@@ -1,5 +1,5 @@
 /*
- * matchmaker_b200 -- C ABI of the B200-native interaction-scoring library.
+ * matchmaker_b200 -- C ABI of the H100-native (sm_90a) interaction-scoring library.
  *
  * This is the drop-in boundary for the query-document interaction hot path of
  * sebastian-hofstaetter/matchmaker.  The reference is pure Python/PyTorch and has no FFI of
@@ -17,7 +17,7 @@
  *     launches are asynchronous with respect to the host and ordered on `stream`;
  *   - tensors are dense row-major ("contiguous" in PyTorch terms) unless a stride is given;
  *   - the library never falls back to a CPU implementation: on a device that is not
- *     compute capability 10.x every compute entry point fails with MMB200_ERR_UNSUPPORTED.
+ *     compute capability 9.0 every compute entry point fails with MMB200_ERR_UNSUPPORTED.
  */
 #ifndef MATCHMAKER_B200_H_
 #define MATCHMAKER_B200_H_
@@ -40,7 +40,7 @@ extern "C" {
 #define MMB200_OK 0
 #define MMB200_ERR_INVALID (-1)     /* bad argument (shape, dtype, alignment, null pointer) */
 #define MMB200_ERR_CUDA (-2)        /* a CUDA runtime / driver call failed */
-#define MMB200_ERR_UNSUPPORTED (-3) /* device is not sm_100, or shape outside kernel limits */
+#define MMB200_ERR_UNSUPPORTED (-3) /* device is not sm_90, or shape outside kernel limits */
 
 /* element types of embedding / vector tensors */
 #define MMB200_F16 0
@@ -58,10 +58,10 @@ extern "C" {
 /* kernel selection for entry points that have more than one device implementation */
 #define MMB200_IMPL_AUTO 0
 #define MMB200_IMPL_SIMT 1    /* CUDA-core kernel, any shape/dtype */
-#define MMB200_IMPL_TCGEN05 2 /* TMA + tcgen05 tensor-core kernel (fails if shape unsupported) */
-#define MMB200_IMPL_TCGEN05_DOCM 3 /* max-sim only: the first-generation "documents on M" tcgen05 kernel */
-#define MMB200_IMPL_TCGEN05_RAGGED 4 /* max-sim only: tcgen05 kernel that fetches each document only up to its
-                                        last unmasked row (padding rows never leave HBM / host memory) */
+#define MMB200_IMPL_TCGEN05 2 /* TMA + wgmma tensor-core kernel (fails if shape unsupported); the name is historical */
+#define MMB200_IMPL_TCGEN05_DOCM 3 /* max-sim only: the "documents on M" tensor-core kernel */
+#define MMB200_IMPL_TCGEN05_RAGGED 4 /* max-sim only: tensor-core kernel that fetches each document only up to its
+                                        last unmasked row (padding rows never leave HBM) */
 
 MMB200_API int mmb200_version(void);
 MMB200_API const char* mmb200_last_error(void);
@@ -113,10 +113,7 @@ MMB200_API int mmb200_maxsim_bwd(const void* q, const void* d, const float* grad
  * gives full PCIe bandwidth, pageable works).  Documents are streamed to the device in chunks
  * on internal streams, overlapped with the kernel; scores are copied back before returning.
  * Synchronous.  Same semantics as mmb200_maxsim_fwd with pair_q = pair_d = NULL.
- * When d_host is pinned (device-mapped) memory and the shape fits the queries-on-M kernel, the
- * documents are not staged at all: the kernel's TMA reads them directly over PCIe, 16 rows at a time, and
- * only up to each document's last unmasked row.  chunk_pairs: 0 = default slab size, -1 = force the
- * staged (slab) pipeline. */
+ * chunk_pairs: documents per slab; 0 or -1 = default slab size (~96 MB). */
 MMB200_API int mmb200_maxsim_fwd_host(const void* q_host, const void* d_host, const void* q_mask_host,
                            const void* d_mask_host, float* out_host, int64_t n_q, int64_t n_d,
                            int32_t docs_per_query, int32_t Lq, int32_t Ld, int32_t dim, int32_t dtype,
@@ -189,12 +186,12 @@ MMB200_API int mmb200_kernel_pool_bwd_ex(const float* q, const float* d, const v
                                          void* stream);
 
 /* Training pair on the tensor cores (the step of train.py:330-360 for KNRM / TK: forward, loss, backward).
- *   mmb200_kernel_pool_fwd_train = mmb200_kernel_pool_fwd_ex (tcgen05 kernel; doc_gate as there, or NULL) that additionally leaves
+ *   mmb200_kernel_pool_fwd_train = mmb200_kernel_pool_fwd_ex (tensor-core kernel; doc_gate as there, or NULL) that additionally leaves
  *   `saved` for the backward: mmb200_kernel_pool_saved_floats(B, Ld) = B * (33 * Ld + 32) floats, 16-byte aligned
  *   (cosines document-row-major [B][Ld][32], then 1 / (|d_j| + eps) [B][Ld], then 1 / (|q_i| + eps) [B][32]); the
  *   layout is private to the pair of calls.
  *   mmb200_kernel_pool_bwd_saved = mmb200_kernel_pool_bwd_ex (doc_gate / grad_gate as there, or NULL) computed from `saved` with both contractions
- *   (G q^ and G^T d^) as kind::tf32 UMMAs on the raw fp32 tiles; gradients agree with the fp32 expression to a few
+ *   (G q^ and G^T d^) as tf32 wgmma on the raw fp32 embeddings; gradients agree with the fp32 expression to a few
  *   1e-4 relative (tf32 operands; the reference trains under fp16 autocast).  grad_q / grad_d must be 16-byte aligned.
  *   Envelope: mmb200_kernel_pool_train_tc_supported(Lq, Ld, D, K) != 0  (Lq <= 32, K <= 32, D % 4 == 0, D <= 320);
  *   outside it both calls return MMB200_ERR_UNSUPPORTED and the caller uses _fwd_ex / _bwd_ex. */
@@ -242,7 +239,7 @@ MMB200_API int mmb200_dot_pairs(const void* q, const void* d, float* out, int64_
  * saturation 1 ("log", :245-246): sat_params[K] = kernel_mult[0]
  * window_score  [B, W] f32 out, W = (C*40 - 30)/2 + 1  (raw dense output, sentinel not yet applied)
  * n_chunks      Nc (rows of `chunks` / `chunk_mask`)
- * impl          MMB200_IMPL_AUTO: the TMA + tcgen05 kernel (Lq * K <= 512) when the kernel set activates on every cosine
+ * impl          MMB200_IMPL_AUTO: the TMA + wgmma kernel (Lq * K <= 512) when the kernel set activates on every cosine
  *               in [-1, 1] -- decided on the device, no host sync -- else the FFMA kernel; _TCGEN05 / _SIMT force one.
  * ------------------------------------------------------------------------------------------ */
 MMB200_API int mmb200_tkl_window_scores(const float* q, const void* q_mask, const float* chunks,

@@ -35,7 +35,7 @@ def maxsim(q: torch.Tensor, d: torch.Tensor, q_mask: Optional[torch.Tensor] = No
     return _MaxSim.apply(q, d, q_mask, d_mask, docs_per_query)
 
 
-# "auto": forward that saves its cosines + tcgen05 backward where the shape allows; "simt": always the FFMA backward
+# "auto": forward that saves its cosines + tensor-core backward where the shape allows; "simt": always the FFMA backward
 KP_TRAIN_IMPL = "auto"
 
 

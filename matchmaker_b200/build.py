@@ -1,4 +1,4 @@
-"""Build ``libmatchmaker_b200.so`` (hand-written CUDA for sm_100a + the C ABI) in-tree.
+"""Build ``libmatchmaker_b200.so`` (hand-written CUDA for sm_90a + the C ABI) in-tree.
 
     python -m matchmaker_b200.build [--force] [--verbose]
 
@@ -24,7 +24,7 @@ LIB_PATH = os.path.join(CSRC, LIB_NAME)
 OBJ_DIR = os.path.join(CSRC, "build")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "-Xcompiler", "-fvisibility=hidden",
@@ -61,8 +61,8 @@ def _all_inputs():
 
 
 def build(force: bool = False, verbose: bool = False, prof: bool = False) -> str:
-    """prof=True adds -DMMB200_ENABLE_PROF: the MMB200_*_PROF / MMB200_KP_RAW debugging switches (they allocate and
-    synchronise inside the launch path) exist only in such a build, never in the product library."""
+    """prof=True adds -DMMB200_ENABLE_PROF: the MMB200_*_PROF debugging switches (they allocate and synchronise inside
+    the launch path) exist only in such a build, never in the product library."""
     stamp = os.path.join(OBJ_DIR, "stamp.sha256")
     digest = _digest(_all_inputs()) + ("+prof" if prof else "")
     if not force and os.path.isfile(LIB_PATH) and os.path.isfile(stamp) and open(stamp).read() == digest:
@@ -83,7 +83,7 @@ def build(force: bool = False, verbose: bool = False, prof: bool = False) -> str
 
     with ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1)) as ex:
         objs = list(ex.map(compile_one, sources()))
-    link = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static",
+    link = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static",
             "-Xcompiler", "-fPIC", "-o", LIB_PATH, *objs]
     r = subprocess.run(link, capture_output=True, text=True)
     if r.returncode != 0:

@@ -60,8 +60,8 @@ extern "C" int mmb200_dot_pairs(const void* q, const void* d, float* out, int64_
   if (B == 0) return MMB200_OK;
   DeviceInfo dev;
   if (int rc = current_device_info(&dev)) return rc;
-  if (!is_sm100(dev)) {
-    set_error("matchmaker_b200 kernels are built for sm_100a only");
+  if (!is_sm90(dev)) {
+    set_error("matchmaker_b200 kernels are built for sm_90a only");
     return MMB200_ERR_UNSUPPORTED;
   }
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);

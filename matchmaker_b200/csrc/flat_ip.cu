@@ -7,19 +7,18 @@
 //
 //   flat_ip_tc_kernel   persistent CTAs over work items (block of 128 queries) x (range of passages); clusters of 2
 //               CTAs take consecutive query blocks and share every passage tile by TMA multicast.
-//       warp 0  TMA producer: per k-block one 16 KB query tile + this CTA's slice of the 32 KB passage tile
-//       warp 1  tcgen05.mma issuer (whole-warp loop, elect.sync): D[128 queries x 256 passages] fp32 in TMEM, 2 slots
-//       warps 2-9 epilogue: two warps per TMEM lane quarter, each filtering one 128-column half of every tile, thread =
-//               query row: tcgen05.ld, FMNMX tree -> maxima of 8-column sub-groups, compare against the row's running
-//               threshold tau (the k-th best seen so far); sub-groups holding a candidate for SOME row of the warp (~1/3
-//               of them) are scanned with warp-uniform control flow and a predicated shared-memory atomic + global
-//               store into the row's candidate list (ONE list per row, capacity 1024, global memory).  The pair of
-//               warps meets at a named barrier at the start of every tile; rows whose list could overflow during the
-//               tile are compacted there (split between the two warps): 32-step bisection on the order-preserving
-//               integer image of the scores finds the k-th largest, survivors are rewritten in place and tau rises.
-//               tau is also published per query (atomicMax) so items working on other passage ranges of the same
-//               queries filter harder.  The per-tile loop must stay inside the instruction cache (compact_row is
-//               __noinline__).
+//       warp 8  TMA producer: per k-block one 16 KB query tile + this CTA's slice of the 16 KB passage tile
+//       warpgroups 0, 1  wgmma m64n128k16: warpgroup c scores query rows 64c .. 64c + 63 against the 128 passages of a
+//               tile (fp32 registers) and writes them to a shared-memory score tile; then its four warps filter them,
+//               thread = query row, one 64-column half per warp: FMNMX tree -> maxima of 8-column sub-groups, compare
+//               against the row's running threshold tau (the k-th best seen so far); sub-groups holding a candidate for
+//               SOME row of the warp are scanned with warp-uniform control flow and a predicated shared-memory atomic +
+//               global store into the row's candidate list (ONE list per row, capacity 1024, global memory).  The pair of
+//               warps of a row quarter meets at a named barrier at the start of every tile; rows whose list could
+//               overflow during the tile are compacted there (split between the two warps): 32-step bisection on the
+//               order-preserving integer image of the scores finds the k-th largest, survivors are rewritten in place
+//               and tau rises.  tau is also published per query (atomicMax) so items working on other passage ranges
+//               of the same queries filter harder.  compact_row is __noinline__ to keep the per-tile loop small.
 //   topk_merge_kernel   per query: bitonic sort of the candidate lists of all ranges (or, after the NCCL
 //       all-gather, of all ranks) under the total order (score desc, id asc) -> [k] scores + ids.
 //
@@ -32,6 +31,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
+#include <type_traits>
 
 #include "host_util.cuh"
 #include "ptx.cuh"
@@ -40,27 +40,23 @@ namespace mmb {
 
 namespace {
 
-constexpr int kEpiPerQuarter = 2;        // epilogue warps per TMEM lane quarter (column halves of a tile, ONE list per row)
-constexpr int kThreads = 64 + 128 * kEpiPerQuarter;  // TMA warp, MMA warp, 8 epilogue warps
+constexpr int kThreads = 384;            // two consumer warpgroups (warps 0-7), TMA warp 8 (warps 9-11 idle)
+constexpr int kRegsProducer = 40, kRegsConsumer = 232;  // setmaxnreg: 128 x 40 + 256 x 232 <= 384 x 168 (the launch)
 // list entries per lane in a compaction: EPL = 32 -> capacity 1024 per row (k <= 256), EPL = 64 -> 2048 (k <= 1024)
 constexpr int kMaxK = 1024;
 __host__ __device__ constexpr int epl_for_k(int k) { return k <= 256 ? 32 : 64; }
-constexpr int BM = 128;                 // queries per block (UMMA M)
-constexpr int BN = 256;                 // passages per tile (UMMA N)
+constexpr int BM = 128;                 // queries per block (two wgmma M = 64 halves)
+constexpr int BN = 128;                 // passages per tile (wgmma N)
 constexpr int kABytes = BM * 128;       // one k-block (64 halfs) of the query tile
 constexpr int kBBytes = BN * 128;
-constexpr int kStageBytes = kABytes + kBBytes;  // 48 KB
+constexpr int kStageBytes = kABytes + kBBytes;  // 32 KB
 constexpr int kStages = 4;
-constexpr int kAccSlots = 2;
+constexpr int kCsStride = BN + 4;       // floats per row of the score tile: 16-byte row reads by 8 threads hit 32 banks
 constexpr int kMaxRanges = 32;
 
 struct FipShared {
   uint64_t full[kStages];
   uint64_t empty[kStages];
-  uint64_t accfull[kAccSlots];
-  uint64_t accempty[kAccSlots];
-  uint32_t tmem_base;
-  uint32_t pad;
   int cnt[BM];        // entries in each row's candidate list (appended to by both warps of the row's quarter)
   uint32_t tau[BM];   // order-preserving image of each row's threshold
 };
@@ -72,7 +68,6 @@ struct FipParams {
   int32_t dim, k, kpad;             // kpad = k rounded up to 32 (list capacity per row is 32 * EPL)
   int32_t kblocks, kb_wrap;         // k-blocks of 64 along the QUERY rows; passage k-block = kb < kb_wrap ? kb : kb - kb_wrap
   int32_t n_qblocks, n_ranges, tiles_per_range, n_tiles;
-  int32_t fmt;
   uint2* lists;             // [grid][BM][cap]  (score bits, position)
   uint32_t* tau_glob;       // [nq] order-preserving image of the per-query threshold
   float* cand_scores;       // [nq][n_ranges * kpad]
@@ -189,31 +184,28 @@ __device__ __noinline__ int compact_row(const FipParams& P, uint2* list, int cnt
 
 // CL = thread-block cluster size.  The CL CTAs of a cluster work on CL consecutive query blocks against the SAME passage
 // tiles: each CTA fetches 1/CL of every passage tile and multicasts it to the whole cluster, so the L2 -> SM traffic per
-// CTA drops from 48 KB to (16 + 32 / CL) KB per k-block (7.2 TB/s of L2 reads at CL = 1).  A stage may be refilled only
-// when EVERY CTA of the cluster has consumed it, hence the multicast commit onto all `empty` barriers (count CL).
-// PROF (MMB200_FLATIP_PROF=1): debugging aid, one thread per role of CTA 0 accumulates the cycles it spends blocked
-#define FIP_TIMED(slot, stmt)                                 \
-  do {                                                        \
-    if constexpr (PROF) {                                     \
-      const long long t0_ = clock64();                        \
-      stmt;                                                   \
-      pc[slot] += clock64() - t0_;                            \
-    } else {                                                  \
-      stmt;                                                   \
-    }                                                         \
-  } while (0)
+// CTA drops from 32 KB to (16 + 16 / CL) KB per k-block.  A stage may be refilled only when EVERY CTA of the cluster has
+// consumed it, hence the consumers arrive on the `empty` barriers of all CTAs (count 8 * CL).
+template <typename T>
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc);
+template <>
+__device__ __forceinline__ void wgmma_n128<__half>(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) {
+  wgmma_m64n128k16_f16(d, a, b, acc);
+}
+template <>
+__device__ __forceinline__ void wgmma_n128<__nv_bfloat16>(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) {
+  wgmma_m64n128k16_bf16(d, a, b, acc);
+}
 
-template <int CL, bool PROF = false, int EPL = 32>
+template <typename T, int CL, int EPL = 32>
 __global__ void __launch_bounds__(kThreads, 1)
-flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_p, FipParams P,
-                  long long* prof = nullptr) {
-  long long pc[3] = {0, 0, 0};
-  const long long t_start = PROF ? clock64() : 0;
+flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_p, FipParams P) {
   extern __shared__ uint8_t smem_raw[];
   // 1024-B alignment for SWIZZLE_128B tiles, derived by pointer arithmetic on the __shared__ array so the
   // compiler keeps the shared address space (LDS/STS instead of generic LD/ST)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  FipShared* S = reinterpret_cast<FipShared*>(smem + (size_t)kStages * kStageBytes);
+  float* cs = reinterpret_cast<float*>(smem + (size_t)kStages * kStageBytes);     // [BM][kCsStride] score tile
+  FipShared* S = reinterpret_cast<FipShared*>(cs + BM * kCsStride);
   constexpr int kCap = 32 * EPL;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int kblocks = P.kblocks;
@@ -226,97 +218,67 @@ flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
   if (threadIdx.x == 0) {
     prefetch_tensormap(&tmap_q);
     prefetch_tensormap(&tmap_p);
-    for (int s = 0; s < kStages; ++s) { mbar_init(&S->full[s], 1); mbar_init(&S->empty[s], CL); }
-    for (int s = 0; s < kAccSlots; ++s) { mbar_init(&S->accfull[s], 1); mbar_init(&S->accempty[s], 4 * kEpiPerQuarter); }
+    for (int s = 0; s < kStages; ++s) { mbar_init(&S->full[s], 1); mbar_init(&S->empty[s], 8 * CL); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(&S->tmem_base, 512);
-  tc_fence_before_sync();
   if (CL > 1) cluster_sync_all(); else __syncthreads();   // peers signal our barriers: their init must be visible cluster-wide
-  tc_fence_after_sync();
-  const uint32_t tmem_base = S->tmem_base;
 
-  if (warp == 0) {
+  if (warp >= 8) {
+    setmaxnreg_dec<kRegsProducer>();
+  }
+  if (warp == 8) {
     // the whole warp walks the loop (uniform control flow and operands); one elected lane issues the TMA: inside an
-    // `if (lane == 0)` region the compiler wraps every TMA / MMA in an ELECT / R2UR waterfall loop (ptx.cuh)
-    {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int item = cluster_id; item < n_items; item += n_clusters) {
-        const int rg = item / n_qgroups, qb = (item % n_qgroups) * CL + rank;  // range-major: co-running CTAs share passages
-        const int t0 = rg * P.tiles_per_range, t1 = min(P.n_tiles, t0 + P.tiles_per_range);
-        for (int t = t0; t < t1; ++t) {
-          for (int kb = 0; kb < kblocks; ++kb) {
-            FIP_TIMED(0, mbar_wait(&S->empty[stage], phase ^ 1u));
-            uint8_t* st = smem + (size_t)stage * kStageBytes;
-            if (elect_one_sync()) {
-              mbar_arrive_expect_tx(&S->full[stage], (uint32_t)kStageBytes);
-              const int kbp = kb < P.kb_wrap ? kb : kb - P.kb_wrap;   // fp32-split storage: [q_hi|q_lo|q_hi] x [p_hi|p_hi|p_lo]
-              tma_load_2d(&tmap_q, st, &S->full[stage], kb * 64, qb * BM, kEvictLast);
-              if (CL == 1)
-                tma_load_2d(&tmap_p, st + kABytes, &S->full[stage], kbp * 64, t * BN, kEvictFirst);
-              else  // this CTA's slice of the passage tile, written into every CTA of the cluster
-                tma_load_2d_multicast(&tmap_p, st + kABytes + rank * (kBBytes / CL), &S->full[stage], kbp * 64,
-                                      t * BN + rank * (BN / CL), kAllCtas, kEvictFirst);
-            }
-            __syncwarp();
-            if (++stage == kStages) { stage = 0; phase ^= 1u; }
+    // `if (lane == 0)` region the compiler wraps every TMA in an ELECT / R2UR waterfall loop (ptx.cuh)
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int item = cluster_id; item < n_items; item += n_clusters) {
+      const int rg = item / n_qgroups, qb = (item % n_qgroups) * CL + rank;  // range-major: co-running CTAs share passages
+      const int t0 = rg * P.tiles_per_range, t1 = min(P.n_tiles, t0 + P.tiles_per_range);
+      for (int t = t0; t < t1; ++t) {
+        for (int kb = 0; kb < kblocks; ++kb) {
+          mbar_wait(&S->empty[stage], phase ^ 1u);
+          uint8_t* st = smem + (size_t)stage * kStageBytes;
+          if (elect_one_sync()) {
+            mbar_arrive_expect_tx(&S->full[stage], (uint32_t)kStageBytes);
+            const int kbp = kb < P.kb_wrap ? kb : kb - P.kb_wrap;   // fp32-split storage: [q_hi|q_lo|q_hi] x [p_hi|p_hi|p_lo]
+            tma_load_2d(&tmap_q, st, &S->full[stage], kb * 64, qb * BM, kEvictLast);
+            if (CL == 1)
+              tma_load_2d(&tmap_p, st + kABytes, &S->full[stage], kbp * 64, t * BN, kEvictFirst);
+            else  // this CTA's slice of the passage tile, written into every CTA of the cluster
+              tma_load_2d_multicast(&tmap_p, st + kABytes + rank * (kBBytes / CL), &S->full[stage], kbp * 64,
+                                    t * BN + rank * (BN / CL), kAllCtas, kEvictFirst);
           }
+          __syncwarp();
+          if (++stage == kStages) { stage = 0; phase ^= 1u; }
         }
       }
     }
-  } else if (warp == 1) {
-    {
-      const uint32_t idesc = make_idesc((uint32_t)P.fmt, BM, BN);
-      int stage = 0, acc = 0;
-      uint32_t phase = 0, accphase = 0;
-      for (int item = cluster_id; item < n_items; item += n_clusters) {
-        const int rg = item / n_qgroups;
-        const int t0 = rg * P.tiles_per_range, t1 = min(P.n_tiles, t0 + P.tiles_per_range);
-        for (int t = t0; t < t1; ++t) {
-          FIP_TIMED(0, mbar_wait(&S->accempty[acc], accphase ^ 1u));
-          tc_fence_after_sync();
-          const uint32_t tmem_d = tmem_base + (uint32_t)(acc * BN);
-          for (int kb = 0; kb < kblocks; ++kb) {
-            FIP_TIMED(1, mbar_wait(&S->full[stage], phase));
-            tc_fence_after_sync();
-            const long long t_i = PROF ? clock64() : 0;
-            const uint32_t a = smem_u32(smem + (size_t)stage * kStageBytes);
-            const uint64_t da = make_sw128_kmajor_desc(a), db = make_sw128_kmajor_desc(a + kABytes);
-            if (elect_one_sync()) {
-#pragma unroll
-              for (int k = 0; k < 4; ++k)  // +32 bytes along K inside the 128-byte swizzle atom = +2 in the address field
-                umma_f16(tmem_d, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (uint32_t)((kb | k) != 0));
-              if (CL == 1) umma_commit(&S->empty[stage]); else umma_commit_multicast(&S->empty[stage], kAllCtas);
-              if (kb == kblocks - 1) umma_commit(&S->accfull[acc]);
-            }
-            __syncwarp();
-            if (PROF) pc[2] += clock64() - t_i;
-            if (++stage == kStages) { stage = 0; phase ^= 1u; }
-          }
-          if (++acc == kAccSlots) { acc = 0; accphase ^= 1u; }
-        }
-      }
-    }
-  } else {
-    // ------------------------------- epilogue: filter + top-k lists ---------------------------------
-    // Two warps per TMEM lane quarter (one epilogue warp per scheduler runs its dependent chains at ~0.2 IPC and cannot
-    // keep up with the tensor pipe): warp (quarter, half) filters columns [128 half, 128 half + 128) of every tile.  Both
-    // append to the SAME per-row list (shared-memory counter, atomicAdd) under the SAME threshold, so nothing about the
-    // selection changes.  The pair meets at a named barrier at the start of every tile: counters are final there, both
-    // warps see the same set of nearly-full rows and split their compaction.  A row gains at most 256 entries per
-    // tile, so compacting when cnt > cap - 256 keeps every append in bounds.
-    const int quarter = warp & 3;
-    const int half = (warp - 2) >> 2;
-    const int row = quarter * 32 + lane;  // query row inside the block == TMEM lane
+  } else if (warp < 8) {
+    // ------------------------------- consumers: wgmma, then filter + top-k lists ----------------------------
+    // Warpgroup c computes the scores of query rows 64c .. 64c + 63 (wgmma m64n128k16, registers) and writes them to the
+    // score tile; its four warps then filter them like this, thread = query row: warp (quarter, half) takes rows
+    // [32 quarter, +32) and columns [64 half, +64) of every tile.  Both warps of a quarter append to the SAME per-row
+    // list (shared-memory counter, atomicAdd) under the SAME threshold, so nothing about the selection changes.  The pair
+    // meets at a named barrier at the start of every tile: counters are final there, both warps see the same set of
+    // nearly-full rows and split their compaction.  A row gains at most BN entries per tile, so compacting when
+    // cnt > cap - BN keeps every append in bounds.
+    setmaxnreg_inc<kRegsConsumer>();
+    const int c = warp >> 2;
+    const int wq = warp & 3;
+    const int quarter = 2 * c + (wq & 1);
+    const int half = wq >> 1;
+    const int row = quarter * 32 + lane;  // query row inside the block
     const uint32_t pair_bar = 1u + (uint32_t)quarter;
-    int acc = 0;
-    uint32_t accphase = 0;
+    const uint32_t wg_bar = 5u + (uint32_t)c;
+    int stage = 0;
+    uint32_t phase = 0;
     uint2* my_list = P.lists + ((size_t)blockIdx.x * BM + row) * kCap;
     uint2* warp_lists = P.lists + ((size_t)blockIdx.x * BM + quarter * 32) * kCap;
     int* cnt_s = S->cnt + quarter * 32;
     uint32_t* tau_s = S->tau + quarter * 32;
     const uint32_t my_cnt_addr = smem_u32(cnt_s + lane);
+    const int fr0 = 64 * c + 16 * wq + (lane >> 2);   // score-tile rows of this thread's accumulator fragment: fr0, fr0 + 8
+    const int fc0 = 2 * (lane & 3);
     for (int item = cluster_id; item < n_items; item += n_clusters) {
       const int rg = item / n_qgroups, qb = (item % n_qgroups) * CL + rank;  // range-major: co-running CTAs share passages
       const int t0 = rg * P.tiles_per_range, t1 = min(P.n_tiles, t0 + P.tiles_per_range);
@@ -325,9 +287,53 @@ flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
       uint32_t tau_seen = live ? P.tau_glob[q] : 0xffffffffu;  // dead rows accept nothing
       if (half == 0) { cnt_s[lane] = 0; tau_s[lane] = tau_seen; }
       for (int t = t0; t < t1; ++t) {
-        FIP_TIMED(0, mbar_wait(&S->accfull[acc], accphase));
-        tc_fence_after_sync();
-        const long long t_e = PROF ? clock64() : 0;
+        {  // scores of the tile: 64 rows x 128 passages per warpgroup
+          float acc[64];
+#pragma unroll
+          for (int j = 0; j < 64; ++j) acc[j] = 0.f;
+          // one k-block's MMAs stay in flight while the next k-block is issued; a stage is released once its MMAs are done
+          auto release = [&](int st) {
+            __syncwarp();
+            if (lane == 0) {
+              if (CL == 1) mbar_arrive(&S->empty[st]);
+              else
+                for (int r = 0; r < CL; ++r) mbar_arrive_cluster(&S->empty[st], (uint32_t)r);
+            }
+          };
+          int prev = -1;
+          for (int kb = 0; kb < kblocks; ++kb) {
+            mbar_wait(&S->full[stage], phase);
+            const uint32_t a = smem_u32(smem + (size_t)stage * kStageBytes);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 4; ++k)  // +32 bytes along K inside the 128-byte swizzle atom
+              wgmma_n128<T>(acc, make_wgmma_sw128_desc(a + 64 * c * 128 + 32 * k), make_wgmma_sw128_desc(a + kABytes + 32 * k), 1u);
+            wgmma_commit();
+            wgmma_wait<1>();
+            if (prev >= 0) release(prev);
+            prev = stage;
+            if (++stage == kStages) { stage = 0; phase ^= 1u; }
+          }
+          wgmma_wait<0>();
+          release(prev);
+          wgmma_fence_regs(acc);
+          named_bar_sync(wg_bar, 128);     // every warp of the warpgroup has read the previous tile's scores
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
+            *reinterpret_cast<float2*>(cs + fr0 * kCsStride + 8 * j + fc0) = make_float2(acc[4 * j], acc[4 * j + 1]);
+            *reinterpret_cast<float2*>(cs + (fr0 + 8) * kCsStride + 8 * j + fc0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+          }
+          named_bar_sync(wg_bar, 128);
+        }
+        // this warp's 64 columns of its row into registers
+        uint32_t r4[BN / 2 / 32][32];
+#pragma unroll
+        for (int cc = 0; cc < BN / 2 / 32; ++cc)
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const uint4 v = *reinterpret_cast<const uint4*>(cs + row * kCsStride + half * (BN / 2) + cc * 32 + 4 * j);
+            r4[cc][4 * j] = v.x; r4[cc][4 * j + 1] = v.y; r4[cc][4 * j + 2] = v.z; r4[cc][4 * j + 3] = v.w;
+          }
         if (half == 0 && live) tau_s[lane] = max(tau_s[lane], tau_seen);   // other ranges' progress, fetched a tile ago
         named_bar_sync(pair_bar, 64);      // appends of the previous tile are complete, counters and thresholds final
         if (live) tau_seen = *reinterpret_cast<volatile const uint32_t*>(P.tau_glob + q);  // consumed one tile later
@@ -351,22 +357,12 @@ flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
           named_bar_sync(pair_bar, 64);
         }
         const float tau = key2f(tau_s[lane]);
-        const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * BN + half * (BN / 2));
         const int64_t col0 = (int64_t)t * BN + half * (BN / 2);
         const bool ragged = (int64_t)t * BN + BN > P.n_pass;
-        // all 128 columns of this warp into registers, then the accumulator slot goes straight back to the MMA warp:
-        // with two slots the tensor pipe otherwise idles while the filter below works its way through the tile
-        uint32_t r4[BN / 2 / 32][32];
 #pragma unroll
-        for (int c = 0; c < BN / 2 / 32; ++c) tmem_ld_32x32b_x32(taddr + c * 32, r4[c]);
-        tmem_ld_wait();
-        tc_fence_before_sync();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&S->accempty[acc]);
-#pragma unroll
-        for (int c = 0; c < BN / 2 / 32; ++c) {
-          uint32_t (&r)[32] = r4[c];
-          const uint32_t pbase = (uint32_t)(col0 + c * 32);
+        for (int cc = 0; cc < BN / 2 / 32; ++cc) {
+          uint32_t (&r)[32] = r4[cc];
+          const uint32_t pbase = (uint32_t)(col0 + cc * 32);
           // A row sees a candidate in a few % of its 32-column groups, but SOME row of the warp does in most of them,
           // so the path behind the maxima has to be cheap for the idle lanes too: four sub-groups of 8 whose maxima
           // come out of one FMNMX tree, votes issued back to back, and only sub-groups with a candidate are scanned --
@@ -413,11 +409,8 @@ flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
             }
           }
         }
-        if (PROF) pc[1] += clock64() - t_e;
-        if (++acc == kAccSlots) { acc = 0; accphase ^= 1u; }
       }
       // item done: final compaction of every row (split between the two warps), then publish (score, id) candidates
-      const long long t_f = PROF ? clock64() : 0;
       named_bar_sync(pair_bar, 64);
       for (int rr = half; rr < 32; rr += 2) {
         uint32_t kth;
@@ -426,15 +419,15 @@ flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
         if (qq < P.nq) {
           if (lane == 0 && nc == P.k) atomicMax(P.tau_glob + qq, kth);
           const uint2* lst = warp_lists + (size_t)rr * kCap;
-          float* cs = P.cand_scores + (size_t)qq * P.n_ranges * P.kpad + (size_t)rg * P.kpad;
+          float* cso = P.cand_scores + (size_t)qq * P.n_ranges * P.kpad + (size_t)rg * P.kpad;
           int64_t* ci = P.cand_ids + (size_t)qq * P.n_ranges * P.kpad + (size_t)rg * P.kpad;
           for (int e = lane; e < P.kpad; e += 32) {
             if (e < nc) {
               const uint2 v = lst[e];
-              cs[e] = __uint_as_float(v.x);
+              cso[e] = __uint_as_float(v.x);
               ci[e] = pos_to_id(P, v.y);
             } else {
-              cs[e] = -INFINITY;
+              cso[e] = -INFINITY;
               ci[e] = -1;
             }
           }
@@ -442,24 +435,12 @@ flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
         __syncwarp();
       }
       named_bar_sync(pair_bar, 64);   // the counters are reset by the next item only after both warps are done with them
-      if (PROF) pc[2] += clock64() - t_f;
     }
-    if (PROF && blockIdx.x == 0 && threadIdx.x == 64) { prof[5] = pc[0]; prof[6] = pc[1]; prof[7] = pc[2]; }
-  }
-  if (PROF && blockIdx.x == 0 && lane == 0) {
-    if (warp == 0) prof[0] = pc[0];
-    if (warp == 1) { prof[1] = pc[0]; prof[2] = pc[1]; prof[3] = pc[2]; }
   }
 
-  tc_fence_before_sync();
   if (CL > 1) cluster_sync_all(); else __syncthreads();   // no CTA may exit while peers still multicast into it
-  if (PROF && blockIdx.x == 0 && threadIdx.x == 0) prof[4] = clock64() - t_start;
-  if (warp == 1) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 512);
-  }
 }
-#undef FIP_TIMED
+
 
 // ---------------------------------------------------------------------------------------------
 // merge: per query, sort L candidates by (score desc, id asc), emit the first k.
@@ -686,8 +667,8 @@ extern "C" int mmb200_flat_ip_topk(const void* queries, const void* passages, co
   MMB_REQUIRE(((reinterpret_cast<uintptr_t>(queries) | reinterpret_cast<uintptr_t>(passages)) & 15) == 0, "16-byte alignment");
   DeviceInfo dev;
   if (int rc = current_device_info(&dev)) return rc;
-  if (!is_sm100(dev)) {
-    set_error("matchmaker_b200 kernels are built for sm_100a only");
+  if (!is_sm90(dev)) {
+    set_error("matchmaker_b200 kernels are built for sm_90a only");
     return MMB200_ERR_UNSUPPORTED;
   }
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
@@ -722,7 +703,6 @@ extern "C" int mmb200_flat_ip_topk(const void* queries, const void* passages, co
     P.cand_ids = reinterpret_cast<int64_t*>(w);
     P.ids = pass_ids; P.id_base = pass_id_base; P.nq = nq; P.n_pass = n_rows; P.dim = dim; P.k = k; P.kpad = pp.kpad;
     P.n_qblocks = pp.n_qblocks; P.n_ranges = pp.n_ranges; P.tiles_per_range = pp.tiles_per_range; P.n_tiles = pp.n_tiles;
-    P.fmt = dtype == MMB200_BF16 ? kFmtBF16 : kFmtF16;
     P.kblocks = (int32_t)(q_cols / 64);
     P.kb_wrap = split ? dim / 64 : P.kblocks;
     CUtensorMap tp;
@@ -734,7 +714,7 @@ extern "C" int mmb200_flat_ip_topk(const void* queries, const void* passages, co
                                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B))
         return rc;
     }
-    const size_t smem = (size_t)kStages * kStageBytes + sizeof(FipShared) + 1024;
+    const size_t smem = (size_t)kStages * kStageBytes + (size_t)BM * kCsStride * sizeof(float) + sizeof(FipShared) + 1024;
     auto launch = [&](auto kernel) -> int {
       MMB_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
       cudaLaunchConfig_t cfg{};
@@ -749,35 +729,21 @@ extern "C" int mmb200_flat_ip_topk(const void* queries, const void* passages, co
       attr.val.clusterDim.z = 1;
       cfg.attrs = &attr;
       cfg.numAttrs = 1;
-      MMB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel, tq, tp, P, (long long*)nullptr));
+      MMB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel, tq, tp, P));
       return MMB200_OK;
     };
     if (out_params) *out_params = P;
-#ifdef MMB200_ENABLE_PROF
-    if (pp.cl == 1 && out_params && epl_for_k(k) == 32 && getenv("MMB200_FLATIP_PROF")) {  // debugging aid: per-role wait cycles
-      long long* prof = nullptr;
-      long long h[12] = {0};
-      MMB_CHECK_CUDA(cudaMalloc(&prof, sizeof(h)));
-      MMB_CHECK_CUDA(cudaMemset(prof, 0, sizeof(h)));
-      MMB_CHECK_CUDA(cudaFuncSetAttribute(flat_ip_tc_kernel<1, true, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      flat_ip_tc_kernel<1, true, 32><<<pp.grid, kThreads, smem, stream>>>(tq, tp, P, prof);
-      MMB_CHECK_CUDA(cudaStreamSynchronize(stream));
-      MMB_CHECK_CUDA(cudaMemcpy(h, prof, sizeof(h), cudaMemcpyDeviceToHost));
-      MMB_CHECK_CUDA(cudaFree(prof));
-      fprintf(stderr,
-              "fip_prof cycles: total %lld | tma wait_empty %lld | mma wait_accempty %lld wait_full %lld issue %lld | "
-              "epi wait_accfull %lld tile %lld item_end %lld\n",
-              h[4], h[0], h[1], h[2], h[3], h[5], h[6], h[7]);
-      return MMB200_OK;
-    }
-#endif
-    if (epl_for_k(k) == 32)
-      return pp.cl == 1   ? launch(flat_ip_tc_kernel<1, false, 32>)
-             : pp.cl == 2 ? launch(flat_ip_tc_kernel<2, false, 32>)
-                          : launch(flat_ip_tc_kernel<4, false, 32>);
-    return pp.cl == 1   ? launch(flat_ip_tc_kernel<1, false, 64>)
-           : pp.cl == 2 ? launch(flat_ip_tc_kernel<2, false, 64>)
-                        : launch(flat_ip_tc_kernel<4, false, 64>);
+    auto by_cluster = [&](auto t, auto epl) -> int {
+      using T = decltype(t);
+      constexpr int E = decltype(epl)::value;
+      return pp.cl == 1   ? launch(flat_ip_tc_kernel<T, 1, E>)
+             : pp.cl == 2 ? launch(flat_ip_tc_kernel<T, 2, E>)
+                          : launch(flat_ip_tc_kernel<T, 4, E>);
+    };
+    using E32 = std::integral_constant<int, 32>;
+    using E64 = std::integral_constant<int, 64>;
+    if (dtype == MMB200_BF16) return epl_for_k(k) == 32 ? by_cluster(__nv_bfloat16{}, E32{}) : by_cluster(__nv_bfloat16{}, E64{});
+    return epl_for_k(k) == 32 ? by_cluster(__half{}, E32{}) : by_cluster(__half{}, E64{});
   };
 
   FipParams P{};
@@ -793,8 +759,8 @@ extern "C" int mmb200_topk_merge(const float* cand_scores, const int64_t* cand_i
   if (nq == 0) return MMB200_OK;
   DeviceInfo dev;
   if (int rc = current_device_info(&dev)) return rc;
-  if (!is_sm100(dev)) {
-    set_error("matchmaker_b200 kernels are built for sm_100a only");
+  if (!is_sm90(dev)) {
+    set_error("matchmaker_b200 kernels are built for sm_90a only");
     return MMB200_ERR_UNSUPPORTED;
   }
   return launch_merge(cand_scores, cand_ids, nq, n_candidates, k, out_scores, out_ids, dev, static_cast<cudaStream_t>(stream_));

@@ -43,8 +43,8 @@ struct DeviceInfo {
 // Properties of the current device (cached per device id).  Returns nonzero on failure.
 int current_device_info(DeviceInfo* out);
 
-// True when the current device can run the sm_100a tcgen05/TMA kernels.
-inline bool is_sm100(const DeviceInfo& d) { return d.cc_major == 10; }
+// True when the current device can run the sm_90a wgmma/TMA kernels (sm_90a code loads on compute capability 9.0 only).
+inline bool is_sm90(const DeviceInfo& d) { return d.cc_major == 9 && d.cc_minor == 0; }
 
 // cuTensorMapEncodeTiled through cudaGetDriverEntryPoint; returns nonzero on failure.
 int encode_tensor_map(CUtensorMap* map, CUtensorMapDataType dtype, uint32_t rank, const void* base,

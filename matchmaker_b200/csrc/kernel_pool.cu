@@ -11,7 +11,7 @@
 //
 // This file is the fp32-exact FFMA implementation: one CTA per pair, the normalised query block
 // (32 rows) resident in shared memory, document rows streamed in tiles.  It serves every shape and is the
-// validated baseline for the tensor-core kernels: forward kernel_pool_ts.cu, backward kernel_pool_bwd_tc.cu (the
+// validated baseline for the tensor-core kernels: forward kernel_pool_ts.cu, backward kernel_pool_bwd_wg.cu (the
 // training pair mmb200_kernel_pool_fwd_train / _bwd_saved below routes to them).
 #include <algorithm>
 
@@ -509,7 +509,7 @@ extern "C" int mmb200_kernel_pool_fwd(const float* q, const float* d, const void
 }
 
 namespace mmb {
-// the envelope of the tcgen05 training pair (forward that saves its cosines + backward that consumes them)
+// the envelope of the tensor-core training pair (forward that saves its cosines + backward that consumes them)
 static bool kp_train_tc_shape_ok(int Lq, int Ld, int D, int K) {
   return Lq >= 1 && Lq <= 32 && Ld >= 1 && K >= 1 && K <= 32 && D >= 4 && D % 4 == 0 && D <= 320;
 }
@@ -551,7 +551,7 @@ extern "C" int mmb200_kernel_pool_fwd_train(const float* q, const float* d, cons
   using namespace mmb;
   MMB_REQUIRE(saved != nullptr && per_kernel_query != nullptr, "saved and per_kernel_query must be non-null");
   if (!kp_train_tc_shape_ok(Lq, Ld, D, K)) {
-    set_error("kernel_pool_fwd_train: shape outside the tcgen05 training envelope (Lq <= 32, K <= 32, D % 4 == 0, D <= 320)");
+    set_error("kernel_pool_fwd_train: shape outside the tensor-core training envelope (Lq <= 32, K <= 32, D % 4 == 0, D <= 320)");
     return MMB200_ERR_UNSUPPORTED;
   }
   return kp_fwd_impl(q, d, q_mask, d_mask, doc_gate, mu, sigma, alpha, weight, score, per_kernel, per_kernel_query, nullptr,
@@ -568,7 +568,7 @@ extern "C" int mmb200_kernel_pool_bwd_saved(const float* q, const float* d, cons
   using namespace mmb;
   MMB_REQUIRE(saved != nullptr, "saved must be non-null");
   if (!kp_train_tc_shape_ok(Lq, Ld, D, K)) {
-    set_error("kernel_pool_bwd_saved: shape outside the tcgen05 training envelope (Lq <= 32, K <= 32, D % 4 == 0, D <= 320)");
+    set_error("kernel_pool_bwd_saved: shape outside the tensor-core training envelope (Lq <= 32, K <= 32, D % 4 == 0, D <= 320)");
     return MMB200_ERR_UNSUPPORTED;
   }
   return kp_bwd_impl(q, d, q_mask, d_mask, doc_gate, mu, sigma, alpha, weight, per_kernel_query, saved, grad_score, grad_q,
@@ -594,8 +594,8 @@ static int mmb::kp_fwd_impl(const float* q, const float* d, const void* q_mask, 
   if (B == 0) return MMB200_OK;
   DeviceInfo dev;
   if (int rc = current_device_info(&dev)) return rc;
-  if (!is_sm100(dev)) {
-    set_error("matchmaker_b200 kernels are built for sm_100a only");
+  if (!is_sm90(dev)) {
+    set_error("matchmaker_b200 kernels are built for sm_90a only");
     return MMB200_ERR_UNSUPPORTED;
   }
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
@@ -604,7 +604,7 @@ static int mmb::kp_fwd_impl(const float* q, const float* d, const void* q_mask, 
     int rc = kernel_pool_fwd_ts(P, dev, stream, &handled);
     if (handled) return rc;
     if (impl == MMB200_IMPL_TCGEN05) {
-      if (rc == MMB200_OK) { set_error("kernel_pool: shape not supported by the tcgen05 kernel"); rc = MMB200_ERR_UNSUPPORTED; }
+      if (rc == MMB200_OK) { set_error("kernel_pool: shape not supported by the tensor-core kernel"); rc = MMB200_ERR_UNSUPPORTED; }
       return rc;
     }
   }
@@ -648,8 +648,7 @@ static int mmb::kp_bwd_impl(const float* q, const float* d, const void* q_mask, 
   KpParams P{};
   P.saved = const_cast<float*>(saved);
   // the tensor core drops the low 13 mantissa bits of the raw fp32 tiles: relative shrink 2^-10 u / m with u uniform in
-  // [0, 1) and the mantissa m log-uniform in [1, 2) -> mean 2^-11 / ln 2 * (1 - 1/2) = 0.72 * 2^-11 (measured on B200:
-  // -3.3e-4 without the factor, profiles/r02_kernel_pool_bwd_investigation.md)
+  // [0, 1) and the mantissa m log-uniform in [1, 2) -> mean 2^-11 / ln 2 * (1 - 1/2) = 0.72 * 2^-11
   P.tf32_comp = 1.0f + 0.72f / 2048.0f;
 #ifdef MMB200_ENABLE_PROF
   if (const char* e = getenv("MMB200_KPB_COMP")) P.tf32_comp = (float)atof(e);
@@ -666,8 +665,8 @@ static int mmb::kp_bwd_impl(const float* q, const float* d, const void* q_mask, 
   if (B == 0) return MMB200_OK;
   DeviceInfo dev;
   if (int rc = current_device_info(&dev)) return rc;
-  if (!is_sm100(dev)) {
-    set_error("matchmaker_b200 kernels are built for sm_100a only");
+  if (!is_sm90(dev)) {
+    set_error("matchmaker_b200 kernels are built for sm_90a only");
     return MMB200_ERR_UNSUPPORTED;
   }
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
@@ -676,7 +675,7 @@ static int mmb::kp_bwd_impl(const float* q, const float* d, const void* q_mask, 
     bool handled = false;
     rc = kernel_pool_bwd_tc(P, dev, stream, &handled);
     if (!handled) {
-      if (rc == MMB200_OK) { set_error("kernel_pool_bwd_saved: arguments outside the tcgen05 backward's envelope"); rc = MMB200_ERR_UNSUPPORTED; }
+      if (rc == MMB200_OK) { set_error("kernel_pool_bwd_saved: arguments outside the tensor-core backward's envelope"); rc = MMB200_ERR_UNSUPPORTED; }
       return rc;
     }
     if (rc) return rc;

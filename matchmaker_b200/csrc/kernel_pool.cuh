@@ -1,5 +1,5 @@
 // Parameter block shared by the kernel-pooling kernels (kernel_pool.cu: FFMA forward/backward;
-// kernel_pool_ts.cu: tcgen05 forward).
+// kernel_pool_ts.cu: tensor-core forward).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -37,11 +37,11 @@ struct KpParams {
   float* grad_d;
   float* ws_weight;  // [B,K]
   float* ws_alpha;   // [B,K]
-  // state the tcgen05 forward leaves for the tcgen05 backward (kernel_pool_bwd_tc.cu), B * (33 Ld + 32) floats:
+  // state the tensor-core forward leaves for the tensor-core backward (kernel_pool_bwd_wg.cu), B * (33 Ld + 32) floats:
   // cosines document-row-major [B][Ld][32] (query term contiguous: one 128-byte row per document term, rows >= Lq
   // of a row are 0), then 1 / (|d_j| + eps) [B][Ld], then 1 / (|q_i| + eps) [B][32].  nullptr = do not save.
   float* saved;
-  // tcgen05 forward on a block of <= 32 query rows of a longer query (kernel_pool_ts.cu, Lq > 32): the kernel sees Lq =
+  // tensor-core forward on a block of <= 32 query rows of a longer query (kernel_pool_ts.cu, Lq > 32): the kernel sees Lq =
   // rows of the block; the rows sit at q_row0 .. of Lq_total in q, q_mask and per_kernel_query.  0 / Lq otherwise.
   int32_t q_row0, Lq_total;
   float tf32_comp;   // backward: factor undoing the mean truncation of the raw fp32 operands to tf32 (1 + 2^-11), or 1
@@ -53,10 +53,10 @@ __host__ __device__ inline int64_t kp_saved_rsd_off(int64_t B, int64_t p, int Ld
 __host__ __device__ inline int64_t kp_saved_rsq_off(int64_t B, int64_t p, int Ld) { return B * (int64_t)Ld * 33 + p * 32; }
 
 struct DeviceInfo;
-// tcgen05 forward with the document operand in tensor memory (kernel_pool_ts.cu); *handled = false when the shape is
+// tensor-core forward (kernel_pool_ts.cu); *handled = false when the shape is
 // outside the kernel's envelope
 int kernel_pool_fwd_ts(const KpParams& P, const DeviceInfo& dev, cudaStream_t stream, bool* handled);
-// tcgen05 backward from the state saved by the forward (kernel_pool_bwd_tc.cu); same convention
+// tensor-core backward from the state saved by the forward (kernel_pool_bwd_wg.cu); same convention
 int kernel_pool_bwd_tc(const KpParams& P, const DeviceInfo& dev, cudaStream_t stream, bool* handled);
 
 }  // namespace mmb

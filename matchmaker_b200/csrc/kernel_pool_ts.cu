@@ -1,33 +1,27 @@
-// Cosine + RBF kernel pooling forward (KNRM / TK) on the tensor cores with fp32-grade accuracy -- second
-// generation: the document operand of the MMA lives in TENSOR MEMORY.
+// Cosine + RBF kernel pooling forward (KNRM / TK) on the tensor cores with fp32-grade accuracy.
 //
 // Arithmetic (x = hi + lo, hi = x & 0xffffe000, [Qhi;Qlo] stacked along N):
 //
 //     D[128 doc rows x 64] = Dhi[128 x K] * [Qhi; Qlo]^T  +  Dlo[128 x K] * [Qhi; Qlo]^T
 //
-// What changed is where the operands sit.  The first generation wrote Dhi / Dlo to shared memory and let the
-// tensor core read them back: per 128x32 chunk that is 160 (TMA fill) + 352 (convert LDS/STS) + 384 (MMA operand
-// reads) shared-memory wavefronts, ~900 of the ~900 cycles the chunk may take at HBM speed -- the kernel was bound
-// by the shared-memory data path (profiles/r01_kernel_pool_investigation.md).  Here the convert warps write Dhi / Dlo
-// straight into TMEM with tcgen05.st (thread = document row = TMEM lane) and the MMA takes its A operand from
-// there (tcgen05.mma [d], [a_tmem], b_desc): shared memory only carries the TMA fill, one read of the raw tile and
-// the small query operand -- ~510 wavefronts per chunk.
+// The document operand never goes back to shared memory: the MMA warpgroups read the raw fp32 tile TMA delivered in the
+// wgmma A-fragment layout, split it into hi / lo in registers and issue wgmma kind tf32 with A from registers; only the
+// small query operand [Qhi;Qlo] is written to shared memory (K-major, SWIZZLE_128B) for the B descriptor.
 //
 // Padding is skipped instead of computed: the last document tile is fetched with a box of exactly
-// round8(Ld mod 128) rows, convert warps whose 32 rows are all beyond Ld do nothing, and the last K-chunk only
-// converts / multiplies the 8-column steps that hold data (D = 300 -> 2 of 4).
+// round8(Ld mod 128) rows (rows past it hold stale, finite data whose results are masked), and the last K-chunk only
+// multiplies the 8-column steps that hold data (D = 300 -> 2 of 4).
 //
 // Per CTA (persistent, one per SM, 640 threads = 5 warpgroups; registers are re-dealt with setmaxnreg):
 //   warp 0      TMA producer: fp32 chunks [<=128 doc rows x 32] + [32 query rows x 32], SWIZZLE_128B, raw ring
-//   warp 1      tcgen05.mma kind::tf32 issuer (A from TMEM, B = [Qhi;Qlo] from shared memory), 4 accumulators
 //   warps 2-3   query convert, two threads per query row: hi / lo into the B-operand ring, query norms
-//   warps 4-11  document convert, two threads per document row (16 of the chunk's 32 columns each): warp w owns
-//               TMEM lane quarter w % 4 = rows 32(w%4) .. +31 and column half (w-4)/4
-//   warps 12-19 epilogue.  Phase A: tcgen05.ld, add the two halves, scale by the norms, cosine tile to shared memory
-//               (masked rows -> sentinel), last live row published.  Phase B: lane = query row, rows dealt round-robin
-//               to the warps two at a time, K activations ex2(-((c-mu)a)^2) accumulated in registers.
-//
-// TMEM map (512 columns): [0,256) 4 accumulators of 64 columns; [256,512) A ring, 4 slots of (32 hi + 32 lo).
+//   warps 4-11  two MMA warpgroups, warpgroup c = document rows 64c .. 64c + 63: A fragments (hi, lo) from the raw
+//               tile, wgmma m64n64k8 tf32 into registers, document norms by quad shuffles; then phase A: add the two
+//               halves, scale by the norms, cosine tile to shared memory (masked rows -> sentinel), last live row
+//               published
+//   warps 12-19 epilogue, phase B: lane = query row, rows dealt round-robin to the warps two at a time, K activations
+//               ex2(-((c-mu)a)^2) accumulated in registers; end of pair: log, per-kernel sums, score.
+// The two cosine tiles are handed over between phase A and phase B through mbarriers (cs_full / cs_empty).
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
@@ -43,42 +37,34 @@ namespace {
 
 constexpr int kThreads = 640;           // 20 warps, see the role table above
 constexpr int kMaxRaw = 8;            // raw ring (TMA targets): 20 KB per slot
-constexpr int kOps = 4;               // operand ring: A slot in TMEM (64 columns) + B slot in shared memory (8 KB)
-constexpr int kAcc = 4;
-constexpr int kAccCols = 64;
-constexpr int kACol0 = kAcc * kAccCols;  // first TMEM column of the A ring
-constexpr int kNormRing = kAcc + kOps + 1;
+constexpr int kOps = 4;               // query-operand ring: B slot in shared memory (8 KB)
+constexpr int kNormRing = kOps + 2;
 constexpr int kDxBytes = 128 * 128;   // [128 rows][32 fp32]
 constexpr int kQxBytes = 32 * 128;    // [32 query rows][32 fp32]
 constexpr int kRawBytes = kDxBytes + kQxBytes;          // 20 KB
 constexpr int kQ64Bytes = 64 * 128;   // rows 0-31 Q hi, rows 32-63 Q lo
 constexpr int kEpiThreads = 256;
-constexpr int kReleaseArrivals = 8 + 64;  // lane 0 of each document convert warp + every lane of the two query warps
+constexpr int kReleaseArrivals = 8 + 64;  // lane 0 of each MMA warp + every lane of the two query warps
 constexpr int kFirstDocWarp = 4, kFirstEpiWarp = 12;
-constexpr int kRegsLight = 56, kRegsConvert = 80, kRegsEpilogue = 128;  // setmaxnreg budgets per warpgroup
+constexpr int kRegsLight = 56, kRegsMma = 88, kRegsEpilogue = 120;  // setmaxnreg budgets per warpgroup (<= 640 x 96)
 constexpr float kSentinel = 1.0e6f;   // "cosine" of a masked row: ex2(-((1e6 - mu) a)^2) is exactly 0 for any sigma < 1e4
 constexpr float kTinyNorm = 1e-13f;
 
 struct KpShared {
-  uint64_t raw_full[kMaxRaw];    // TMA -> convert
-  uint64_t raw_empty[kMaxRaw];   // convert -> TMA
-  uint64_t op_full[kOps];        // convert -> MMA
-  uint64_t op_empty[kOps];       // tcgen05.commit -> convert
-  uint64_t accfull[kAcc];
-  uint64_t accempty[kAcc];
-  uint32_t tmem_base;
-  uint32_t pad;
-  // |d|^2 (one partial per column half: two convert threads per document row) and 1 / (|q| + eps) travel from the
-  // convert warps to the epilogue in their own ring: the convert warps run up to kOps k-chunks ahead of the MMA warp,
-  // which runs up to kAcc tiles ahead of the epilogue -- kAcc + kOps tiles when a tile is a single k-chunk (D <= 32),
-  // so a ring indexed by the accumulator slot could be overwritten before it is read
-  float ss_d[kNormRing][2][128];
+  uint64_t raw_full[kMaxRaw];    // TMA -> query convert, MMA warps
+  uint64_t raw_empty[kMaxRaw];   // query convert, MMA warps -> TMA
+  uint64_t op_full[kOps];        // query convert -> MMA warps
+  uint64_t op_empty[kOps];       // MMA warps -> query convert
+  uint64_t cs_full[2];           // phase A (MMA warps) -> phase B (epilogue warps)
+  uint64_t cs_empty[2];          // phase B -> phase A
+  // 1 / (|q| + eps) travels from the query convert warps to phase A in its own ring: the convert warps run up to kOps
+  // k-chunks ahead of the MMA warps -- kOps tiles when a tile is a single k-chunk (D <= 32)
   float rs_q[kNormRing][32];
   float mu[32], a[32], alpha[32], w[32];
   float pk[32];
   float qm[32];
   float lg[2][128];              // per cosine tile: log2 of the document-term gate (0 without a gate)
-  int live[2][4];                // per cosine tile: last unmasked document row + 1 of each 32-row quarter
+  int live[2][8];                // per cosine tile: last unmasked document row + 1 of each MMA warp's 16 rows
 };
 
 __device__ __forceinline__ float ex2f(float x) {
@@ -94,26 +80,10 @@ __device__ __forceinline__ void split4(const float4 v, uint32_t* hi, uint32_t* l
   hi[3] = __float_as_uint(v.w) & 0xffffe000u; lo[3] = __float_as_uint(v.w - __uint_as_float(hi[3]));
 }
 
-// PROF: debugging aid (MMB200_KP_PROF=1): one thread per role of CTA 0 accumulates the cycles it spends blocked on
-// each barrier; prof[] is printed by the launcher.  Compiled out of the product instantiation.
-#define KP_TIMED(slot, stmt)                                  \
-  do {                                                        \
-    if constexpr (PROF) {                                     \
-      const long long t0_ = clock64();                        \
-      stmt;                                                   \
-      pc[slot] += clock64() - t0_;                            \
-    } else {                                                  \
-      stmt;                                                   \
-    }                                                         \
-  } while (0)
-
-template <int KB, bool PROF, bool SAVE>
+template <int KB, bool SAVE>
 __global__ void __launch_bounds__(kThreads, 1)
 kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_d,
-                      const __grid_constant__ CUtensorMap tmap_d_last, KpParams P, int n_raw, int last_box_rows,
-                      long long* prof) {
-  long long pc[3] = {0, 0, 0};
-  const long long t_start = PROF ? clock64() : 0;
+                      const __grid_constant__ CUtensorMap tmap_d_last, KpParams P, int n_raw, int last_box_rows) {
   extern __shared__ uint8_t smem_raw[];
   // 1024-B alignment for SWIZZLE_128B tiles, derived by pointer arithmetic on the __shared__ array so the
   // compiler keeps the shared address space (LDS/STS instead of generic LD/ST)
@@ -121,10 +91,8 @@ kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
   uint8_t* qring = smem;                                                        // [kOps][Qhi;Qlo]
   uint8_t* raws = smem + kOps * kQ64Bytes;                                      // [n_raw][Dx | Qx]
   float* cs = reinterpret_cast<float*>(raws + (size_t)n_raw * kRawBytes);       // [2][128][32] cosine tiles
-  // the end-of-pair scratch aliases the cosine tiles (free between the last phase B of a pair and the first
-  // phase A of the next one; fenced by named barriers 5 and 4)
-  float* spart = cs;                                                           // [8][KB][32]  (<= 32 KB)
-  KpShared* S = reinterpret_cast<KpShared*>(cs + 2 * 128 * 32);
+  float* spart = cs + 2 * 128 * 32;                                            // [8][KB][32] end-of-pair scratch
+  KpShared* S = reinterpret_cast<KpShared*>(spart + 8 * 32 * 32);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles = (P.Ld + 127) / 128;
@@ -138,8 +106,8 @@ kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     prefetch_tensormap(&tmap_d);
     prefetch_tensormap(&tmap_d_last);
     for (int s = 0; s < n_raw; ++s) { mbar_init(&S->raw_full[s], 1); mbar_init(&S->raw_empty[s], kReleaseArrivals); }
-    for (int s = 0; s < kOps; ++s) { mbar_init(&S->op_full[s], kReleaseArrivals); mbar_init(&S->op_empty[s], 1); }
-    for (int s = 0; s < kAcc; ++s) { mbar_init(&S->accfull[s], 1); mbar_init(&S->accempty[s], 8); }
+    for (int s = 0; s < kOps; ++s) { mbar_init(&S->op_full[s], 64); mbar_init(&S->op_empty[s], 8); }
+    for (int s = 0; s < 2; ++s) { mbar_init(&S->cs_full[s], 8); mbar_init(&S->cs_empty[s], 8); }
     fence_barrier_init();
   }
   if (threadIdx.x < 32) {
@@ -150,74 +118,34 @@ kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     S->alpha[t] = ok ? (P.alpha ? P.alpha[t] : 1.f) : 1.f;
     S->w[t] = ok ? P.weight[t] : 0.f;
   }
-  if (warp == 1) tmem_alloc(&S->tmem_base, 512);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = S->tmem_base;
 
   // every role branch starts with its setmaxnreg so that ptxas allocates each branch against its own budget
   if (warp == 0) {
     // ------------------------------- TMA producer -------------------------------
+    // The whole warp walks the loop (uniform control flow and operands); one elected lane issues: inside an
+    // `if (lane == 0)` region the compiler wraps every TMA in an ELECT / R2UR waterfall loop (ptx.cuh)
     setmaxnreg_dec<kRegsLight>();
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      const uint32_t last_bytes = (uint32_t)(last_box_rows * 128 + kQxBytes);
-      for (int64_t p = p_begin; p < p_end; ++p)
-        for (int t = 0; t < tiles; ++t) {
-          const bool last = t == tiles - 1;
-          for (int ck = 0; ck < nch; ++ck) {
-            KP_TIMED(0, mbar_wait(&S->raw_empty[stage], phase ^ 1u));
-            uint8_t* st = raws + (size_t)stage * kRawBytes;
+    int stage = 0;
+    uint32_t phase = 0;
+    const uint32_t last_bytes = (uint32_t)(last_box_rows * 128 + kQxBytes);
+    for (int64_t p = p_begin; p < p_end; ++p)
+      for (int t = 0; t < tiles; ++t) {
+        const bool last = t == tiles - 1;
+        for (int ck = 0; ck < nch; ++ck) {
+          mbar_wait(&S->raw_empty[stage], phase ^ 1u);
+          uint8_t* st = raws + (size_t)stage * kRawBytes;
+          if (elect_one_sync()) {
             mbar_arrive_expect_tx(&S->raw_full[stage], last ? last_bytes : (uint32_t)kRawBytes);
             tma_load_3d(last ? &tmap_d_last : &tmap_d, st, &S->raw_full[stage], ck * 32, t * 128, (int)p, kEvictFirst);
             tma_load_3d(&tmap_q, st + kDxBytes, &S->raw_full[stage], ck * 32, P.q_row0, (int)p, kEvictLast);
-            if (++stage == n_raw) { stage = 0; phase ^= 1u; }
           }
+          __syncwarp();
+          if (++stage == n_raw) { stage = 0; phase ^= 1u; }
         }
-      if (PROF && blockIdx.x == 0) prof[0] = pc[0];
-    }
+      }
   } else if (warp == 1) {
-    // ------------------------------- MMA issuer ---------------------------------
-    // The whole warp walks the loop (uniform control flow, uniform operands); one elected lane issues.
     setmaxnreg_dec<kRegsLight>();
-    {
-      const uint32_t idesc = make_idesc(kFmtTF32, 128, 64);
-      int stage = 0, acc = 0;
-      uint32_t phase = 0, accphase = 0;
-      for (int64_t p = p_begin; p < p_end; ++p)
-        for (int t = 0; t < tiles; ++t) {
-          KP_TIMED(0, mbar_wait(&S->accempty[acc], accphase ^ 1u));
-          tc_fence_after_sync();
-          const uint32_t tmem_d = tmem_base + (uint32_t)(acc * kAccCols);
-          for (int ck = 0; ck < nch; ++ck) {
-            const int ksteps = (min(32, P.D - ck * 32) + 7) >> 3;  // 8 fp32 per UMMA K-step
-            KP_TIMED(1, mbar_wait(&S->op_full[stage], phase));
-            tc_fence_after_sync();
-            const uint32_t abase = tmem_base + (uint32_t)(kACol0 + stage * 64);
-            const uint64_t b0 = make_sw128_kmajor_desc(smem_u32(qring + (size_t)stage * kQ64Bytes));
-            const long long t_i = PROF ? clock64() : 0;
-            if (elect_one_sync()) {
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                if (k < ksteps) {
-                  const uint64_t bq = b0 + (uint64_t)(k * 2);  // +32 bytes along K inside the 128-byte swizzle atom
-                  umma_tf32_ts(tmem_d, abase + (uint32_t)(k * 8), bq, idesc, (uint32_t)((ck | k) != 0));
-                  umma_tf32_ts(tmem_d, abase + (uint32_t)(32 + k * 8), bq, idesc, 1u);
-                }
-              }
-              umma_commit(&S->op_empty[stage]);
-              if (ck == nch - 1) umma_commit(&S->accfull[acc]);
-            }
-            __syncwarp();
-            if (PROF) pc[2] += clock64() - t_i;
-            if (++stage == kOps) { stage = 0; phase ^= 1u; }
-          }
-          if (++acc == kAcc) { acc = 0; accphase ^= 1u; }
-        }
-      if (PROF && blockIdx.x == 0 && lane == 0) { prof[1] = pc[0]; prof[2] = pc[1]; prof[12] = pc[2]; }
-    }
   } else if (warp < 4) {
     // ------------------------------- query convert: [Qhi;Qlo] B operand, norms ------
     setmaxnreg_dec<kRegsLight>();
@@ -231,7 +159,7 @@ kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
         float4 ss4 = make_float4(0.f, 0.f, 0.f, 0.f);
         for (int ck = 0; ck < nch; ++ck) {
           const bool have = half == 0 || P.D - ck * 32 > 16;  // this thread's 16 columns hold data
-          KP_TIMED(0, mbar_wait(&S->raw_full[rs_], rphase));
+          mbar_wait(&S->raw_full[rs_], rphase);
           const uint8_t* xrow = raws + (size_t)rs_ * kRawBytes + kDxBytes + row * 128;
           float4 x[4];
 #pragma unroll
@@ -242,7 +170,7 @@ kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
             const float4 v = x[c];
             ss4.x = fmaf(v.x, v.x, ss4.x); ss4.y = fmaf(v.y, v.y, ss4.y); ss4.z = fmaf(v.z, v.z, ss4.z); ss4.w = fmaf(v.w, v.w, ss4.w);
           }
-          KP_TIMED(1, mbar_wait(&S->op_empty[os_], ophase ^ 1u));
+          mbar_wait(&S->op_empty[os_], ophase ^ 1u);
           uint8_t* hrow = qring + (size_t)os_ * kQ64Bytes + row * 128;
           uint8_t* lrow = hrow + 32 * 128;
           if (have) {
@@ -261,7 +189,8 @@ kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
             if (half == 0) S->rs_q[nr][row] = 1.0f / (sqrtf(ss) + kTinyNorm);
           }
           // release the raw slot only after the stores that consumed the loaded values: an arrive placed right after
-          // the LDS is hoisted above their completion by ptxas and the TMA overwrites rows that are still being read
+          // the LDS is hoisted above their completion by ptxas and the TMA overwrites rows that are still being read;
+          // the operand stores are made visible to the tensor core's async proxy before the MMA warps are told
           fence_proxy_async_smem();
           mbar_arrive(&S->raw_empty[rs_]);
           mbar_arrive(&S->op_full[os_]);
@@ -270,71 +199,114 @@ kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
         }
         if (++nr == kNormRing) nr = 0;
       }
-    if (PROF && blockIdx.x == 0 && warp == 2 && lane == 0) { prof[6] = pc[0]; prof[7] = pc[1]; }
   } else if (warp < kFirstEpiWarp) {
-    // ------------------------------- document convert: hi / lo into TMEM, norms ----
-    setmaxnreg_dec<kRegsConvert>();
-    const int qd = warp & 3;                  // TMEM lane quarter this warp may access
-    const int half = (warp - kFirstDocWarp) >> 2;  // which 16 of the chunk's 32 columns
-    const int row = qd * 32 + lane;           // document row inside the tile = TMEM lane
-    const int sw = row & 7;
+    // ------------------------------- document operand + wgmma + cosine tile (phase A) ------------------------------
+    setmaxnreg_dec<kRegsMma>();
+    const int c = (warp - kFirstDocWarp) >> 2;   // warpgroup: document rows 64c .. 64c + 63 of the tile
+    const int wq = warp & 3;
+    const int ew = 4 * c + wq;                   // 0..7
+    const int r0 = 64 * c + 16 * wq + (lane >> 2), r1 = r0 + 8;   // this thread's two document rows
+    const int tq = lane & 3;
+    const int dmt = P.d_mask ? P.mask_dtype : MMB200_MASK_NONE;
     int rs_ = 0, os_ = 0, nr = 0;
     uint32_t rphase = 0, ophase = 0;
+    int64_t tile_seq = 0;
     for (int64_t p = p_begin; p < p_end; ++p)
-      for (int t = 0; t < tiles; ++t) {
-        const bool in_doc = qd * 32 < P.Ld - t * 128;   // warp-uniform: any of this warp's rows inside the document
-        float4 ss4 = make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int t = 0; t < tiles; ++t, ++tile_seq) {
+        const int g0 = t * 128 + r0, g1 = t * 128 + r1;
+        const uint64_t draw0 = g0 < P.Ld ? (dmt != MMB200_MASK_NONE ? mask_raw(P.d_mask, dmt, p * (int64_t)P.Ld + g0) : 1) : 0;
+        const uint64_t draw1 = g1 < P.Ld ? (dmt != MMB200_MASK_NONE ? mask_raw(P.d_mask, dmt, p * (int64_t)P.Ld + g1) : 1) : 0;
+        float acc[32];   // columns 0..31: D . Qhi, 32..63: D . Qlo (rows r0 / r1)
+#pragma unroll
+        for (int j = 0; j < 32; ++j) acc[j] = 0.f;
+        float ss0 = 0.f, ss1 = 0.f;
         for (int ck = 0; ck < nch; ++ck) {
-          const bool active = in_doc && (half == 0 || P.D - ck * 32 > 16);  // ... and these 16 columns hold data
-          KP_TIMED(0, mbar_wait(&S->raw_full[rs_], rphase));
-          const uint8_t* xrow = raws + (size_t)rs_ * kRawBytes + row * 128;
-          float4 x[4];
+          const int ksteps = (min(32, P.D - ck * 32) + 7) >> 3;  // 8 fp32 per wgmma K-step
+          mbar_wait(&S->raw_full[rs_], rphase);
+          const float* x = reinterpret_cast<const float*>(raws + (size_t)rs_ * kRawBytes);
+          // A fragments straight from the raw SWIZZLE_128B tile: element (row, col) sits in 16-byte chunk (col / 4) ^ (row & 7)
+          uint32_t ahi[4][4], alo[4][4];
 #pragma unroll
-          for (int c = 0; c < 4; ++c)
-            x[c] = active ? *reinterpret_cast<const float4*>(xrow + (((4 * half + c) ^ sw) << 4)) : make_float4(0.f, 0.f, 0.f, 0.f);
+          for (int k = 0; k < 4; ++k) {
+            const int ch0 = (2 * k) ^ (r0 & 7), ch1 = (2 * k + 1) ^ (r0 & 7);   // r1 & 7 == r0 & 7
+            const float v[4] = {x[r0 * 32 + ch0 * 4 + tq], x[r1 * 32 + ch0 * 4 + tq], x[r0 * 32 + ch1 * 4 + tq], x[r1 * 32 + ch1 * 4 + tq]};
 #pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            const float4 v = x[c];
-            ss4.x = fmaf(v.x, v.x, ss4.x); ss4.y = fmaf(v.y, v.y, ss4.y); ss4.z = fmaf(v.z, v.z, ss4.z); ss4.w = fmaf(v.w, v.w, ss4.w);
+            for (int e = 0; e < 4; ++e) {
+              ahi[k][e] = __float_as_uint(v[e]) & 0xffffe000u;
+              alo[k][e] = __float_as_uint(v[e] - __uint_as_float(ahi[k][e]));
+            }
+            ss0 = fmaf(v[0], v[0], fmaf(v[2], v[2], ss0));
+            ss1 = fmaf(v[1], v[1], fmaf(v[3], v[3], ss1));
           }
-          KP_TIMED(1, mbar_wait(&S->op_empty[os_], ophase ^ 1u));
-          tc_fence_after_sync();
-          const long long t_st = PROF ? clock64() : 0;
-          if (active) {
-            const uint32_t taddr = tmem_base + ((uint32_t)(qd * 32) << 16) + (uint32_t)(kACol0 + os_ * 64 + 16 * half);
-            uint32_t hi[16], lo[16];
+          mbar_wait(&S->op_full[os_], ophase);
+          const uint64_t b0 = make_wgmma_sw128_desc(smem_u32(qring + (size_t)os_ * kQ64Bytes));
+          wgmma_fence();
 #pragma unroll
-            for (int c = 0; c < 4; ++c) split4(x[c], hi + 4 * c, lo + 4 * c);
-            tmem_st_32x32b_x16(taddr, hi);
-            tmem_st_32x32b_x16(taddr + 32, lo);
-            tmem_st_wait();
+          for (int k = 0; k < 4; ++k) {
+            if (k < ksteps) {
+              wgmma_m64n64k8_tf32_rs(acc, ahi[k], b0 + (uint64_t)(k * 2), 1u);   // +32 bytes along K
+              wgmma_m64n64k8_tf32_rs(acc, alo[k], b0 + (uint64_t)(k * 2), 1u);
+            }
           }
-          if (PROF) pc[2] += clock64() - t_st;
-          if (ck == nch - 1) S->ss_d[nr][half][row] = (ss4.x + ss4.y) + (ss4.z + ss4.w);
-          // the tcgen05.st above consumed every loaded value and has completed: the raw slot may be refilled and the
-          // A slot may be read (an arrive placed right after the LDS would be hoisted above their completion)
-          tc_fence_before_sync();
+          wgmma_commit();
+          wgmma_wait<0>();
           __syncwarp();
           if (lane == 0) {
             mbar_arrive(&S->raw_empty[rs_]);
-            mbar_arrive(&S->op_full[os_]);
+            mbar_arrive(&S->op_empty[os_]);
           }
           if (++rs_ == n_raw) { rs_ = 0; rphase ^= 1u; }
           if (++os_ == kOps) { os_ = 0; ophase ^= 1u; }
         }
+        wgmma_fence_regs(acc);
+        ss0 += __shfl_xor_sync(0xffffffffu, ss0, 1); ss0 += __shfl_xor_sync(0xffffffffu, ss0, 2);
+        ss1 += __shfl_xor_sync(0xffffffffu, ss1, 1); ss1 += __shfl_xor_sync(0xffffffffu, ss1, 2);
+        const float rsd0 = 1.0f / (sqrtf(ss0) + kTinyNorm), rsd1 = 1.0f / (sqrtf(ss1) + kTinyNorm);
+        const bool valid0 = g0 < P.Ld && mask_test(draw0, dmt), valid1 = g1 < P.Ld && mask_test(draw1, dmt);
+        const int buf = (int)(tile_seq & 1);
+        float* cbuf = cs + buf * (128 * 32);
+        mbar_wait(&S->cs_empty[buf], (uint32_t)((tile_seq >> 1) & 1) ^ 1u);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int col = 8 * j + 2 * tq;   // query columns col, col + 1
+          const float q0 = S->rs_q[nr][col], q1 = S->rs_q[nr][col + 1];
+          const float c00 = (acc[4 * j + 0] + acc[4 * (j + 4) + 0]) * rsd0 * q0;
+          const float c01 = (acc[4 * j + 1] + acc[4 * (j + 4) + 1]) * rsd0 * q1;
+          const float c10 = (acc[4 * j + 2] + acc[4 * (j + 4) + 2]) * rsd1 * q0;
+          const float c11 = (acc[4 * j + 3] + acc[4 * (j + 4) + 3]) * rsd1 * q1;
+          *reinterpret_cast<float2*>(cbuf + r0 * 32 + ((((col >> 2) ^ (r0 & 7))) << 2) + (col & 3)) =
+              make_float2(valid0 ? c00 : kSentinel, valid0 ? c01 : kSentinel);
+          *reinterpret_cast<float2*>(cbuf + r1 * 32 + ((((col >> 2) ^ (r1 & 7))) << 2) + (col & 3)) =
+              make_float2(valid1 ? c10 : kSentinel, valid1 ? c11 : kSentinel);
+          if constexpr (SAVE) {  // training: leave the unmasked cosines and the norms for the tensor-core backward
+            if (g0 < P.Ld) *reinterpret_cast<float2*>(P.saved + kp_saved_cos_off(p, P.Ld) + (int64_t)g0 * 32 + col) = make_float2(c00, c01);
+            if (g1 < P.Ld) *reinterpret_cast<float2*>(P.saved + kp_saved_cos_off(p, P.Ld) + (int64_t)g1 * 32 + col) = make_float2(c10, c11);
+          }
+        }
+        if constexpr (SAVE) {
+          if (tq == 0) {
+            if (g0 < P.Ld) P.saved[kp_saved_rsd_off(P.B, p, P.Ld) + g0] = rsd0;
+            if (g1 < P.Ld) P.saved[kp_saved_rsd_off(P.B, p, P.Ld) + g1] = rsd1;
+          }
+          if (t == 0 && ew == 0) P.saved[kp_saved_rsq_off(P.B, p, P.Ld) + lane] = S->rs_q[nr][lane];
+        }
+        // last live row + 1 of this warp's 16 rows: phase B stops there instead of testing every row
+        const int live = __reduce_max_sync(0xffffffffu, valid1 ? r1 + 1 : valid0 ? r0 + 1 : 0);
+        if (lane == 0) S->live[buf][ew] = live;
+        if (tq == 0) {
+          // gate g_j * exp(-x^2) = 2^(-u^2 + log2 g_j): one exponent term per document row, no extra multiply
+          S->lg[buf][r0] = (P.gate && g0 < P.Ld) ? __log2f(fmaxf(P.gate[p * (int64_t)P.Ld + g0], 0.f)) : 0.f;
+          S->lg[buf][r1] = (P.gate && g1 < P.Ld) ? __log2f(fmaxf(P.gate[p * (int64_t)P.Ld + g1], 0.f)) : 0.f;
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&S->cs_full[buf]);
         if (++nr == kNormRing) nr = 0;
       }
-    if (PROF && blockIdx.x == 0 && warp == kFirstDocWarp && lane == 0) { prof[3] = pc[0]; prof[4] = pc[1]; prof[5] = pc[2]; }
   } else {
-    // ------------------------------- epilogue ------------------------------------
+    // ------------------------------- epilogue (phase B) ------------------------------------
     setmaxnreg_inc<kRegsEpilogue>();
     const int ew = warp - kFirstEpiWarp;  // 0..7
-    const int qd = warp & 3;            // TMEM lane quarter
-    const int h = ew >> 2;              // which 16 query columns of the 32 this warp extracts in phase A
-    const int dmt = P.d_mask ? P.mask_dtype : MMB200_MASK_NONE;
     const int qmt = P.q_mask ? P.mask_dtype : MMB200_MASK_NONE;
-    int acc_slot = 0, nr = 0;
-    uint32_t accphase = 0;
     int64_t tile_seq = 0;
     // kernel centres / widths in registers when they fit (the reference's 11- and 21-kernel models); otherwise they are
     // re-read from shared memory inside the activation loop
@@ -364,72 +336,19 @@ kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
       const int sub16 = 16 * (lane / qp);        // document-row offset of this lane's sub-stream
       const int rstep = 16 * (32 / qp);          // document rows one warp iteration advances by
       for (int t = 0; t < tiles; ++t, ++tile_seq) {
-        const int row = qd * 32 + lane;          // document row inside the tile
-        const int g = t * 128 + row;
-        uint64_t draw = 0;
-        if (g < P.Ld) draw = dmt != MMB200_MASK_NONE ? mask_raw(P.d_mask, dmt, p * (int64_t)P.Ld + g) : 1;
-        float* cbuf = cs + (tile_seq & 1) * (128 * 32);
-        KP_TIMED(0, mbar_wait(&S->accfull[acc_slot], accphase));
-        tc_fence_after_sync();
-        {  // phase A
-          const uint32_t taddr = tmem_base + ((uint32_t)(qd * 32) << 16) + (uint32_t)(acc_slot * 64);
-          uint32_t rh[16], rl[16];
-          tmem_ld_32x32b_x16(taddr + 16 * h, rh);
-          tmem_ld_32x32b_x16(taddr + 32 + 16 * h, rl);
-          tmem_ld_wait();
-          const bool valid = g < P.Ld && mask_test(draw, dmt);
-          const float rsd = 1.0f / (sqrtf(S->ss_d[nr][0][row] + S->ss_d[nr][1][row]) + kTinyNorm);
-          float v[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const float c = (__uint_as_float(rh[j]) + __uint_as_float(rl[j])) * rsd * S->rs_q[nr][16 * h + j];
-            v[j] = valid ? c : kSentinel;
-          }
-          if constexpr (SAVE) {  // training: leave the unmasked cosines and the norms for the tcgen05 backward
-            if (g < P.Ld) {
-              float* crow = P.saved + kp_saved_cos_off(p, P.Ld) + (int64_t)g * 32 + 16 * h;
-#pragma unroll
-              for (int cc = 0; cc < 4; ++cc) {
-                float4 o;
-                o.x = (__uint_as_float(rh[4 * cc + 0]) + __uint_as_float(rl[4 * cc + 0])) * rsd * S->rs_q[nr][16 * h + 4 * cc + 0];
-                o.y = (__uint_as_float(rh[4 * cc + 1]) + __uint_as_float(rl[4 * cc + 1])) * rsd * S->rs_q[nr][16 * h + 4 * cc + 1];
-                o.z = (__uint_as_float(rh[4 * cc + 2]) + __uint_as_float(rl[4 * cc + 2])) * rsd * S->rs_q[nr][16 * h + 4 * cc + 2];
-                o.w = (__uint_as_float(rh[4 * cc + 3]) + __uint_as_float(rl[4 * cc + 3])) * rsd * S->rs_q[nr][16 * h + 4 * cc + 3];
-                *reinterpret_cast<float4*>(crow + 4 * cc) = o;
-              }
-              if (h == 0) P.saved[kp_saved_rsd_off(P.B, p, P.Ld) + g] = rsd;
-            }
-            if (t == 0 && ew == 0) P.saved[kp_saved_rsq_off(P.B, p, P.Ld) + lane] = S->rs_q[nr][lane];
-          }
-          if (h == 0) {  // last live row of this quarter: phase B stops there instead of testing every row
-            const uint32_t live = __ballot_sync(0xffffffffu, valid);
-            if (lane == 0) S->live[tile_seq & 1][qd] = live ? qd * 32 + 32 - __clz(live) : 0;
-            // gate g_j * exp(-x^2) = 2^(-u^2 + log2 g_j): one exponent term per document row, no extra multiply
-            S->lg[tile_seq & 1][row] = (P.gate && g < P.Ld) ? __log2f(fmaxf(P.gate[p * (int64_t)P.Ld + g], 0.f)) : 0.f;
-          }
-          tc_fence_before_sync();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&S->accempty[acc_slot]);
-#pragma unroll
-          for (int cc = 0; cc < 4; ++cc) {
-            const int phys = (4 * h + cc) ^ (row & 7);
-            *reinterpret_cast<float4*>(cbuf + row * 32 + phys * 4) = make_float4(v[4 * cc], v[4 * cc + 1], v[4 * cc + 2], v[4 * cc + 3]);
-          }
-        }
-        if (++acc_slot == kAcc) { acc_slot = 0; accphase ^= 1u; }
-        if (++nr == kNormRing) nr = 0;
-        KP_TIMED(1, named_bar_sync(1, kEpiThreads));
-        const long long t_b = PROF ? clock64() : 0;
+        const int buf = (int)(tile_seq & 1);
+        const float* cbuf = cs + buf * (128 * 32);
+        mbar_wait(&S->cs_full[buf], (uint32_t)((tile_seq >> 1) & 1));
         {  // phase B: lane = query row; document rows are dealt round-robin to the 8 warps, two at a time (rows r and
            // r + 8 give the MUFU two independent streams).  Masked rows below the last live row carry the sentinel
            // and contribute exactly 0; rows above it are not visited.  The next pair of cosines is loaded before the
            // current one is consumed so that the MUFU stream does not drain at every iteration.
-          const int* lv = S->live[tile_seq & 1];
-          const int rows_live = max(max(lv[0], lv[1]), max(lv[2], lv[3]));
+          const int* lv = S->live[buf];
+          const int rows_live = max(max(max(lv[0], lv[1]), max(lv[2], lv[3])), max(max(lv[4], lv[5]), max(lv[6], lv[7])));
           auto cos_at = [&](int r) -> float {
             return r < rows_live ? cbuf[r * 32 + (((qi >> 2) ^ (r & 7)) << 2) + (qi & 3)] : kSentinel;
           };
-          const float* lgs = S->lg[tile_seq & 1];
+          const float* lgs = S->lg[buf];
           float c0 = cos_at(ew + sub16), c1 = cos_at(ew + sub16 + 8);
           float l0 = lgs[(ew + sub16) & 127], l1 = lgs[(ew + sub16 + 8) & 127];
           for (int r0 = ew; r0 < rows_live; r0 += rstep) {   // uniform trip count: rows past rows_live read the sentinel
@@ -446,10 +365,10 @@ kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
             l0 = m0; l1 = m1;
           }
         }
-        if (PROF) pc[2] += clock64() - t_b;
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&S->cs_empty[buf]);
       }
       // ---- end of pair: S_ik = sum over the 8 warps, log, mask, per-kernel sums, score ----
-      named_bar_sync(5, kEpiThreads);  // every warp is done reading the cosine tiles that spart aliases
       if (qp < 32) {   // warp-uniform: add the sub-streams; afterwards every lane holds the total of its query row
 #pragma unroll
         for (int k = 0; k < KB; ++k) {
@@ -487,60 +406,28 @@ kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
         for (int o = 16; o > 0; o >>= 1) sc += __shfl_xor_sync(0xffffffffu, sc, o);
         if (lane == 0) P.score[p] = sc + P.bias;
       }
-      // spart / pk / qm are rewritten only after the next pair's tiles, i.e. after further barriers
     }
   }
-
-  if (PROF && blockIdx.x == 0 && threadIdx.x == kFirstEpiWarp * 32) { prof[8] = pc[0]; prof[9] = pc[1]; prof[10] = pc[2]; }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (PROF && blockIdx.x == 0 && threadIdx.x == 0) prof[11] = clock64() - t_start;
-  if (warp == 1) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 512);
-  }
 }
-#undef KP_TIMED
 
 template <int KB>
 int launch(const KpParams& P, const DeviceInfo& dev, cudaStream_t stream, const CUtensorMap& tq, const CUtensorMap& td,
            const CUtensorMap& td_last, int last_box_rows) {
-  static_assert(8 * KB * 32 <= 2 * 128 * 32, "end-of-pair scratch must fit inside the cosine tiles");
-  const size_t fixed = (size_t)(2 * 128 * 32) * sizeof(float) + sizeof(KpShared) + 1024 + (size_t)kOps * kQ64Bytes;
-  int n_raw = std::min<int>(kMaxRaw, (int)(((size_t)dev.max_smem_optin - fixed) / kRawBytes));
-#ifdef MMB200_ENABLE_PROF
-  if (const char* e = getenv("MMB200_KP_RAW")) n_raw = std::max(2, std::min(n_raw, atoi(e)));
-#endif
+  static_assert(KB <= 32, "end-of-pair scratch holds 32 kernels");
+  const size_t fixed = (size_t)(2 * 128 * 32 + 8 * 32 * 32) * sizeof(float) + sizeof(KpShared) + 1024 + (size_t)kOps * kQ64Bytes;
+  const int n_raw = std::min<int>(kMaxRaw, (int)(((size_t)dev.max_smem_optin - fixed) / kRawBytes));
   const size_t smem = fixed + (size_t)n_raw * kRawBytes;
   if (n_raw < 2 || smem > (size_t)dev.max_smem_optin) {
-    set_error("kernel_pool tcgen05: shared-memory plan does not fit");
+    set_error("kernel_pool tensor-core forward: shared-memory plan does not fit");
     return MMB200_ERR_UNSUPPORTED;
   }
   const int grid = (int)std::min<int64_t>(dev.sm_count, P.B);
-#ifdef MMB200_ENABLE_PROF  // debugging builds only (python -m matchmaker_b200.build --prof): cudaMalloc + sync in the launch path
-  if (KB == 21 && getenv("MMB200_KP_PROF")) {  // where does each role of CTA 0 wait?
-    long long* prof = nullptr;
-    long long h[13] = {0};
-    MMB_CHECK_CUDA(cudaMalloc(&prof, sizeof(h)));
-    MMB_CHECK_CUDA(cudaMemset(prof, 0, sizeof(h)));
-    MMB_CHECK_CUDA(cudaFuncSetAttribute(kernel_pool_ts_kernel<21, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kernel_pool_ts_kernel<21, true, false><<<grid, kThreads, smem, stream>>>(tq, td, td_last, P, n_raw, last_box_rows, prof);
-    MMB_CHECK_CUDA(cudaStreamSynchronize(stream));
-    MMB_CHECK_CUDA(cudaMemcpy(h, prof, sizeof(h), cudaMemcpyDeviceToHost));
-    MMB_CHECK_CUDA(cudaFree(prof));
-    fprintf(stderr,
-            "kp_prof cycles: total %lld | tma wait_raw_empty %lld | mma wait_accempty %lld wait_op_full %lld | dconv wait_raw_full "
-            "%lld wait_op_empty %lld st %lld | mma issue %lld | qconv wait_raw_full %lld wait_op_empty %lld | epi wait_accfull %lld bar1 %lld phaseB %lld\n",
-            h[11], h[0], h[1], h[2], h[3], h[4], h[5], h[12], h[6], h[7], h[8], h[9], h[10]);
-    return MMB200_OK;
-  }
-#endif
   if (P.saved) {
-    MMB_CHECK_CUDA(cudaFuncSetAttribute(kernel_pool_ts_kernel<KB, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kernel_pool_ts_kernel<KB, false, true><<<grid, kThreads, smem, stream>>>(tq, td, td_last, P, n_raw, last_box_rows, nullptr);
+    MMB_CHECK_CUDA(cudaFuncSetAttribute(kernel_pool_ts_kernel<KB, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel_pool_ts_kernel<KB, true><<<grid, kThreads, smem, stream>>>(tq, td, td_last, P, n_raw, last_box_rows);
   } else {
-    MMB_CHECK_CUDA(cudaFuncSetAttribute(kernel_pool_ts_kernel<KB, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kernel_pool_ts_kernel<KB, false, false><<<grid, kThreads, smem, stream>>>(tq, td, td_last, P, n_raw, last_box_rows, nullptr);
+    MMB_CHECK_CUDA(cudaFuncSetAttribute(kernel_pool_ts_kernel<KB, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel_pool_ts_kernel<KB, false><<<grid, kThreads, smem, stream>>>(tq, td, td_last, P, n_raw, last_box_rows);
   }
   MMB_CHECK_CUDA(cudaGetLastError());
   return MMB200_OK;

@@ -1,4 +1,4 @@
-// ColBERT late-interaction max-sim for sm_100a.
+// ColBERT late-interaction max-sim for sm_90a.
 //
 //   score[p] = sum_i qmask[i] * max_j ( dmask[j] ? <q_i, d_j> : -1000 )
 //
@@ -8,21 +8,21 @@
 // over it; here one persistent kernel streams the document token matrices through shared
 // memory once and never writes the score matrix.
 //
-// Kernel `maxsim_tc_kernel` (the hot path; HBM-bound, 2 bytes per document element):
+// Kernel `maxsim_tc_kernel` (documents on M; any Lq <= 128, dim % 64 == 0):
 //   * one CTA per SM, persistent over a contiguous range of pairs;
 //   * warp 0 (one lane): TMA producer.  A document tile is 128 token rows x dim, fetched as
 //     [KBS k-blocks][128 rows][64 halfs] with SWIZZLE_128B by ONE 4-D cp.async.bulk.tensor
 //     per stage (rows past Ld are zero-filled by the TMA unit, no HBM traffic); the query
 //     matrix ([NPAD rows][dim]) lives in a 2-slot ring and is re-fetched only when the query
 //     of consecutive pairs changes;
-//   * warp 1 (one lane): tcgen05.mma issuer.  D[128 doc rows x NPAD query cols] (fp32, TMEM)
-//     = Doc_tile[128 x dim] * Q[NPAD x dim]^T, kind::f16, UMMA_K = 16; 4 accumulator stages
-//     in TMEM so the tensor pipe never waits for the epilogue;
-//   * warps 2..5: epilogue.  tcgen05.ld the accumulator (lane = document row, register =
-//     query column), apply the document mask (-1000) / tile padding (-inf), column-wise max
-//     across the 32 lanes by a shuffle "transpose-reduce" (31 SHFL + 31 FMNMX for 32 columns),
-//     running max over the tiles of a pair in registers, cross-warp combine through 2 KB of
-//     shared memory, query mask, warp-sum, one fp32 store per pair.
+//   * warpgroups 1 and 2: warpgroup c computes D[64 doc rows x NPAD query cols] (fp32,
+//     registers) = Doc_tile[rows 64c..64c+63] * Q^T with wgmma m64n32k16 chunks, applies the
+//     document mask (-1000) / tile padding (-inf) per row, and keeps a running column max over
+//     the tiles of a pair (per thread over its two rows, then across the warp by shuffles);
+//     the 8 warps combine through 8 KB of shared memory, query mask, warp-sum, one fp32 store
+//     per pair.
+//
+// The hot path for Lq <= 32 is the transposed "queries on M" kernel in maxsim_qm.cu.
 //
 // Kernel `maxsim_simt_kernel`: CUDA-core version for any dtype / dim / length (fp32 inputs,
 // dim % 64 != 0, argmax for backward); also the in-library cross-check of the tensor-core path.
@@ -142,85 +142,49 @@ __global__ void __launch_bounds__(kSimtThreads) maxsim_simt_kernel(MaxsimParams 
 }
 
 // ---------------------------------------------------------------------------------------------
-// tcgen05 kernel
+// wgmma kernel (documents on M)
 // ---------------------------------------------------------------------------------------------
-constexpr int kTcThreads = 192;        // warp 0 TMA, warp 1 MMA, warps 2-5 epilogue
-constexpr int kTileRows = 128;         // UMMA M
+constexpr int kTcThreads = 384;        // warp 0 TMA (warps 1-3 idle), warpgroups 1 and 2: MMA + epilogue
+constexpr int kTileRows = 128;         // document rows per stage: warpgroup c takes rows 64c .. 64c + 63
 constexpr int kKBlockElems = 64;       // 64 x 16-bit = 128 B = one SWIZZLE_128B row
 constexpr int kKBlockBytes = kTileRows * 128;  // 16 KB: [128 rows][128 B]
 constexpr int kMaxStages = 12;
-constexpr int kAccStages = 4;
 constexpr int kQSlots = 2;
 
 struct TcShared {  // control block placed after the tile storage
   uint64_t full[kMaxStages];
-  uint64_t empty[kMaxStages];
+  uint64_t empty[kMaxStages];   // 8 arrivals: every consumer warp
   uint64_t qfull[kQSlots];
-  uint64_t qempty[kQSlots];
-  uint64_t accfull[kAccStages];
-  uint64_t accempty[kAccStages];
-  uint32_t tmem_base;
-  uint32_t pad;
-  float colmax[2][4][128];  // [pair parity][epilogue warp][query column]
+  uint64_t qempty[kQSlots];     // 8 arrivals
+  float colmax[2][8][128];      // [pair parity][consumer warp][query column]
 };
 
 struct TcLaunch {
-  int32_t npad;        // query rows padded to a multiple of 32 (UMMA N, TMEM columns per stage)
+  int32_t npad;        // query rows padded to a multiple of 32 (wgmma N)
   int32_t kblocks;     // dim / 64
   int32_t kbs;         // k-blocks per stage (1 or 2)
   int32_t stages;      // document stages in the ring
   int32_t tiles;       // ceil(Ld / 128)
-  int32_t fmt;         // kFmtF16 / kFmtBF16
-  int32_t tmem_cols;   // power of two >= kAccStages * npad
   int32_t qslot_bytes; // kblocks * npad * 128
 };
 
-// Column-wise max over the 32 lanes of a warp for 32 per-lane values: afterwards lane l holds
-// max over lanes of v[l].  Halving exchange: 16+8+4+2+1 shuffles.
-__device__ __forceinline__ float warp_transpose_max32(float (&v)[32], int lane) {
-#pragma unroll
-  for (int i = 0; i < 16; ++i) {
-    const bool up = (lane & 16) != 0;
-    const float send = up ? v[i] : v[i + 16];
-    const float keep = up ? v[i + 16] : v[i];
-    v[i] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, 16));
-  }
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const bool up = (lane & 8) != 0;
-    const float send = up ? v[i] : v[i + 8];
-    const float keep = up ? v[i + 8] : v[i];
-    v[i] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, 8));
-  }
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const bool up = (lane & 4) != 0;
-    const float send = up ? v[i] : v[i + 4];
-    const float keep = up ? v[i + 4] : v[i];
-    v[i] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, 4));
-  }
-#pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    const bool up = (lane & 2) != 0;
-    const float send = up ? v[i] : v[i + 2];
-    const float keep = up ? v[i + 2] : v[i];
-    v[i] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, 2));
-  }
-  {
-    const bool up = (lane & 1) != 0;
-    const float send = up ? v[0] : v[1];
-    const float keep = up ? v[1] : v[0];
-    v[0] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, 1));
-  }
-  return v[0];
+template <typename T>
+__device__ __forceinline__ void wgmma_n32(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc);
+template <>
+__device__ __forceinline__ void wgmma_n32<__half>(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc) {
+  wgmma_m64n32k16_f16(d, a, b, acc);
+}
+template <>
+__device__ __forceinline__ void wgmma_n32<__nv_bfloat16>(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc) {
+  wgmma_m64n32k16_bf16(d, a, b, acc);
 }
 
-template <int KBS>
+// NC = npad / 32 accumulator chunks of 16 registers per thread.
+template <typename T, int KBS, int NC>
 __global__ void __launch_bounds__(kTcThreads, 1)
 maxsim_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_d,
                  MaxsimParams P, TcLaunch L) {
   extern __shared__ uint8_t smem_raw[];
-  // SWIZZLE_128B tiles need 1024-B alignment
   // 1024-B alignment for SWIZZLE_128B tiles, derived by pointer arithmetic on the __shared__ array so the
   // compiler keeps the shared address space (LDS/STS instead of generic LD/ST)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -240,16 +204,11 @@ maxsim_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   if (threadIdx.x == 0) {
     prefetch_tensormap(&tmap_q);
     prefetch_tensormap(&tmap_d);
-    for (int s = 0; s < L.stages; ++s) { mbar_init(&S->full[s], 1); mbar_init(&S->empty[s], 1); }
-    for (int s = 0; s < kQSlots; ++s) { mbar_init(&S->qfull[s], 1); mbar_init(&S->qempty[s], 1); }
-    for (int s = 0; s < kAccStages; ++s) { mbar_init(&S->accfull[s], 1); mbar_init(&S->accempty[s], 4); }
+    for (int s = 0; s < L.stages; ++s) { mbar_init(&S->full[s], 1); mbar_init(&S->empty[s], 8); }
+    for (int s = 0; s < kQSlots; ++s) { mbar_init(&S->qfull[s], 1); mbar_init(&S->qempty[s], 8); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(&S->tmem_base, (uint32_t)L.tmem_cols);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = S->tmem_base;
 
   const int ksteps = L.kblocks / KBS;
 
@@ -282,134 +241,114 @@ maxsim_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------- MMA issuer ---------------------------------
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc((uint32_t)L.fmt, kTileRows, (uint32_t)L.npad);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t accphase = 0;
-      int64_t prev_q = -1;
-      uint32_t qcount = 0;
-      int cur_slot = 0;
-      for (int64_t p = p_begin; p < p_end; ++p) {
-        const int64_t qi = pair_query(P, p);
-        if (qi != prev_q) {
-          if (prev_q >= 0) umma_commit(&S->qempty[cur_slot]);  // all MMAs reading the old Q are done
-          cur_slot = (int)(qcount & 1u);
-          mbar_wait(&S->qfull[cur_slot], (qcount >> 1) & 1u);
-          ++qcount;
-          prev_q = qi;
-        }
-        const uint32_t qaddr = smem_u32(q_base + (size_t)cur_slot * L.qslot_bytes);
-        for (int t = 0; t < L.tiles; ++t) {
-          mbar_wait(&S->accempty[acc], accphase ^ 1u);
-          tc_fence_after_sync();
-          const uint32_t tmem_d = tmem_base + (uint32_t)(acc * L.npad);
-          for (int ks = 0; ks < ksteps; ++ks) {
-            mbar_wait(&S->full[stage], phase);
-            tc_fence_after_sync();
-            const uint32_t aaddr = smem_u32(stage_base + (size_t)stage * kStageBytes);
-#pragma unroll
-            for (int kb = 0; kb < KBS; ++kb) {
-              const uint32_t a_kb = aaddr + kb * kKBlockBytes;
-              const uint32_t b_kb = qaddr + (uint32_t)((ks * KBS + kb) * L.npad * 128);
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {  // 64 / UMMA_K(16)
-                umma_f16(tmem_d, make_sw128_kmajor_desc(a_kb + k * 32), make_sw128_kmajor_desc(b_kb + k * 32),
-                         idesc, (uint32_t)((ks | kb | k) != 0));
-              }
-            }
-            umma_commit(&S->empty[stage]);  // smem stage free once these MMAs retire
-            if (++stage == L.stages) { stage = 0; phase ^= 1u; }
-          }
-          umma_commit(&S->accfull[acc]);
-          if (++acc == kAccStages) { acc = 0; accphase ^= 1u; }
-        }
-      }
-    }
-  } else {
-    // ------------------------------- epilogue ------------------------------------
-    const int ew = warp - 2;          // 0..3
-    const int lq = warp & 3;          // TMEM lane quarter this warp may access
-    const int ncol32 = L.npad >> 5;   // 32-column groups
-    int acc = 0;
-    uint32_t accphase = 0;
+  } else if (warp >= 4) {
+    // ------------------------------- consumers: wgmma + masked column max -------------------
+    const int c = (warp >> 2) - 1;     // warpgroup 0 / 1: document rows 64c .. 64c + 63 of every tile
+    const int wq = warp & 3;
+    const int ew = 4 * c + wq;         // 0..7
+    const int cq = 2 * (lane & 3);     // first column of this thread inside an 8-column group
     const int dmt = P.d_mask ? P.mask_dtype : MMB200_MASK_NONE;
     const int qmt = P.q_mask ? P.mask_dtype : MMB200_MASK_NONE;
-    // Mask words are fetched two tiles ahead and only *tested* when their tile is processed, so the
-    // global-load latency hides behind the TMEM loads / shuffles of the tiles in between.
-    int64_t fp = p_begin;  // (pair, tile) whose mask word is fetched next
-    int ft = 0;
-    auto fetch = [&](uint64_t& raw) -> bool {  // returns "row lies inside the document"
-      bool in_doc = false;
-      raw = 1;
-      if (fp < p_end) {
-        const int row = ft * kTileRows + lq * 32 + lane;
-        in_doc = row < P.Ld;
-        if (in_doc && dmt != MMB200_MASK_NONE) raw = mask_raw(P.d_mask, dmt, pair_dmask_row(P, fp) * (int64_t)P.Ld + row);
-      }
-      if (++ft == L.tiles) { ft = 0; ++fp; }
-      return in_doc;
-    };
-    uint64_t raw0, raw1;
-    bool in0 = fetch(raw0);
-    bool in1 = fetch(raw1);
+    int stage = 0;
+    uint32_t phase = 0;
+    int64_t prev_q = -1;
+    uint32_t qcount = 0;
+    int cur_slot = 0;
     for (int64_t p = p_begin; p < p_end; ++p) {
       const int64_t qi = pair_query(P, p);
-      // query-mask words for this lane's columns: fetched now, tested after the pair's tiles
-      uint64_t qraw[4];
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        const int col = c * 32 + lane;
-        qraw[c] = (c < ncol32 && col < P.Lq) ? (qmt != MMB200_MASK_NONE ? mask_raw(P.q_mask, qmt, qi * (int64_t)P.Lq + col) : 1) : 0;
+      if (qi != prev_q) {
+        if (prev_q >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&S->qempty[cur_slot]); }  // old Q no longer read
+        cur_slot = (int)(qcount & 1u);
+        mbar_wait(&S->qfull[cur_slot], (qcount >> 1) & 1u);
+        ++qcount;
+        prev_q = qi;
       }
-      float colmax[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
+      const uint32_t qaddr = smem_u32(q_base + (size_t)cur_slot * L.qslot_bytes);
+      const int64_t dmrow = pair_dmask_row(P, p);
+      float colmax[NC][8];
+#pragma unroll
+      for (int h = 0; h < NC; ++h)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) colmax[h][j] = -INFINITY;
       for (int t = 0; t < L.tiles; ++t) {
-        const bool in_doc = in0;
-        const uint64_t raw = raw0;
-        in0 = in1;
-        raw0 = raw1;
-        in1 = fetch(raw1);
-        mbar_wait(&S->accfull[acc], accphase);
-        tc_fence_after_sync();
-        const bool tok_ok = mask_test(raw, dmt);
-        const uint32_t taddr = tmem_base + ((uint32_t)(lq * 32) << 16) + (uint32_t)(acc * L.npad);
+        // this thread's two document rows; mask words fetched before the MMAs so their latency hides behind them
+        const int g0 = t * kTileRows + 64 * c + 16 * wq + (lane >> 2), g1 = g0 + 8;
+        const bool in0 = g0 < P.Ld, in1 = g1 < P.Ld;
+        const uint64_t raw0 = (in0 && dmt != MMB200_MASK_NONE) ? mask_raw(P.d_mask, dmt, dmrow * (int64_t)P.Ld + g0) : 1;
+        const uint64_t raw1 = (in1 && dmt != MMB200_MASK_NONE) ? mask_raw(P.d_mask, dmt, dmrow * (int64_t)P.Ld + g1) : 1;
+        float acc[NC][16];
 #pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          if (c < ncol32) {
-            uint32_t r[32];
-            tmem_ld_32x32b_x32(taddr + c * 32, r);
-            tmem_ld_wait();
-            float v[32];
+        for (int h = 0; h < NC; ++h)
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              v[j] = in_doc ? (tok_ok ? __uint_as_float(r[j]) : kMaskedScore) : -INFINITY;
+          for (int j = 0; j < 16; ++j) acc[h][j] = 0.f;
+        for (int ks = 0; ks < ksteps; ++ks) {
+          mbar_wait(&S->full[stage], phase);
+          const uint32_t aaddr = smem_u32(stage_base + (size_t)stage * kStageBytes) + 64 * c * 128;
+          wgmma_fence();
+#pragma unroll
+          for (int kb = 0; kb < KBS; ++kb) {
+            const uint32_t a_kb = aaddr + kb * kKBlockBytes;
+            const uint32_t b_kb = qaddr + (uint32_t)((ks * KBS + kb) * L.npad * 128);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {  // 64 / wgmma K (16)
+              const uint64_t adesc = make_wgmma_sw128_desc(a_kb + k * 32);
+#pragma unroll
+              for (int h = 0; h < NC; ++h)
+                wgmma_n32<T>(acc[h], adesc, make_wgmma_sw128_desc(b_kb + h * 32 * 128 + k * 32), 1u);
             }
-            colmax[c] = fmaxf(colmax[c], warp_transpose_max32(v, lane));
           }
+          wgmma_commit();
+          wgmma_wait<0>();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&S->empty[stage]);  // smem stage free: these MMAs have completed
+          if (++stage == L.stages) { stage = 0; phase ^= 1u; }
         }
-        tc_fence_before_sync();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&S->accempty[acc]);
-        if (++acc == kAccStages) { acc = 0; accphase ^= 1u; }
-      }
-      const int buf = (int)((p - p_begin) & 1);
 #pragma unroll
-      for (int c = 0; c < 4; ++c)
-        if (c < ncol32) S->colmax[buf][ew][c * 32 + lane] = colmax[c];
-      named_bar_sync(1, 128);
-      if (ew == (int)((p - p_begin) & 3)) {  // rotate the final reduction over the 4 warps
+        for (int h = 0; h < NC; ++h) wgmma_fence_regs(acc[h]);
+        const float f0 = in0 ? (mask_test(raw0, dmt) ? 0.f : kMaskedScore) : -INFINITY;
+        const float f1 = in1 ? (mask_test(raw1, dmt) ? 0.f : kMaskedScore) : -INFINITY;
+        const bool keep0 = in0 && mask_test(raw0, dmt), keep1 = in1 && mask_test(raw1, dmt);
+#pragma unroll
+        for (int h = 0; h < NC; ++h)
+#pragma unroll
+          for (int j = 0; j < 4; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const float v0 = keep0 ? acc[h][4 * j + e] : f0;
+              const float v1 = keep1 ? acc[h][4 * j + 2 + e] : f1;
+              colmax[h][2 * j + e] = fmaxf(colmax[h][2 * j + e], fmaxf(v0, v1));
+            }
+      }
+      // max over the 8 row groups of the warp (lanes with the same lane % 4 hold the same columns)
+#pragma unroll
+      for (int h = 0; h < NC; ++h)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          float v = colmax[h][j];
+          v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 4));
+          v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 8));
+          v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 16));
+          colmax[h][j] = v;
+        }
+      const int buf = (int)((p - p_begin) & 1);
+      if (lane < 4) {
+#pragma unroll
+        for (int h = 0; h < NC; ++h)
+#pragma unroll
+          for (int j = 0; j < 4; ++j)
+            *reinterpret_cast<float2*>(&S->colmax[buf][ew][h * 32 + 8 * j + cq]) = make_float2(colmax[h][2 * j], colmax[h][2 * j + 1]);
+      }
+      named_bar_sync(1, 256);
+      if (ew == (int)((p - p_begin) & 7)) {  // rotate the final reduction over the 8 warps
         float total = 0.f;
 #pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          if (c < ncol32) {
-            const int col = c * 32 + lane;
-            float m = fmaxf(fmaxf(S->colmax[buf][0][col], S->colmax[buf][1][col]),
-                            fmaxf(S->colmax[buf][2][col], S->colmax[buf][3][col]));
-            total += mask_test(qraw[c], qmt) ? m : 0.f;
-          }
+        for (int h = 0; h < NC; ++h) {
+          const int col = h * 32 + lane;
+          float m = S->colmax[buf][0][col];
+#pragma unroll
+          for (int w = 1; w < 8; ++w) m = fmaxf(m, S->colmax[buf][w][col]);
+          const bool qok = col < P.Lq && mask_test(qmt != MMB200_MASK_NONE ? mask_raw(P.q_mask, qmt, qi * (int64_t)P.Lq + col) : 1, qmt);
+          total += qok ? m : 0.f;
         }
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) total += __shfl_xor_sync(0xffffffffu, total, o);
@@ -417,26 +356,42 @@ maxsim_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
       }
     }
   }
-
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, (uint32_t)L.tmem_cols);
-  }
 }
 
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
 static bool tc_supported(const MaxsimParams& P, int dtype, std::string* why) {
-  if (dtype != MMB200_F16 && dtype != MMB200_BF16) { *why = "tcgen05 path needs f16/bf16 inputs"; return false; }
-  if (P.dim % 64 != 0 || P.dim < 64 || P.dim > 1024) { *why = "tcgen05 path needs dim % 64 == 0, 64 <= dim <= 1024"; return false; }
-  if (P.Lq < 1 || P.Lq > 128) { *why = "tcgen05 path needs 1 <= Lq <= 128"; return false; }
+  if (dtype != MMB200_F16 && dtype != MMB200_BF16) { *why = "tensor-core path needs f16/bf16 inputs"; return false; }
+  if (P.dim % 64 != 0 || P.dim < 64 || P.dim > 1024) { *why = "tensor-core path needs dim % 64 == 0, 64 <= dim <= 1024"; return false; }
+  if (P.Lq < 1 || P.Lq > 128) { *why = "tensor-core path needs 1 <= Lq <= 128"; return false; }
   if (P.Ld < 1) { *why = "Ld < 1"; return false; }
   if (P.argmax) { *why = "argmax output is produced by the SIMT kernel"; return false; }
   if ((reinterpret_cast<uintptr_t>(P.q) | reinterpret_cast<uintptr_t>(P.d)) & 15) { *why = "q/d must be 16-byte aligned"; return false; }
   return true;
+}
+
+template <typename T, int KBS>
+static int launch_tc_nc(int nc, int grid, size_t smem_bytes, cudaStream_t stream, const CUtensorMap& tq, const CUtensorMap& td,
+                        const MaxsimParams& P, const TcLaunch& L) {
+#define MMB_TC_CASE(N)                                                                                                  \
+  case N:                                                                                                               \
+    MMB_CHECK_CUDA(cudaFuncSetAttribute(maxsim_tc_kernel<T, KBS, N>, cudaFuncAttributeMaxDynamicSharedMemorySize,       \
+                                        (int)smem_bytes));                                                              \
+    maxsim_tc_kernel<T, KBS, N><<<grid, kTcThreads, smem_bytes, stream>>>(tq, td, P, L);                                \
+    break;
+  switch (nc) {
+    MMB_TC_CASE(1)
+    MMB_TC_CASE(2)
+    MMB_TC_CASE(3)
+    MMB_TC_CASE(4)
+    default:
+      set_error("maxsim documents-on-M: query tile out of range");
+      return MMB200_ERR_INVALID;
+  }
+#undef MMB_TC_CASE
+  MMB_CHECK_CUDA(cudaGetLastError());
+  return MMB200_OK;
 }
 
 static int launch_tc(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cudaStream_t stream) {
@@ -445,17 +400,13 @@ static int launch_tc(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cu
   L.kblocks = P.dim / 64;
   L.kbs = (L.kblocks % 2 == 0) ? 2 : 1;
   L.tiles = (P.Ld + kTileRows - 1) / kTileRows;
-  L.fmt = dtype == MMB200_F16 ? kFmtF16 : kFmtBF16;
   L.qslot_bytes = L.kblocks * L.npad * 128;
-  int tc = kAccStages * L.npad;
-  L.tmem_cols = 32;
-  while (L.tmem_cols < tc) L.tmem_cols <<= 1;
   const int stage_bytes = L.kbs * kKBlockBytes;
   const int fixed = kQSlots * L.qslot_bytes + (int)sizeof(TcShared) + 1024 /* alignment slack */;
   const int budget = dev.max_smem_optin - fixed;
   L.stages = std::min(kMaxStages, budget / stage_bytes);
   if (L.stages < 2) {
-    set_error("maxsim tcgen05: query tile too large for shared memory");
+    set_error("maxsim documents-on-M: query tile too large for shared memory");
     return MMB200_ERR_UNSUPPORTED;
   }
   const size_t smem_bytes = (size_t)L.stages * stage_bytes + fixed;
@@ -479,15 +430,12 @@ static int launch_tc(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cu
       return rc;
   }
   const int grid = (int)std::min<int64_t>(dev.sm_count, P.n_pairs);
-  if (L.kbs == 2) {
-    MMB_CHECK_CUDA(cudaFuncSetAttribute(maxsim_tc_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
-    maxsim_tc_kernel<2><<<grid, kTcThreads, smem_bytes, stream>>>(tq, td, P, L);
-  } else {
-    MMB_CHECK_CUDA(cudaFuncSetAttribute(maxsim_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
-    maxsim_tc_kernel<1><<<grid, kTcThreads, smem_bytes, stream>>>(tq, td, P, L);
-  }
-  MMB_CHECK_CUDA(cudaGetLastError());
-  return MMB200_OK;
+  const int nc = L.npad / 32;
+  if (dtype == MMB200_F16)
+    return L.kbs == 2 ? launch_tc_nc<__half, 2>(nc, grid, smem_bytes, stream, tq, td, P, L)
+                      : launch_tc_nc<__half, 1>(nc, grid, smem_bytes, stream, tq, td, P, L);
+  return L.kbs == 2 ? launch_tc_nc<__nv_bfloat16, 2>(nc, grid, smem_bytes, stream, tq, td, P, L)
+                    : launch_tc_nc<__nv_bfloat16, 1>(nc, grid, smem_bytes, stream, tq, td, P, L);
 }
 
 static int launch_simt(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cudaStream_t stream) {
@@ -521,8 +469,8 @@ int maxsim_fwd_device(const MaxsimParams& P, int dtype, int impl, cudaStream_t s
   if (P.n_pairs == 0) return MMB200_OK;
   DeviceInfo dev;
   if (int rc = current_device_info(&dev)) return rc;
-  if (!is_sm100(dev)) {
-    set_error("matchmaker_b200 kernels are built for sm_100a only; device is sm_" + std::to_string(dev.cc_major) +
+  if (!is_sm90(dev)) {
+    set_error("matchmaker_b200 kernels are built for sm_90a only; device is sm_" + std::to_string(dev.cc_major) +
               std::to_string(dev.cc_minor));
     return MMB200_ERR_UNSUPPORTED;
   }

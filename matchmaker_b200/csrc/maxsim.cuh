@@ -23,12 +23,12 @@ struct MaxsimParams {
 };
 
 struct DeviceInfo;
-// maxsim_qm.cu: "queries on M" tcgen05 kernel (Lq <= 32, dim 64/128); *handled = false if out of envelope.
+// maxsim_qm.cu: "queries on M" wgmma kernel (Lq <= 32, dim 64/128); *handled = false if out of envelope.
 int maxsim_qm_launch(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cudaStream_t stream, bool* handled);
 // rows_needed[di] = 1 + index of the last unmasked row of document di (Ld when d_mask == NULL)
 int maxsim_rows_needed_launch(const void* d_mask, int mask_dtype, int32_t* rows_needed, int64_t n_d, int Ld, cudaStream_t stream);
 
-// Validates, picks SIMT or tcgen05 and launches on `stream`.
+// Validates, picks the SIMT or a tensor-core kernel and launches on `stream`.
 int maxsim_fwd_device(const MaxsimParams& P, int dtype, int impl, cudaStream_t stream);
 
 }  // namespace mmb

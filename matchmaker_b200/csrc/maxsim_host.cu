@@ -125,8 +125,8 @@ extern "C" int mmb200_maxsim_bwd(const void* q, const void* d, const float* grad
               "pair counts inconsistent");
   DeviceInfo dev;
   if (int rc = current_device_info(&dev)) return rc;
-  if (!is_sm100(dev)) {
-    set_error("matchmaker_b200 kernels are built for sm_100a only");
+  if (!is_sm90(dev)) {
+    set_error("matchmaker_b200 kernels are built for sm_90a only");
     return MMB200_ERR_UNSUPPORTED;
   }
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
@@ -165,48 +165,8 @@ extern "C" int mmb200_maxsim_fwd_host(const void* q_host, const void* d_host, co
   HostPipe* hp = nullptr;
   if (int rc = get_pipe(&hp)) return rc;
 
-  // ---- zero-copy path: documents in pinned (device-mapped) host memory are fetched by the kernel's TMA
-  // straight over PCIe, and only up to each document's last unmasked row (chunk_pairs == -1 disables it)
-  if (chunk_pairs != -1) {
-    cudaPointerAttributes attr{};
-    const bool pinned = cudaPointerGetAttributes(&attr, d_host) == cudaSuccess && attr.type == cudaMemoryTypeHost &&
-                        attr.devicePointer != nullptr;
-    (void)cudaGetLastError();
-    DeviceInfo dev;
-    if (int rc = current_device_info(&dev)) return rc;
-    if (pinned && is_sm100(dev)) {
-      const size_t es0 = dtype_size(dtype), ms0 = mask_dtype_size(mask_dtype);
-      const size_t qb = (size_t)n_q * Lq * dim * es0;
-      const size_t qmb = q_mask_host ? (size_t)n_q * Lq * ms0 : 0;
-      const size_t dmb = d_mask_host ? (size_t)n_d * Ld * ms0 : 0;
-      const size_t rows_b = (size_t)n_d * sizeof(int32_t);
-      const size_t need = align_up(qb, 256) + align_up(qmb, 256) + align_up(dmb, 256) + align_up(rows_b, 256);
-      if (int rc = ensure(&hp->qbuf, &hp->q_bytes, need)) return rc;
-      if (int rc = ensure(reinterpret_cast<void**>(&hp->out), &hp->out_bytes, (size_t)n_d * sizeof(float))) return rc;
-      uint8_t* w = static_cast<uint8_t*>(hp->qbuf);
-      void* dq = w; w += align_up(qb, 256);
-      void* dqm = q_mask_host ? w : nullptr; w += align_up(qmb, 256);
-      void* ddm = d_mask_host ? w : nullptr; w += align_up(dmb, 256);
-      int32_t* rows = reinterpret_cast<int32_t*>(w);
-      MMB_CHECK_CUDA(cudaMemcpyAsync(dq, q_host, qb, cudaMemcpyHostToDevice, hp->compute));
-      if (q_mask_host) MMB_CHECK_CUDA(cudaMemcpyAsync(dqm, q_mask_host, qmb, cudaMemcpyHostToDevice, hp->compute));
-      if (d_mask_host) MMB_CHECK_CUDA(cudaMemcpyAsync(ddm, d_mask_host, dmb, cudaMemcpyHostToDevice, hp->compute));
-      if (int rc = maxsim_rows_needed_launch(ddm, mask_dtype, rows, n_d, Ld, hp->compute)) return rc;
-      MaxsimParams P;
-      P.q = dq; P.d = attr.devicePointer; P.q_mask = dqm; P.d_mask = ddm;
-      P.pair_q = nullptr; P.pair_d = nullptr; P.pair_dmask = nullptr; P.rows_needed = rows;
-      P.out = hp->out; P.argmax = nullptr; P.n_q = n_q; P.n_d = n_d; P.n_pairs = n_d; P.pair_base = 0;
-      P.docs_per_query = docs_per_query; P.Lq = Lq; P.Ld = Ld; P.dim = dim; P.mask_dtype = mask_dtype;
-      bool handled = false;
-      if (int rc = maxsim_qm_launch(P, dtype, dev, hp->compute, &handled)) return rc;
-      if (handled) {
-        MMB_CHECK_CUDA(cudaMemcpyAsync(out_host, hp->out, (size_t)n_d * sizeof(float), cudaMemcpyDeviceToHost, hp->compute));
-        MMB_CHECK_CUDA(cudaStreamSynchronize(hp->compute));
-        return MMB200_OK;
-      }
-      // shape outside the queries-on-M kernel: fall through to the slab pipeline
-    }
-  }
+  // Documents are staged through device slabs by the copy engine, also when they sit in pinned host memory: the H100's
+  // TMA unit does not fetch from mapped host memory (the kernel faults), so there is no zero-copy path on this GPU.
   if (chunk_pairs == -1) chunk_pairs = 0;
 
   const size_t es = dtype_size(dtype), ms = mask_dtype_size(mask_dtype);

@@ -1,27 +1,29 @@
-// ColBERT max-sim, second-generation tcgen05 kernel ("queries on M"): the hot path for Lq <= 32.
+// ColBERT max-sim, "queries on M" wgmma kernel: the hot path for Lq <= 32.
 //
-// Why a second orientation: in maxsim.cu the accumulator is [128 document rows (TMEM lanes) x 32 query
-// columns], so the max over document rows is a cross-lane reduction -- ~460 warp instructions per
-// 128-row tile on warps that have nobody to hide latency behind (ncu: 28 % issue-slot use, epilogue-bound
-// at 56 % of HBM peak).  Here the accumulator is transposed:
+// Why this orientation: with documents on M (maxsim.cu) the max over document rows is a reduction across the rows of
+// the accumulator, i.e. across threads.  Here the accumulator is transposed:
 //
-//     D[128 x TN] = Qrep[128 x dim] * Doc[TN x dim]^T        (one tcgen05.mma chain per document)
+//     D[64 x TN] = Qrep[64 x dim] * Doc[TN x dim]^T        (one wgmma chain per document tile)
 //
-// TMEM lane = query token, TMEM column = document row, so the max over a document is a per-thread
-// FMNMX chain over registers (no shuffles, no cross-warp combine, no barrier).  Rows 0..31 of Qrep are
-// the query, rows 32..63 a second copy (so two epilogue warps, TMEM lane quarters 0 and 1, can each
-// take every other pair); rows 64..127 read whatever follows in shared memory and are never looked at.
+// row = query token, column = document row, so the max over a document is a per-thread FMNMX chain over the
+// accumulator registers plus two quad shuffles.  Rows 0..31 of Qrep are the query; rows 32..63 of the instruction read
+// whatever follows the query in shared memory and are never looked at.
 //
-// The document mask is applied BY THE TENSOR CORE: one extra UMMA K-step multiplies a column of ones
-// (query side) with a per-row penalty (document side): 0 for real tokens, -inf for padding and for the
-// tile's rows past Ld, so masked rows can never win the max.  The reference's -1000 fill
-// (matchmaker/models/colbert.py:69) only matters when it IS the max; that is reproduced exactly by one
-// "virtual" document row (index Ld, zero data from TMA out-of-bounds fill) whose penalty is -1000 when
-// the document has at least one masked position and -inf otherwise.  A helper warp writes the 6 KB
-// penalty tile per document while TMA streams the 48 KB of token vectors.
+// The document mask is applied in the epilogue as an fp32 penalty per document row, added to every query's score of
+// that row: 0 for real tokens, -inf for padding and for the tile's rows past Ld, so masked rows can never win the max.
+// The reference's -1000 fill (matchmaker/models/colbert.py:69) only matters when it IS the max; that is reproduced
+// exactly by one "virtual" document row (the last row of the last tile, index >= Ld, zero data from TMA out-of-bounds
+// fill) whose penalty is -1000 when the document has at least one masked position and -inf otherwise.  A helper warp
+// writes the penalty row per document tile while TMA streams the token vectors.
 //
-// Per document: 1 TMA (box 64 x TN x KB), 4*KB+1 MMAs (M=128, N=TN<=256, K=16), TN/32 tcgen05.ld + TN/3
-// FMNMX3 in one warp, one fp32 store.  HBM-bound by design.
+// Per CTA (persistent, one per SM, 384 threads = 3 warpgroups):
+//   warp 0        TMA producer: query tile (2-slot ring, re-fetched when the query changes), document tiles
+//   warp 1        penalty writer
+//   warpgroups 1, 2  consumers: warpgroup c takes the CTA's documents c, c + 2, ...; per tile 4 * dim / 64 * TN / 64
+//                 wgmma m64n64k16 into registers, then the masked max over the tile in the same registers.  While one
+//                 warpgroup reduces, the other one's MMAs run.  Each warpgroup has its own half of the stage ring, so
+//                 every stage barrier has one consumer that waits for its phases in order.
+// HBM-bound by design: per document one TMA box, one fp32 store.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -36,62 +38,60 @@ namespace mmb {
 
 namespace {
 
-constexpr int kThreads = 192;  // warp 0,1: epilogue (TMEM lane quarters 0,1); 2: TMA; 3: MMA; 4: penalty writer; 5: spare
-constexpr int kMaxStages = 4;
-constexpr int kMaxAcc = 4;
+constexpr int kThreads = 384;
+constexpr int kMaxStages = 8;                // even: half of the ring per consumer warpgroup
 constexpr int kQSlots = 2;
-constexpr int kQRep = 2;                     // copies of the 32 query rows
 constexpr int kQRows = 32;
-constexpr int kQBlockBytes = kQRep * kQRows * 128;  // one k-block of the replicated query tile (8 KB)
+constexpr int kQBlockBytes = kQRows * 128;   // one k-block of the query tile (4 KB)
 
 struct QmShared {
   uint64_t full[kMaxStages];   // 2 arrivals: TMA producer (with tx bytes) + penalty writer
-  uint64_t empty[kMaxStages];  // tcgen05.commit
+  uint64_t empty[kMaxStages];  // 4 arrivals: the warps of the warpgroup that owns the stage
   uint64_t qfull[kQSlots];
-  uint64_t qempty[kQSlots];
-  uint64_t accfull[kMaxAcc];
-  uint64_t accempty[kMaxAcc];
-  uint32_t tmem_base;
-  uint32_t pad;
+  uint64_t qempty[kQSlots];    // 8 arrivals: every warp of both consumer warpgroups
+  float part[2][2];            // [consumer][pair parity]: row sum of query rows 16..31
 };
 
 struct QmLaunch {
   int32_t kblocks;      // dim / 64 (1 or 2)
-  int32_t tn;           // document rows per tile (multiple of 16, <= 256)
+  int32_t tn;           // document rows per tile (multiple of 64, <= 256)
   int32_t tiles;        // tiles per document; tiles * tn >= Ld + 1
-  int32_t stages;
-  int32_t acc_slots;
-  int32_t tmem_cols;
-  int32_t fmt;
+  int32_t stages;       // even: stages [0, stages / 2) serve warpgroup 0, the rest warpgroup 1
   int32_t doc_bytes;    // kblocks * tn * 128
-  int32_t stage_bytes;  // doc_bytes + tn * 32
-  uint16_t neg_inf, neg_1000, one;  // bit patterns in the storage dtype
+  int32_t stage_bytes;  // doc_bytes + penalty row (tn fp32, rounded to 1 KB)
 };
-
-// K-major operand with NO swizzle, 16 elements (32 B) along K: core matrices of 8 rows x 16 B;
-// second K chunk at +128 B (LBO), next 8-row group at +256 B (SBO).
-__device__ __forceinline__ uint64_t make_noswz_k16_desc(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
-  d |= static_cast<uint64_t>(128 >> 4) << 16;
-  d |= static_cast<uint64_t>(256 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  return d;
-}
-
-__device__ __forceinline__ uint32_t penalty_offset(int row) { return (uint32_t)((row >> 3) * 256 + (row & 7) * 16); }
-
-__device__ __forceinline__ float max3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
 
 __device__ __forceinline__ int64_t pair_dmask_row_of(const MaxsimParams& P, int64_t p) {
   if (P.pair_dmask) return (int64_t)P.pair_dmask[p];
   return P.pair_d ? (int64_t)P.pair_d[p] : p;
 }
 
-// kArgmax: the training instantiation also tracks WHICH document row won each query token's max (what backward needs,
-// matchmaker/models/colbert.py:71 through autograd): a compare + two selects per accumulator element instead of a third
-// of an FMNMX3 -- ~9x the epilogue instructions, still a fraction of the ~2000 cycles a document's bytes take to arrive.
+template <typename T>
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc);
+template <>
+__device__ __forceinline__ void wgmma_n64<__half>(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
+  wgmma_m64n64k16_f16(d, a, b, acc);
+}
+template <>
+__device__ __forceinline__ void wgmma_n64<__nv_bfloat16>(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
+  wgmma_m64n64k16_bf16(d, a, b, acc);
+}
+
+// running maximum of (v, column) in column order; ties keep the first column
 template <bool kArgmax>
+__device__ __forceinline__ void take(float v, int col, float& m, int& am) {
+  if constexpr (kArgmax) {
+    const bool gt = v > m;
+    m = gt ? v : m;
+    am = gt ? col : am;
+  } else {
+    m = fmaxf(m, v);
+  }
+}
+
+// kArgmax: the training instantiation also tracks WHICH document row won each query token's max (what backward needs,
+// matchmaker/models/colbert.py:71 through autograd).  NCH = tn / 64 accumulator chunks of 32 registers.
+template <typename T, int NCH, bool kArgmax>
 __global__ void __launch_bounds__(kThreads, 1)
 maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_d,
                  const __grid_constant__ CUtensorMap tmap_d16, MaxsimParams P, QmLaunch L) {
@@ -100,10 +100,9 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   // compiler keeps the shared address space (LDS/STS instead of generic LD/ST)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int qslot_bytes = L.kblocks * kQBlockBytes;
-  uint8_t* q_base = smem;                                            // [kQSlots][kblocks][2 x 32 rows][128 B]
-  uint8_t* stage_base = q_base + kQSlots * qslot_bytes;              // [stages][doc tile | penalty tile]
-  uint8_t* ones_tile = stage_base + (size_t)L.stages * L.stage_bytes;  // [128 rows][16 elems], no swizzle
-  QmShared* S = reinterpret_cast<QmShared*>(ones_tile + 4096);
+  uint8_t* q_base = smem;                                            // [kQSlots][kblocks][32 rows][128 B]
+  uint8_t* stage_base = q_base + kQSlots * qslot_bytes;              // [stages][doc tile | penalty row]
+  QmShared* S = reinterpret_cast<QmShared*>(stage_base + (size_t)L.stages * L.stage_bytes);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -115,46 +114,26 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   if (threadIdx.x == 0) {
     prefetch_tensormap(&tmap_q);
     prefetch_tensormap(&tmap_d);
-    for (int s = 0; s < L.stages; ++s) { mbar_init(&S->full[s], 2); mbar_init(&S->empty[s], 1); }
-    for (int s = 0; s < kQSlots; ++s) { mbar_init(&S->qfull[s], 1); mbar_init(&S->qempty[s], 1); }
-    for (int s = 0; s < L.acc_slots; ++s) { mbar_init(&S->accfull[s], 1); mbar_init(&S->accempty[s], 1); }
+    for (int s = 0; s < L.stages; ++s) { mbar_init(&S->full[s], 2); mbar_init(&S->empty[s], 4); }
+    for (int s = 0; s < kQSlots; ++s) { mbar_init(&S->qfull[s], 1); mbar_init(&S->qempty[s], 8); }
     fence_barrier_init();
-  }
-  if (warp == 4) {
-    // zero every penalty tile (only element 0 of each row's first 16-B chunk is rewritten per document)
-    // and build the ones tile: element (row, k=0) = 1, everything else 0
-    for (int s = 0; s < L.stages; ++s) {
-      uint4* pt = reinterpret_cast<uint4*>(stage_base + (size_t)s * L.stage_bytes + L.doc_bytes);
-      for (int e = lane; e < L.tn * 2; e += 32) pt[e] = make_uint4(0, 0, 0, 0);
-    }
-    uint4* ot = reinterpret_cast<uint4*>(ones_tile);
-    for (int e = lane; e < 256; e += 32) {
-      // 16-B chunk e: row group e/16, k-chunk (e/8)%2, row e%8
-      const bool first_chunk = ((e >> 3) & 1) == 0;
-      ot[e] = make_uint4(first_chunk ? (uint32_t)L.one : 0u, 0, 0, 0);
-    }
-    fence_proxy_async_smem();
   }
   if (P.rows_needed) {
     // ragged fetch leaves rows of a stage untouched: start from zeros so that stale rows are always finite
-    // and the virtual row (index TN-1 >= Ld, only ever written by TMA zero fill) is zero
+    // and the virtual row (index >= Ld, only ever written by TMA zero fill) is zero
     for (int s = 0; s < L.stages; ++s) {
       uint4* z = reinterpret_cast<uint4*>(stage_base + (size_t)s * L.stage_bytes);
       for (int e = threadIdx.x; e < L.doc_bytes / 16; e += kThreads) z[e] = make_uint4(0, 0, 0, 0);
     }
     fence_proxy_async_smem();
   }
-  if (warp == 3) tmem_alloc(&S->tmem_base, (uint32_t)L.tmem_cols);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = S->tmem_base;
 
-  if (warp == 2) {
+  if (warp == 0) {
     // ------------------------------- TMA producer -------------------------------
     if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
+      const int ring = L.stages >> 1;
+      int64_t seq0 = 0, seq1 = 0;   // tiles filled so far into each warpgroup's half of the ring
       int64_t prev_q = -1;
       uint32_t qcount = 0;
       for (int64_t p = p_begin; p < p_end; ++p) {
@@ -163,16 +142,19 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
         if (qi != prev_q) {
           const uint32_t slot = qcount & 1u, use = qcount >> 1;
           mbar_wait(&S->qempty[slot], (use & 1u) ^ 1u);
-          mbar_arrive_expect_tx(&S->qfull[slot], (uint32_t)(L.kblocks * kQRep * kQRows * 128));
+          mbar_arrive_expect_tx(&S->qfull[slot], (uint32_t)(L.kblocks * kQBlockBytes));
           for (int kb = 0; kb < L.kblocks; ++kb)
-            for (int r = 0; r < kQRep; ++r)
-              tma_load_4d(&tmap_q, q_base + (size_t)slot * qslot_bytes + kb * kQBlockBytes + r * (kQRows * 128),
-                          &S->qfull[slot], 0, 0, kb, (int)qi, kEvictLast);
+            tma_load_4d(&tmap_q, q_base + (size_t)slot * qslot_bytes + kb * kQBlockBytes, &S->qfull[slot], 0, 0, kb, (int)qi,
+                        kEvictLast);
           ++qcount;
           prev_q = qi;
         }
         const int need_rows = P.rows_needed ? P.rows_needed[di] : 0;
+        const int c = (int)((p - p_begin) & 1);
         for (int t = 0; t < L.tiles; ++t) {
+          const int64_t j = c ? seq1++ : seq0++;
+          const int stage = c * ring + (int)(j % ring);
+          const uint32_t phase = (uint32_t)((j / ring) & 1);
           mbar_wait(&S->empty[stage], phase ^ 1u);
           uint8_t* dst = stage_base + (size_t)stage * L.stage_bytes;
           if (!P.rows_needed) {
@@ -180,7 +162,7 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
             tma_load_4d(&tmap_d, dst, &S->full[stage], 0, t * L.tn, 0, (int)di, kEvictFirst);
           } else {
             // 16-row blocks up to the document's last unmasked row; the rest of the stage keeps stale
-            // (finite) rows, which the penalty tile masks with -inf
+            // (finite) rows, which the penalty row masks with -inf
             const int rows_here = min(max(need_rows - t * L.tn, 0), L.tn);
             const int nb = (rows_here + 15) >> 4;
             if (nb == 0) {
@@ -193,58 +175,14 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
                               (int)di, kEvictFirst);
             }
           }
-          if (++stage == L.stages) { stage = 0; phase ^= 1u; }
         }
       }
     }
-  } else if (warp == 3) {
-    // ------------------------------- MMA issuer ---------------------------------
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc((uint32_t)L.fmt, 128, (uint32_t)L.tn);
-      const uint64_t ones_desc = make_noswz_k16_desc(smem_u32(ones_tile));
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t accphase = 0;
-      int64_t prev_q = -1;
-      uint32_t qcount = 0;
-      int cur_slot = 0;
-      for (int64_t p = p_begin; p < p_end; ++p) {
-        const int64_t qi = P.pair_q ? (int64_t)P.pair_q[p] : (p + P.pair_base) / P.docs_per_query;
-        if (qi != prev_q) {
-          if (prev_q >= 0) umma_commit(&S->qempty[cur_slot]);
-          cur_slot = (int)(qcount & 1u);
-          mbar_wait(&S->qfull[cur_slot], (qcount >> 1) & 1u);
-          ++qcount;
-          prev_q = qi;
-        }
-        const uint32_t qaddr = smem_u32(q_base + (size_t)cur_slot * qslot_bytes);
-        for (int t = 0; t < L.tiles; ++t) {
-          mbar_wait(&S->accempty[acc], accphase ^ 1u);
-          mbar_wait(&S->full[stage], phase);
-          tc_fence_after_sync();
-          const uint32_t tmem_d = tmem_base + (uint32_t)(acc * L.tn);
-          const uint32_t daddr = smem_u32(stage_base + (size_t)stage * L.stage_bytes);
-          for (int kb = 0; kb < L.kblocks; ++kb) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-              umma_f16(tmem_d, make_sw128_kmajor_desc(qaddr + kb * kQBlockBytes + k * 32),
-                       make_sw128_kmajor_desc(daddr + kb * L.tn * 128 + k * 32), idesc, (uint32_t)((kb | k) != 0));
-          }
-          // + ones[128 x 16] * penalty[TN x 16]^T : adds penalty[row] to every query's score of that row
-          umma_f16(tmem_d, ones_desc, make_noswz_k16_desc(daddr + L.doc_bytes), idesc, 1u);
-          umma_commit(&S->empty[stage]);
-          umma_commit(&S->accfull[acc]);
-          if (++stage == L.stages) { stage = 0; phase ^= 1u; }
-          if (++acc == L.acc_slots) { acc = 0; accphase ^= 1u; }
-        }
-      }
-    }
-  } else if (warp == 4) {
+  } else if (warp == 1) {
     // ------------------------------- penalty writer -----------------------------
     const int dmt = P.d_mask ? P.mask_dtype : MMB200_MASK_NONE;
-    int stage = 0;
-    uint32_t phase = 0;
+    const int ring = L.stages >> 1;
+    int64_t seq0 = 0, seq1 = 0;
     uint64_t raw[8], raw_next[8];
     auto fetch = [&](int64_t p, int t, uint64_t (&dst)[8]) {
 #pragma unroll
@@ -267,7 +205,7 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
           if (nt == L.tiles) { nt = 0; ++np; }
           fetch(np, nt, raw_next);
         }
-        uint16_t pen[8];
+        float pen[8];
         bool masked_here = false;
 #pragma unroll
         for (int k = 0; k < 8; ++k) {
@@ -275,108 +213,151 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
           const bool in_doc = r < L.tn && g < P.Ld;
           const bool ok = in_doc && mask_test(raw[k], dmt);
           masked_here |= in_doc && !ok;
-          pen[k] = ok ? (uint16_t)0 : L.neg_inf;
+          pen[k] = ok ? 0.f : -INFINITY;
         }
         any_masked |= __any_sync(0xffffffffu, masked_here);
+        const int c = (int)((p - p_begin) & 1);
+        const int64_t j = c ? seq1++ : seq0++;
+        const int stage = c * ring + (int)(j % ring);
+        const uint32_t phase = (uint32_t)((j / ring) & 1);
         mbar_wait(&S->empty[stage], phase ^ 1u);
-        uint8_t* pt = stage_base + (size_t)stage * L.stage_bytes + L.doc_bytes;
+        float* pt = reinterpret_cast<float*>(stage_base + (size_t)stage * L.stage_bytes + L.doc_bytes);
 #pragma unroll
         for (int k = 0; k < 8; ++k) {
           const int r = lane + 32 * k, g = t * L.tn + r;
-          if (r < L.tn) {
-            const uint16_t v = (g == L.tiles * L.tn - 1) ? (any_masked ? L.neg_1000 : L.neg_inf) : pen[k];
-            *reinterpret_cast<uint16_t*>(pt + penalty_offset(r)) = v;
-          }
+          if (r < L.tn) pt[r] = (g == L.tiles * L.tn - 1) ? (any_masked ? -1000.f : -INFINITY) : pen[k];
         }
-        fence_proxy_async_smem();
         __syncwarp();
         if (lane == 0) mbar_arrive(&S->full[stage]);
-        if (++stage == L.stages) { stage = 0; phase ^= 1u; }
       }
     }
-  } else if (warp < 2) {
-    // ------------------------------- epilogue ------------------------------------
+  } else if (warp >= 4) {
+    // ------------------------------- consumers: wgmma + masked max ------------------------
+    const int c = (warp >> 2) - 1;        // consumer warpgroup 0 / 1
+    const int wq = warp & 3;              // warp inside the warpgroup: rows 16 wq .. 16 wq + 15
+    const int r0 = 16 * wq + (lane >> 2), r1 = r0 + 8;   // this thread's query rows (< 32 for wq < 2)
+    const int cq = 2 * (lane & 3);        // this thread's first column inside an 8-column group
     const int qmt = P.q_mask ? P.mask_dtype : MMB200_MASK_NONE;
-    const int n32 = L.tn >> 5, tail16 = (L.tn & 16) != 0;
-    for (int64_t n = warp; p_begin + n < p_end; n += 2) {
+    const int ring = L.stages >> 1;
+    int64_t seq = 0;   // tiles consumed from this warpgroup's half of the ring
+    int64_t prev_q = -1;
+    uint32_t qcount = 0;
+    int cur_slot = 0;
+    for (int64_t n = 0; p_begin + n < p_end; ++n) {
       const int64_t p = p_begin + n;
       const int64_t qi = P.pair_q ? (int64_t)P.pair_q[p] : (p + P.pair_base) / P.docs_per_query;
-      uint64_t qraw = 0;
-      if (lane < P.Lq) qraw = (qmt != MMB200_MASK_NONE) ? mask_raw(P.q_mask, qmt, qi * (int64_t)P.Lq + lane) : 1;
-      float m = -INFINITY;
-      int am = -1;   // row of the running maximum (first one on ties); stays -1 when nothing beats -inf
+      if (qi != prev_q) {
+        // every MMA of this warpgroup that read the old query tile has completed (wgmma_wait below)
+        if (prev_q >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&S->qempty[cur_slot]); }
+        cur_slot = (int)(qcount & 1u);
+        mbar_wait(&S->qfull[cur_slot], (qcount >> 1) & 1u);
+        ++qcount;
+        prev_q = qi;
+      }
+      if ((int)(n & 1) != c) continue;
+      const uint32_t qaddr = smem_u32(q_base + (size_t)cur_slot * qslot_bytes);
+      uint64_t qraw0 = 0, qraw1 = 0;
+      if (wq < 2) {
+        if (r0 < P.Lq) qraw0 = (qmt != MMB200_MASK_NONE) ? mask_raw(P.q_mask, qmt, qi * (int64_t)P.Lq + r0) : 1;
+        if (r1 < P.Lq) qraw1 = (qmt != MMB200_MASK_NONE) ? mask_raw(P.q_mask, qmt, qi * (int64_t)P.Lq + r1) : 1;
+      }
+      float m0 = -INFINITY, m1 = -INFINITY;
+      int a0 = -1, a1 = -1;   // row of the running maximum (first one on ties); stays -1 when nothing beats -inf
       for (int t = 0; t < L.tiles; ++t) {
-        const int64_t u = n * L.tiles + t;  // tile sequence number inside this CTA
-        const int acc = (int)(u % L.acc_slots);
-        const uint32_t accphase = (uint32_t)((u / L.acc_slots) & 1);
-        mbar_wait(&S->accfull[acc], accphase);
-        tc_fence_after_sync();
-        const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(acc * L.tn);
-        for (int c = 0; c < n32; ++c) {
-          uint32_t r[32];
-          tmem_ld_32x32b_x32(taddr + c * 32, r);
-          tmem_ld_wait();
-          if constexpr (kArgmax) {
-            const int col0 = t * L.tn + c * 32;
+        const int stage = c * ring + (int)(seq % ring);
+        mbar_wait(&S->full[stage], (uint32_t)((seq / ring) & 1));
+        ++seq;
+        const uint32_t daddr = smem_u32(stage_base + (size_t)stage * L.stage_bytes);
+        float acc[NCH][32];   // the first K-step overwrites (scale-d = 0): no zeroing inside the wgmma pipeline
+        wgmma_fence();
+        for (int kb = 0; kb < L.kblocks; ++kb) {
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const float v = __uint_as_float(r[j]);
-              const bool gt = v > m;
-              m = gt ? v : m;
-              am = gt ? col0 + j : am;
-            }
-            continue;
-          }
-          float a = max3(__uint_as_float(r[0]), __uint_as_float(r[1]), __uint_as_float(r[2]));
-          float b = max3(__uint_as_float(r[3]), __uint_as_float(r[4]), __uint_as_float(r[5]));
+          for (int k = 0; k < 4; ++k) {
+            const uint64_t adesc = make_wgmma_sw128_desc(qaddr + kb * kQBlockBytes + k * 32);
 #pragma unroll
-          for (int j = 6; j + 3 < 32; j += 4) {
-            a = max3(a, __uint_as_float(r[j]), __uint_as_float(r[j + 1]));
-            b = max3(b, __uint_as_float(r[j + 2]), __uint_as_float(r[j + 3]));
-          }
-          m = max3(m, a, b);
-          m = max3(m, __uint_as_float(r[30]), __uint_as_float(r[31]));
-        }
-        if (tail16) {
-          uint32_t r[16];
-          tmem_ld_32x32b_x16(taddr + n32 * 32, r);
-          tmem_ld_wait();
-          if constexpr (kArgmax) {
-            const int col0 = t * L.tn + n32 * 32;
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              const float v = __uint_as_float(r[j]);
-              const bool gt = v > m;
-              m = gt ? v : m;
-              am = gt ? col0 + j : am;
-            }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 16; j += 2) m = max3(m, __uint_as_float(r[j]), __uint_as_float(r[j + 1]));
+            for (int h = 0; h < NCH; ++h)
+              wgmma_n64<T>(acc[h], adesc, make_wgmma_sw128_desc(daddr + kb * L.tn * 128 + h * 64 * 128 + k * 32), (kb | k) != 0);
           }
         }
-        tc_fence_before_sync();
+        wgmma_commit();
+        wgmma_wait<0>();
+#pragma unroll
+        for (int h = 0; h < NCH; ++h) wgmma_fence_regs(acc[h]);
+        if (wq < 2) {
+          const float* pen = reinterpret_cast<const float*>(stage_base + (size_t)stage * L.stage_bytes + L.doc_bytes);
+#pragma unroll
+          for (int h = 0; h < NCH; ++h) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              const int col = h * 64 + 8 * j + cq;
+              const float2 pv = *reinterpret_cast<const float2*>(pen + col);
+              const int gcol = t * L.tn + col;
+              take<kArgmax>(acc[h][4 * j + 0] + pv.x, gcol, m0, a0);
+              take<kArgmax>(acc[h][4 * j + 1] + pv.y, gcol + 1, m0, a0);
+              take<kArgmax>(acc[h][4 * j + 2] + pv.x, gcol, m1, a1);
+              take<kArgmax>(acc[h][4 * j + 3] + pv.y, gcol + 1, m1, a1);
+            }
+          }
+        }
         __syncwarp();
-        if (lane == 0) mbar_arrive(&S->accempty[acc]);
+        if (lane == 0) mbar_arrive(&S->empty[stage]);
       }
-      if constexpr (kArgmax) {
-        // rows >= Ld are the -inf padding and the virtual -1000 row: a max taken there carries no gradient (-1), like a
-        // masked query token
-        if (lane < P.Lq) P.argmax[p * (int64_t)P.Lq + lane] = (mask_test(qraw, qmt) && am < P.Ld) ? am : -1;
-      }
-      float total = mask_test(qraw, qmt) ? m : 0.f;  // lanes >= Lq carry qraw = 0
+      if (wq < 2) {
+        // the four threads of a quad hold the same two rows: combine (larger value, then first column)
 #pragma unroll
-      for (int o = 16; o > 0; o >>= 1) total += __shfl_xor_sync(0xffffffffu, total, o);
-      if (lane == 0) P.out[p] = total;
+        for (int o = 1; o <= 2; o <<= 1) {
+          const float om0 = __shfl_xor_sync(0xffffffffu, m0, o), om1 = __shfl_xor_sync(0xffffffffu, m1, o);
+          if constexpr (kArgmax) {
+            const int oa0 = __shfl_xor_sync(0xffffffffu, a0, o), oa1 = __shfl_xor_sync(0xffffffffu, a1, o);
+            if (om0 > m0 || (om0 == m0 && (unsigned)oa0 < (unsigned)a0)) { m0 = om0; a0 = oa0; }
+            if (om1 > m1 || (om1 == m1 && (unsigned)oa1 < (unsigned)a1)) { m1 = om1; a1 = oa1; }
+          } else {
+            m0 = fmaxf(m0, om0);
+            m1 = fmaxf(m1, om1);
+          }
+        }
+        const bool ok0 = mask_test(qraw0, qmt), ok1 = mask_test(qraw1, qmt);   // qraw = 0 for rows >= Lq
+        if constexpr (kArgmax) {
+          // rows >= Ld are the -inf padding and the virtual -1000 row: a max taken there carries no gradient (-1), like a
+          // masked query token
+          if ((lane & 3) == 0) {
+            if (r0 < P.Lq) P.argmax[p * (int64_t)P.Lq + r0] = (ok0 && a0 < P.Ld) ? a0 : -1;
+            if (r1 < P.Lq) P.argmax[p * (int64_t)P.Lq + r1] = (ok1 && a1 < P.Ld) ? a1 : -1;
+          }
+        }
+        float total = (lane & 3) == 0 ? (ok0 ? m0 : 0.f) + (ok1 ? m1 : 0.f) : 0.f;
+#pragma unroll
+        for (int o = 4; o < 32; o <<= 1) total += __shfl_xor_sync(0xffffffffu, total, o);
+        const int buf = (int)((n >> 1) & 1);
+        if (wq == 1 && lane == 0) S->part[c][buf] = total;
+        named_bar_sync(1 + c, 64);
+        if (wq == 0 && lane == 0) P.out[p] = total + S->part[c][buf];
+      }
     }
   }
+}
 
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 3) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, (uint32_t)L.tmem_cols);
+template <typename T, bool kArgmax>
+int launch_qm(int nch, int grid, size_t smem_bytes, cudaStream_t stream, const CUtensorMap& tq, const CUtensorMap& td,
+              const CUtensorMap& td16, const MaxsimParams& P, const QmLaunch& L) {
+#define MMB_QM_CASE(N)                                                                                                  \
+  case N:                                                                                                               \
+    MMB_CHECK_CUDA(cudaFuncSetAttribute(maxsim_qm_kernel<T, N, kArgmax>, cudaFuncAttributeMaxDynamicSharedMemorySize,   \
+                                        (int)smem_bytes));                                                              \
+    maxsim_qm_kernel<T, N, kArgmax><<<grid, kThreads, smem_bytes, stream>>>(tq, td, td16, P, L);                        \
+    break;
+  switch (nch) {
+    MMB_QM_CASE(1)
+    MMB_QM_CASE(2)
+    MMB_QM_CASE(3)
+    MMB_QM_CASE(4)
+    default:
+      set_error("maxsim queries-on-M: tile width out of range");
+      return MMB200_ERR_INVALID;
   }
+#undef MMB_QM_CASE
+  MMB_CHECK_CUDA(cudaGetLastError());
+  return MMB200_OK;
 }
 
 }  // namespace
@@ -416,18 +397,12 @@ int maxsim_qm_launch(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cu
   L.kblocks = P.dim / 64;
   const int rows = P.Ld + 1;  // + the virtual row that carries the reference's -1000 fill
   L.tiles = (rows + 255) / 256;
-  L.tn = (((rows + L.tiles - 1) / L.tiles) + 15) / 16 * 16;
+  L.tn = (((rows + L.tiles - 1) / L.tiles) + 63) / 64 * 64;
   L.doc_bytes = L.kblocks * L.tn * 128;
-  L.stage_bytes = L.doc_bytes + L.tn * 32;
-  L.acc_slots = std::min(kMaxAcc, 512 / L.tn);
-  L.tmem_cols = 32;
-  while (L.tmem_cols < L.acc_slots * L.tn) L.tmem_cols <<= 1;
-  L.fmt = dtype == MMB200_F16 ? kFmtF16 : kFmtBF16;
-  if (dtype == MMB200_F16) { L.neg_inf = 0xFC00; L.neg_1000 = 0xE3D0; L.one = 0x3C00; }
-  else { L.neg_inf = 0xFF80; L.neg_1000 = 0xC47A; L.one = 0x3F80; }
-  const int fixed = kQSlots * L.kblocks * kQBlockBytes + 4096 + (int)sizeof(QmShared) + 1024;
-  L.stages = std::min(kMaxStages, (dev.max_smem_optin - fixed) / L.stage_bytes);
-  if (L.stages < 2 || L.acc_slots < 2) return MMB200_OK;
+  L.stage_bytes = L.doc_bytes + (L.tn * 4 + 1023) / 1024 * 1024;
+  const int fixed = kQSlots * L.kblocks * kQBlockBytes + (int)sizeof(QmShared) + 1024;
+  L.stages = std::min(kMaxStages, (dev.max_smem_optin - fixed) / L.stage_bytes) & ~1;
+  if (L.stages < 2) return MMB200_OK;
   const size_t smem_bytes = (size_t)L.stages * L.stage_bytes + fixed;
 
   const CUtensorMapDataType tdt = dtype == MMB200_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
@@ -459,15 +434,12 @@ int maxsim_qm_launch(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cu
   }
   *handled = true;
   const int grid = (int)std::min<int64_t>(dev.sm_count, P.n_pairs);
-  if (P.argmax) {
-    MMB_CHECK_CUDA(cudaFuncSetAttribute(maxsim_qm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
-    maxsim_qm_kernel<true><<<grid, kThreads, smem_bytes, stream>>>(tq, td, td16, P, L);
-  } else {
-    MMB_CHECK_CUDA(cudaFuncSetAttribute(maxsim_qm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
-    maxsim_qm_kernel<false><<<grid, kThreads, smem_bytes, stream>>>(tq, td, td16, P, L);
-  }
-  MMB_CHECK_CUDA(cudaGetLastError());
-  return MMB200_OK;
+  const int nch = L.tn / 64;
+  if (dtype == MMB200_F16)
+    return P.argmax ? launch_qm<__half, true>(nch, grid, smem_bytes, stream, tq, td, td16, P, L)
+                    : launch_qm<__half, false>(nch, grid, smem_bytes, stream, tq, td, td16, P, L);
+  return P.argmax ? launch_qm<__nv_bfloat16, true>(nch, grid, smem_bytes, stream, tq, td, td16, P, L)
+                  : launch_qm<__nv_bfloat16, false>(nch, grid, smem_bytes, stream, tq, td, td16, P, L);
 }
 
 }  // namespace mmb

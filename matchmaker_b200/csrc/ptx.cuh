@@ -1,7 +1,7 @@
-// Thin inline-PTX wrappers for the sm_100a features the interaction kernels use:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld), proxies.
-// Hand-written for this project; bit layouts follow the PTX ISA 8.7 descriptions of the
-// tcgen05 shared-memory matrix descriptor and instruction descriptor.
+// Thin inline-PTX wrappers for the sm_90a features the interaction kernels use:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA from shared-memory descriptors), proxies,
+// clusters.  Hand-written for this project; bit layouts follow the PTX ISA descriptions of the wgmma
+// shared-memory matrix descriptor and of the wgmma accumulator fragments.
 #pragma once
 
 #include <cuda.h>
@@ -47,19 +47,16 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
                : "memory");
 }
 
-// Two flavours of the blocking wait, selected per kernel (template argument of mbar_wait):
-//   * polling (default): try_wait returns at once when the phase is still open; the loop re-issues it and checks a clock
-//     watchdog.  Lowest wake-up latency -- right for pipelines whose stages hand over every few hundred cycles and whose
-//     waiting roles have issue slots to spare (max-sim, kernel pooling, flat-IP: same-box A/B, profiles/r02_ab_*.log).
-//   * napping (kNap = true): try_wait carries a suspend-time hint, the hardware parks the warp (ptxas: NANOSLEEP.SYNCS)
-//     until the phase completes or something wakes it, and the watchdog counts wake-ups (3 instructions per turn instead
-//     of 6).  Right when the waiting roles share their schedulers with an issue-bound role: in tkl_ts_kernel the convert
-//     warps, waiting on the epilogue-bound pipeline, executed 30 % of all warp instructions as polling loops.
-// Either way a protocol bug ends in a trap (the launch fails with an error the host reports) instead of a hung GPU.
+// Blocking wait: try_wait returns at once when the phase is still open; the loop re-issues it and checks a clock
+// watchdog, so a protocol bug ends in a trap (the launch fails with an error the host reports) instead of a hung GPU.
+// No printf in the product build: any function call in a kernel makes ptxas serialise its wgmma pipeline (and spill
+// around the call).  Debugging builds (-DMMB200_ENABLE_PROF) print which barrier timed out.
+//
+// Parity waits are unambiguous only while the barrier is at most one phase behind the phase waited for: every barrier
+// here has waiters that pass through all of its phases in order.
 #ifndef MMB_WATCHDOG_CYCLES
-#define MMB_WATCHDOG_CYCLES (4000000000ll)  // ~2 s at 1.9 GHz
+#define MMB_WATCHDOG_CYCLES (4000000000ll)  // ~2 s at 1.98 GHz
 #endif
-constexpr uint32_t kMbarSuspendHintNs = 50000u;  // 50 us: upper bound of one nap
 
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
@@ -73,41 +70,17 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   return ok != 0;
 }
 
-__device__ __forceinline__ bool mbar_try_wait_nap(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity), "r"(kMbarSuspendHintNs)
-      : "memory");
-  return ok != 0;
-}
-
-template <bool kNap = false>
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  if constexpr (kNap) {
-    if (mbar_try_wait_nap(bar, parity)) return;
-    uint32_t spins = 0;   // 2^18 futile wake-ups: 13 s of naps in a true deadlock, milliseconds of back-to-back wake-ups
-    while (!mbar_try_wait_nap(bar, parity)) {
-      if (++spins > (1u << 18)) {
-        printf("mmb200: mbarrier watchdog (block %d thread %d bar %u parity %u)\n", (int)blockIdx.x, (int)threadIdx.x,
-               smem_u32(bar), parity);
-        __trap();
-      }
+  if (mbar_try_wait(bar, parity)) return;
+  const long long t0 = clock64();
+  while (!mbar_try_wait(bar, parity))
+    if (clock64() - t0 > MMB_WATCHDOG_CYCLES) {
+#ifdef MMB200_ENABLE_PROF
+      printf("mmb200: mbarrier watchdog (block %d thread %d bar %u parity %u)\n", (int)blockIdx.x, (int)threadIdx.x,
+             smem_u32(bar), parity);
+#endif
+      __trap();
     }
-  } else {
-    if (mbar_try_wait(bar, parity)) return;
-    const long long t0 = clock64();
-    while (!mbar_try_wait(bar, parity)) {
-      if (clock64() - t0 > MMB_WATCHDOG_CYCLES) {
-        printf("mmb200: mbarrier watchdog (block %d thread %d bar %u parity %u)\n", (int)blockIdx.x, (int)threadIdx.x,
-               smem_u32(bar), parity);
-        __trap();
-      }
-    }
-  }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -152,196 +125,84 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, void* smem_d
       : "memory");
 }
 
-// shared memory -> global through a tensor map (bulk async-group completion).  The generic-proxy writes that
-// filled the box must be ordered before it with fence.proxy.async + a barrier.
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, const void* smem_src, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
-               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
-}
-__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-// at most kPending of this thread's bulk groups still READ their shared-memory source afterwards
-template <int kPending>
-__device__ __forceinline__ void bulk_wait_group_read() {
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(kPending) : "memory");
-}
-template <int kPending>
-__device__ __forceinline__ void bulk_wait_group() {
-  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(kPending) : "memory");
-}
-
 // ---------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation
+// wgmma (sm_90a): D[64 x N] (+)= A[64 x K] * B[N x K]^T, issued by all 128 threads of a warpgroup (4 consecutive
+// warps starting at a multiple of 4), accumulator in registers.  Fragment of thread (warp w of the warpgroup, lane l),
+// for every 8-column group j:  d[4j + 0..1] = row 16w + l/4,     columns 8j + 2(l%4) + 0..1
+//                              d[4j + 2..3] = row 16w + l/4 + 8, same columns
 // ---------------------------------------------------------------------------------------------
-// Whole warp, converged.  ncols: power of two in [32, 512].
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-__device__ __forceinline__ void tc_fence_before_sync() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after_sync() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-
-// ---------------------------------------------------------------------------------------------
-// tcgen05: descriptors
-// ---------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor for a K-major operand stored as rows of exactly 128 bytes
-// (64 x 16-bit or 32 x 32-bit elements along K) written by TMA with CU_TENSOR_MAP_SWIZZLE_128B:
+// Shared-memory matrix descriptor for a K-major operand stored as rows of exactly 128 bytes (64 x 16-bit or 32 x 32-bit
+// elements along K) written by TMA with CU_TENSOR_MAP_SWIZZLE_128B:
 //   bits [0,14)  start address >> 4
 //   bits [16,30) leading-dimension byte offset >> 4 (unused for swizzled K-major; canonical value 1)
 //   bits [32,46) stride-dimension byte offset >> 4 = 1024 B: distance between 8-row groups
-//   bits [46,48) descriptor version = 1 on sm_100
 //   bits [49,52) base offset = 0 (tiles are 1024-B aligned)
-//   bits [61,64) layout type: 2 = SWIZZLE_128B
-__device__ __forceinline__ uint64_t make_sw128_kmajor_desc(uint32_t smem_addr) {
+//   bits [62,64) layout type: 1 = SWIZZLE_128B
+// A K-step inside the 128-byte row advances the start address (32 bytes per k16 of 16-bit data).
+__device__ __forceinline__ uint64_t make_wgmma_sw128_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>(1) << 16;
   d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
 
-// MN-major fp32 / tf32 operand (the contraction index K runs over the ROWS of the stored tile, the M / N index is
-// contiguous): what a TMA box [K rows][32 fp32] is when the MMA reduces over its rows.  For 32-bit elements the tensor
-// core accepts exactly one shared-memory layout here, "128-byte swizzle with 32-byte atomicity" (descriptor layout type
-// 1; the TMA side is CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B): rows of 128 bytes whose four 32-byte units are XORed with
-// (row & 3).  Canonical form: atom = 4 K-rows x 128 bytes; the next 32 M/N elements sit lbo_bytes further (the next
-// box), the next 4 K-rows sbo_bytes = 512 further.  A kind::tf32 instruction (K = 8) consumes two 4-row groups: the
-// K-step advances the start address by 1024 bytes.  (With the ordinary 16-byte-atom SWIZZLE_128B the instruction
-// executes and writes zeros.)
-__device__ __forceinline__ uint64_t make_sw128x32_mnmajor_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes = 512) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(1) << 61;
-  return d;
-}
-// byte offset of 16-byte chunk `chunk` (0..7) of row `row` inside a [rows][128 B] tile in that layout
-__device__ __forceinline__ uint32_t sw128x32_offset(int row, int chunk) {
-  return (uint32_t)(row * 128 + ((((chunk >> 1) ^ row) & 3) << 5) + ((chunk & 1) << 4));
-}
-constexpr uint32_t kIdescBMajorMN = 1u << 16;   // instruction-descriptor bit: B operand is MN-major
-constexpr uint32_t kIdescAMajorMN = 1u << 15;
-
-enum : uint32_t { kFmtF16 = 0, kFmtBF16 = 1, kFmtTF32 = 2 };
-
-// Instruction descriptor (kind::f16 / kind::tf32), fp32 accumulate, both operands K-major:
-//   [4,6) D format (1 = f32)   [7,10) A format   [10,13) B format   [15] A major (0 = K)
-//   [16] B major (0 = K)       [17,23) N >> 3     [24,29) M >> 4
-__device__ __host__ __forceinline__ uint32_t make_idesc(uint32_t fmt, uint32_t M, uint32_t N) {
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
+// Orders this thread's earlier register / shared-memory accesses before the wgmma that follow (all 128 threads).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// at most kPending committed groups of this warpgroup still in flight afterwards
+template <int kPending>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kPending) : "memory"); }
+// Keeps the compiler from moving reads of an accumulator above the wgmma_wait that completes it.
+template <int N>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// D[tmem] (+)= A[smem] * B[smem]^T, issued by ONE thread.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
+// The wrappers: accumulator operands first ("+f", NR registers), then the A descriptor / A registers, the B descriptor
+// and the scale-d flag (0: D = A * B, else D += A * B), which selects the predicate p.
+#define MMB_ACC4(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3])
+#define MMB_ACC16(i) MMB_ACC4(i), MMB_ACC4(i + 4), MMB_ACC4(i + 8), MMB_ACC4(i + 12)
+#define MMB_REGS16 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+#define MMB_REGS20 MMB_REGS16 ", %16, %17, %18, %19"
+#define MMB_REGS32 MMB_REGS16 ", %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+#define MMB_REGS64                                                                                               \
+  MMB_REGS32 ", %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "                    \
+             "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
 
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
+// 16-bit inputs, both operands from shared-memory descriptors (K-major)
+#define MMB_WGMMA_SS(N, TY, NR, REGS, PI, AI, BI, ...)                                                               \
+  __device__ __forceinline__ void wgmma_m64n##N##k16_##TY(float (&d)[NR], uint64_t adesc, uint64_t bdesc,              \
+                                                          uint32_t accumulate) {                                     \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, " PI ", 0;\n\t"                                                 \
+                 "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32." #TY "." #TY " {" REGS "}, " AI ", " BI              \
+                 ", p, 1, 1, 0, 0;\n\t}"                                                                               \
+                 : __VA_ARGS__                                                                                       \
+                 : "l"(adesc), "l"(bdesc), "r"(accumulate));                                                        \
+  }
+MMB_WGMMA_SS(32, f16, 16, MMB_REGS16, "%18", "%16", "%17", MMB_ACC16(0))
+MMB_WGMMA_SS(32, bf16, 16, MMB_REGS16, "%18", "%16", "%17", MMB_ACC16(0))
+MMB_WGMMA_SS(64, f16, 32, MMB_REGS32, "%34", "%32", "%33", MMB_ACC16(0), MMB_ACC16(16))
+MMB_WGMMA_SS(64, bf16, 32, MMB_REGS32, "%34", "%32", "%33", MMB_ACC16(0), MMB_ACC16(16))
+MMB_WGMMA_SS(128, f16, 64, MMB_REGS64, "%66", "%64", "%65", MMB_ACC16(0), MMB_ACC16(16), MMB_ACC16(32), MMB_ACC16(48))
+MMB_WGMMA_SS(128, bf16, 64, MMB_REGS64, "%66", "%64", "%65", MMB_ACC16(0), MMB_ACC16(16), MMB_ACC16(32), MMB_ACC16(48))
 
-// Same, A operand read from tensor memory (128 lanes = M rows, one 32-bit column per K element), B from shared memory
-__device__ __forceinline__ void umma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// Arrive on an mbarrier when all tcgen05.mma issued so far by this thread have completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// ---------------------------------------------------------------------------------------------
-// tcgen05: TMEM -> registers.  Warp w of a warpgroup may touch lanes [32*(w%4), 32*(w%4)+32).
-// 32x32b.xN: thread t gets N consecutive 32-bit columns of lane (32*(w%4) + t).
-// ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld_32x32b_x8(uint32_t taddr, uint32_t (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld_32x32b_x2(uint32_t taddr, uint32_t (&r)[2]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x2.b32 {%0, %1}, [%2];" : "=r"(r[0]), "=r"(r[1]) : "r"(taddr) : "memory");
-}
-
-// registers -> tensor memory: lane i of the warp writes TMEM lane (base lane + i), 16 consecutive 32-bit columns
-__device__ __forceinline__ void tmem_st_32x32b_x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_st_32x32b_x8(uint32_t taddr, const uint32_t (&r)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-               ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
+// tf32 with the A operand in registers (K = 8): thread (warp w, lane l) supplies
+//   a[0] = A[16w + l/4][l%4], a[1] = A[16w + l/4 + 8][l%4], a[2] = A[16w + l/4][l%4 + 4], a[3] = A[16w + l/4 + 8][l%4 + 4]
+// as tf32 bit patterns; B from a K-major SWIZZLE_128B descriptor (+32 bytes per K-step).
+#define MMB_WGMMA_RS_TF32(N, NR, REGS, A0, PI, BI, ...)                                                             \
+  __device__ __forceinline__ void wgmma_m64n##N##k8_tf32_rs(float (&d)[NR], const uint32_t (&a)[4], uint64_t bdesc,     \
+                                                            uint32_t accumulate) {                                   \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, " PI ", 0;\n\t"                                                 \
+                 "wgmma.mma_async.sync.aligned.m64n" #N "k8.f32.tf32.tf32 {" REGS "}, {" A0 "}, " BI ", p, 1, 1;\n\t}"   \
+                 : __VA_ARGS__                                                                                       \
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));                        \
+  }
+MMB_WGMMA_RS_TF32(64, 32, MMB_REGS32, "%32, %33, %34, %35", "%37", "%36", MMB_ACC16(0), MMB_ACC16(16))
+MMB_WGMMA_RS_TF32(40, 20, MMB_REGS20, "%20, %21, %22, %23", "%25", "%24", MMB_ACC16(0), MMB_ACC4(16))
+MMB_WGMMA_RS_TF32(32, 16, MMB_REGS16, "%16, %17, %18, %19", "%21", "%20", MMB_ACC16(0))
 
 // fp32 -> tf32, round to nearest (the tensor core itself drops the low 13 bits)
 __device__ __forceinline__ uint32_t f32_to_tf32_rna(float x) {
@@ -350,12 +211,9 @@ __device__ __forceinline__ uint32_t f32_to_tf32_rna(float x) {
   return r;
 }
 
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
 // Re-deal the CTA's registers between warpgroups (4 consecutive warps, all of which must execute the instruction):
-// light roles shrink, the register-hungry role grows.  The sum over the CTA must fit the 64 K register file.
+// light roles shrink, the register-hungry role grows.  The sum over the CTA must fit the registers the CTA was
+// launched with.
 template <int kRegs>
 __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs)); }
 template <int kRegs>
@@ -369,7 +227,7 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
   return r;
 }
-// all threads of all CTAs of the cluster (release / acquire: mbarrier inits and TMEM allocations are visible after it)
+// all threads of all CTAs of the cluster (release / acquire: mbarrier inits are visible after it)
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
@@ -384,17 +242,18 @@ __device__ __forceinline__ void tma_load_2d_multicast(const CUtensorMap* map, vo
       "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask), "l"(cache_hint)
       : "memory");
 }
-// tcgen05.commit whose arrival is delivered to the mbarrier at this offset in every CTA of `cta_mask`
-__device__ __forceinline__ void umma_commit_multicast(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"(cta_mask)
-               : "memory");
+// Arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster (release at cluster scope).
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}"
+      ::"r"(smem_u32(bar)), "r"(cta)
+      : "memory");
 }
-
-// One lane of a CONVERGED warp.  tcgen05.mma / commit / TMA take their operands from uniform registers: issue them
+// One lane of a CONVERGED warp.  TMA instructions take their operands from uniform registers: issue them
 // as `if (elect_one_sync()) { ... }` from warp-uniform control flow with operands computed OUTSIDE the branch, so the
 // compiler keeps them uniform.  Inside an `if (lane == 0)` region it cannot prove uniformity and wraps every
-// instruction in an ELECT / R2UR.BROADCAST / BRA.U.ANY waterfall loop (~11 extra instructions per MMA).
+// instruction in an ELECT / R2UR.BROADCAST / BRA.U.ANY waterfall loop.
 __device__ __forceinline__ bool elect_one_sync() {
   uint32_t pred;
   asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));

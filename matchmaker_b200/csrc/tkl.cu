@@ -153,7 +153,7 @@ __global__ void __launch_bounds__(kThreads) tkl_window_kernel(TklParams P, long 
   float* pk = sp + 16;                              // [20][KB] per-kernel sums over query rows
   float* T = pk + 20 * KB;                          // [20 windows][40][KB] saturated activations
   const int t = threadIdx.x;
-  if (P.plan && P.plan[0] == 1) return;  // the tcgen05 kernel (tkl_ts.cu) took this call
+  if (P.plan && P.plan[0] == 1) return;  // the tensor-core kernel (tkl_ts.cu) took this call
 
   if (t < KB) {
     const bool ok = t < K;
@@ -421,8 +421,8 @@ extern "C" int mmb200_tkl_window_scores(const float* q, const void* q_mask, cons
   if (B == 0) return MMB200_OK;
   DeviceInfo dev;
   if (int rc = current_device_info(&dev)) return rc;
-  if (!is_sm100(dev)) {
-    set_error("matchmaker_b200 kernels are built for sm_100a only");
+  if (!is_sm90(dev)) {
+    set_error("matchmaker_b200 kernels are built for sm_90a only");
     return MMB200_ERR_UNSUPPORTED;
   }
   TklParams P{};
@@ -452,7 +452,7 @@ extern "C" int mmb200_tkl_window_scores(const float* q, const void* q_mask, cons
     bool handled = false;
     if (int rc = tkl_window_ts_launch(P, dev, stream, &handled, &plan)) return rc;
     if (impl == MMB200_IMPL_TCGEN05 && !handled) {
-      set_error("tkl_window_scores: shape outside the tcgen05 kernel's envelope (Lq <= 40, K <= 16, Lq * K <= 512)");
+      set_error("tkl_window_scores: shape outside the tensor-core kernel's envelope (Lq <= 40, K <= 16, Lq * K <= 512)");
       return MMB200_ERR_UNSUPPORTED;
     }
     if (handled && (impl == MMB200_IMPL_TCGEN05 || !ffma_fits)) {
@@ -501,8 +501,8 @@ extern "C" int mmb200_tkl_top_hills(const float* window_score, float* orig_score
   if (B == 0) return MMB200_OK;
   DeviceInfo dev;
   if (int rc = current_device_info(&dev)) return rc;
-  if (!is_sm100(dev)) {
-    set_error("matchmaker_b200 kernels are built for sm_100a only");
+  if (!is_sm90(dev)) {
+    set_error("matchmaker_b200 kernels are built for sm_90a only");
     return MMB200_ERR_UNSUPPORTED;
   }
   const size_t smem = (size_t)2 * W * sizeof(float);

@@ -1,5 +1,5 @@
 // Parameter block shared by the TKL window-score kernels (tkl.cu: FFMA kernel, any activation pattern;
-// tkl_ts.cu: TMA + tcgen05 kernel for kernel sets whose activations cover the whole cosine range).
+// tkl_ts.cu: TMA + wgmma kernel for kernel sets whose activations cover the whole cosine range).
 #pragma once
 
 #include <cuda_runtime.h>

@@ -369,8 +369,8 @@ extern "C" int mmb200_tkl_bwd(const float* q, const void* q_mask, const float* c
   MMB_REQUIRE(saturation == 1 || sat_red_w != nullptr, "embedding saturation needs sat_emb_reduce1 weights");
   DeviceInfo dev;
   if (int rc = current_device_info(&dev)) return rc;
-  if (!is_sm100(dev)) {
-    set_error("matchmaker_b200 kernels are built for sm_100a only");
+  if (!is_sm90(dev)) {
+    set_error("matchmaker_b200 kernels are built for sm_90a only");
     return MMB200_ERR_UNSUPPORTED;
   }
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);

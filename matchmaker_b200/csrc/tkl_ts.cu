@@ -1,4 +1,4 @@
-// TKL (SIGIR'20) window scores on TMA + tcgen05: the cosine of every (query row, document position) pair comes from
+// TKL (SIGIR'20) window scores on TMA + wgmma: the cosine of every (query row, document position) pair comes from
 // the tensor cores with fp32-grade accuracy, the RBF activations, the sliding-window sums, the learned saturation
 // and the dense layer are fused behind it; only [B, W] window scores are written.
 //
@@ -16,18 +16,17 @@
 // starts inside a document first replays the previous tile's last block -- its "halo" -- to rebuild the suffix sums).
 // Windows outside every share are exactly 0 and come from one cudaMemsetAsync.
 //
-// Per CTA (768 threads = 6 warpgroups, registers re-dealt with setmaxnreg), same operand pipeline as
-// kernel_pool_ts.cu (x = hi + lo with hi = x & 0xffffe000; [Qhi;Qlo] stacked along the UMMA N dimension, the
-// document operand written to TENSOR MEMORY by the convert warps):
+// Per CTA (768 threads = 6 warpgroups, registers re-dealt with setmaxnreg), same operand scheme as kernel_pool_ts.cu
+// (x = hi + lo with hi = x & 0xffffe000, the document operand split in registers):
 //   warp 0      TMA producer: per 32-column k-chunk up to three [40 x 32] chunk boxes + one [40 x 32] query box
-//   warp 1      tcgen05.mma kind::tf32, M = 128 (120 used), N = 80 = [40 hi | 40 lo], A from TMEM, 3 accumulators
-//   warps 2-3   query convert (hi / lo B operand, query norms)
-//   warps 4-7   document convert, one thread per position (hi / lo straight into TMEM, position norms)
-//   warps 8-23  epilogue.  Phase A: thread = position, 10 query columns per warp: cosine tile to shared memory (masked
-//               positions -> a sentinel whose activations are exactly 0).  Phase B: thread = (query row i, kernel k),
-//               walks the tile's 60 pairs in registers: activation pair sums, block prefix / suffix, window sum,
-//               saturation (per-document table indexed by the window's token count), w_k * T; a 16-value transposed
-//               butterfly per block reduces over the warp, 60 threads add the per-warp partials in a fixed order.
+//   warps 2-3   query convert (Qhi / Qlo B operands, query norms)
+//   warps 4-7   MMA warpgroup: A fragments of the tile's 120 positions (two 64-row halves) from the raw tile, hi / lo in
+//               registers, wgmma m64n40k8 tf32 against Qhi and Qlo; then phase A: cosine tile to shared memory (masked
+//               positions -> a sentinel whose activations are exactly 0) and the position flags
+//   warps 8-23  epilogue, thread = (query row i, kernel k): walks the tile's 60 pairs in registers: activation pair sums,
+//               block prefix / suffix, window sum, saturation (per-document table indexed by the window's token count),
+//               w_k * T; a 16-value transposed butterfly per block reduces over the warp, 60 threads add the per-warp
+//               partials in a fixed order.  Two cosine tiles travel between phase A and the epilogue through mbarriers.
 //
 // The window "length" of sigir20_tkl.py:210 counts positions whose K activations do not all vanish.  When every
 // cosine in [-1, 1] activates at least one kernel (checked on the device by the plan kernel: true for every kernel
@@ -52,23 +51,21 @@ constexpr int kTileSlots = 3, kTileRows = kTileSlots * kChunk;   // 120 position
 constexpr int kTilePairs = kTileRows / 2;                       // 60
 constexpr int kBlk = 15, kBlocks = kTilePairs / kBlk;           // 4 blocks of 15 pairs
 constexpr int kMaxLq = 40;
-constexpr int kNq = 2 * kMaxLq;           // UMMA N: hi columns 0..39, lo columns 40..79
 constexpr int kMaxRaw = 6;
 constexpr int kOps = 4;
-constexpr int kAcc = 3;
-constexpr int kNormRing = kAcc + kOps + 1;
-constexpr int kAccCol0 = kOps * 64;       // TMEM: [0, 256) A ring (4 x (32 hi + 32 lo)), [256, 496) 3 accumulators of 80
+constexpr int kNormRing = kOps + 2;
 constexpr int kDxBytes = 128 * 128;       // [128 rows][32 fp32], rows 0..119 written
 constexpr int kSlotBytes = kChunk * 128;  // one chunk's 40 rows of a k-chunk
 constexpr int kQxBytes = kMaxLq * 128;
 constexpr int kRawBytes = kDxBytes + kQxBytes;   // 21 KB
-constexpr int kQopBytes = kNq * 128;      // B operand: rows 0-39 Q hi, rows 40-79 Q lo
+constexpr int kQopBytes = 2 * kMaxLq * 128;  // B operands: rows 0-39 Q hi, rows 40-79 Q lo
 constexpr int kEpiWarps = 16, kEpiThreads = kEpiWarps * 32;
 constexpr int kFirstDocWarp = 4, kFirstEpiWarp = 8;
-constexpr int kReleaseArrivals = 4 + 64;   // lane 0 of each document convert warp + every lane of the two query warps
+constexpr int kReleaseArrivals = 4 + 64;   // lane 0 of each MMA warp + every lane of the two query warps
 // The re-deal must fit the registers the CTA was LAUNCHED with (768 threads x 80 = 61 440), not the SM's 64 K: a
 // setmaxnreg.inc beyond that pool never returns.  Only the light warpgroup gives registers back; the others keep 80.
-constexpr int kRegsLight = 56;   // convert and epilogue warps keep the 80 registers of the launch
+constexpr int kRegsLight = 56, kRegsMma = 104;   // the MMA warpgroup takes what the light one gives back; epilogue keeps 80
+constexpr int kDmRing = 512;     // position flags of the last tiles (a window reaches 29 positions into the previous tile)
 constexpr int kCsStride = 122;            // floats per QUERY ROW of the cosine tile cs[i][position]: even (8-byte pair loads), 122 mod 32 = 26
                                           // puts the 3-4 query rows a warp reads at once on distinct bank pairs
 constexpr int kSatStride = 33;            // table row stride (token counts 0..30)
@@ -81,21 +78,17 @@ struct TsShared {
   uint64_t raw_empty[kMaxRaw];
   uint64_t op_full[kOps];
   uint64_t op_empty[kOps];
-  uint64_t accfull[kAcc];
-  uint64_t accempty[kAcc];
-  uint32_t tmem_base;
-  uint32_t pad;
-  // norms travel from the convert warps to the epilogue in their own ring: the convert warps run up to kOps k-chunks
-  // ahead of the MMA warp, which runs up to kAcc tiles ahead of the epilogue -- with a single k-chunk per tile
-  // (D <= 32) that is kAcc + kOps tiles, so a ring indexed by the accumulator slot would be overwritten early
-  float ss_d[kNormRing][128];
+  uint64_t cs_full[2];        // phase A (MMA warps) -> epilogue: cosine tile and position flags written
+  uint64_t cs_empty[2];       // epilogue -> phase A: every epilogue warp is done with the cosine tile
+  // query norms travel from the convert warps to phase A in their own ring: the convert warps run up to kOps k-chunks
+  // ahead of the MMA warps -- kOps tiles when a tile is a single k-chunk (D <= 32)
   float rs_q[kNormRing][kMaxLq];
   float red[kMaxLq];          // sat_emb_reduce1(q_i)
   float qm[kMaxLq];
   float sp[16];
   alignas(16) uint16_t lenw[kBlocks][16]; // 16 x token count of the window ending at each pair of the tile (byte offset into a sat row),
                               // 15 per block in a 32-byte row: two 16-byte loads per block
-  float dmring[256];          // unmasked flag of the document's positions, indexed by position & 255
+  float dmring[kDmRing];      // unmasked flag of the positions, indexed by (tile sequence number * 120 + position) % kDmRing
   float part[kEpiWarps][64];  // per-warp partial window scores
   float4 sat[kMaxLq * kSatStride];   // (sat1 * gate, sat2, sat3 * gate, -) per (query row, token count)
 };
@@ -317,43 +310,16 @@ struct TileWalk {
   }
 };
 
-// MMB200_ENABLE_PROF builds (python -m matchmaker_b200.build --prof) + MMB200_TKL_TS_PROF=1: one thread per role of CTA 0
-// accumulates the cycles it spends in each wait / phase; printed by the launcher.  Compiled out of the product build.
-#ifdef MMB200_ENABLE_PROF
-#define TKL_T(slot, stmt)                    \
-  do {                                       \
-    const long long t0_ = clock64();         \
-    stmt;                                    \
-    pc[slot] += clock64() - t0_;             \
-  } while (0)
-#define TKL_MARK(slot)                       \
-  do {                                       \
-    const long long now_ = clock64();        \
-    pc[slot] += now_ - t_mark;               \
-    t_mark = now_;                           \
-  } while (0)
-#else
-#define TKL_T(slot, stmt) stmt
-#define TKL_MARK(slot) \
-  do {                 \
-  } while (0)
-#endif
-
 template <int SAT>
 __global__ void __launch_bounds__(kThreads, 1)
 tkl_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_c, TklParams P,
-              int n_raw, int fallback_available, long long* prof) {
-#ifdef MMB200_ENABLE_PROF
-  long long pc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  long long t_mark = clock64();
-  const long long t_start = t_mark;
-#endif
+              int n_raw, int fallback_available) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* qring = smem;                                                    // [kOps][Qhi;Qlo]
   uint8_t* raws = smem + kOps * kQopBytes;                                  // [n_raw][Dx | Qx]
-  float* cs = reinterpret_cast<float*>(raws + (size_t)n_raw * kRawBytes);   // [40 query rows][kCsStride] cosine tile
-  TsShared* S = reinterpret_cast<TsShared*>(cs + kMaxLq * kCsStride);
+  float* cs = reinterpret_cast<float*>(raws + (size_t)n_raw * kRawBytes);   // [2][40 query rows][kCsStride] cosine tiles
+  TsShared* S = reinterpret_cast<TsShared*>(cs + 2 * kMaxLq * kCsStride);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nch = (P.D + 31) / 32;
@@ -362,25 +328,20 @@ tkl_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant_
     prefetch_tensormap(&tmap_q);
     prefetch_tensormap(&tmap_c);
     for (int s = 0; s < n_raw; ++s) { mbar_init(&S->raw_full[s], 1); mbar_init(&S->raw_empty[s], kReleaseArrivals); }
-    for (int s = 0; s < kOps; ++s) { mbar_init(&S->op_full[s], kReleaseArrivals); mbar_init(&S->op_empty[s], 1); }
-    for (int s = 0; s < kAcc; ++s) { mbar_init(&S->accfull[s], 1); mbar_init(&S->accempty[s], kEpiWarps); }
+    for (int s = 0; s < kOps; ++s) { mbar_init(&S->op_full[s], 64); mbar_init(&S->op_empty[s], 4); }
+    for (int s = 0; s < 2; ++s) { mbar_init(&S->cs_full[s], 4); mbar_init(&S->cs_empty[s], kEpiWarps); }
     fence_barrier_init();
   }
   if (threadIdx.x < 16) S->sp[threadIdx.x] = (SAT == 0 && threadIdx.x < 13) ? P.sat_params[threadIdx.x] : 0.f;
-  if (warp == 1) tmem_alloc(&S->tmem_base, 512);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = S->tmem_base;
 
   // Programmatic dependent launch: this grid is launched while the plan kernel still runs (it triggers its dependents at
   // its first instruction), so the launch latency and the prologue above overlap with it; everything below reads the plan.
   asm volatile("griddepcontrol.wait;" ::: "memory");
   const bool covered = P.plan[0] == 1;
-  if (!covered && !fallback_available && blockIdx.x == 0 && threadIdx.x == 0) {
-    printf("mmb200 tkl: kernel set does not cover the cosine range and the FFMA kernel cannot run this shape\n");
-    __trap();
-  }
+  // a kernel set without cover on a shape the FFMA kernel cannot run either: fail the launch (no printf here -- a
+  // function call in the kernel would serialise its wgmma pipeline)
+  if (!covered && !fallback_available && blockIdx.x == 0 && threadIdx.x == 0) __trap();
 
   // every role walks the same tile sequence with its own copy of the iterator (set up inside the role branch, after
   // setmaxnreg, so that it lives in that role's registers); without cover nobody has work and the FFMA kernel takes over
@@ -404,7 +365,7 @@ tkl_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant_
         }
         const uint32_t bytes = (uint32_t)(n_present * kSlotBytes + kQxBytes);
         for (int ck = 0; ck < nch; ++ck) {
-          TKL_T(0, mbar_wait<true>(&S->raw_empty[stage], phase ^ 1u));
+          mbar_wait(&S->raw_empty[stage], phase ^ 1u);
           uint8_t* st = raws + (size_t)stage * kRawBytes;
           mbar_arrive_expect_tx(&S->raw_full[stage], bytes);
 #pragma unroll
@@ -416,41 +377,7 @@ tkl_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant_
       }
     }
   } else if (warp == 1) {
-    // ------------------------------- MMA issuer ---------------------------------
     setmaxnreg_dec<kRegsLight>();
-    TKL_WALK();
-    if (have_work) {
-      const uint32_t idesc = make_idesc(kFmtTF32, 128, kNq);
-      int stage = 0, acc = 0;
-      uint32_t phase = 0, accphase = 0;
-      for (; tw.valid(); tw.next()) {
-        TKL_T(0, mbar_wait<true>(&S->accempty[acc], accphase ^ 1u));
-        tc_fence_after_sync();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(kAccCol0 + acc * kNq);
-        for (int ck = 0; ck < nch; ++ck) {
-          const int ksteps = (min(32, P.D - ck * 32) + 7) >> 3;
-          TKL_T(1, mbar_wait<true>(&S->op_full[stage], phase));
-          tc_fence_after_sync();
-          const uint32_t abase = tmem_base + (uint32_t)(stage * 64);
-          const uint64_t b0 = make_sw128_kmajor_desc(smem_u32(qring + (size_t)stage * kQopBytes));
-          if (elect_one_sync()) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              if (k < ksteps) {
-                const uint64_t bq = b0 + (uint64_t)(k * 2);
-                umma_tf32_ts(tmem_d, abase + (uint32_t)(k * 8), bq, idesc, (uint32_t)((ck | k) != 0));
-                umma_tf32_ts(tmem_d, abase + (uint32_t)(32 + k * 8), bq, idesc, 1u);
-              }
-            }
-            umma_commit(&S->op_empty[stage]);
-            if (ck == nch - 1) umma_commit(&S->accfull[acc]);
-          }
-          __syncwarp();
-          if (++stage == kOps) { stage = 0; phase ^= 1u; }
-        }
-        if (++acc == kAcc) { acc = 0; accphase ^= 1u; }
-      }
-    }
   } else if (warp < 4) {
     // ------------------------------- query convert ------------------------------
     // 40 rows x 8 float4 per k-chunk = 320 float4 over 64 threads: thread qt owns 16-byte column c = qt & 7 of rows
@@ -465,7 +392,7 @@ tkl_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant_
       for (; tw.valid(); tw.next()) {
         float ss[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
         for (int ck = 0; ck < nch; ++ck) {
-          TKL_T(0, mbar_wait<true>(&S->raw_full[rs_], rphase));
+          mbar_wait(&S->raw_full[rs_], rphase);
           const uint8_t* xq = raws + (size_t)rs_ * kRawBytes + kDxBytes;
           float4 x[5];
 #pragma unroll
@@ -474,7 +401,7 @@ tkl_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant_
             x[j] = *reinterpret_cast<const float4*>(xq + row * 128 + ((c ^ (row & 7)) << 4));
             ss[j] = fmaf(x[j].x, x[j].x, fmaf(x[j].y, x[j].y, fmaf(x[j].z, x[j].z, fmaf(x[j].w, x[j].w, ss[j]))));
           }
-          TKL_T(1, mbar_wait<true>(&S->op_empty[os_], ophase ^ 1u));
+          mbar_wait(&S->op_empty[os_], ophase ^ 1u);
           uint8_t* qo = qring + (size_t)os_ * kQopBytes;
 #pragma unroll
           for (int j = 0; j < 5; ++j) {
@@ -505,67 +432,113 @@ tkl_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant_
       }
     }
   } else if (warp < kFirstEpiWarp) {
-    // ------------------------------- document convert ---------------------------
-    // one thread per position (TMEM lane): this kernel is bound by the SM's issue slots (ncu: 65 % issue-active, the
-    // MUFU-heavy epilogue next door), not by the latency of the convert chain, so the per-chunk bookkeeping (barrier
-    // waits, address arithmetic, arrivals) is paid by 4 warps instead of 8
+    // ------------------------------- MMA warpgroup: document operand, wgmma, cosine tile (phase A) -------------------
+    // Thread (warp wq, lane) owns positions rb, rb + 8 (M-block 0) and 64 + rb, 72 + rb (M-block 1), rb = 16 wq + lane / 4.
+    // Per 8-column K-step: the four positions' A fragments straight from the raw SWIZZLE_128B tile, split into hi / lo in
+    // registers; D += Dhi Qhi^T + Dhi Qlo^T + Dlo Qhi^T + Dlo Qlo^T, wgmma m64n40k8 tf32 with A from registers.
+    setmaxnreg_inc<kRegsMma>();
     TKL_WALK();
     if (have_work) {
-      const int qd = warp & 3;
-      const int row = qd * 32 + lane;
-      const int sw = row & 7;
-      const uint32_t trow = tmem_base + ((uint32_t)(qd * 32) << 16);
+      const int wq = warp & 3;
+      const int tq = lane & 3;
+      const int rb = 16 * wq + (lane >> 2);
+      const int dmt = P.chunk_mask ? P.mask_dtype : MMB200_MASK_NONE;
       int rs_ = 0, os_ = 0, nr = 0;
       uint32_t rphase = 0, ophase = 0;
-      for (; tw.valid(); tw.next()) {
-        float4 ss4 = make_float4(0.f, 0.f, 0.f, 0.f);
+      int64_t tile_seq = 0;
+      for (; tw.valid(); tw.next(), ++tile_seq) {
+        const int t = tw.t;
+        uint64_t draw[4];
+        bool present[4];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {   // the position's packed chunk, then its mask word: in flight during the MMAs
+          const int row = rb + 8 * (e & 1) + 64 * (e >> 1);
+          const int c = t * kTileSlots + row / kChunk;
+          const int pk = (row < kTileRows && c < P.C) ? P.slot_to_packed[(int64_t)tw.b * P.C + c] : -1;
+          present[e] = pk >= 0;
+          draw[e] = pk < 0 ? 0 : dmt != MMB200_MASK_NONE ? mask_raw(P.chunk_mask, dmt, (int64_t)pk * kChunk + (row % kChunk)) : 1;
+        }
+        float acc0[20], acc1[20];
+#pragma unroll
+        for (int j = 0; j < 20; ++j) { acc0[j] = 0.f; acc1[j] = 0.f; }
+        float ss[4] = {0.f, 0.f, 0.f, 0.f};
         for (int ck = 0; ck < nch; ++ck) {
-          const bool second = P.D - ck * 32 > 16;   // columns 16..31 of this chunk hold data (warp-uniform)
-          TKL_T(0, mbar_wait<true>(&S->raw_full[rs_], rphase));
-          const uint8_t* xrow = raws + (size_t)rs_ * kRawBytes + row * 128;
-          float4 x[4];
+          const int ksteps = (min(32, P.D - ck * 32) + 7) >> 3;   // 8 fp32 per wgmma K-step
+          mbar_wait(&S->raw_full[rs_], rphase);
+          mbar_wait(&S->op_full[os_], ophase);
+          const float* x = reinterpret_cast<const float*>(raws + (size_t)rs_ * kRawBytes);
+          const uint32_t qb = smem_u32(qring + (size_t)os_ * kQopBytes);
+          const uint64_t bhi = make_wgmma_sw128_desc(qb), blo = make_wgmma_sw128_desc(qb + kMaxLq * 128);
 #pragma unroll
-          for (int c = 0; c < 4; ++c) x[c] = *reinterpret_cast<const float4*>(xrow + ((c ^ sw) << 4));
+          for (int k = 0; k < 4; ++k) {
+            if (k < ksteps) {
+              uint32_t ah[2][4], al[2][4];
 #pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            const float4 v = x[c];
-            ss4.x = fmaf(v.x, v.x, ss4.x); ss4.y = fmaf(v.y, v.y, ss4.y); ss4.z = fmaf(v.z, v.z, ss4.z); ss4.w = fmaf(v.w, v.w, ss4.w);
-          }
-          TKL_T(1, mbar_wait<true>(&S->op_empty[os_], ophase ^ 1u));
-          tc_fence_after_sync();
-          const uint32_t taddr = trow + (uint32_t)(os_ * 64);
-          {   // columns 0..15 of the chunk
-            uint32_t hi[16], lo[16];
+              for (int mb = 0; mb < 2; ++mb) {
+                const int ra = 64 * mb + rb, rc = ra + 8;   // rc & 7 == ra & 7
+                const int ch0 = (2 * k) ^ (ra & 7), ch1 = (2 * k + 1) ^ (ra & 7);
+                const float v[4] = {x[ra * 32 + ch0 * 4 + tq], x[rc * 32 + ch0 * 4 + tq], x[ra * 32 + ch1 * 4 + tq], x[rc * 32 + ch1 * 4 + tq]};
 #pragma unroll
-            for (int c = 0; c < 4; ++c) split4(x[c], hi + 4 * c, lo + 4 * c);
-            tmem_st_32x32b_x16(taddr, hi);
-            tmem_st_32x32b_x16(taddr + 32, lo);
-          }
-          if (second) {   // columns 16..31: second pass over the same registers
-#pragma unroll
-            for (int c = 0; c < 4; ++c) x[c] = *reinterpret_cast<const float4*>(xrow + (((4 + c) ^ sw) << 4));
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-              const float4 v = x[c];
-              ss4.x = fmaf(v.x, v.x, ss4.x); ss4.y = fmaf(v.y, v.y, ss4.y); ss4.z = fmaf(v.z, v.z, ss4.z); ss4.w = fmaf(v.w, v.w, ss4.w);
+                for (int e = 0; e < 4; ++e) {
+                  ah[mb][e] = __float_as_uint(v[e]) & 0xffffe000u;
+                  al[mb][e] = __float_as_uint(v[e] - __uint_as_float(ah[mb][e]));
+                }
+                ss[2 * mb] = fmaf(v[0], v[0], fmaf(v[2], v[2], ss[2 * mb]));
+                ss[2 * mb + 1] = fmaf(v[1], v[1], fmaf(v[3], v[3], ss[2 * mb + 1]));
+              }
+              const uint64_t kh = bhi + (uint64_t)(2 * k), kl = blo + (uint64_t)(2 * k);   // +32 bytes along K
+              wgmma_fence();
+              wgmma_m64n40k8_tf32_rs(acc0, ah[0], kh, 1u);
+              wgmma_m64n40k8_tf32_rs(acc0, ah[0], kl, 1u);
+              wgmma_m64n40k8_tf32_rs(acc0, al[0], kh, 1u);
+              wgmma_m64n40k8_tf32_rs(acc0, al[0], kl, 1u);
+              wgmma_m64n40k8_tf32_rs(acc1, ah[1], kh, 1u);
+              wgmma_m64n40k8_tf32_rs(acc1, ah[1], kl, 1u);
+              wgmma_m64n40k8_tf32_rs(acc1, al[1], kh, 1u);
+              wgmma_m64n40k8_tf32_rs(acc1, al[1], kl, 1u);
+              wgmma_commit();
+              wgmma_wait<0>();
             }
-            uint32_t hi[16], lo[16];
-#pragma unroll
-            for (int c = 0; c < 4; ++c) split4(x[c], hi + 4 * c, lo + 4 * c);
-            tmem_st_32x32b_x16(taddr + 16, hi);
-            tmem_st_32x32b_x16(taddr + 48, lo);
           }
-          tmem_st_wait();
-          if (ck == nch - 1) S->ss_d[nr][row] = (ss4.x + ss4.y) + (ss4.z + ss4.w);
-          tc_fence_before_sync();
           __syncwarp();
           if (lane == 0) {
             mbar_arrive(&S->raw_empty[rs_]);
-            mbar_arrive(&S->op_full[os_]);
+            mbar_arrive(&S->op_empty[os_]);
           }
           if (++rs_ == n_raw) { rs_ = 0; rphase ^= 1u; }
           if (++os_ == kOps) { os_ = 0; ophase ^= 1u; }
         }
+        wgmma_fence_regs(acc0);
+        wgmma_fence_regs(acc1);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          ss[e] += __shfl_xor_sync(0xffffffffu, ss[e], 1);
+          ss[e] += __shfl_xor_sync(0xffffffffu, ss[e], 2);
+        }
+        const int buf = (int)(tile_seq & 1);
+        float* cb = cs + buf * (kMaxLq * kCsStride);   // transposed: consecutive positions of one query row are adjacent
+        mbar_wait(&S->cs_empty[buf], (uint32_t)((tile_seq >> 1) & 1) ^ 1u);
+        const float* rq = S->rs_q[nr];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int row = rb + 8 * (e & 1) + 64 * (e >> 1);
+          if (row < kTileRows) {
+            const bool valid = present[e] && mask_test(draw[e], dmt);
+            const float rsd = 1.0f / (sqrtf(ss[e]) + kTinyNorm);
+            const float* a = (e >> 1) ? acc1 : acc0;
+            const int ri = 2 * (e & 1);
+#pragma unroll
+            for (int j = 0; j < 5; ++j)
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const int col = 8 * j + 2 * tq + h;
+                cb[col * kCsStride + row] = valid ? a[4 * j + ri + h] * rsd * rq[col] : kSentinel;
+              }
+            if (tq == 0) S->dmring[(tile_seq * kTileRows + row) & (kDmRing - 1)] = valid ? 1.f : 0.f;
+          }
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&S->cs_full[buf]);
         if (++nr == kNormRing) nr = 0;
       }
     }
@@ -575,10 +548,6 @@ tkl_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant_
     if (have_work) {
       const int ew = warp - kFirstEpiWarp;       // 0..15
       const int et = ew * 32 + lane;             // 0..511
-      const int qd = warp & 3;                   // TMEM lane quarter
-      const int cg = ew >> 2;                    // query columns 10 cg .. 10 cg + 9 in phase A
-      const int row = qd * 32 + lane;            // position inside the tile
-      const int dmt = P.chunk_mask ? P.mask_dtype : MMB200_MASK_NONE;
       const int qmt = P.q_mask ? P.mask_dtype : MMB200_MASK_NONE;
       const int n_ik = P.Lq * P.K;
       const bool ik_live = et < n_ik;
@@ -591,30 +560,16 @@ tkl_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant_
       float suf[kBlk];
 #pragma unroll
       for (int r = 0; r < kBlk; ++r) suf[r] = 0.f;
-      int acc_slot = 0, nr = 0;
-      uint32_t accphase = 0;
-      // This position's mask word needs two dependent global loads (slot map, then mask).  They are issued one and two
-      // tiles ahead -- the packed index of tile n + 2 and, with the index fetched a tile earlier, the mask word of tile
-      // n + 1 -- at the end of phase A, so each has a whole phase B to arrive.
-      auto fetch_slot = [&](int bb, int tt) -> int {
-        if (row >= kTileRows) return -1;
-        const int c = tt * kTileSlots + row / kChunk;
-        return c < P.C ? P.slot_to_packed[(int64_t)bb * P.C + c] : -1;
-      };
-      auto fetch_word = [&](int pk) -> uint64_t {
-        if (pk < 0) return 0;
-        return dmt != MMB200_MASK_NONE ? mask_raw(P.chunk_mask, dmt, (int64_t)pk * kChunk + (row % kChunk)) : 1;
-      };
-      int have_ahead = 0;          // how many of the following tiles have their prefetches in flight (0, 1 or 2)
-      int pk_n1 = -1, pk_n2 = -1;  // packed chunk index of this position in tiles n + 1, n + 2
-      uint64_t draw_n1 = 0;
+      int64_t tile_seq = 0;
       int cur_doc = -1;
       int n_doc_warps = 0;   // epilogue warps holding an unmasked query row of the current document
       float qm_i = 0.f;
 
-      for (; tw.valid(); tw.next()) {
+      for (; tw.valid(); tw.next(), ++tile_seq) {
         const int b = tw.b;
         const int t = tw.t;
+        const int buf = (int)(tile_seq & 1);
+        const float* cb = cs + buf * (kMaxLq * kCsStride);
         if (b != cur_doc) {
           // ---- new document: query mask, sat_emb_reduce1(q_i), saturation table indexed by (query row, token count)
           cur_doc = b;
@@ -673,66 +628,7 @@ tkl_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant_
           n_doc_warps = (q_hi * P.K + 31) >> 5;
         }
 
-        // ---- phase A: accumulator -> cosine tile -------------------------------------------------------------
-        // this position's mask word was fetched while the previous tile was in phase B (two dependent global loads --
-        // slot map, then mask -- that the accumulator wait no longer hides: the producers run ahead of the epilogue)
-        int pk_cur;
-        uint64_t draw;
-        if (have_ahead == 0) {   // first tile of the share: nothing was prefetched
-          pk_cur = fetch_slot(b, t);
-          draw = fetch_word(pk_cur);
-        } else {
-          pk_cur = pk_n1;
-          draw = draw_n1;
-        }
-        const bool present = pk_cur >= 0;
-        TKL_MARK(7);   // bookkeeping between tiles, document switch
-        mbar_wait<true>(&S->accfull[acc_slot], accphase);
-        TKL_MARK(0);   // wait for the accumulator
-        tc_fence_after_sync();
-        {
-          const uint32_t taddr = tmem_base + ((uint32_t)(qd * 32) << 16) + (uint32_t)(kAccCol0 + acc_slot * kNq + 10 * cg);
-          uint32_t h8[8], h2[2], l8[8], l2[2];
-          tmem_ld_32x32b_x8(taddr, h8);
-          tmem_ld_32x32b_x2(taddr + 8, h2);
-          tmem_ld_32x32b_x8(taddr + kMaxLq, l8);
-          tmem_ld_32x32b_x2(taddr + kMaxLq + 8, l2);
-          tmem_ld_wait();
-          tc_fence_before_sync();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&S->accempty[acc_slot]);
-          const bool valid = present && mask_test(draw, dmt);
-          if (row < kTileRows) {
-            const float rsd = 1.0f / (sqrtf(S->ss_d[nr][row]) + kTinyNorm);
-            const float* rq = S->rs_q[nr] + 10 * cg;
-            float v[10];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) v[j] = valid ? (__uint_as_float(h8[j]) + __uint_as_float(l8[j])) * rsd * rq[j] : kSentinel;
-#pragma unroll
-            for (int j = 0; j < 2; ++j) v[8 + j] = valid ? (__uint_as_float(h2[j]) + __uint_as_float(l2[j])) * rsd * rq[8 + j] : kSentinel;
-            float* dst = cs + (10 * cg) * kCsStride + row;   // transposed: consecutive positions of one query row are adjacent
-#pragma unroll
-            for (int j = 0; j < 10; ++j) dst[j * kCsStride] = v[j];
-            if (cg == 0) S->dmring[(t * kTileRows + row) & 255] = valid ? 1.f : 0.f;
-          }
-        }
-        if (++acc_slot == kAcc) { acc_slot = 0; accphase ^= 1u; }
-        if (++nr == kNormRing) nr = 0;
-        {   // prefetches for the next two tiles (see fetch_slot above)
-          TileWalk tn = tw;
-          tn.next();
-          if (!tn.valid()) {
-            have_ahead = 0;
-          } else {
-            pk_n1 = have_ahead == 2 ? pk_n2 : fetch_slot(tn.b, tn.t);
-            draw_n1 = fetch_word(pk_n1);   // waits for pk_n1 only on the first tile of a share
-            tn.next();
-            if (tn.valid()) { pk_n2 = fetch_slot(tn.b, tn.t); have_ahead = 2; } else { have_ahead = 1; }
-          }
-        }
-        TKL_MARK(1);   // phase A
-        named_bar_sync(2, kEpiThreads);
-        TKL_MARK(2);   // barrier 2
+        mbar_wait(&S->cs_full[buf], (uint32_t)((tile_seq >> 1) & 1));   // cosine tile and position flags of the tile
         // ---- token count of the window ending at each pair of this tile (sigir20_tkl.py:210 under "cover") ----
         if (et < 8 * kTilePairs) {   // eight threads per window, four positions each, three shuffle steps
           const int wl = et >> 3, sub = et & 7;
@@ -741,21 +637,19 @@ tkl_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant_
 #pragma unroll
           for (int u = sub; u < kWindow; u += 8) {
             const int pos = last - u;
-            if (pos >= 0) n += S->dmring[pos & 255];
+            if (pos >= 0) n += S->dmring[(tile_seq * kTileRows + 2 * wl + 1 - u) & (kDmRing - 1)];
           }
           n += __shfl_xor_sync(0xffffffffu, n, 1);
           n += __shfl_xor_sync(0xffffffffu, n, 2);
           n += __shfl_xor_sync(0xffffffffu, n, 4);
           if (sub == 0) S->lenw[wl / kBlk][wl % kBlk] = (uint16_t)(16 * (int)n);
         }
-        TKL_MARK(3);   // token counts
         named_bar_sync(3, kEpiThreads);
-        TKL_MARK(2);
         // ---- phase B: activations, block prefix / suffix, windows ------------------------------------------------
         if (ew < n_doc_warps) {
           if (tw.halo) {
             // halo tile: only the suffix sums of its last block are wanted
-            const float2* cblk = reinterpret_cast<const float2*>(cs + qi * kCsStride + 2 * kBlk * (kBlocks - 1));
+            const float2* cblk = reinterpret_cast<const float2*>(cb + qi * kCsStride + 2 * kBlk * (kBlocks - 1));
 #pragma unroll
             for (int r = 0; r < kBlk; ++r) {
               const float2 c = cblk[r];
@@ -771,7 +665,7 @@ tkl_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant_
             for (int j = 0; j < kBlocks; ++j) {
               float tv[16];
               float pre = 0.f;
-              const float2* cblk = reinterpret_cast<const float2*>(cs + qi * kCsStride + 2 * kBlk * j);
+              const float2* cblk = reinterpret_cast<const float2*>(cb + qi * kCsStride + 2 * kBlk * j);
               uint32_t lw[8];   // the block's 15 window token counts: two 16-byte loads instead of 15 scalar ones
               {
                 const uint4 la = *reinterpret_cast<const uint4*>(&S->lenw[j][0]), lb = *reinterpret_cast<const uint4*>(&S->lenw[j][8]);
@@ -832,9 +726,9 @@ tkl_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant_
             }
           }
         }
-        TKL_MARK(4);   // phase B
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&S->cs_empty[buf]);   // this warp is done with the cosine tile
         named_bar_sync(4, kEpiThreads);
-        TKL_MARK(5);   // barrier 4
         if (!tw.halo && et < kTilePairs) {
           const int w = t * kTilePairs - (kBlk - 1) + et;
           if (w >= 0 && w < P.W) {
@@ -851,24 +745,6 @@ tkl_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant_
     }
   }
 
-#ifdef MMB200_ENABLE_PROF
-  if (prof && blockIdx.x == 0 && lane == 0 && (warp == 0 || warp == 1 || warp == 2 || warp == kFirstDocWarp || warp == kFirstEpiWarp)) {
-    const int role = warp == 0 ? 0 : warp == 1 ? 1 : warp == 2 ? 2 : warp == kFirstDocWarp ? 3 : 4;
-    for (int i = 0; i < 8; ++i) prof[role * 9 + i] = pc[i];
-    prof[role * 9 + 8] = clock64() - t_start;
-  }
-  if (prof && lane == 0 && (warp == kFirstEpiWarp || warp == 1)) {   // per CTA: epilogue / MMA role totals, phase B, accumulator wait
-    long long* pq = prof + 45 + (long long)blockIdx.x * 4;
-    if (warp == 1) pq[3] = clock64() - t_start;
-    else { pq[0] = clock64() - t_start; pq[1] = pc[4]; pq[2] = pc[0]; }
-  }
-#endif
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 512);
-  }
 }
 
 #undef TKL_WALK
@@ -880,7 +756,7 @@ int tkl_window_ts_launch(TklParams& P, const DeviceInfo& dev, cudaStream_t strea
   *plan_out = nullptr;
   if (P.Lq > kMaxLq || P.K > 16 || P.Lq * P.K > kEpiThreads || P.D % 4 != 0) return MMB200_OK;
   if (P.B * (int64_t)P.C >= (1ll << 31) || P.B >= (1ll << 31) - 8) return MMB200_OK;
-  const size_t fixed = (size_t)kOps * kQopBytes + (size_t)kMaxLq * kCsStride * sizeof(float) + sizeof(TsShared) + 1024;
+  const size_t fixed = (size_t)kOps * kQopBytes + 2 * (size_t)kMaxLq * kCsStride * sizeof(float) + sizeof(TsShared) + 1024;
   const int n_raw = std::min<int>(kMaxRaw, (int)(((size_t)dev.max_smem_optin - fixed) / kRawBytes));
   if (n_raw < 2) return MMB200_OK;
   const size_t smem = fixed + (size_t)n_raw * kRawBytes;
@@ -918,14 +794,6 @@ int tkl_window_ts_launch(TklParams& P, const DeviceInfo& dev, cudaStream_t strea
   P.plan = plan;
   *plan_out = plan;
   const int fallback = P.segs > 0 ? 1 : 0;
-  long long* prof = nullptr;
-#ifdef MMB200_ENABLE_PROF
-  const bool do_prof = getenv("MMB200_TKL_TS_PROF") != nullptr;
-  if (do_prof) {
-    MMB_CHECK_CUDA(cudaMalloc(&prof, (45 + 4 * 160) * sizeof(long long)));
-    MMB_CHECK_CUDA(cudaMemset(prof, 0, (45 + 4 * 160) * sizeof(long long)));
-  }
-#endif
   auto launch_pdl = [&](auto kernel) -> cudaError_t {
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3((unsigned)grid);
@@ -937,7 +805,7 @@ int tkl_window_ts_launch(TklParams& P, const DeviceInfo& dev, cudaStream_t strea
     attr.val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = &attr;
     cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, kernel, tq, tc, P, n_raw, fallback, prof);
+    return cudaLaunchKernelEx(&cfg, kernel, tq, tc, P, n_raw, fallback);
   };
   static bool attr_set[2][64] = {};
   const int di = dev.device & 63;
@@ -955,32 +823,6 @@ int tkl_window_ts_launch(TklParams& P, const DeviceInfo& dev, cudaStream_t strea
     MMB_CHECK_CUDA(launch_pdl(tkl_ts_kernel<1>));
   }
   MMB_CHECK_CUDA(cudaGetLastError());
-#ifdef MMB200_ENABLE_PROF
-  if (do_prof) {
-    long long h[45 + 4 * 160];
-    MMB_CHECK_CUDA(cudaStreamSynchronize(stream));
-    MMB_CHECK_CUDA(cudaMemcpy(h, prof, sizeof(h), cudaMemcpyDeviceToHost));
-    {
-      long long mx[4] = {0, 0, 0, 0}, sm[4] = {0, 0, 0, 0};
-      int arg = 0;
-      for (int x = 0; x < grid && x < 160; ++x)
-        for (int i = 0; i < 4; ++i) {
-          const long long v = h[45 + 4 * x + i];
-          sm[i] += v;
-          if (v > mx[i]) { mx[i] = v; if (i == 0) arg = x; }
-        }
-      fprintf(stderr, "tkl_ts_prof per CTA (max / mean): epilogue total %lld / %lld (slowest CTA %d: phaseB %lld wait_accfull %lld) | phaseB %lld / %lld | "
-              "wait_accfull %lld / %lld | mma role total %lld / %lld\n", mx[0], sm[0] / grid, arg, h[45 + 4 * arg + 1], h[45 + 4 * arg + 2], mx[1],
-              sm[1] / grid, mx[2], sm[2] / grid, mx[3], sm[3] / grid);
-    }
-    MMB_CHECK_CUDA(cudaFree(prof));
-    fprintf(stderr,
-            "tkl_ts_prof cycles (CTA 0): tma total %lld wait_raw_empty %lld | mma total %lld wait_accempty %lld wait_op_full %lld | qconv total %lld "
-            "wait_raw_full %lld wait_op_empty %lld | dconv total %lld wait_raw_full %lld wait_op_empty %lld | epi total %lld wait_accfull %lld "
-            "phaseA %lld barriers23 %lld counts %lld phaseB %lld barrier4 %lld between %lld\n",
-            h[8], h[0], h[17], h[9], h[10], h[26], h[18], h[19], h[35], h[27], h[28], h[44], h[36], h[37], h[38], h[39], h[40], h[41], h[43]);
-  }
-#endif
   *handled = true;
   return MMB200_OK;
 }

@@ -25,7 +25,7 @@ def _require_cuda(*tensors: Optional[torch.Tensor]) -> torch.device:
             continue
         if not t.is_cuda:
             raise _lib.MatchmakerB200Error(
-                "matchmaker_b200 interaction ops run on CUDA (sm_100a) tensors only; got a "
+                "matchmaker_b200 interaction ops run on CUDA (sm_90a) tensors only; got a "
                 f"{t.device} tensor and there is no CPU fallback")
         if dev is None:
             dev = t.device
@@ -244,7 +244,7 @@ def kernel_pool(q: torch.Tensor, d: torch.Tensor, q_mask: torch.Tensor, d_mask: 
 
 
 def kernel_pool_train_supported(Lq: int, Ld: int, D: int, K: int) -> bool:
-    """True when the tensor-core training pair (forward that saves its cosines + tcgen05 backward) covers the shape."""
+    """True when the tensor-core training pair (forward that saves its cosines + tensor-core backward) covers the shape."""
     return bool(_lib.load().mmb200_kernel_pool_train_tc_supported(int(Lq), int(Ld), int(D), int(K)))
 
 
@@ -366,7 +366,7 @@ def tkl_window_scores(q_ctx: torch.Tensor, q_mask: torch.Tensor, doc_chunks: tor
     out = torch.empty((B, W), dtype=torch.float32, device=dev)
     if impl == "auto":
         # decide on the host (cached per parameter version) so that only ONE of the two kernels is enqueued; the library's
-        # own device-side check stays in force (a forced tcgen05 call on a kernel set without cover writes zeros)
+        # own device-side check stays in force (a forced tensor-core call on a kernel set without cover writes zeros)
         impl = "tcgen05" if (Lq * K <= 512 and K <= 16 and tkl_kernel_set_covers(mu, sigma)) else "simt"
     lib = _lib.load()
     with torch.cuda.device(dev):

@@ -1,6 +1,6 @@
 """Drop-in counterparts of the reference's interaction models (``matchmaker/models``): same class names,
 constructor / ``from_config`` keys, ``forward`` signatures, state-dict keys and secondary-output keys; the
-interaction arithmetic runs in the sm_100a kernels (``libmatchmaker_b200.so``), everything upstream of it
+interaction arithmetic runs in the sm_90a kernels (``libmatchmaker_b200.so``), everything upstream of it
 (embeddings, transformer / BERT encoders) stays ordinary PyTorch exactly as in the reference.
 
     reference                                        here

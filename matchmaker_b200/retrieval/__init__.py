@@ -1,5 +1,5 @@
 """Index API of matchmaker/retrieval (base_index.py:4-32) for the exact inner-product index
-(`faiss_index_type: "full"`, dense_retrieval.py:310-311) on the B200 kernels."""
+(`faiss_index_type: "full"`, dense_retrieval.py:310-311) on the H100 kernels."""
 from .base_index import BaseNNIndexer  # noqa: F401
 from .flat_ip_index import FlatIPIndexer  # noqa: F401
 from .colbert_rerank import ColBERTTokenIndex  # noqa: F401

@@ -1,4 +1,4 @@
-"""Exact (brute-force) maximum-inner-product index with id mapping on the B200 kernels.
+"""Exact (brute-force) maximum-inner-product index with id mapping on the H100 kernels.
 
 Drop-in for ``FaissIdIndexer`` (matchmaker/retrieval/faiss_indices.py:49-74) as driven by
 dense_retrieval.py:328 (``index``) and :391 (``search``): same constructor config keys (``token_dim``,

@@ -311,7 +311,7 @@ def flat_ip_check_exact(queries: torch.Tensor, passages: torch.Tensor, ids: torc
     """Checker for exact inner-product top-k results against an fp64 ranking.
 
     The products of fp16 / bf16 values are exact in fp32; what differs between any two fp32 implementations
-    (faiss's cuBLAS tiles, torch's CPU sgemm, our tcgen05 chain) is the ORDER of the dim additions.  The fp64 scores
+    (faiss's cuBLAS tiles, torch's CPU sgemm, our wgmma chain) is the ORDER of the dim additions.  The fp64 scores
     s64 are the arbiter: with ``tol[q,p] = 4 * sqrt(dim/16) * 2^-24 * sum_i |q_i p_i|`` (a random-walk bound on the
     accumulation error of dim/16 fp32 accumulator updates, x4 margin; the worst case dim * 2^-24 * sum|q_i p_i| is never
     approached)

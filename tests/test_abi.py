@@ -64,7 +64,7 @@ def test_flat_ip_plan_invariants(sm_count):
                 assert lib.mmb200_flat_ip_plan(nq, n_pass, k, sm_count, out) == _lib.OK, _lib.last_error()
                 n_qb, n_tiles, n_ranges, tpr, grid, cl, ws_lo, ws_hi = [int(v) for v in out]
                 ws = (ws_lo & 0xffffffff) | ((ws_hi & 0xffffffff) << 32)
-                assert n_qb == (nq + 127) // 128 and n_tiles == (n_pass + 255) // 256
+                assert n_qb == (nq + 127) // 128 and n_tiles == (n_pass + 127) // 128   # 128 x 128 score tiles
                 assert 1 <= n_ranges <= 32 and n_ranges * tpr >= n_tiles and (n_ranges - 1) * tpr < n_tiles
                 assert cl in (1, 2, 4) and grid >= cl and grid % cl == 0 and grid <= max(cl, sm_count)
                 n_groups = (n_qb + cl - 1) // cl

@@ -218,7 +218,7 @@ def test_tcgen05_forward_vs_oracle(shape):
     assert_close_rel(out["per_kernel_query"].cpu()[valid], sec["per_kernel_query"][valid], rel=5e-3, what="S (valid query rows)")
     simt = interaction.kernel_pool(*_c(q, d, qm, dm, mu, sg, w), alpha=None if alpha is None else alpha.to(DEV),
                                    log_scale=ls, impl="simt")
-    assert_score_close(out["score"], simt["score"], sec["per_kernel"], w, what="tcgen05 vs FFMA kernel")
+    assert_score_close(out["score"], simt["score"], sec["per_kernel"], w, what="tensor-core vs FFMA kernel")
 
 
 def test_tcgen05_golden():
@@ -271,7 +271,7 @@ def test_tcgen05_run_to_run_determinism():
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# training pair on the tensor cores: forward that saves its cosines + tcgen05 backward (kernel_pool_bwd_tc.cu)
+# training pair on the tensor cores: forward that saves its cosines + tensor-core backward (kernel_pool_bwd_wg.cu)
 # ---------------------------------------------------------------------------------------------------------------
 def _grad_close(a, b, what, rel=1e-3):
     """1e-3 of the largest entry of the tensor (elementwise tiny entries are cancellation noise), the bar of the FFMA

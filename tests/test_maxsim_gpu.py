@@ -40,7 +40,7 @@ SHAPES = [  # n_q, docs_per_query, Lq, Ld, dim, dtype
     (5, 3, 32, 180, 128, torch.float16),
     (3, 7, 17, 300, 64, torch.float16),     # KBS=1, 3 tiles, ragged Lq
     (4, 2, 64, 57, 256, torch.bfloat16),    # NPAD=64, single tile
-    (2, 5, 128, 129, 192, torch.float16),   # NPAD=128 (512 TMEM cols), odd k-block count
+    (2, 5, 128, 129, 192, torch.float16),   # NPAD=128 (four wgmma N = 32 chunks), odd k-block count
     (300, 1, 32, 180, 128, torch.float16),  # query changes every pair; more pairs than SMs
     (1, 1, 1, 1, 64, torch.float16),
     (2, 4, 32, 255, 128, torch.bfloat16),   # Ld + 1 == 256: one 256-row tile in the queries-on-M kernel
@@ -133,7 +133,7 @@ def test_argmax_and_backward_vs_autograd():
 
 def test_backward_is_deterministic_with_many_docs_per_query():
     """grad_q sums the contributions of a query's docs_per_query pairs: a fixed order (no atomics), so two runs agree
-    bit for bit; fp16 inputs take the tcgen05 forward with argmax."""
+    bit for bit; fp16 inputs take the tensor-core forward with argmax."""
     from matchmaker_b200 import autograd
     q, d, qm, dm = O.synth_colbert_inputs(5, 300, 32, 180, 128, seed=77, full_q=False)
     g = torch.randn(5 * 300, generator=torch.Generator().manual_seed(2)).to(DEV)
@@ -158,7 +158,7 @@ def test_backward_is_deterministic_with_many_docs_per_query():
 
 def test_baseline_size_properties():
     """BASELINE config 3 (64 queries x 1000 docs, Lq=32, Ld=180, dim=128, fp16): size-independent properties
-    -- tcgen05 == SIMT, permutation equivariance over documents, chunking invariance, oracle on a sample."""
+    -- tensor cores == SIMT, permutation equivariance over documents, chunking invariance, oracle on a sample."""
     n_q, dpq = 64, 1000
     q, d, qm, dm = O.synth_colbert_inputs(n_q, dpq, 32, 180, 128, seed=1237)
     cq, cd, cqm, cdm = _cuda(q, d, qm, dm)

@@ -1,5 +1,5 @@
 """Checkpoint compatibility: the drop-in rankers expose exactly the state-dict keys and shapes of the reference's
-classes (fixture recorded from /root/reference by oracle/make_state_dict_fixture.py).  The reference loads checkpoints
+classes (fixture recorded from the reference's own classes by oracle/make_state_dict_fixture.py).  The reference loads checkpoints
 with load_state_dict(strict=False) (train.py:107, dense_retrieval.py:138), which silently skips mismatching keys -- a
 renamed parameter would train from scratch without an error."""
 import json

@@ -20,7 +20,7 @@ def _sat_args(params, sat):
     return params["kernel_mult0"], None
 
 
-IMPLS = ["simt", "tcgen05"]   # the FFMA kernel (tkl.cu) and the TMA + tcgen05 kernel (tkl_ts.cu)
+IMPLS = ["simt", "tcgen05"]   # the FFMA kernel (tkl.cu) and the TMA + wgmma kernel (tkl_ts.cu); the impl name is historical
 
 
 def _run(g, params, sat, impl="auto"):
@@ -182,7 +182,7 @@ def test_chunk_holes_and_many_documents(impl):
 def test_kernel_set_without_cover_takes_the_ffma_kernel():
     """Narrow kernels that leave parts of [-1, 1] without any activation: the window token count is then NOT the mask
     count (sigir20_tkl.py:210 tests the activations), the plan kernel detects it on the device and the FFMA kernel,
-    which tests the activations themselves, produces the result; forcing the tcgen05 kernel alone leaves the output of
+    which tests the activations themselves, produces the result; forcing the tensor-core kernel alone leaves the output of
     the memset (all zero), which is how the test knows which kernel ran."""
     B, Lq, Ld, D, K = 3, 6, 200, 32, 3
     g = torch.Generator().manual_seed(4)
@@ -206,7 +206,7 @@ def test_kernel_set_without_cover_takes_the_ffma_kernel():
     assert_close_rel(orig, sec["orig_score"], what="orig_score")
     assert ((orig.cpu() == 0) == (sec["orig_score"] == 0)).all()
     ws_tc, _ = _run(gd, params, "log", "tcgen05")
-    assert (ws_tc == 0).all(), "the tcgen05 kernel must decline a kernel set without cover"
+    assert (ws_tc == 0).all(), "the tensor-core kernel must decline a kernel set without cover"
 
 
 def test_dropin_class_matches_reference_golden():

@@ -1,6 +1,6 @@
 """Kernel-pooling variants of SURVEY 8(f) row 3 against golden vectors recorded from the reference's own classes
 (CIKM20_TK_Sparse, Conv_KNRM) and against the oracle restatement (IDCM's ESM scorer): the document-term gate, the
-n x n n-gram cross match, the 1e-4 clamp floor + bias.  Forward on both kernels (tcgen05 / FFMA), gradients against fp64
+n x n n-gram cross match, the 1e-4 clamp floor + bias.  Forward on both kernels (tensor-core / FFMA), gradients against fp64
 autograd of the oracle."""
 import pytest
 import torch

@@ -1,4 +1,4 @@
-"""Bring-up of the tcgen05 kernel-pooling forward: staged parity (each stage in a subprocess) + timing."""
+"""Bring-up of the tensor-core kernel-pooling forward: staged parity (each stage in a subprocess) + timing."""
 import os, subprocess, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
@@ -70,7 +70,7 @@ def bwd():
     for _ in range(5): step()
     e1.record(); torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / 5
-    print(f"TK fwd+bwd B={B}: {ms:.3f} ms per step -> {B / ms * 1e3 / 1e6:.2f} M pairs/s (forward tcgen05 + backward FFMA)", flush=True)
+    print(f"TK fwd+bwd B={B}: {ms:.3f} ms per step -> {B / ms * 1e3 / 1e6:.2f} M pairs/s (forward tensor cores + backward FFMA)", flush=True)
 
 if __name__ == "__main__":
     if len(sys.argv) > 1 and sys.argv[1] == "bwd": bwd(); sys.exit(0)

@@ -39,7 +39,7 @@ def win(impl):
 
 
 timed("window scores (auto)", lambda: win("auto"))
-timed("window scores (tcgen05)", lambda: win("tcgen05"))
+timed("window scores (tensor cores)", lambda: win("tcgen05"))
 timed("window scores (simt)", lambda: win("simt"), n=5)
 timed("top hills", lambda: interaction.tkl_top_hills(ws_holder["ws"], c["cs"]))
 timed("full step", wl.kernel_step)
