@@ -119,6 +119,23 @@ MMB200_API int mmb200_maxsim_fwd_host(const void* q_host, const void* d_host, co
                            int32_t docs_per_query, int32_t Lq, int32_t Ld, int32_t dim, int32_t dtype,
                            int32_t mask_dtype, int64_t chunk_pairs);
 
+/* Store mode: max-sim against a ragged token store (passages keep only their real token rows, as the reference's
+ * encode loop writes them, matchmaker/dense_retrieval.py:244), ColBERT.forward_aggregation semantics
+ * (colbert.py:100-112, no masks):
+ *
+ *   out[p] = sum_{i < Lq} max_{off[d] <= r < off[d+1]} <q[pair_q[p]][i], store[r]>,   d = pair_d[p]
+ *
+ * store [n_rows, dim]; doc_offsets [n_docs + 1] int64, non-decreasing, doc_offsets[n_docs] <= n_rows (passage d is
+ * rows [off[d], off[d+1]); empty ranges allowed; at most max_doc_len rows of a passage are read).
+ * q [n_q, Lq, dim]; pair_q / pair_d [n_pairs] int32; pair_d[p] < 0 skips the pair (nothing is fetched) and, like a
+ * passage without rows, scores -inf.  dtype / impl as mmb200_maxsim_fwd (AUTO picks the kernel it would pick for
+ * the padded [n_docs, max_doc_len, dim] layout; scores are bit-identical to that layout with masks).  The tensor-core
+ * kernels address the store with the passage's first row as the TMA row coordinate: n_rows < 2^31 - 1024. */
+MMB200_API int mmb200_maxsim_store_fwd(const void* q, const void* store, const int64_t* doc_offsets,
+                                       const int32_t* pair_q, const int32_t* pair_d, float* out, int64_t n_q,
+                                       int64_t n_rows, int64_t n_docs, int64_t n_pairs, int32_t Lq, int32_t max_doc_len,
+                                       int32_t dim, int32_t dtype, int32_t impl, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Cosine match matrix + RBF kernel pooling (KNRM / TK)
  *
@@ -314,6 +331,14 @@ MMB200_API int mmb200_flat_ip_topk(const void* queries, const void* passages, co
  * the host). */
 MMB200_API int mmb200_topk_merge(const float* cand_scores, const int64_t* cand_ids, float* out_scores,
                                  int64_t* out_ids, int64_t nq, int32_t n_candidates, int32_t k, void* stream);
+
+/* Per-query de-duplication + top-k: the k best DISTINCT ids of cand_scores / cand_ids [nq, n_candidates], each id with
+ * its highest score, ordered by (score desc, id asc).  Void candidates, any n_candidates (passes over groups of 8192)
+ * and the (-FLT_MAX, -1) tail are as in mmb200_topk_merge.  1 <= k <= 4096; larger k returns MMB200_ERR_UNSUPPORTED.
+ * Replaces the per-passage de-duplication loop of the maxP aggregation, matchmaker/dense_retrieval.py:414-427, and
+ * builds the candidate passage lists of ColBERT end-to-end retrieval. */
+MMB200_API int mmb200_topk_unique(const float* cand_scores, const int64_t* cand_ids, float* out_scores,
+                                  int64_t* out_ids, int64_t nq, int32_t n_candidates, int32_t k, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Storage block loader: byte ranges of files -> one contiguous DEVICE buffer.

@@ -43,6 +43,8 @@ SIGNATURES = {
     "mmb200_flat_ip_plan": (_c.c_int, [_i64, _i64, _i32, _i32, _c.POINTER(_i32)]),
     "mmb200_flat_ip_topk": (_c.c_int, [_vp] * 6 + [_i64, _i64, _i64, _i32, _i32, _i32, _i64, _vp]),
     "mmb200_topk_merge": (_c.c_int, [_vp] * 4 + [_i64, _i32, _i32, _vp]),
+    "mmb200_topk_unique": (_c.c_int, [_vp] * 4 + [_i64, _i32, _i32, _vp]),
+    "mmb200_maxsim_store_fwd": (_c.c_int, [_vp] * 6 + [_i64, _i64, _i64, _i64, _i32, _i32, _i32, _i32, _i32, _vp]),
     "mmb200_dot_pairs": (_c.c_int, [_vp, _vp, _vp, _i64, _i32, _i32, _vp]),
     "mmb200_kernel_pool_bwd": (_c.c_int, [_vp] * 15 + [_i64, _i32, _i32, _i32, _i32, _f32, _i32, _vp]),
     "mmb200_kernel_pool_fwd_ex": (_c.c_int, [_vp] * 13 + [_i64, _i32, _i32, _i32, _i32, _f32, _f32, _f32, _i32, _i32, _vp]),

@@ -455,14 +455,42 @@ __device__ __forceinline__ bool cand_before(const Cand& a, const Cand& b) {
   if (a.s != b.s) return a.s > b.s;
   return a.id < b.id;
 }
+// (valid desc, id asc, score desc): the order in which the first entry of every id is its best one
+__device__ __forceinline__ bool cand_before_by_id(const Cand& a, const Cand& b) {
+  if (a.valid != b.valid) return a.valid > b.valid;
+  if (a.id != b.id) return a.id < b.id;
+  return a.s > b.s;
+}
+
+// In-place bitonic sort of c[0, Lpow2) by the order `kById ? cand_before_by_id : cand_before`; ends with __syncthreads.
+template <bool kById>
+__device__ __forceinline__ void bitonic_sort(Cand* c, int Lpow2) {
+  for (int size = 2; size <= Lpow2; size <<= 1) {
+    for (int stride = size >> 1; stride > 0; stride >>= 1) {
+      for (int e = threadIdx.x; e < Lpow2 / 2; e += blockDim.x) {
+        const int i = 2 * e - (e & (stride - 1));
+        const int j = i + stride;
+        const bool up = ((i & size) == 0);
+        const Cand a = c[i], b = c[j];
+        const bool swap = kById ? (up ? cand_before_by_id(b, a) : cand_before_by_id(a, b))
+                                : (up ? cand_before(b, a) : cand_before(a, b));
+        if (swap) { c[i] = b; c[j] = a; }
+      }
+      __syncthreads();
+    }
+  }
+}
 
 // Block (q, grp) sorts candidates [grp * seg, min(L, (grp + 1) * seg)) of query q and writes its k best to row
 // q * n_groups + grp of the output.  A candidate is void when its score is NaN, -inf or faiss's "no result" value
 // (-FLT_MAX) -- NOT by the sign of its id: faiss IndexIDMap accepts negative user ids.  `final_pass` selects the
 // filler for missing results: (-FLT_MAX, -1) as faiss returns them, or (-inf, -1) between passes.
+// `unique` (mmb200_topk_unique): every id is kept once, with its highest score -- a first sort by (id, score desc)
+// voids all but the first entry of each id, then the usual sort ranks the survivors.  Unique-with-max composes over
+// groups, so the pass structure stays exact.
 __global__ void __launch_bounds__(256) topk_merge_kernel(const float* __restrict__ cand_scores,
                                                          const int64_t* __restrict__ cand_ids, int64_t nq, int L, int seg,
-                                                         int n_groups, int Lpow2, int k, int final_pass,
+                                                         int n_groups, int Lpow2, int k, int final_pass, int unique,
                                                          float* __restrict__ out_scores, int64_t* __restrict__ out_ids) {
   extern __shared__ __align__(16) uint8_t msm[];
   Cand* c = reinterpret_cast<Cand*>(msm);
@@ -483,19 +511,17 @@ __global__ void __launch_bounds__(256) topk_merge_kernel(const float* __restrict
       c[e] = v;
     }
     __syncthreads();
-    for (int size = 2; size <= Lpow2; size <<= 1) {
-      for (int stride = size >> 1; stride > 0; stride >>= 1) {
-        for (int e = threadIdx.x; e < Lpow2 / 2; e += blockDim.x) {
-          const int i = 2 * e - (e & (stride - 1));
-          const int j = i + stride;
-          const bool up = ((i & size) == 0);
-          const Cand a = c[i], b = c[j];
-          const bool swap = up ? cand_before(b, a) : cand_before(a, b);
-          if (swap) { c[i] = b; c[j] = a; }
-        }
-        __syncthreads();
-      }
+    if (unique) {
+      bitonic_sort<true>(c, Lpow2);
+      uint32_t dup = 0;   // bit b: element threadIdx.x + b * blockDim.x repeats the id before it (Lpow2 <= 32 * 256)
+      for (int e = threadIdx.x, b = 0; e < Lpow2; e += blockDim.x, ++b)
+        if (e > 0 && c[e].valid && c[e - 1].valid && c[e].id == c[e - 1].id) dup |= 1u << b;
+      __syncthreads();
+      for (int e = threadIdx.x, b = 0; e < Lpow2; e += blockDim.x, ++b)
+        if ((dup >> b) & 1u) c[e].valid = 0;
+      __syncthreads();
     }
+    bitonic_sort<false>(c, Lpow2);
     for (int e = threadIdx.x; e < k; e += blockDim.x) {
       const bool ok = e < Lpow2 && c[e].valid;
       out_scores[item * k + e] = ok ? c[e].s : (final_pass ? -3.4028234663852886e38f : -INFINITY);
@@ -570,9 +596,10 @@ __global__ void fill_u32(uint32_t* p, int64_t n, uint32_t v) {
 // k = 1024, or sharding.topk_all_gather_merge over a shard with thousands of local scores per query -- is merged in
 // passes: groups of kMergeSeg candidates are cut to their k best, the survivors merged again.
 constexpr int kMergeSeg = 8192;
+constexpr int kMaxUniqueK = kMergeSeg / 2;
 
 int launch_merge(const float* cand_scores, const int64_t* cand_ids, int64_t nq, int L, int k, float* out_scores,
-                 int64_t* out_ids, const DeviceInfo& dev, cudaStream_t stream) {
+                 int64_t* out_ids, const DeviceInfo& dev, cudaStream_t stream, bool unique = false) {
   MMB_CHECK_CUDA(cudaFuncSetAttribute(topk_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       (int)(kMergeSeg * sizeof(Cand))));
   const float* in_s = cand_scores;
@@ -602,7 +629,7 @@ int launch_merge(const float* cand_scores, const int64_t* cand_ids, int64_t nq, 
     }
     const int grid = (int)std::min<int64_t>(nq * groups, (int64_t)dev.sm_count * 4);
     topk_merge_kernel<<<grid, 256, (size_t)lp * sizeof(Cand), stream>>>(in_s, in_i, nq, L, seg, groups, lp, k_out, last ? 1 : 0,
-                                                                        o_s, o_i);
+                                                                        unique ? 1 : 0, o_s, o_i);
     if (cudaGetLastError() != cudaSuccess) {
       set_error("topk merge: kernel launch failed");
       rc = MMB200_ERR_CUDA;
@@ -764,4 +791,25 @@ extern "C" int mmb200_topk_merge(const float* cand_scores, const int64_t* cand_i
     return MMB200_ERR_UNSUPPORTED;
   }
   return launch_merge(cand_scores, cand_ids, nq, n_candidates, k, out_scores, out_ids, dev, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int mmb200_topk_unique(const float* cand_scores, const int64_t* cand_ids, float* out_scores, int64_t* out_ids,
+                                  int64_t nq, int32_t n_candidates, int32_t k, void* stream_) {
+  using namespace mmb;
+  MMB_REQUIRE(cand_scores && cand_ids && out_scores && out_ids, "null pointer");
+  MMB_REQUIRE(nq >= 0 && n_candidates >= 1 && k >= 1, "bad sizes");
+  if (k > kMaxUniqueK) {
+    // a pass over groups of kMergeSeg candidates shrinks the list only while k <= kMergeSeg / 2
+    set_error("topk_unique supports k <= 4096");
+    return MMB200_ERR_UNSUPPORTED;
+  }
+  if (nq == 0) return MMB200_OK;
+  DeviceInfo dev;
+  if (int rc = current_device_info(&dev)) return rc;
+  if (!is_sm90(dev)) {
+    set_error("matchmaker_b200 kernels are built for sm_90a only");
+    return MMB200_ERR_UNSUPPORTED;
+  }
+  return launch_merge(cand_scores, cand_ids, nq, n_candidates, k, out_scores, out_ids, dev, static_cast<cudaStream_t>(stream_),
+                      true);
 }

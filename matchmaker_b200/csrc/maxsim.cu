@@ -13,8 +13,8 @@
 //   * warp 0 (one lane): TMA producer.  A document tile is 128 token rows x dim, fetched as
 //     [KBS k-blocks][128 rows][64 halfs] with SWIZZLE_128B by ONE 4-D cp.async.bulk.tensor
 //     per stage (rows past Ld are zero-filled by the TMA unit, no HBM traffic); the query
-//     matrix ([NPAD rows][dim]) lives in a 2-slot ring and is re-fetched only when the query
-//     of consecutive pairs changes;
+//     matrix ([NPAD rows][dim]) lives in a 2-slot ring (1 slot when two leave no room for two
+//     stages) and is re-fetched only when the query of consecutive pairs changes;
 //   * warpgroups 1 and 2: warpgroup c computes D[64 doc rows x NPAD query cols] (fp32,
 //     registers) = Doc_tile[rows 64c..64c+63] * Q^T with wgmma m64n32k16 chunks, applies the
 //     document mask (-1000) / tile padding (-inf) per row, and keeps a running column max over
@@ -26,6 +26,11 @@
 //
 // Kernel `maxsim_simt_kernel`: CUDA-core version for any dtype / dim / length (fp32 inputs,
 // dim % 64 != 0, argmax for backward); also the in-library cross-check of the tensor-core path.
+//
+// Store mode (MaxsimParams::doc_offsets, mmb200_maxsim_store_fwd): every kernel reads passage d
+// as rows [off[d], off[d+1]) of a ragged [n_rows, dim] token store instead of a padded, masked
+// [n_d, Ld, dim] tensor; rows past the passage's length are excluded like padding, without the
+// -1000 fill (there is no mask).
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -83,7 +88,10 @@ __global__ void __launch_bounds__(kSimtThreads) maxsim_simt_kernel(MaxsimParams 
   for (int64_t p = blockIdx.x; p < P.n_pairs; p += gridDim.x) {
     const int64_t qi = pair_query(P, p), di = pair_doc(P, p), dmi = pair_dmask_row(P, p);
     const T* qptr = static_cast<const T*>(P.q) + qi * (int64_t)Lq * dim;
-    const T* dptr = static_cast<const T*>(P.d) + di * (int64_t)Ld * dim;
+    int64_t row0 = di * (int64_t)Ld;
+    int nrows = Ld;
+    if (P.doc_offsets) nrows = store_doc_rows(P, di, &row0);  // store mode: the passage's own rows, no mask
+    const T* dptr = static_cast<const T*>(P.d) + row0 * dim;
     __syncthreads();
     for (int e = threadIdx.x; e < Lq * dim; e += kSimtThreads) {
       sq[(e / dim) * qstride + (e % dim)] = to_float(qptr[e]);
@@ -93,7 +101,7 @@ __global__ void __launch_bounds__(kSimtThreads) maxsim_simt_kernel(MaxsimParams 
     int barg[kSimtMaxQPerLane];
 #pragma unroll
     for (int t = 0; t < kSimtMaxQPerLane; ++t) { best[t] = -INFINITY; barg[t] = -1; }
-    for (int j = warp; j < Ld; j += 4) {
+    for (int j = warp; j < nrows; j += 4) {
       const bool ok = mask_at(P.d_mask, P.d_mask ? P.mask_dtype : MMB200_MASK_NONE, dmi * (int64_t)Ld + j);
       float acc[kSimtMaxQPerLane] = {0.f, 0.f, 0.f, 0.f};
       if (ok) {
@@ -166,6 +174,7 @@ struct TcLaunch {
   int32_t stages;      // document stages in the ring
   int32_t tiles;       // ceil(Ld / 128)
   int32_t qslot_bytes; // kblocks * npad * 128
+  int32_t qslots;      // query tiles in the ring: 2, or 1 when two do not leave room for two stages (dim 768, Lq > 32)
 };
 
 template <typename T>
@@ -191,7 +200,7 @@ maxsim_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   constexpr int kStageBytes = KBS * kKBlockBytes;
   uint8_t* stage_base = smem;
   uint8_t* q_base = smem + (size_t)L.stages * kStageBytes;
-  TcShared* S = reinterpret_cast<TcShared*>(q_base + (size_t)kQSlots * L.qslot_bytes);
+  TcShared* S = reinterpret_cast<TcShared*>(q_base + (size_t)L.qslots * L.qslot_bytes);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -222,7 +231,7 @@ maxsim_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
       for (int64_t p = p_begin; p < p_end; ++p) {
         const int64_t qi = pair_query(P, p), di = pair_doc(P, p);
         if (qi != prev_q) {
-          const uint32_t slot = qcount & 1u, use = qcount >> 1;
+          const uint32_t slot = L.qslots == 2 ? (qcount & 1u) : 0u, use = L.qslots == 2 ? (qcount >> 1) : qcount;
           mbar_wait(&S->qempty[slot], (use & 1u) ^ 1u);
           mbar_arrive_expect_tx(&S->qfull[slot], (uint32_t)L.qslot_bytes);
           tma_load_4d(&tmap_q, q_base + (size_t)slot * L.qslot_bytes, &S->qfull[slot], 0, 0, 0, (int)qi,
@@ -230,12 +239,21 @@ maxsim_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
           ++qcount;
           prev_q = qi;
         }
+        // store mode: rows [row0, row0 + nrows) of the [n_rows, dim] store; tiles past the passage are not fetched
+        int64_t row0 = 0;
+        int nrows = P.Ld;
+        if (P.doc_offsets) nrows = store_doc_rows(P, di, &row0);
+        const int dcoord = P.doc_offsets ? 0 : (int)di;
         for (int t = 0; t < L.tiles; ++t) {
           for (int ks = 0; ks < ksteps; ++ks) {
             mbar_wait(&S->empty[stage], phase ^ 1u);
-            mbar_arrive_expect_tx(&S->full[stage], (uint32_t)kStageBytes);
-            tma_load_4d(&tmap_d, stage_base + (size_t)stage * kStageBytes, &S->full[stage], 0, t * kTileRows,
-                        ks * KBS, (int)di, kEvictFirst);
+            if (t * kTileRows < nrows) {
+              mbar_arrive_expect_tx(&S->full[stage], (uint32_t)kStageBytes);
+              tma_load_4d(&tmap_d, stage_base + (size_t)stage * kStageBytes, &S->full[stage], 0, (int)row0 + t * kTileRows,
+                          ks * KBS, dcoord, kEvictFirst);
+            } else {
+              mbar_arrive(&S->full[stage]);
+            }
             if (++stage == L.stages) { stage = 0; phase ^= 1u; }
           }
         }
@@ -258,13 +276,18 @@ maxsim_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
       const int64_t qi = pair_query(P, p);
       if (qi != prev_q) {
         if (prev_q >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&S->qempty[cur_slot]); }  // old Q no longer read
-        cur_slot = (int)(qcount & 1u);
-        mbar_wait(&S->qfull[cur_slot], (qcount >> 1) & 1u);
+        cur_slot = L.qslots == 2 ? (int)(qcount & 1u) : 0;
+        mbar_wait(&S->qfull[cur_slot], (L.qslots == 2 ? (qcount >> 1) : qcount) & 1u);
         ++qcount;
         prev_q = qi;
       }
       const uint32_t qaddr = smem_u32(q_base + (size_t)cur_slot * L.qslot_bytes);
       const int64_t dmrow = pair_dmask_row(P, p);
+      int nrows = P.Ld;   // store mode: the passage's length (0 for a skipped pair)
+      if (P.doc_offsets) {
+        int64_t row0;
+        nrows = store_doc_rows(P, pair_doc(P, p), &row0);
+      }
       float colmax[NC][8];
 #pragma unroll
       for (int h = 0; h < NC; ++h)
@@ -273,7 +296,7 @@ maxsim_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
       for (int t = 0; t < L.tiles; ++t) {
         // this thread's two document rows; mask words fetched before the MMAs so their latency hides behind them
         const int g0 = t * kTileRows + 64 * c + 16 * wq + (lane >> 2), g1 = g0 + 8;
-        const bool in0 = g0 < P.Ld, in1 = g1 < P.Ld;
+        const bool in0 = g0 < nrows, in1 = g1 < nrows;
         const uint64_t raw0 = (in0 && dmt != MMB200_MASK_NONE) ? mask_raw(P.d_mask, dmt, dmrow * (int64_t)P.Ld + g0) : 1;
         const uint64_t raw1 = (in1 && dmt != MMB200_MASK_NONE) ? mask_raw(P.d_mask, dmt, dmrow * (int64_t)P.Ld + g1) : 1;
         float acc[NC][16];
@@ -402,10 +425,15 @@ static int launch_tc(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cu
   L.tiles = (P.Ld + kTileRows - 1) / kTileRows;
   L.qslot_bytes = L.kblocks * L.npad * 128;
   const int stage_bytes = L.kbs * kKBlockBytes;
-  const int fixed = kQSlots * L.qslot_bytes + (int)sizeof(TcShared) + 1024 /* alignment slack */;
-  const int budget = dev.max_smem_optin - fixed;
-  L.stages = std::min(kMaxStages, budget / stage_bytes);
-  if (L.stages < 2) {
+  // two query tiles when they leave room for at least two document stages; otherwise (large dim with Lq > 32) one,
+  // re-fetched after the consumers release it
+  int fixed = 0;
+  for (L.qslots = kQSlots; L.qslots >= 1; --L.qslots) {
+    fixed = L.qslots * L.qslot_bytes + (int)sizeof(TcShared) + 1024 /* alignment slack */;
+    L.stages = std::min(kMaxStages, (dev.max_smem_optin - fixed) / stage_bytes);
+    if (L.stages >= 2) break;
+  }
+  if (L.qslots < 1 || L.stages < 2) {
     set_error("maxsim documents-on-M: query tile too large for shared memory");
     return MMB200_ERR_UNSUPPORTED;
   }
@@ -422,8 +450,11 @@ static int launch_tc(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cu
       return rc;
   }
   {
-    const uint64_t dims[4] = {64, (uint64_t)P.Ld, (uint64_t)L.kblocks, (uint64_t)P.n_d};
-    const uint64_t strides[3] = {(uint64_t)P.dim * 2, 128, (uint64_t)P.Ld * P.dim * 2};
+    // store mode: the [n_rows, dim] store is one "document"; a passage's tile starts at its first row
+    const uint64_t d_rows = P.doc_offsets ? (uint64_t)P.n_rows : (uint64_t)P.Ld;
+    const uint64_t d_count = P.doc_offsets ? 1 : (uint64_t)P.n_d;
+    const uint64_t dims[4] = {64, d_rows, (uint64_t)L.kblocks, d_count};
+    const uint64_t strides[3] = {(uint64_t)P.dim * 2, 128, d_rows * P.dim * 2};
     const uint32_t box[4] = {64, (uint32_t)kTileRows, (uint32_t)L.kbs, 1};
     if (int rc = encode_tensor_map(&td, tdt, 4, P.d, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B,
                                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B))
@@ -517,5 +548,23 @@ extern "C" int mmb200_maxsim_fwd(const void* q, const void* d, const void* q_mas
   P.out = out; P.argmax = argmax; P.n_q = n_q; P.n_d = n_d; P.n_pairs = n_pairs;
   P.pair_base = 0;
   P.docs_per_query = docs_per_query; P.Lq = Lq; P.Ld = Ld; P.dim = dim; P.mask_dtype = mask_dtype;
+  P.doc_offsets = nullptr; P.n_rows = 0;
+  return mmb::maxsim_fwd_device(P, dtype, impl, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int mmb200_maxsim_store_fwd(const void* q, const void* store, const int64_t* doc_offsets,
+                                       const int32_t* pair_q, const int32_t* pair_d, float* out, int64_t n_q,
+                                       int64_t n_rows, int64_t n_docs, int64_t n_pairs, int32_t Lq, int32_t max_doc_len,
+                                       int32_t dim, int32_t dtype, int32_t impl, void* stream) {
+  MMB_REQUIRE(doc_offsets && pair_q && pair_d, "doc_offsets, pair_q and pair_d must be non-null");
+  MMB_REQUIRE(n_rows >= 1 && n_docs >= 1 && max_doc_len >= 1, "the store needs at least one row, one passage, max_doc_len >= 1");
+  MMB_REQUIRE(n_rows < (1ll << 31) - 1024, "at most 2^31 - 1024 store rows per device (TMA row coordinates are int32)");
+  MMB_REQUIRE(impl != MMB200_IMPL_TCGEN05_RAGGED, "store mode already fetches only each passage's own rows");
+  mmb::MaxsimParams P;
+  P.q = q; P.d = store; P.q_mask = nullptr; P.d_mask = nullptr; P.pair_q = pair_q; P.pair_d = pair_d; P.pair_dmask = nullptr;
+  P.rows_needed = nullptr; P.out = out; P.argmax = nullptr; P.n_q = n_q; P.n_d = n_docs;
+  P.n_pairs = n_pairs; P.pair_base = 0; P.docs_per_query = 1; P.Lq = Lq; P.Ld = max_doc_len; P.dim = dim;
+  P.mask_dtype = MMB200_MASK_NONE;
+  P.doc_offsets = doc_offsets; P.n_rows = n_rows;
   return mmb::maxsim_fwd_device(P, dtype, impl, static_cast<cudaStream_t>(stream));
 }

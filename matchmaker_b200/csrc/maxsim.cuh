@@ -20,7 +20,20 @@ struct MaxsimParams {
   int64_t n_q, n_d, n_pairs;
   int64_t pair_base;  // query of pair p (when pair_q == NULL) is (p + pair_base) / docs_per_query
   int32_t docs_per_query, Lq, Ld, dim, mask_dtype;
+  // Store mode (doc_offsets != NULL): d is a ragged token store [n_rows, dim]; document di is rows
+  // [doc_offsets[di], doc_offsets[di + 1]), at most Ld of them are read.  No masks; pair_d < 0 and documents without
+  // rows score -inf.  NULL: the padded [n_d, Ld, dim] layout above.
+  const int64_t* doc_offsets;
+  int64_t n_rows;
 };
+
+// Rows [*lo, *lo + return value) of document di in store mode; 0 rows for a skipped pair (di < 0).
+__device__ __forceinline__ int store_doc_rows(const MaxsimParams& P, int64_t di, int64_t* lo) {
+  if (di < 0) { *lo = 0; return 0; }
+  const int64_t a = P.doc_offsets[di], b = P.doc_offsets[di + 1];
+  *lo = a;
+  return (int)max((int64_t)0, min(b - a, (int64_t)P.Ld));
+}
 
 struct DeviceInfo;
 // maxsim_qm.cu: "queries on M" wgmma kernel (Lq <= 32, dim 64/128); *handled = false if out of envelope.

@@ -209,6 +209,7 @@ extern "C" int mmb200_maxsim_fwd_host(const void* q_host, const void* d_host, co
     MaxsimParams P;
     P.q = dq; P.d = slab; P.q_mask = dqm; P.d_mask = d_mask_host ? slab + slab_docs : nullptr;
     P.pair_q = nullptr; P.pair_d = nullptr; P.pair_dmask = nullptr; P.rows_needed = nullptr; P.out = hp->out + lo; P.argmax = nullptr;
+    P.doc_offsets = nullptr; P.n_rows = 0;
     P.n_q = n_q; P.n_d = n; P.n_pairs = n; P.pair_base = lo; P.docs_per_query = docs_per_query;
     P.Lq = Lq; P.Ld = Ld; P.dim = dim; P.mask_dtype = mask_dtype;
     if (int rc = maxsim_fwd_device(P, dtype, MMB200_IMPL_AUTO, hp->compute)) return rc;

@@ -91,7 +91,8 @@ __device__ __forceinline__ void take(float v, int col, float& m, int& am) {
 
 // kArgmax: the training instantiation also tracks WHICH document row won each query token's max (what backward needs,
 // matchmaker/models/colbert.py:71 through autograd).  NCH = tn / 64 accumulator chunks of 32 registers.
-template <typename T, int NCH, bool kArgmax>
+// kStore: store mode (P.doc_offsets != NULL) -- a template parameter so that the padded instantiations compile as before.
+template <typename T, int NCH, bool kArgmax, bool kStore>
 __global__ void __launch_bounds__(kThreads, 1)
 maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_d,
                  const __grid_constant__ CUtensorMap tmap_d16, MaxsimParams P, QmLaunch L) {
@@ -118,9 +119,9 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     for (int s = 0; s < kQSlots; ++s) { mbar_init(&S->qfull[s], 1); mbar_init(&S->qempty[s], 8); }
     fence_barrier_init();
   }
-  if (P.rows_needed) {
-    // ragged fetch leaves rows of a stage untouched: start from zeros so that stale rows are always finite
-    // and the virtual row (index >= Ld, only ever written by TMA zero fill) is zero
+  if (P.rows_needed || kStore) {
+    // ragged fetch (and store mode) leaves rows of a stage untouched: start from zeros so that stale rows are always
+    // finite and the virtual row (index >= Ld, only ever written by TMA zero fill) is zero
     for (int s = 0; s < L.stages; ++s) {
       uint4* z = reinterpret_cast<uint4*>(stage_base + (size_t)s * L.stage_bytes);
       for (int e = threadIdx.x; e < L.doc_bytes / 16; e += kThreads) z[e] = make_uint4(0, 0, 0, 0);
@@ -149,7 +150,12 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
           ++qcount;
           prev_q = qi;
         }
-        const int need_rows = P.rows_needed ? P.rows_needed[di] : 0;
+        // store mode: the passage's rows start at row `row0` of the [n_rows, dim] store (tensor-map dim 3 has extent 1)
+        int64_t row0 = 0;
+        int need_rows = 0;
+        if constexpr (kStore) need_rows = store_doc_rows(P, di, &row0);
+        else if (P.rows_needed) need_rows = P.rows_needed[di];
+        const int dcoord = kStore ? 0 : (int)di;
         const int c = (int)((p - p_begin) & 1);
         for (int t = 0; t < L.tiles; ++t) {
           const int64_t j = c ? seq1++ : seq0++;
@@ -157,12 +163,12 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
           const uint32_t phase = (uint32_t)((j / ring) & 1);
           mbar_wait(&S->empty[stage], phase ^ 1u);
           uint8_t* dst = stage_base + (size_t)stage * L.stage_bytes;
-          if (!P.rows_needed) {
+          if (!P.rows_needed && !kStore) {
             mbar_arrive_expect_tx(&S->full[stage], (uint32_t)L.doc_bytes);
             tma_load_4d(&tmap_d, dst, &S->full[stage], 0, t * L.tn, 0, (int)di, kEvictFirst);
           } else {
-            // 16-row blocks up to the document's last unmasked row; the rest of the stage keeps stale
-            // (finite) rows, which the penalty row masks with -inf
+            // 16-row blocks up to the document's last unmasked row (store mode: its last row); the rest of the stage
+            // keeps stale (finite) rows, which the penalty row masks with -inf
             const int rows_here = min(max(need_rows - t * L.tn, 0), L.tn);
             const int nb = (rows_here + 15) >> 4;
             if (nb == 0) {
@@ -171,8 +177,8 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
               mbar_arrive_expect_tx(&S->full[stage], (uint32_t)(nb * L.kblocks * 2048));
               for (int kb = 0; kb < L.kblocks; ++kb)
                 for (int b16 = 0; b16 < nb; ++b16)
-                  tma_load_4d(&tmap_d16, dst + kb * L.tn * 128 + b16 * 2048, &S->full[stage], 0, t * L.tn + b16 * 16, kb,
-                              (int)di, kEvictFirst);
+                  tma_load_4d(&tmap_d16, dst + kb * L.tn * 128 + b16 * 2048, &S->full[stage], 0,
+                              (int)row0 + t * L.tn + b16 * 16, kb, dcoord, kEvictFirst);
             }
           }
         }
@@ -196,6 +202,11 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     fetch(p_begin, 0, raw_next);
     for (int64_t p = p_begin; p < p_end; ++p) {
       bool any_masked = false;
+      int lim = P.Ld;   // rows of this document; store mode: the passage's length, 0 for a skipped pair
+      if constexpr (kStore) {
+        int64_t row0;
+        lim = store_doc_rows(P, P.pair_d ? (int64_t)P.pair_d[p] : p, &row0);
+      }
       for (int t = 0; t < L.tiles; ++t) {
 #pragma unroll
         for (int k = 0; k < 8; ++k) raw[k] = raw_next[k];
@@ -210,7 +221,7 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
 #pragma unroll
         for (int k = 0; k < 8; ++k) {
           const int r = lane + 32 * k, g = t * L.tn + r;
-          const bool in_doc = r < L.tn && g < P.Ld;
+          const bool in_doc = r < L.tn && g < lim;
           const bool ok = in_doc && mask_test(raw[k], dmt);
           masked_here |= in_doc && !ok;
           pen[k] = ok ? 0.f : -INFINITY;
@@ -225,7 +236,8 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
 #pragma unroll
         for (int k = 0; k < 8; ++k) {
           const int r = lane + 32 * k, g = t * L.tn + r;
-          if (r < L.tn) pt[r] = (g == L.tiles * L.tn - 1) ? (any_masked ? -1000.f : -INFINITY) : pen[k];
+          // the virtual -1000 row exists only in the masked (padded) layout
+          if (r < L.tn) pt[r] = (!kStore && g == L.tiles * L.tn - 1) ? (any_masked ? -1000.f : -INFINITY) : pen[k];
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(&S->full[stage]);
@@ -337,14 +349,14 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   }
 }
 
-template <typename T, bool kArgmax>
+template <typename T, bool kArgmax, bool kStore>
 int launch_qm(int nch, int grid, size_t smem_bytes, cudaStream_t stream, const CUtensorMap& tq, const CUtensorMap& td,
               const CUtensorMap& td16, const MaxsimParams& P, const QmLaunch& L) {
 #define MMB_QM_CASE(N)                                                                                                  \
   case N:                                                                                                               \
-    MMB_CHECK_CUDA(cudaFuncSetAttribute(maxsim_qm_kernel<T, N, kArgmax>, cudaFuncAttributeMaxDynamicSharedMemorySize,   \
+    MMB_CHECK_CUDA(cudaFuncSetAttribute(maxsim_qm_kernel<T, N, kArgmax, kStore>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
                                         (int)smem_bytes));                                                              \
-    maxsim_qm_kernel<T, N, kArgmax><<<grid, kThreads, smem_bytes, stream>>>(tq, td, td16, P, L);                        \
+    maxsim_qm_kernel<T, N, kArgmax, kStore><<<grid, kThreads, smem_bytes, stream>>>(tq, td, td16, P, L);                \
     break;
   switch (nch) {
     MMB_QM_CASE(1)
@@ -395,7 +407,7 @@ int maxsim_qm_launch(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cu
   if ((reinterpret_cast<uintptr_t>(P.q) | reinterpret_cast<uintptr_t>(P.d)) & 15) return MMB200_OK;
   QmLaunch L;
   L.kblocks = P.dim / 64;
-  const int rows = P.Ld + 1;  // + the virtual row that carries the reference's -1000 fill
+  const int rows = P.Ld + (P.doc_offsets ? 0 : 1);  // + the virtual row that carries the reference's -1000 fill
   L.tiles = (rows + 255) / 256;
   L.tn = (((rows + L.tiles - 1) / L.tiles) + 63) / 64 * 64;
   L.doc_bytes = L.kblocks * L.tn * 128;
@@ -415,9 +427,13 @@ int maxsim_qm_launch(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cu
                                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B))
       return rc;
   }
+  // documents: [n_d][Ld rows][kblocks][64], or in store mode the [n_rows][kblocks][64] store as one "document" whose
+  // row coordinate is the passage's first row (rows past n_rows are zero-filled by TMA)
+  const uint64_t d_rows = P.doc_offsets ? (uint64_t)P.n_rows : (uint64_t)P.Ld;
+  const uint64_t d_count = P.doc_offsets ? 1 : (uint64_t)P.n_d;
   {
-    const uint64_t dims[4] = {64, (uint64_t)P.Ld, (uint64_t)L.kblocks, (uint64_t)P.n_d};
-    const uint64_t strides[3] = {(uint64_t)P.dim * 2, 128, (uint64_t)P.Ld * P.dim * 2};
+    const uint64_t dims[4] = {64, d_rows, (uint64_t)L.kblocks, d_count};
+    const uint64_t strides[3] = {(uint64_t)P.dim * 2, 128, d_rows * P.dim * 2};
     const uint32_t box[4] = {64, (uint32_t)L.tn, (uint32_t)L.kblocks, 1};
     if (int rc = encode_tensor_map(&td, tdt, 4, P.d, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B,
                                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B))
@@ -425,8 +441,8 @@ int maxsim_qm_launch(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cu
   }
   CUtensorMap td16;
   {
-    const uint64_t dims[4] = {64, (uint64_t)P.Ld, (uint64_t)L.kblocks, (uint64_t)P.n_d};
-    const uint64_t strides[3] = {(uint64_t)P.dim * 2, 128, (uint64_t)P.Ld * P.dim * 2};
+    const uint64_t dims[4] = {64, d_rows, (uint64_t)L.kblocks, d_count};
+    const uint64_t strides[3] = {(uint64_t)P.dim * 2, 128, d_rows * P.dim * 2};
     const uint32_t box[4] = {64, 16, 1, 1};
     if (int rc = encode_tensor_map(&td16, tdt, 4, P.d, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B,
                                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B))
@@ -435,11 +451,16 @@ int maxsim_qm_launch(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cu
   *handled = true;
   const int grid = (int)std::min<int64_t>(dev.sm_count, P.n_pairs);
   const int nch = L.tn / 64;
+  if (P.doc_offsets) {   // store mode never asks for argmax
+    if (P.argmax) { *handled = false; return MMB200_OK; }
+    return dtype == MMB200_F16 ? launch_qm<__half, false, true>(nch, grid, smem_bytes, stream, tq, td, td16, P, L)
+                               : launch_qm<__nv_bfloat16, false, true>(nch, grid, smem_bytes, stream, tq, td, td16, P, L);
+  }
   if (dtype == MMB200_F16)
-    return P.argmax ? launch_qm<__half, true>(nch, grid, smem_bytes, stream, tq, td, td16, P, L)
-                    : launch_qm<__half, false>(nch, grid, smem_bytes, stream, tq, td, td16, P, L);
-  return P.argmax ? launch_qm<__nv_bfloat16, true>(nch, grid, smem_bytes, stream, tq, td, td16, P, L)
-                  : launch_qm<__nv_bfloat16, false>(nch, grid, smem_bytes, stream, tq, td, td16, P, L);
+    return P.argmax ? launch_qm<__half, true, false>(nch, grid, smem_bytes, stream, tq, td, td16, P, L)
+                    : launch_qm<__half, false, false>(nch, grid, smem_bytes, stream, tq, td, td16, P, L);
+  return P.argmax ? launch_qm<__nv_bfloat16, true, false>(nch, grid, smem_bytes, stream, tq, td, td16, P, L)
+                  : launch_qm<__nv_bfloat16, false, false>(nch, grid, smem_bytes, stream, tq, td, td16, P, L);
 }
 
 }  // namespace mmb

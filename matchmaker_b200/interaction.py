@@ -480,6 +480,59 @@ def topk_merge(cand_scores: torch.Tensor, cand_ids: torch.Tensor, k: int) -> Tup
     return out_s, out_i
 
 
+TOPK_UNIQUE_MAX_K = 4096
+
+
+def topk_unique(cand_scores: torch.Tensor, cand_ids: torch.Tensor, k: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Per-query de-duplication + top-k of candidate lists [nq, L]: the k best DISTINCT ids, each with its highest
+    score, under (score desc, id asc).  Void candidates (score NaN / -inf / -FLT_MAX) are dropped; missing results are
+    (-FLT_MAX, -1).  1 <= k <= 4096."""
+    dev = _require_cuda(cand_scores, cand_ids)
+    cand_scores = cand_scores.to(torch.float32).contiguous()
+    cand_ids = cand_ids.to(torch.int64).contiguous()
+    nq, L = cand_scores.shape
+    if tuple(cand_ids.shape) != (nq, L):
+        raise _lib.MatchmakerB200Error(f"topk_unique: scores {tuple(cand_scores.shape)} vs ids {tuple(cand_ids.shape)}")
+    out_s = torch.empty((nq, k), dtype=torch.float32, device=dev)
+    out_i = torch.empty((nq, k), dtype=torch.int64, device=dev)
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        rc = lib.mmb200_topk_unique(_ptr(cand_scores), _ptr(cand_ids), _ptr(out_s), _ptr(out_i), nq, L, k, _stream(dev))
+    _lib.check(rc, "mmb200_topk_unique")
+    return out_s, out_i
+
+
+def maxsim_store(q: torch.Tensor, store: torch.Tensor, doc_offsets: torch.Tensor, pair_q: torch.Tensor,
+                 pair_d: torch.Tensor, max_doc_len: int, impl: str = "auto") -> torch.Tensor:
+    """ColBERT max-sim against a ragged token store, fp32 [n_pairs] (colbert.py:100-112, no masks).
+
+    store [n_rows, dim]; passage d is rows ``doc_offsets[d] : doc_offsets[d+1]`` (int64 [n_docs+1], non-decreasing,
+    at most ``max_doc_len`` rows read).  Pair p scores query ``pair_q[p]`` of q [n_q, Lq, dim] against passage
+    ``pair_d[p]``; ``pair_d[p] < 0`` and passages without rows score -inf.  Same kernels and bit-identical scores as
+    :func:`maxsim` on the passages padded to ``max_doc_len`` with a mask."""
+    dev = _require_cuda(q, store, doc_offsets, pair_q, pair_d)
+    if q.dtype != store.dtype or q.dtype not in _DTYPES:
+        raise _lib.MatchmakerB200Error(f"q/store must share a dtype in fp16/bf16/fp32, got {q.dtype}, {store.dtype}")
+    if q.dim() != 3 or store.dim() != 2 or q.shape[-1] != store.shape[-1]:
+        raise _lib.MatchmakerB200Error(f"expected q [n_q,Lq,dim], store [n_rows,dim]; got {tuple(q.shape)}, "
+                                       f"{tuple(store.shape)}")
+    q, store = q.contiguous(), store.contiguous()
+    doc_offsets = doc_offsets.to(torch.int64).contiguous()
+    pair_q = pair_q.to(torch.int32).contiguous().view(-1)
+    pair_d = pair_d.to(torch.int32).contiguous().view(-1)
+    if pair_q.numel() != pair_d.numel():
+        raise _lib.MatchmakerB200Error("pair_q / pair_d length mismatch")
+    n_q, Lq, dim = q.shape
+    out = torch.empty(pair_q.numel(), dtype=torch.float32, device=dev)
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        rc = lib.mmb200_maxsim_store_fwd(_ptr(q), _ptr(store), _ptr(doc_offsets), _ptr(pair_q), _ptr(pair_d), _ptr(out),
+                                         n_q, store.shape[0], doc_offsets.numel() - 1, pair_q.numel(), Lq, int(max_doc_len),
+                                         dim, _DTYPES[q.dtype], _IMPLS[impl], _stream(dev))
+    _lib.check(rc, "mmb200_maxsim_store_fwd")
+    return out
+
+
 def _tkl_slot_map(packed_indices: torch.Tensor) -> torch.Tensor:
     """Packed index of every chunk slot (-1 = dropped by the packing), one kernel launch (mmb200_tkl_slot_map)."""
     pk = packed_indices.reshape(-1)

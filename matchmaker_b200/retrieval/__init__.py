@@ -3,3 +3,4 @@
 from .base_index import BaseNNIndexer  # noqa: F401
 from .flat_ip_index import FlatIPIndexer  # noqa: F401
 from .colbert_rerank import ColBERTTokenIndex  # noqa: F401
+from .colbert_e2e import ColBERTEndToEndIndexer  # noqa: F401

@@ -1,0 +1,171 @@
+"""Exact (brute-force) ColBERT end-to-end retrieval over the encoded token store.
+
+The ColBERT paper's two-stage search with exact token search in place of its approximate index:
+
+1. candidate generation -- every live query token is searched against all token rows of the store (``flat_ip_topk``,
+   the rows' passage ids as ids), keeping its ``token_top_k`` best rows; the candidate passages of a query are the
+   union of those rows' passages (``topk_unique``);
+2. exact scoring -- the query against each candidate with ``forward_aggregation`` semantics (colbert.py:100-112):
+   sum over query tokens of the max over the passage's stored rows (``maxsim_store``, no padding in HBM);
+3. ranking -- the ``top_n`` best per query under (score desc, id asc), merged across ranks.
+
+Everything is enqueued on the current stream without a host synchronisation between the stages.  Candidate lists
+have a static width ``C = min(Lq * token_top_k, 4096)`` with void entries.  Candidate cap: the candidate set is the
+exact union of the token hits whenever ``Lq * token_top_k <= 4096``; beyond that, the 4096 distinct passages with the
+highest single-token score (ties by passage id) are kept.
+
+The store is what the reference's encode loop writes (``token_reps_N.npy`` + ``doc_infos.npz``, read by
+``token_storage.load_token_storage``): each passage keeps only its real token rows (dense_retrieval.py:244), and the
+``id_mapping`` value of a row is its passage's position in ``seq_ids`` -- which is also the id this index returns.
+Multi-GPU: one process per GPU, each rank owns a contiguous range of whole passages (``sharding.passage_shard_bounds``)
+and the per-rank top lists are merged with ``sharding.all_gather_merge``.
+"""
+from __future__ import annotations
+
+from typing import List, Optional
+
+import numpy
+import torch
+
+from .. import _lib, interaction, sharding
+from .base_index import BaseNNIndexer
+
+CANDIDATE_CAP = 4096          # candidate passages per query and rank (the topk_unique limit)
+_VOID_SCORE = -3.4028234663852886e38
+
+
+def doc_offsets_from_id_mapping(id_mapping: List[numpy.ndarray]) -> numpy.ndarray:
+    """Row offsets [n_docs + 1] of the passages of a token store from its per-block ``id_mapping`` (row -> passage
+    position in ``seq_ids``): passage d is rows [off[d], off[d+1]), n_docs = 1 + the largest position.  Passages whose
+    rows were all stripped get an empty range.  Raises on a mapping that is not non-decreasing (the reference's writer
+    appends passages in order, so anything else is malformed input)."""
+    rows = numpy.concatenate([numpy.asarray(x, dtype=numpy.int64).reshape(-1) for x in id_mapping]) if id_mapping \
+        else numpy.zeros(0, dtype=numpy.int64)
+    if rows.size and (rows[0] < 0 or (numpy.diff(rows) < 0).any()):
+        raise _lib.MatchmakerB200Error("id_mapping must be non-negative and non-decreasing over the concatenated blocks "
+                                       "(rows of one passage are contiguous, passages in seq_ids order)")
+    n_docs = int(rows[-1]) + 1 if rows.size else 0
+    return numpy.searchsorted(rows, numpy.arange(n_docs + 1, dtype=numpy.int64), side="left").astype(numpy.int64)
+
+
+class ColBERTEndToEndIndexer(BaseNNIndexer):
+    def __init__(self, config, device: Optional[torch.device] = None, process_group=None):
+        super().__init__(config)
+        if not self.use_gpu:
+            raise _lib.MatchmakerB200Error("ColBERTEndToEndIndexer runs on the GPU only (faiss_use_gpu must be True); "
+                                           "there is no CPU fallback")
+        self.store_dtype = torch.float16 if self.use_fp16 else torch.float32
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        self.group = process_group
+        self.store: Optional[torch.Tensor] = None       # [rows of this rank, dim] in store_dtype
+        self.flat: Optional[torch.Tensor] = None        # what flat_ip_topk reads (the fp16 hi / lo split for fp32)
+        self.split_scale = None
+        self.row_ids: Optional[torch.Tensor] = None     # [rows] int64 passage id (seq_ids position) of every row
+        self.offsets: Optional[torch.Tensor] = None     # [passages of this rank + 1] int64, local row offsets
+        self.max_doc_len = 1
+        self.d_lo = self.d_hi = 0
+        self.n_docs = 0
+
+    def _world(self):
+        import torch.distributed as dist
+        if dist.is_available() and dist.is_initialized():
+            return dist.get_rank(self.group), dist.get_world_size(self.group)
+        return 0, 1
+
+    def index(self, id_mapping: List[numpy.ndarray], storage: List[numpy.ndarray]):
+        """id_mapping, storage: the first two results of ``token_storage.load_token_storage`` (per-block row -> passage
+        position arrays, and the [rows, token_dim] blocks).  Every rank is given the same lists and keeps its passage
+        range; its rows reach HBM through ``token_storage.blocks_to_device``."""
+        from .token_storage import blocks_to_device
+        if len(id_mapping) != len(storage) or any(len(a) != len(b) for a, b in zip(id_mapping, storage)):
+            raise _lib.MatchmakerB200Error("id_mapping and storage must have one entry per stored row, block by block")
+        if storage and storage[0].shape[1] != self.token_dim:
+            raise _lib.MatchmakerB200Error(f"storage rows have dim {storage[0].shape[1]}, config token_dim is "
+                                           f"{self.token_dim}")
+        off = doc_offsets_from_id_mapping(id_mapping)
+        rank, world = self._world()
+        self.n_docs = len(off) - 1
+        d_lo, d_hi, r_lo, r_hi = sharding.passage_shard_bounds(off, rank, world) if self.n_docs else (0, 0, 0, 0)
+        self.d_lo, self.d_hi = d_lo, d_hi
+        if r_hi > r_lo:
+            with torch.cuda.device(self.device):
+                rows = blocks_to_device(storage, r_lo, r_hi, self.device)
+            self.index_device(rows, off[d_lo:d_hi + 1] - r_lo, d_lo)
+        else:
+            self.store = torch.empty((0, self.token_dim), dtype=self.store_dtype, device=self.device)
+            self.flat, self.offsets, self.row_ids = self.store, None, None
+
+    def index_device(self, rows: torch.Tensor, doc_offsets: numpy.ndarray, first_doc: int = 0):
+        """Index this rank's passages from a device tensor: rows [n_rows, token_dim]; passage first_doc + d is rows
+        [doc_offsets[d], doc_offsets[d+1]) (int64 [n + 1], non-decreasing, from 0 to n_rows)."""
+        off = numpy.asarray(doc_offsets, dtype=numpy.int64)
+        if rows.dim() != 2 or rows.shape[1] != self.token_dim or off[0] != 0 or off[-1] != rows.shape[0] or \
+                (numpy.diff(off) < 0).any():
+            raise _lib.MatchmakerB200Error("index_device: rows [n_rows, token_dim] and non-decreasing offsets from 0")
+        self.store = rows.to(self.device, self.store_dtype)
+        if self.store_dtype == torch.float16:
+            self.flat, self.split_scale = self.store, None
+        else:
+            self.flat, self.split_scale = interaction.flat_ip_split_f32(self.store, "passages")
+        lens = torch.from_numpy(numpy.diff(off)).to(self.device)
+        self.offsets = torch.from_numpy(off).to(self.device)
+        self.max_doc_len = max(1, int(numpy.diff(off).max())) if len(off) > 1 else 1
+        self.row_ids = torch.repeat_interleave(torch.arange(first_doc, first_doc + len(off) - 1, device=self.device), lens)
+        self.d_lo, self.d_hi = first_doc, first_doc + len(off) - 1
+
+    def search(self, query_vec: numpy.ndarray, top_n: int, token_top_k: Optional[int] = None):
+        """query_vec [Nq, Lq, dim] (the query_encode output of ColBERT.forward_representation: padded tokens are
+        all-zero rows).  Returns (scores [Nq, top_n] f32, ids [Nq, top_n] i64): ids are positions in ``seq_ids``,
+        missing results (-3.4028235e38, -1)."""
+        if self.store is None:
+            raise _lib.MatchmakerB200Error("search() before index()")
+        q = torch.from_numpy(numpy.ascontiguousarray(query_vec))
+        if q.dim() == 2:
+            q = q.unsqueeze(0)
+        scores, ids = self.search_device(q.to(self.device), top_n, token_top_k)
+        return scores.cpu().numpy(), ids.cpu().numpy()
+
+    def search_device(self, q: torch.Tensor, top_n: int, token_top_k: Optional[int] = None):
+        """search() with device tensors in and out.  token_top_k (k') defaults to min(top_n, 1024)."""
+        if self.store is None:
+            raise _lib.MatchmakerB200Error("search() before index()")
+        if q.dim() != 3 or q.shape[-1] != self.token_dim:
+            raise _lib.MatchmakerB200Error(f"expected queries [Nq, Lq, {self.token_dim}], got {tuple(q.shape)}")
+        kp = min(top_n, interaction.FLAT_IP_MAX_K) if token_top_k is None else int(token_top_k)
+        if not 1 <= kp <= interaction.FLAT_IP_MAX_K:
+            raise _lib.MatchmakerB200Error(f"token_top_k must be in [1, {interaction.FLAT_IP_MAX_K}], got {kp}")
+        if not 1 <= top_n <= CANDIDATE_CAP:
+            raise _lib.MatchmakerB200Error(f"top_n must be in [1, {CANDIDATE_CAP}], got {top_n}")
+        rank, world = self._world()
+        nq, lq, dim = q.shape
+        q = q.to(self.device, self.store_dtype).contiguous()
+        if self.store.shape[0] == 0:
+            s = torch.full((nq, top_n), _VOID_SCORE, device=self.device)
+            i = torch.full((nq, top_n), -1, dtype=torch.int64, device=self.device)
+        else:
+            s, i = self._search_local(q, top_n, kp)
+        if world > 1:
+            s, i = sharding.all_gather_merge(s, i, top_n, self.group)
+        return s, i
+
+    def candidates_device(self, q: torch.Tensor, kp: int):
+        """Stage 1 on this rank: (best single-token score, passage id) [Nq, C] of every candidate passage, best first;
+        void entries are (-3.4028235e38, -1).  q [Nq, Lq, dim] in the store dtype on the device."""
+        nq, lq, dim = q.shape
+        toks = q.reshape(nq * lq, dim)
+        # token hits -> passage ids; all-zero query rows are padding and their hits are voided
+        hs, hi = interaction.flat_ip_topk(toks, self.flat, kp, ids=self.row_ids, split_scale=self.split_scale)
+        pad = (toks == 0).all(dim=1, keepdim=True)
+        hs = hs.masked_fill(pad, float("-inf"))
+        c = min(lq * kp, CANDIDATE_CAP)
+        return interaction.topk_unique(hs.view(nq, lq * kp), hi.view(nq, lq * kp), c)
+
+    def _search_local(self, q: torch.Tensor, top_n: int, kp: int):
+        nq = q.shape[0]
+        _, cand = self.candidates_device(q, kp)
+        c = cand.shape[1]
+        # stage 2: exact max-sim of every candidate; void candidates (id -1) are skipped and score -inf
+        pair_d = torch.where(cand >= 0, cand - self.d_lo, torch.full_like(cand, -1))
+        pair_q = torch.arange(nq, device=self.device, dtype=torch.int32).repeat_interleave(c)
+        scores = interaction.maxsim_store(q, self.store, self.offsets, pair_q, pair_d, self.max_doc_len).view(nq, c)
+        return interaction.topk_merge(scores, cand, top_n)

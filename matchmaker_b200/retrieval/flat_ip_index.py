@@ -99,6 +99,21 @@ class FlatIPIndexer(BaseNNIndexer):
             s, i = sharding.all_gather_merge(s, i, top_n, self.group)
         return s, i
 
+    def search_unique(self, query_vec: numpy.ndarray, top_n: int, index_hit_top_n: int):
+        """The ``maxP->bert_dot`` aggregation (dense_retrieval.py:414-427): search ``index_hit_top_n`` vector hits and
+        keep the ``top_n`` best distinct ids, each at its best hit's score -- on the device, after the cross-rank merge,
+        so a passage whose vectors straddle two ranks is still counted once.  Missing results are
+        (-3.4028235e38, -1)."""
+        if self.passages is None:
+            raise _lib.MatchmakerB200Error("search() before index()")
+        if query_vec.ndim == 1:
+            query_vec = query_vec[numpy.newaxis, :]
+        q = torch.from_numpy(numpy.ascontiguousarray(query_vec)).to(
+            self.device, dtype=torch.float16 if self.store_dtype == torch.float16 else torch.float32)
+        s, i = self.search_device(q, index_hit_top_n)
+        s, i = interaction.topk_unique(s, i, top_n)
+        return s.cpu().numpy(), i.cpu().numpy()
+
     def _shard_path(self, path: str) -> str:
         rank, world = self._world()
         return path if world == 1 else f"{path}.rank{rank}of{world}"

@@ -22,6 +22,24 @@ def shard_bounds(n_items: int, rank: int, world: int) -> Tuple[int, int]:
     return lo, lo + per + (1 if rank < rem else 0)
 
 
+def passage_shard_bounds(doc_offsets, rank: int, world: int) -> Tuple[int, int, int, int]:
+    """Passage-aligned split of a ragged token store: passage d owns rows [doc_offsets[d], doc_offsets[d+1]).
+    Returns (first passage, end passage, first row, end row) of rank `rank`.  Every passage lands on exactly one rank
+    and rank r's range starts at the first passage that begins at or after row shard_bounds(n_rows, r, world)[0], so
+    row ranges are contiguous, cover every row and are balanced up to one passage; a rank may get no passage."""
+    import numpy as np
+    off = np.asarray(doc_offsets, dtype=np.int64).reshape(-1)
+    n_docs, n_rows = len(off) - 1, int(off[-1])
+
+    def start(r: int) -> int:
+        if r >= world:
+            return n_docs
+        return int(min(n_docs, np.searchsorted(off, shard_bounds(n_rows, r, world)[0], side="left")))
+
+    d_lo, d_hi = start(rank), start(rank + 1)
+    return d_lo, d_hi, int(off[d_lo]), int(off[d_hi])
+
+
 def rank_topk(scores: torch.Tensor, ids: torch.Tensor, k: int) -> Tuple[torch.Tensor, torch.Tensor]:
     """Top-k per row under the project-wide total order (score descending, id ascending).
     scores [Nq, n] f32, ids [Nq, n] or [n] i64."""
