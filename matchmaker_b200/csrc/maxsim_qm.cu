@@ -13,12 +13,17 @@
 // that row: 0 for real tokens, -inf for padding and for the tile's rows past Ld, so masked rows can never win the max.
 // The reference's -1000 fill (matchmaker/models/colbert.py:69) only matters when it IS the max; that is reproduced
 // exactly by one "virtual" document row (the last row of the last tile, index >= Ld, zero data from TMA out-of-bounds
-// fill) whose penalty is -1000 when the document has at least one masked position and -inf otherwise.  A helper warp
-// writes the penalty row per document tile while TMA streams the token vectors.
+// fill) whose penalty is -1000 when the document has at least one masked position and -inf otherwise.  Two helper warps
+// write the penalty row per document tile while TMA streams the token vectors.
+//
+// Nothing on a warp's per-document path waits for a global load: the per-pair indices and lengths arrive 32 pairs at a
+// time, a batch ahead (PairStream; the consumers, which only need the query, keep just a batch of pair_q), and the
+// penalty writers keep the mask words of their next two tiles in flight.  setmaxnreg moves registers from the helper
+// warpgroup to the consumers, whose accumulators are the kernel's register peak.
 //
 // Per CTA (persistent, one per SM, 384 threads = 3 warpgroups):
 //   warp 0        TMA producer: query tile (2-slot ring, re-fetched when the query changes), document tiles
-//   warp 1        penalty writer
+//   warps 1, 2    penalty writers, warp 1 + c for consumer warpgroup c's documents
 //   warpgroups 1, 2  consumers: warpgroup c takes the CTA's documents c, c + 2, ...; per tile 4 * dim / 64 * TN / 64
 //                 wgmma m64n64k16 into registers, then the masked max over the tile in the same registers.  While one
 //                 warpgroup reduces, the other one's MMAs run.  Each warpgroup has its own half of the stage ring, so
@@ -43,6 +48,9 @@ constexpr int kMaxStages = 8;                // even: half of the ring per consu
 constexpr int kQSlots = 2;
 constexpr int kQRows = 32;
 constexpr int kQBlockBytes = kQRows * 128;   // one k-block of the query tile (4 KB)
+// setmaxnreg budgets: the helper warpgroup (producer, penalty writers) gives registers to the two consumer warpgroups, whose
+// NCH x 32 accumulators are the kernel's register peak.  128 x 104 + 256 x 200 = 384 x 168 (the launch).
+constexpr int kRegsHelper = 104, kRegsConsumer = 200;
 
 struct QmShared {
   uint64_t full[kMaxStages];   // 2 arrivals: TMA producer (with tx bytes) + penalty writer
@@ -61,10 +69,76 @@ struct QmLaunch {
   int32_t stage_bytes;  // doc_bytes + penalty row (tn fp32, rounded to 1 KB)
 };
 
-__device__ __forceinline__ int64_t pair_dmask_row_of(const MaxsimParams& P, int64_t p) {
-  if (P.pair_dmask) return (int64_t)P.pair_dmask[p];
-  return P.pair_d ? (int64_t)P.pair_d[p] : p;
-}
+// One warp's own sequence of pairs p = first, first + step, ... < end and what the warp needs of each: its query, its
+// document, its document-mask row, and (ragged fetch, store mode) its first row and the rows worth fetching.  Lane l
+// holds element l of a batch of 32.  A batch's index arrays are read with one coalesced load per array two batches
+// ahead of use, store mode's doc_offsets of those documents one batch ahead, and elements are handed out by
+// __shfl_sync: the warp never waits on a per-pair global load.  Every lane of the warp calls next() and the accessors
+// together.
+template <bool kStore>
+struct PairStream {
+  // Indices are int32 like the pair arrays of the C ABI; the implicit document index p (< n_pairs <= n_d) is one too:
+  // it becomes the TMA box's int32 document coordinate, and the mask row index is widened to int64 before it is scaled.
+  struct Batch {
+    int32_t q, d, dm, rows;
+    int64_t row0, row_end;   // store mode: [doc_offsets[d], doc_offsets[d + 1])
+  };
+  const MaxsimParams& P;
+  int64_t first, end, step;
+  int64_t pre_batch;   // batch index held in `pre`
+  int k;               // current element of `cur` (-1 before the first next())
+  int lane;
+  Batch cur, nxt, pre;   // cur: resolved; nxt: second-level loads in flight; pre: first-level loads in flight
+
+  __device__ __forceinline__ PairStream(const MaxsimParams& P_, int64_t first_, int64_t end_, int64_t step_, int lane_)
+      : P(P_), first(first_), end(end_), step(step_), lane(lane_) {
+    load1(cur, 0);
+    load1(nxt, 1);
+    load2(cur);
+    load2(nxt);
+    resolve(cur);
+    pre_batch = 2;
+    load1(pre, pre_batch);
+    k = -1;
+  }
+  // indices: pair_q / pair_d / pair_dmask / rows_needed of this lane's pair
+  __device__ __forceinline__ void load1(Batch& b, int64_t bi) {
+    const int64_t p = first + (bi * 32 + lane) * step;
+    b.q = 0; b.d = -1; b.dm = 0; b.rows = 0; b.row0 = 0; b.row_end = 0;
+    if (p >= end) return;
+    b.q = P.pair_q ? P.pair_q[p] : (int32_t)((p + P.pair_base) / P.docs_per_query);
+    b.d = P.pair_d ? P.pair_d[p] : (int32_t)p;
+    if (P.pair_dmask) b.dm = P.pair_dmask[p];
+    if (!kStore && P.rows_needed) b.rows = P.rows_needed[p];   // ragged fetch has no pair_d: the document is p
+  }
+  // what depends on the indices (waits for load1's results)
+  __device__ __forceinline__ void load2(Batch& b) {
+    if (!P.pair_dmask) b.dm = b.d;
+    if constexpr (kStore) {
+      if (b.d >= 0) { b.row0 = P.doc_offsets[b.d]; b.row_end = P.doc_offsets[b.d + 1]; }
+    }
+  }
+  __device__ __forceinline__ void resolve(Batch& b) {
+    if constexpr (kStore) b.rows = (int)max((int64_t)0, min(b.row_end - b.row0, (int64_t)P.Ld));   // 0 for d < 0
+  }
+  // moves to the next pair of the sequence; the accessors below read the current one (a shuffle each: a role shuffles
+  // only what it uses, so the loads of the rest are dead code)
+  __device__ __forceinline__ void next() {
+    if (++k == 32) {   // the loads waited for here were issued one batch ago
+      cur = nxt;
+      resolve(cur);
+      nxt = pre;
+      load2(nxt);
+      load1(pre, ++pre_batch);
+      k = 0;
+    }
+  }
+  __device__ __forceinline__ int64_t q() const { return __shfl_sync(0xffffffffu, cur.q, k); }
+  __device__ __forceinline__ int64_t d() const { return __shfl_sync(0xffffffffu, cur.d, k); }
+  __device__ __forceinline__ int64_t dm() const { return __shfl_sync(0xffffffffu, cur.dm, k); }
+  __device__ __forceinline__ int rows() const { return __shfl_sync(0xffffffffu, cur.rows, k); }
+  __device__ __forceinline__ int64_t row0() const { return __shfl_sync(0xffffffffu, cur.row0, k); }
+};
 
 template <typename T>
 __device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc);
@@ -130,16 +204,24 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   }
   __syncthreads();
 
+  // every role branch starts with its setmaxnreg so that ptxas allocates each branch against its own budget
   if (warp == 0) {
+    setmaxnreg_dec<kRegsHelper>();
     // ------------------------------- TMA producer -------------------------------
-    if (lane == 0) {
-      const int ring = L.stages >> 1;
-      int64_t seq0 = 0, seq1 = 0;   // tiles filled so far into each warpgroup's half of the ring
-      int64_t prev_q = -1;
-      uint32_t qcount = 0;
-      for (int64_t p = p_begin; p < p_end; ++p) {
-        const int64_t qi = P.pair_q ? (int64_t)P.pair_q[p] : (p + P.pair_base) / P.docs_per_query;
-        const int64_t di = P.pair_d ? (int64_t)P.pair_d[p] : p;
+    // the whole warp walks the pairs (it shares out their metadata); lane 0 waits on the barriers and issues the TMA
+    PairStream<kStore> meta(P, p_begin, p_end, 1, lane);
+    const int ring = L.stages >> 1;
+    int64_t seq0 = 0, seq1 = 0;   // tiles filled so far into each warpgroup's half of the ring
+    int64_t prev_q = -1;
+    uint32_t qcount = 0;
+    for (int64_t p = p_begin; p < p_end; ++p) {
+      meta.next();
+      const int64_t qi = meta.q();
+      const int64_t di = meta.d();
+      // store mode: the passage's rows start at row `row0` of the [n_rows, dim] store (tensor-map dim 3 has extent 1)
+      const int64_t row0 = kStore ? meta.row0() : 0;
+      const int need_rows = meta.rows();
+      if (lane == 0) {
         if (qi != prev_q) {
           const uint32_t slot = qcount & 1u, use = qcount >> 1;
           mbar_wait(&S->qempty[slot], (use & 1u) ^ 1u);
@@ -150,11 +232,6 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
           ++qcount;
           prev_q = qi;
         }
-        // store mode: the passage's rows start at row `row0` of the [n_rows, dim] store (tensor-map dim 3 has extent 1)
-        int64_t row0 = 0;
-        int need_rows = 0;
-        if constexpr (kStore) need_rows = store_doc_rows(P, di, &row0);
-        else if (P.rows_needed) need_rows = P.rows_needed[di];
         const int dcoord = kStore ? 0 : (int)di;
         const int c = (int)((p - p_begin) & 1);
         for (int t = 0; t < L.tiles; ++t) {
@@ -183,67 +260,86 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
           }
         }
       }
+      __syncwarp();
     }
-  } else if (warp == 1) {
-    // ------------------------------- penalty writer -----------------------------
+  } else if (warp == 1 || warp == 2) {
+    setmaxnreg_dec<kRegsHelper>();
+    // ------------------------------- penalty writers -----------------------------
+    // writer c fills the penalty rows of consumer warpgroup c's half of the ring (pairs p_begin + c, + 2, ...), so every
+    // stage has one writer that sees its uses in order (a second writer could pass a parity wait one phase early).  The
+    // mask words of the writer's next two tiles (four documents of the CTA at one tile per document) are in flight in
+    // two register sets that take turns; a copy between them would wait for the load.
+    constexpr int kW = 2 * NCH;          // rows of a tile per lane (TN = 64 NCH)
+    const int c = warp - 1;
     const int dmt = P.d_mask ? P.mask_dtype : MMB200_MASK_NONE;
     const int ring = L.stages >> 1;
-    int64_t seq0 = 0, seq1 = 0;
-    uint64_t raw[8], raw_next[8];
-    auto fetch = [&](int64_t p, int t, uint64_t (&dst)[8]) {
-#pragma unroll
-      for (int k = 0; k < 8; ++k) {
-        const int r = lane + 32 * k, g = t * L.tn + r;
-        dst[k] = 1;
-        if (dmt != MMB200_MASK_NONE && p < p_end && r < L.tn && g < P.Ld)
-          dst[k] = mask_raw(P.d_mask, dmt, pair_dmask_row_of(P, p) * (int64_t)P.Ld + g);
+    PairStream<kStore> meta(P, p_begin + c, p_end, 2, lane);
+    int64_t seq = 0;                    // tiles written into this half of the ring
+    int64_t wp = p_begin + c;           // pair and tile being written
+    int wt = 0;
+    bool any_masked = false;
+    int64_t fp = wp;                    // pair and tile being fetched
+    int ft = 0;
+    int64_t f_dm = 0;                   // mask row and row limit of pair fp
+    int f_lim = 0;
+    auto fetch = [&](uint64_t (&raw)[kW], int& lim) {
+      if (fp < p_end && ft == 0) {
+        meta.next();
+        f_dm = meta.dm();
+        f_lim = kStore ? meta.rows() : P.Ld;   // store mode: the passage's length, 0 for a skipped pair
       }
+#pragma unroll
+      for (int k = 0; k < kW; ++k) {
+        const int r = lane + 32 * k, g = ft * L.tn + r;
+        raw[k] = 1;
+        if (dmt != MMB200_MASK_NONE && fp < p_end && r < L.tn && g < P.Ld)
+          raw[k] = mask_raw(P.d_mask, dmt, f_dm * (int64_t)P.Ld + g);
+      }
+      lim = f_lim;
+      if (++ft == L.tiles) { ft = 0; fp += 2; }
     };
-    fetch(p_begin, 0, raw_next);
-    for (int64_t p = p_begin; p < p_end; ++p) {
-      bool any_masked = false;
-      int lim = P.Ld;   // rows of this document; store mode: the passage's length, 0 for a skipped pair
-      if constexpr (kStore) {
-        int64_t row0;
-        lim = store_doc_rows(P, P.pair_d ? (int64_t)P.pair_d[p] : p, &row0);
+    auto write = [&](const uint64_t (&raw)[kW], int lim) {
+      float pen[kW];
+      bool masked_here = false;
+#pragma unroll
+      for (int k = 0; k < kW; ++k) {
+        const int r = lane + 32 * k, g = wt * L.tn + r;
+        const bool in_doc = r < L.tn && g < lim;
+        const bool ok = in_doc && mask_test(raw[k], dmt);
+        masked_here |= in_doc && !ok;
+        pen[k] = ok ? 0.f : -INFINITY;
       }
-      for (int t = 0; t < L.tiles; ++t) {
+      any_masked |= __any_sync(0xffffffffu, masked_here);
+      const int stage = c * ring + (int)(seq % ring);
+      const uint32_t phase = (uint32_t)((seq / ring) & 1);
+      ++seq;
+      mbar_wait(&S->empty[stage], phase ^ 1u);
+      float* pt = reinterpret_cast<float*>(stage_base + (size_t)stage * L.stage_bytes + L.doc_bytes);
 #pragma unroll
-        for (int k = 0; k < 8; ++k) raw[k] = raw_next[k];
-        {  // prefetch the mask words of the next tile
-          int nt = t + 1;
-          int64_t np = p;
-          if (nt == L.tiles) { nt = 0; ++np; }
-          fetch(np, nt, raw_next);
-        }
-        float pen[8];
-        bool masked_here = false;
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const int r = lane + 32 * k, g = t * L.tn + r;
-          const bool in_doc = r < L.tn && g < lim;
-          const bool ok = in_doc && mask_test(raw[k], dmt);
-          masked_here |= in_doc && !ok;
-          pen[k] = ok ? 0.f : -INFINITY;
-        }
-        any_masked |= __any_sync(0xffffffffu, masked_here);
-        const int c = (int)((p - p_begin) & 1);
-        const int64_t j = c ? seq1++ : seq0++;
-        const int stage = c * ring + (int)(j % ring);
-        const uint32_t phase = (uint32_t)((j / ring) & 1);
-        mbar_wait(&S->empty[stage], phase ^ 1u);
-        float* pt = reinterpret_cast<float*>(stage_base + (size_t)stage * L.stage_bytes + L.doc_bytes);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const int r = lane + 32 * k, g = t * L.tn + r;
-          // the virtual -1000 row exists only in the masked (padded) layout
-          if (r < L.tn) pt[r] = (!kStore && g == L.tiles * L.tn - 1) ? (any_masked ? -1000.f : -INFINITY) : pen[k];
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&S->full[stage]);
+      for (int k = 0; k < kW; ++k) {
+        const int r = lane + 32 * k, g = wt * L.tn + r;
+        // the virtual -1000 row exists only in the masked (padded) layout
+        if (r < L.tn) pt[r] = (!kStore && g == L.tiles * L.tn - 1) ? (any_masked ? -1000.f : -INFINITY) : pen[k];
       }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&S->full[stage]);
+      if (++wt == L.tiles) { wt = 0; wp += 2; any_masked = false; }
+    };
+    uint64_t ra[kW], rb[kW];
+    int la, lb;
+    fetch(ra, la);
+    fetch(rb, lb);
+    while (wp < p_end) {
+      write(ra, la);
+      fetch(ra, la);
+      if (wp >= p_end) break;
+      write(rb, lb);
+      fetch(rb, lb);
     }
-  } else if (warp >= 4) {
+  } else if (warp == 3) {
+    setmaxnreg_dec<kRegsHelper>();   // idle: its registers go to the consumers
+  } else {
+    setmaxnreg_inc<kRegsConsumer>();
     // ------------------------------- consumers: wgmma + masked max ------------------------
     const int c = (warp >> 2) - 1;        // consumer warpgroup 0 / 1
     const int wq = warp & 3;              // warp inside the warpgroup: rows 16 wq .. 16 wq + 15
@@ -255,9 +351,20 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     int64_t prev_q = -1;
     uint32_t qcount = 0;
     int cur_slot = 0;
+    // pair_q mode: pair_q of this lane's pair in the current and the next batch of 32 pairs (one coalesced load per batch,
+    // a batch ahead of use); the consumers need nothing else per pair, so they carry no PairStream (register budget)
+    auto load_q = [&](int64_t n0) -> int32_t { return p_begin + n0 + lane < p_end ? P.pair_q[p_begin + n0 + lane] : 0; };
+    int32_t qb_cur = 0, qb_nxt = 0;
+    if (P.pair_q) { qb_cur = load_q(0); qb_nxt = load_q(32); }
     for (int64_t n = 0; p_begin + n < p_end; ++n) {
       const int64_t p = p_begin + n;
-      const int64_t qi = P.pair_q ? (int64_t)P.pair_q[p] : (p + P.pair_base) / P.docs_per_query;
+      int64_t qi;
+      if (P.pair_q) {
+        if ((n & 31) == 0 && n > 0) { qb_cur = qb_nxt; qb_nxt = load_q(n + 32); }
+        qi = __shfl_sync(0xffffffffu, qb_cur, (int)(n & 31));
+      } else {
+        qi = (p + P.pair_base) / P.docs_per_query;
+      }
       if (qi != prev_q) {
         // every MMA of this warpgroup that read the old query tile has completed (wgmma_wait below)
         if (prev_q >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&S->qempty[cur_slot]); }
@@ -268,6 +375,7 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
       }
       if ((int)(n & 1) != c) continue;
       const uint32_t qaddr = smem_u32(q_base + (size_t)cur_slot * qslot_bytes);
+      // query-mask words: first needed in the epilogue, after this document's MMAs (L1 hits after the query's first pair)
       uint64_t qraw0 = 0, qraw1 = 0;
       if (wq < 2) {
         if (r0 < P.Lq) qraw0 = (qmt != MMB200_MASK_NONE) ? mask_raw(P.q_mask, qmt, qi * (int64_t)P.Lq + r0) : 1;
