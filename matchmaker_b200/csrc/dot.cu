@@ -5,18 +5,10 @@
 
 #include <algorithm>
 
+#include "device_util.cuh"
 #include "host_util.cuh"
 
 namespace mmb {
-
-template <typename T>
-__device__ __forceinline__ float dot_to_f(T v);
-template <>
-__device__ __forceinline__ float dot_to_f<float>(float v) { return v; }
-template <>
-__device__ __forceinline__ float dot_to_f<__half>(__half v) { return __half2float(v); }
-template <>
-__device__ __forceinline__ float dot_to_f<__nv_bfloat16>(__nv_bfloat16 v) { return __bfloat162float(v); }
 
 template <typename T>
 __global__ void __launch_bounds__(256) dot_pairs_kernel(const T* __restrict__ q, const T* __restrict__ d,
@@ -38,10 +30,10 @@ __global__ void __launch_bounds__(256) dot_pairs_kernel(const T* __restrict__ q,
         const T* qe = reinterpret_cast<const T*>(&qa);
         const T* de = reinterpret_cast<const T*>(&da);
 #pragma unroll
-        for (int e = 0; e < VEC; ++e) acc = fmaf(dot_to_f(qe[e]), dot_to_f(de[e]), acc);
+        for (int e = 0; e < VEC; ++e) acc = fmaf(to_float(qe[e]), to_float(de[e]), acc);
       }
     } else {
-      for (int c = lane; c < dim; c += 32) acc = fmaf(dot_to_f(qr[c]), dot_to_f(dr[c]), acc);
+      for (int c = lane; c < dim; c += 32) acc = fmaf(to_float(qr[c]), to_float(dr[c]), acc);
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
@@ -59,17 +51,13 @@ extern "C" int mmb200_dot_pairs(const void* q, const void* d, float* out, int64_
   MMB_REQUIRE(dtype_size(dtype) != 0, "unknown dtype");
   if (B == 0) return MMB200_OK;
   DeviceInfo dev;
-  if (int rc = current_device_info(&dev)) return rc;
-  if (!is_sm90(dev)) {
-    set_error("matchmaker_b200 kernels are built for sm_90a only");
-    return MMB200_ERR_UNSUPPORTED;
-  }
+  if (int rc = require_sm90(&dev)) return rc;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const int grid = (int)std::min<int64_t>((B + 7) / 8, (int64_t)dev.sm_count * 8);
-  if (dtype == MMB200_F16) dot_pairs_kernel<__half><<<grid, 256, 0, stream>>>((const __half*)q, (const __half*)d, out, B, dim);
-  else if (dtype == MMB200_BF16)
-    dot_pairs_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>((const __nv_bfloat16*)q, (const __nv_bfloat16*)d, out, B, dim);
-  else dot_pairs_kernel<float><<<grid, 256, 0, stream>>>((const float*)q, (const float*)d, out, B, dim);
-  MMB_CHECK_CUDA(cudaGetLastError());
-  return MMB200_OK;
+  return dispatch_dtype(dtype, [&](auto t) {
+    using T = decltype(t);
+    dot_pairs_kernel<T><<<grid, 256, 0, stream>>>(static_cast<const T*>(q), static_cast<const T*>(d), out, B, dim);
+    MMB_CHECK_CUDA(cudaGetLastError());
+    return MMB200_OK;
+  });
 }

@@ -693,11 +693,7 @@ extern "C" int mmb200_flat_ip_topk(const void* queries, const void* passages, co
   MMB_REQUIRE(n_pass < (1ll << 32) - 512, "at most 2^32 passages per shard");
   MMB_REQUIRE(((reinterpret_cast<uintptr_t>(queries) | reinterpret_cast<uintptr_t>(passages)) & 15) == 0, "16-byte alignment");
   DeviceInfo dev;
-  if (int rc = current_device_info(&dev)) return rc;
-  if (!is_sm90(dev)) {
-    set_error("matchmaker_b200 kernels are built for sm_90a only");
-    return MMB200_ERR_UNSUPPORTED;
-  }
+  if (int rc = require_sm90(&dev)) return rc;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const Plan pl = make_plan(nq, n_pass, k, dev.sm_count);
   MMB_REQUIRE((size_t)workspace_bytes_given >= total_workspace_bytes(nq, n_pass, k, dev.sm_count),
@@ -785,11 +781,7 @@ extern "C" int mmb200_topk_merge(const float* cand_scores, const int64_t* cand_i
   MMB_REQUIRE(nq >= 0 && n_candidates >= 1 && k >= 1, "bad sizes");
   if (nq == 0) return MMB200_OK;
   DeviceInfo dev;
-  if (int rc = current_device_info(&dev)) return rc;
-  if (!is_sm90(dev)) {
-    set_error("matchmaker_b200 kernels are built for sm_90a only");
-    return MMB200_ERR_UNSUPPORTED;
-  }
+  if (int rc = require_sm90(&dev)) return rc;
   return launch_merge(cand_scores, cand_ids, nq, n_candidates, k, out_scores, out_ids, dev, static_cast<cudaStream_t>(stream_));
 }
 
@@ -805,11 +797,7 @@ extern "C" int mmb200_topk_unique(const float* cand_scores, const int64_t* cand_
   }
   if (nq == 0) return MMB200_OK;
   DeviceInfo dev;
-  if (int rc = current_device_info(&dev)) return rc;
-  if (!is_sm90(dev)) {
-    set_error("matchmaker_b200 kernels are built for sm_90a only");
-    return MMB200_ERR_UNSUPPORTED;
-  }
+  if (int rc = require_sm90(&dev)) return rc;
   return launch_merge(cand_scores, cand_ids, nq, n_candidates, k, out_scores, out_ids, dev, static_cast<cudaStream_t>(stream_),
                       true);
 }

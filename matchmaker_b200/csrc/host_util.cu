@@ -31,6 +31,16 @@ int current_device_info(DeviceInfo* out) {
   return MMB200_OK;
 }
 
+int require_sm90(DeviceInfo* dev) {
+  if (int rc = current_device_info(dev)) return rc;
+  if (!(dev->cc_major == 9 && dev->cc_minor == 0)) {
+    set_error("matchmaker_b200 kernels are built for sm_90a only; device is sm_" + std::to_string(dev->cc_major) +
+              std::to_string(dev->cc_minor));
+    return MMB200_ERR_UNSUPPORTED;
+  }
+  return MMB200_OK;
+}
+
 int encode_tensor_map(CUtensorMap* map, CUtensorMapDataType dtype, uint32_t rank, const void* base,
                       const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box,
                       CUtensorMapSwizzle swizzle, CUtensorMapL2promotion l2promo) {

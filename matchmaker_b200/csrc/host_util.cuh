@@ -3,6 +3,8 @@
 #pragma once
 
 #include <cuda.h>
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -43,8 +45,17 @@ struct DeviceInfo {
 // Properties of the current device (cached per device id).  Returns nonzero on failure.
 int current_device_info(DeviceInfo* out);
 
-// True when the current device can run the sm_90a wgmma/TMA kernels (sm_90a code loads on compute capability 9.0 only).
-inline bool is_sm90(const DeviceInfo& d) { return d.cc_major == 9 && d.cc_minor == 0; }
+// current_device_info, then MMB200_ERR_UNSUPPORTED unless the device can run the sm_90a wgmma / TMA kernels (sm_90a code
+// loads on compute capability 9.0 only).
+int require_sm90(DeviceInfo* dev);
+
+// f(T{}) with T the element type of `dtype`: __half, __nv_bfloat16 or float (any other dtype).
+template <class F>
+int dispatch_dtype(int dtype, F&& f) {
+  if (dtype == MMB200_F16) return f(__half{});
+  if (dtype == MMB200_BF16) return f(__nv_bfloat16{});
+  return f(float{});
+}
 
 // cuTensorMapEncodeTiled through cudaGetDriverEntryPoint; returns nonzero on failure.
 int encode_tensor_map(CUtensorMap* map, CUtensorMapDataType dtype, uint32_t rank, const void* base,

@@ -17,6 +17,7 @@
 
 #include <cstdlib>
 
+#include "device_util.cuh"
 #include "host_util.cuh"
 #include "kernel_pool.cuh"
 #include "masks.cuh"
@@ -25,13 +26,6 @@ namespace mmb {
 
 constexpr int kKpThreads = 256;
 constexpr int kKpQ = 32;            // query rows per block pass
-constexpr float kTinyNorm = 1e-13f; // allennlp tiny_value_of_dtype(float32)
-
-__host__ __device__ inline int kp_row_stride(int D) {
-  int dp = (D + 3) & ~3;
-  if (((dp >> 2) & 1) == 0) dp += 4;  // (dp/4) odd -> 8 consecutive rows hit 8 distinct 16-B bank groups
-  return dp;
-}
 
 // Load `nrows` rows (row r of the tile = global row row0 + r, valid while < L) of a [L, D] matrix,
 // L2-normalise them (x / (|x| + 1e-13)) and store into smem with stride dp.  Rows past L become zeros.
@@ -109,12 +103,6 @@ __device__ __forceinline__ void kp_cos_tile(const float* __restrict__ qs, const 
     for (int s = 0; s < JR; ++s) cs[(ti + 8 * r) * cstride + tj + 32 * s] = acc[r][s];
 }
 
-__device__ __forceinline__ float ex2_approx(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
 // ---------------------------------------------------------------------------------------------
 // forward
 // ---------------------------------------------------------------------------------------------
@@ -122,7 +110,7 @@ template <int KB, int JR>
 __global__ void __launch_bounds__(kKpThreads) kernel_pool_fwd_simt(KpParams P) {
   constexpr int TJ = 32 * JR;
   extern __shared__ __align__(16) float sm[];
-  const int D = P.D, dp = kp_row_stride(D), Lq = P.Lq, Ld = P.Ld, K = P.K;
+  const int D = P.D, dp = padded_row_stride(D), Lq = P.Lq, Ld = P.Ld, K = P.K;
   float* qs = sm;                                  // [32][dp]
   float* ds = qs + (size_t)kKpQ * dp;              // [TJ][dp]
   float* cs = ds + (size_t)TJ * dp;                // [32][TJ+1]
@@ -140,7 +128,7 @@ __global__ void __launch_bounds__(kKpThreads) kernel_pool_fwd_simt(KpParams P) {
   if (t < 32) {
     const bool ok = t < K;
     mu_s[t] = ok ? P.mu[t] : 0.f;
-    a_s[t] = ok ? sqrtf(0.5f * 1.4426950408889634f) / P.sigma[t] : 0.f;
+    a_s[t] = ok ? rbf_scale(P.sigma[t]) : 0.f;
     al_s[t] = ok ? (P.alpha ? P.alpha[t] : 1.f) : 1.f;
     w_s[t] = ok ? P.weight[t] : 0.f;
   }
@@ -233,7 +221,7 @@ template <int KB, int NC>
 __global__ void __launch_bounds__(kKpThreads) kernel_pool_bwd_simt(KpParams P) {
   constexpr int TJ = 32;
   extern __shared__ __align__(16) float sm[];
-  const int D = P.D, dp = kp_row_stride(D), Lq = P.Lq, Ld = P.Ld, K = P.K;
+  const int D = P.D, dp = padded_row_stride(D), Lq = P.Lq, Ld = P.Ld, K = P.K;
   float* qs = sm;                          // [32][dp] q^
   float* ds = qs + (size_t)32 * dp;        // [32][dp] d^
   float* gs = ds + (size_t)32 * dp;        // [32][dp] dd^ tile, later dq^
@@ -260,7 +248,7 @@ __global__ void __launch_bounds__(kKpThreads) kernel_pool_bwd_simt(KpParams P) {
     const bool ok = t < K;
     const float sg = ok ? P.sigma[t] : 1.f;
     mu_s[t] = ok ? P.mu[t] : 0.f;
-    a_s[t] = ok ? sqrtf(0.5f * 1.4426950408889634f) / sg : 0.f;
+    a_s[t] = ok ? rbf_scale(sg) : 0.f;
     is2_s[t] = ok ? 1.0f / (sg * sg) : 0.f;
     al_s[t] = ok ? (P.alpha ? P.alpha[t] : 1.f) : 1.f;
     w_s[t] = ok ? P.weight[t] : 0.f;
@@ -469,7 +457,7 @@ static int kp_validate(const KpParams& P) {
 
 template <int KB, int JR>
 static int launch_fwd(const KpParams& P, const DeviceInfo& dev, cudaStream_t stream) {
-  const int dp = kp_row_stride(P.D), TJ = 32 * JR;
+  const int dp = padded_row_stride(P.D), TJ = 32 * JR;
   const size_t need = ((size_t)(kKpQ + TJ) * dp + kKpQ * (TJ + 1) + 32 * 6 + TJ + (size_t)9 * KB * 32) * sizeof(float);
   if (need > (size_t)dev.max_smem_optin) {
     set_error("kernel_pool forward: embedding dim too large for the shared-memory tiles");
@@ -484,7 +472,7 @@ static int launch_fwd(const KpParams& P, const DeviceInfo& dev, cudaStream_t str
 
 template <int KB, int NC>
 static int launch_bwd(const KpParams& P, const DeviceInfo& dev, cudaStream_t stream) {
-  const int dp = kp_row_stride(P.D);
+  const int dp = padded_row_stride(P.D);
   const size_t need = ((size_t)3 * 32 * dp + 32 * 33 + 32 * 32 + 32 * KB + 32 * 13 + (size_t)KB * 32) * sizeof(float);
   if (need > (size_t)dev.max_smem_optin) {
     set_error("kernel_pool backward: embedding dim too large for the shared-memory tiles");
@@ -493,6 +481,100 @@ static int launch_bwd(const KpParams& P, const DeviceInfo& dev, cudaStream_t str
   MMB_CHECK_CUDA(cudaFuncSetAttribute(kernel_pool_bwd_simt<KB, NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)need));
   const int grid = (int)std::min<int64_t>(P.B, (int64_t)dev.sm_count * 4);
   kernel_pool_bwd_simt<KB, NC><<<grid, kKpThreads, need, stream>>>(P);
+  MMB_CHECK_CUDA(cudaGetLastError());
+  return MMB200_OK;
+}
+
+// the envelope of the tensor-core training pair (forward that saves its cosines + backward that consumes them)
+static bool kp_train_tc_shape_ok(int Lq, int Ld, int D, int K) {
+  return Lq >= 1 && Lq <= 32 && Ld >= 1 && K >= 1 && K <= 32 && D >= 4 && D % 4 == 0 && D <= 320;
+}
+
+static int kp_fwd_impl(const float* q, const float* d, const void* q_mask, const void* d_mask, const float* doc_gate,
+                       const float* mu, const float* sigma, const float* alpha, const float* weight, float* score,
+                       float* per_kernel, float* per_kernel_query, float* cosine, float* saved, int64_t B, int32_t Lq,
+                       int32_t Ld, int32_t D, int32_t K, float log_scale, float clamp_min, float score_bias,
+                       int32_t mask_dtype, int32_t impl, void* stream_) {
+  MMB_REQUIRE(clamp_min > 0.f, "clamp_min must be positive");
+  KpParams P{};
+  P.saved = saved;
+  P.gate = doc_gate; P.clamp_min = clamp_min; P.bias = score_bias;
+  P.q = q; P.d = d; P.q_mask = q_mask; P.d_mask = d_mask; P.mu = mu; P.sigma = sigma; P.alpha = alpha; P.weight = weight;
+  P.B = B; P.Lq = Lq; P.Ld = Ld; P.D = D; P.K = K; P.mask_dtype = mask_dtype; P.log_scale = log_scale;
+  P.score = score; P.per_kernel = per_kernel; P.per_kernel_query = per_kernel_query; P.cosine = cosine;
+  if (int rc = kp_validate(P)) return rc;
+  MMB_REQUIRE(score != nullptr, "score must be non-null");
+  if (B == 0) return MMB200_OK;
+  DeviceInfo dev;
+  if (int rc = require_sm90(&dev)) return rc;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (impl != MMB200_IMPL_SIMT) {
+    bool handled = false;
+    int rc = kernel_pool_fwd_ts(P, dev, stream, &handled);
+    if (handled) return rc;
+    if (impl == MMB200_IMPL_TCGEN05) {
+      if (rc == MMB200_OK) { set_error("kernel_pool: shape not supported by the tensor-core kernel"); rc = MMB200_ERR_UNSUPPORTED; }
+      return rc;
+    }
+  }
+  const bool wide = Ld > 48;
+  if (K <= 12) return wide ? launch_fwd<12, 2>(P, dev, stream) : launch_fwd<12, 1>(P, dev, stream);
+  if (K <= 24) return wide ? launch_fwd<24, 2>(P, dev, stream) : launch_fwd<24, 1>(P, dev, stream);
+  return wide ? launch_fwd<32, 2>(P, dev, stream) : launch_fwd<32, 1>(P, dev, stream);
+}
+
+static int kp_bwd_impl(const float* q, const float* d, const void* q_mask, const void* d_mask, const float* doc_gate,
+                       const float* mu, const float* sigma, const float* alpha, const float* weight,
+                       const float* per_kernel_query, const float* saved, const float* grad_score, float* grad_q,
+                       float* grad_d, float* grad_gate, float* grad_alpha, float* grad_weight, float* workspace,
+                       int64_t B, int32_t Lq, int32_t Ld, int32_t D, int32_t K, float log_scale, float clamp_min,
+                       int32_t mask_dtype, void* stream_) {
+  MMB_REQUIRE(clamp_min > 0.f, "clamp_min must be positive");
+  KpParams P{};
+  P.saved = const_cast<float*>(saved);
+  // the tensor core drops the low 13 mantissa bits of the raw fp32 tiles: relative shrink 2^-10 u / m with u uniform in
+  // [0, 1) and the mantissa m log-uniform in [1, 2) -> mean 2^-11 / ln 2 * (1 - 1/2) = 0.72 * 2^-11
+  P.tf32_comp = 1.0f + 0.72f / 2048.0f;
+#ifdef MMB200_ENABLE_PROF
+  if (const char* e = getenv("MMB200_KPB_COMP")) P.tf32_comp = (float)atof(e);
+#endif
+  P.gate = doc_gate; P.clamp_min = clamp_min; P.grad_gate = grad_gate;
+  P.q = q; P.d = d; P.q_mask = q_mask; P.d_mask = d_mask; P.mu = mu; P.sigma = sigma; P.alpha = alpha; P.weight = weight;
+  P.B = B; P.Lq = Lq; P.Ld = Ld; P.D = D; P.K = K; P.mask_dtype = mask_dtype; P.log_scale = log_scale;
+  P.S = per_kernel_query; P.grad_score = grad_score; P.grad_q = grad_q; P.grad_d = grad_d;
+  if (int rc = kp_validate(P)) return rc;
+  MMB_REQUIRE(per_kernel_query && grad_score && grad_q && grad_d && workspace, "null pointer");
+  MMB_REQUIRE(D <= 512, "kernel_pool backward supports embedding dim <= 512");
+  P.ws_weight = workspace;
+  P.ws_alpha = workspace + B * K;
+  if (B == 0) return MMB200_OK;
+  DeviceInfo dev;
+  if (int rc = require_sm90(&dev)) return rc;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  int rc;
+  if (saved) {
+    bool handled = false;
+    rc = kernel_pool_bwd_tc(P, dev, stream, &handled);
+    if (!handled) {
+      if (rc == MMB200_OK) { set_error("kernel_pool_bwd_saved: arguments outside the tensor-core backward's envelope"); rc = MMB200_ERR_UNSUPPORTED; }
+      return rc;
+    }
+    if (rc) return rc;
+    kp_reduce_batch<<<K, 256, 0, stream>>>(P.ws_weight, P.ws_alpha, grad_weight, grad_alpha, B, K);
+    MMB_CHECK_CUDA(cudaGetLastError());
+    return MMB200_OK;
+  }
+  if (D <= 256) {
+    if (K <= 12) rc = launch_bwd<12, 1>(P, dev, stream);
+    else if (K <= 24) rc = launch_bwd<24, 1>(P, dev, stream);
+    else rc = launch_bwd<32, 1>(P, dev, stream);
+  } else {
+    if (K <= 12) rc = launch_bwd<12, 2>(P, dev, stream);
+    else if (K <= 24) rc = launch_bwd<24, 2>(P, dev, stream);
+    else rc = launch_bwd<32, 2>(P, dev, stream);
+  }
+  if (rc) return rc;
+  kp_reduce_batch<<<K, 256, 0, stream>>>(P.ws_weight, P.ws_alpha, grad_weight, grad_alpha, B, K);
   MMB_CHECK_CUDA(cudaGetLastError());
   return MMB200_OK;
 }
@@ -507,24 +589,6 @@ extern "C" int mmb200_kernel_pool_fwd(const float* q, const float* d, const void
   return mmb200_kernel_pool_fwd_ex(q, d, q_mask, d_mask, nullptr, mu, sigma, alpha, weight, score, per_kernel,
                                    per_kernel_query, cosine, B, Lq, Ld, D, K, log_scale, 1e-10f, 0.f, mask_dtype, impl, stream_);
 }
-
-namespace mmb {
-// the envelope of the tensor-core training pair (forward that saves its cosines + backward that consumes them)
-static bool kp_train_tc_shape_ok(int Lq, int Ld, int D, int K) {
-  return Lq >= 1 && Lq <= 32 && Ld >= 1 && K >= 1 && K <= 32 && D >= 4 && D % 4 == 0 && D <= 320;
-}
-static int kp_fwd_impl(const float* q, const float* d, const void* q_mask, const void* d_mask, const float* doc_gate,
-                       const float* mu, const float* sigma, const float* alpha, const float* weight, float* score,
-                       float* per_kernel, float* per_kernel_query, float* cosine, float* saved, int64_t B, int32_t Lq,
-                       int32_t Ld, int32_t D, int32_t K, float log_scale, float clamp_min, float score_bias,
-                       int32_t mask_dtype, int32_t impl, void* stream_);
-static int kp_bwd_impl(const float* q, const float* d, const void* q_mask, const void* d_mask, const float* doc_gate,
-                       const float* mu, const float* sigma, const float* alpha, const float* weight,
-                       const float* per_kernel_query, const float* saved, const float* grad_score, float* grad_q,
-                       float* grad_d, float* grad_gate, float* grad_alpha, float* grad_weight, float* workspace, int64_t B,
-                       int32_t Lq, int32_t Ld, int32_t D, int32_t K, float log_scale, float clamp_min, int32_t mask_dtype,
-                       void* stream_);
-}  // namespace mmb
 
 extern "C" int mmb200_kernel_pool_fwd_ex(const float* q, const float* d, const void* q_mask, const void* d_mask,
                                          const float* doc_gate, const float* mu, const float* sigma, const float* alpha,
@@ -576,44 +640,6 @@ extern "C" int mmb200_kernel_pool_bwd_saved(const float* q, const float* d, cons
                      stream_);
 }
 
-static int mmb::kp_fwd_impl(const float* q, const float* d, const void* q_mask, const void* d_mask, const float* doc_gate,
-                            const float* mu, const float* sigma, const float* alpha, const float* weight, float* score,
-                            float* per_kernel, float* per_kernel_query, float* cosine, float* saved, int64_t B, int32_t Lq,
-                            int32_t Ld, int32_t D, int32_t K, float log_scale, float clamp_min, float score_bias,
-                            int32_t mask_dtype, int32_t impl, void* stream_) {
-  using namespace mmb;
-  MMB_REQUIRE(clamp_min > 0.f, "clamp_min must be positive");
-  KpParams P{};
-  P.saved = saved;
-  P.gate = doc_gate; P.clamp_min = clamp_min; P.bias = score_bias;
-  P.q = q; P.d = d; P.q_mask = q_mask; P.d_mask = d_mask; P.mu = mu; P.sigma = sigma; P.alpha = alpha; P.weight = weight;
-  P.B = B; P.Lq = Lq; P.Ld = Ld; P.D = D; P.K = K; P.mask_dtype = mask_dtype; P.log_scale = log_scale;
-  P.score = score; P.per_kernel = per_kernel; P.per_kernel_query = per_kernel_query; P.cosine = cosine;
-  if (int rc = kp_validate(P)) return rc;
-  MMB_REQUIRE(score != nullptr, "score must be non-null");
-  if (B == 0) return MMB200_OK;
-  DeviceInfo dev;
-  if (int rc = current_device_info(&dev)) return rc;
-  if (!is_sm90(dev)) {
-    set_error("matchmaker_b200 kernels are built for sm_90a only");
-    return MMB200_ERR_UNSUPPORTED;
-  }
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (impl != MMB200_IMPL_SIMT) {
-    bool handled = false;
-    int rc = kernel_pool_fwd_ts(P, dev, stream, &handled);
-    if (handled) return rc;
-    if (impl == MMB200_IMPL_TCGEN05) {
-      if (rc == MMB200_OK) { set_error("kernel_pool: shape not supported by the tensor-core kernel"); rc = MMB200_ERR_UNSUPPORTED; }
-      return rc;
-    }
-  }
-  const bool wide = Ld > 48;
-  if (K <= 12) return wide ? launch_fwd<12, 2>(P, dev, stream) : launch_fwd<12, 1>(P, dev, stream);
-  if (K <= 24) return wide ? launch_fwd<24, 2>(P, dev, stream) : launch_fwd<24, 1>(P, dev, stream);
-  return wide ? launch_fwd<32, 2>(P, dev, stream) : launch_fwd<32, 1>(P, dev, stream);
-}
-
 extern "C" int mmb200_kernel_pool_bwd(const float* q, const float* d, const void* q_mask, const void* d_mask,
                                       const float* mu, const float* sigma, const float* alpha, const float* weight,
                                       const float* per_kernel_query, const float* grad_score, float* grad_q,
@@ -635,65 +661,4 @@ extern "C" int mmb200_kernel_pool_bwd_ex(const float* q, const float* d, const v
   return mmb::kp_bwd_impl(q, d, q_mask, d_mask, doc_gate, mu, sigma, alpha, weight, per_kernel_query, nullptr, grad_score,
                           grad_q, grad_d, grad_gate, grad_alpha, grad_weight, workspace, B, Lq, Ld, D, K, log_scale, clamp_min,
                           mask_dtype, stream_);
-}
-
-static int mmb::kp_bwd_impl(const float* q, const float* d, const void* q_mask, const void* d_mask, const float* doc_gate,
-                            const float* mu, const float* sigma, const float* alpha, const float* weight,
-                            const float* per_kernel_query, const float* saved, const float* grad_score, float* grad_q,
-                            float* grad_d, float* grad_gate, float* grad_alpha, float* grad_weight, float* workspace,
-                            int64_t B, int32_t Lq, int32_t Ld, int32_t D, int32_t K, float log_scale, float clamp_min,
-                            int32_t mask_dtype, void* stream_) {
-  using namespace mmb;
-  MMB_REQUIRE(clamp_min > 0.f, "clamp_min must be positive");
-  KpParams P{};
-  P.saved = const_cast<float*>(saved);
-  // the tensor core drops the low 13 mantissa bits of the raw fp32 tiles: relative shrink 2^-10 u / m with u uniform in
-  // [0, 1) and the mantissa m log-uniform in [1, 2) -> mean 2^-11 / ln 2 * (1 - 1/2) = 0.72 * 2^-11
-  P.tf32_comp = 1.0f + 0.72f / 2048.0f;
-#ifdef MMB200_ENABLE_PROF
-  if (const char* e = getenv("MMB200_KPB_COMP")) P.tf32_comp = (float)atof(e);
-#endif
-  P.gate = doc_gate; P.clamp_min = clamp_min; P.grad_gate = grad_gate;
-  P.q = q; P.d = d; P.q_mask = q_mask; P.d_mask = d_mask; P.mu = mu; P.sigma = sigma; P.alpha = alpha; P.weight = weight;
-  P.B = B; P.Lq = Lq; P.Ld = Ld; P.D = D; P.K = K; P.mask_dtype = mask_dtype; P.log_scale = log_scale;
-  P.S = per_kernel_query; P.grad_score = grad_score; P.grad_q = grad_q; P.grad_d = grad_d;
-  if (int rc = kp_validate(P)) return rc;
-  MMB_REQUIRE(per_kernel_query && grad_score && grad_q && grad_d && workspace, "null pointer");
-  MMB_REQUIRE(D <= 512, "kernel_pool backward supports embedding dim <= 512");
-  P.ws_weight = workspace;
-  P.ws_alpha = workspace + B * K;
-  if (B == 0) return MMB200_OK;
-  DeviceInfo dev;
-  if (int rc = current_device_info(&dev)) return rc;
-  if (!is_sm90(dev)) {
-    set_error("matchmaker_b200 kernels are built for sm_90a only");
-    return MMB200_ERR_UNSUPPORTED;
-  }
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  int rc;
-  if (saved) {
-    bool handled = false;
-    rc = kernel_pool_bwd_tc(P, dev, stream, &handled);
-    if (!handled) {
-      if (rc == MMB200_OK) { set_error("kernel_pool_bwd_saved: arguments outside the tensor-core backward's envelope"); rc = MMB200_ERR_UNSUPPORTED; }
-      return rc;
-    }
-    if (rc) return rc;
-    kp_reduce_batch<<<K, 256, 0, stream>>>(P.ws_weight, P.ws_alpha, grad_weight, grad_alpha, B, K);
-    MMB_CHECK_CUDA(cudaGetLastError());
-    return MMB200_OK;
-  }
-  if (D <= 256) {
-    if (K <= 12) rc = launch_bwd<12, 1>(P, dev, stream);
-    else if (K <= 24) rc = launch_bwd<24, 1>(P, dev, stream);
-    else rc = launch_bwd<32, 1>(P, dev, stream);
-  } else {
-    if (K <= 12) rc = launch_bwd<12, 2>(P, dev, stream);
-    else if (K <= 24) rc = launch_bwd<24, 2>(P, dev, stream);
-    else rc = launch_bwd<32, 2>(P, dev, stream);
-  }
-  if (rc) return rc;
-  kp_reduce_batch<<<K, 256, 0, stream>>>(P.ws_weight, P.ws_alpha, grad_weight, grad_alpha, B, K);
-  MMB_CHECK_CUDA(cudaGetLastError());
-  return MMB200_OK;
 }

@@ -31,6 +31,7 @@
 // bits dropped, mean relative shrink 0.72 * 2^-11), which KpParams::tf32_comp undoes on average.
 #include <algorithm>
 
+#include "device_util.cuh"
 #include "host_util.cuh"
 #include "kernel_pool.cuh"
 #include "masks.cuh"
@@ -59,12 +60,6 @@ struct BwShared {
   float mu[32], a[32], is2[32], sig2[32], alpha[32], w[32];
 };
 
-__device__ __forceinline__ float ex2f(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
 template <int KB, bool GATE>
 __global__ void __launch_bounds__(kThreads, 1)
 kernel_pool_bwd_tc_kernel(KpParams P) {
@@ -83,15 +78,14 @@ kernel_pool_bwd_tc_kernel(KpParams P) {
   const int tiles = (P.Ld + kTile - 1) / kTile;
   const int nfb = (P.D + 63) / 64;
   const int D4 = P.D >> 2, DP4 = DP >> 2;
-  const int64_t per = P.B / gridDim.x, rem = P.B % gridDim.x;
-  const int64_t p_begin = (int64_t)blockIdx.x * per + min((int64_t)blockIdx.x, rem);
-  const int64_t p_end = p_begin + per + ((int64_t)blockIdx.x < rem ? 1 : 0);
+  int64_t p_begin, p_end;
+  cta_share(P.B, &p_begin, &p_end);
 
   if (tid < 32) {
     const bool ok = tid < P.K;
     const float sg = ok ? P.sigma[tid] : 1.f;
     S->mu[tid] = ok ? P.mu[tid] : 0.f;
-    S->a[tid] = ok ? sqrtf(0.5f * 1.4426950408889634f) / sg : 0.f;
+    S->a[tid] = ok ? rbf_scale(sg) : 0.f;
     S->is2[tid] = ok ? 1.0f / (sg * sg) : 0.f;
     S->sig2[tid] = ok ? sg * sg : 0.f;
     S->alpha[tid] = ok ? (P.alpha ? P.alpha[tid] : 1.f) : 1.f;
@@ -193,7 +187,7 @@ kernel_pool_bwd_tc_kernel(KpParams P) {
             for (int y = 0; y < 8; ++y) {
               const float diff = mu_k - c[y];
               const float u = diff * a_k;
-              const float te = Tv[y] * ex2f(-u * u);
+              const float te = Tv[y] * ex2_approx(-u * u);
               G[y] = fmaf(te, diff, G[y]);
               if constexpr (GATE) H = fmaf(te, sig2_k, H);
             }

@@ -1,6 +1,6 @@
 // Cosine + RBF kernel pooling forward (KNRM / TK) on the tensor cores with fp32-grade accuracy.
 //
-// Arithmetic (x = hi + lo, hi = x & 0xffffe000, [Qhi;Qlo] stacked along N):
+// Arithmetic (x = hi + lo from split_tf32, [Qhi;Qlo] stacked along N):
 //
 //     D[128 doc rows x 64] = Dhi[128 x K] * [Qhi; Qlo]^T  +  Dlo[128 x K] * [Qhi; Qlo]^T
 //
@@ -26,6 +26,7 @@
 #include <cstdio>
 #include <cstdlib>
 
+#include "device_util.cuh"
 #include "host_util.cuh"
 #include "kernel_pool.cuh"
 #include "masks.cuh"
@@ -48,7 +49,6 @@ constexpr int kReleaseArrivals = 8 + 64;  // lane 0 of each MMA warp + every lan
 constexpr int kFirstDocWarp = 4, kFirstEpiWarp = 12;
 constexpr int kRegsLight = 56, kRegsMma = 88, kRegsEpilogue = 120;  // setmaxnreg budgets per warpgroup (<= 640 x 96)
 constexpr float kSentinel = 1.0e6f;   // "cosine" of a masked row: ex2(-((1e6 - mu) a)^2) is exactly 0 for any sigma < 1e4
-constexpr float kTinyNorm = 1e-13f;
 
 struct KpShared {
   uint64_t raw_full[kMaxRaw];    // TMA -> query convert, MMA warps
@@ -67,19 +67,6 @@ struct KpShared {
   int live[2][8];                // per cosine tile: last unmasked document row + 1 of each MMA warp's 16 rows
 };
 
-__device__ __forceinline__ float ex2f(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
-__device__ __forceinline__ void split4(const float4 v, uint32_t* hi, uint32_t* lo) {
-  hi[0] = __float_as_uint(v.x) & 0xffffe000u; lo[0] = __float_as_uint(v.x - __uint_as_float(hi[0]));
-  hi[1] = __float_as_uint(v.y) & 0xffffe000u; lo[1] = __float_as_uint(v.y - __uint_as_float(hi[1]));
-  hi[2] = __float_as_uint(v.z) & 0xffffe000u; lo[2] = __float_as_uint(v.z - __uint_as_float(hi[2]));
-  hi[3] = __float_as_uint(v.w) & 0xffffe000u; lo[3] = __float_as_uint(v.w - __uint_as_float(hi[3]));
-}
-
 template <int KB, bool SAVE>
 __global__ void __launch_bounds__(kThreads, 1)
 kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_d,
@@ -97,9 +84,8 @@ kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles = (P.Ld + 127) / 128;
   const int nch = (P.D + 31) / 32;
-  const int64_t per = P.B / gridDim.x, rem = P.B % gridDim.x;
-  const int64_t p_begin = (int64_t)blockIdx.x * per + min((int64_t)blockIdx.x, rem);
-  const int64_t p_end = p_begin + per + ((int64_t)blockIdx.x < rem ? 1 : 0);
+  int64_t p_begin, p_end;
+  cta_share(P.B, &p_begin, &p_end);
 
   if (threadIdx.x == 0) {
     prefetch_tensormap(&tmap_q);
@@ -114,7 +100,7 @@ kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     const int t = threadIdx.x;
     const bool ok = t < P.K;
     S->mu[t] = ok ? P.mu[t] : 0.f;
-    S->a[t] = ok ? sqrtf(0.5f * 1.4426950408889634f) / P.sigma[t] : 0.f;
+    S->a[t] = ok ? rbf_scale(P.sigma[t]) : 0.f;
     S->alpha[t] = ok ? (P.alpha ? P.alpha[t] : 1.f) : 1.f;
     S->w[t] = ok ? P.weight[t] : 0.f;
   }
@@ -177,7 +163,7 @@ kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
 #pragma unroll
             for (int c = 0; c < 4; ++c) {
               uint32_t hi[4], lo[4];
-              split4(x[c], hi, lo);
+              split_tf32(x[c], hi, lo);
               const int off = (((4 * half + c) ^ sw) << 4);
               *reinterpret_cast<uint4*>(hrow + off) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
               *reinterpret_cast<uint4*>(lrow + off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
@@ -231,10 +217,7 @@ kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
             const int ch0 = (2 * k) ^ (r0 & 7), ch1 = (2 * k + 1) ^ (r0 & 7);   // r1 & 7 == r0 & 7
             const float v[4] = {x[r0 * 32 + ch0 * 4 + tq], x[r1 * 32 + ch0 * 4 + tq], x[r0 * 32 + ch1 * 4 + tq], x[r1 * 32 + ch1 * 4 + tq]};
 #pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              ahi[k][e] = __float_as_uint(v[e]) & 0xffffe000u;
-              alo[k][e] = __float_as_uint(v[e] - __uint_as_float(ahi[k][e]));
-            }
+            for (int e = 0; e < 4; ++e) split_tf32(v[e], ahi[k][e], alo[k][e]);
             ss0 = fmaf(v[0], v[0], fmaf(v[2], v[2], ss0));
             ss1 = fmaf(v[1], v[1], fmaf(v[3], v[3], ss1));
           }
@@ -359,7 +342,7 @@ kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
             for (int k = 0; k < KB; ++k) {
               const float m = kRegConst ? mu_r[k] : S->mu[k], a = kRegConst ? a_r[k] : S->a[k];
               const float u0 = (c0 - m) * a, u1 = (c1 - m) * a;
-              acc[k] += ex2f(fmaf(-u0, u0, l0)) + ex2f(fmaf(-u1, u1, l1));
+              acc[k] += ex2_approx(fmaf(-u0, u0, l0)) + ex2_approx(fmaf(-u1, u1, l1));
             }
             c0 = n0; c1 = n1;
             l0 = m0; l1 = m1;

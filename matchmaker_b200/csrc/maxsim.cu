@@ -37,6 +37,7 @@
 #include <algorithm>
 #include <vector>
 
+#include "device_util.cuh"
 #include "host_util.cuh"
 #include "masks.cuh"
 #include "maxsim.cuh"
@@ -47,15 +48,6 @@ namespace mmb {
 // ---------------------------------------------------------------------------------------------
 // shared device helpers
 // ---------------------------------------------------------------------------------------------
-template <typename T>
-__device__ __forceinline__ float to_float(T v);
-template <>
-__device__ __forceinline__ float to_float<float>(float v) { return v; }
-template <>
-__device__ __forceinline__ float to_float<__half>(__half v) { return __half2float(v); }
-template <>
-__device__ __forceinline__ float to_float<__nv_bfloat16>(__nv_bfloat16 v) { return __bfloat162float(v); }
-
 __device__ __forceinline__ int64_t pair_query(const MaxsimParams& P, int64_t p) {
   return P.pair_q ? static_cast<int64_t>(P.pair_q[p]) : (p + P.pair_base) / P.docs_per_query;
 }
@@ -205,10 +197,8 @@ maxsim_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  // contiguous pair range of this CTA
-  const int64_t per = P.n_pairs / gridDim.x, rem = P.n_pairs % gridDim.x;
-  const int64_t p_begin = (int64_t)blockIdx.x * per + min((int64_t)blockIdx.x, rem);
-  const int64_t p_end = p_begin + per + ((int64_t)blockIdx.x < rem ? 1 : 0);
+  int64_t p_begin, p_end;
+  cta_share(P.n_pairs, &p_begin, &p_end);
 
   if (threadIdx.x == 0) {
     prefetch_tensormap(&tmap_q);
@@ -474,18 +464,13 @@ static int launch_simt(const MaxsimParams& P, int dtype, const DeviceInfo& dev, 
   const size_t smem_bytes = ((size_t)P.Lq * (P.dim + 1) + 8 * (size_t)P.Lq) * sizeof(float);
   MMB_REQUIRE(smem_bytes <= (size_t)dev.max_smem_optin, "query tile does not fit in shared memory");
   const int grid = (int)std::min<int64_t>((int64_t)dev.sm_count * 8, P.n_pairs);
-#define MMB_LAUNCH_SIMT(T)                                                                                  \
-  do {                                                                                                      \
-    MMB_CHECK_CUDA(cudaFuncSetAttribute(maxsim_simt_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                        (int)smem_bytes));                                                  \
-    maxsim_simt_kernel<T><<<grid, kSimtThreads, smem_bytes, stream>>>(P);                                  \
-  } while (0)
-  if (dtype == MMB200_F16) MMB_LAUNCH_SIMT(__half);
-  else if (dtype == MMB200_BF16) MMB_LAUNCH_SIMT(__nv_bfloat16);
-  else MMB_LAUNCH_SIMT(float);
-#undef MMB_LAUNCH_SIMT
-  MMB_CHECK_CUDA(cudaGetLastError());
-  return MMB200_OK;
+  return dispatch_dtype(dtype, [&](auto t) {
+    using T = decltype(t);
+    MMB_CHECK_CUDA(cudaFuncSetAttribute(maxsim_simt_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+    maxsim_simt_kernel<T><<<grid, kSimtThreads, smem_bytes, stream>>>(P);
+    MMB_CHECK_CUDA(cudaGetLastError());
+    return MMB200_OK;
+  });
 }
 
 int maxsim_fwd_device(const MaxsimParams& P, int dtype, int impl, cudaStream_t stream) {
@@ -499,12 +484,7 @@ int maxsim_fwd_device(const MaxsimParams& P, int dtype, int impl, cudaStream_t s
   if (!P.pair_d) MMB_REQUIRE(P.n_pairs <= P.n_d, "n_pairs exceeds n_d");
   if (P.n_pairs == 0) return MMB200_OK;
   DeviceInfo dev;
-  if (int rc = current_device_info(&dev)) return rc;
-  if (!is_sm90(dev)) {
-    set_error("matchmaker_b200 kernels are built for sm_90a only; device is sm_" + std::to_string(dev.cc_major) +
-              std::to_string(dev.cc_minor));
-    return MMB200_ERR_UNSUPPORTED;
-  }
+  if (int rc = require_sm90(&dev)) return rc;
   if (impl == MMB200_IMPL_TCGEN05_RAGGED) {
     // skip-padding variant: fetch only rows up to each document's last unmasked row
     MMB_REQUIRE(P.pair_dmask == nullptr, "ragged fetch is incompatible with pair_dmask");
@@ -544,11 +524,9 @@ extern "C" int mmb200_maxsim_fwd(const void* q, const void* d, const void* q_mas
                                  int32_t Ld, int32_t dim, int32_t dtype, int32_t mask_dtype, int32_t impl,
                                  void* stream) {
   mmb::MaxsimParams P;
-  P.q = q; P.d = d; P.q_mask = q_mask; P.d_mask = d_mask; P.pair_q = pair_q; P.pair_d = pair_d; P.pair_dmask = pair_dmask; P.rows_needed = nullptr;
+  P.q = q; P.d = d; P.q_mask = q_mask; P.d_mask = d_mask; P.pair_q = pair_q; P.pair_d = pair_d; P.pair_dmask = pair_dmask;
   P.out = out; P.argmax = argmax; P.n_q = n_q; P.n_d = n_d; P.n_pairs = n_pairs;
-  P.pair_base = 0;
   P.docs_per_query = docs_per_query; P.Lq = Lq; P.Ld = Ld; P.dim = dim; P.mask_dtype = mask_dtype;
-  P.doc_offsets = nullptr; P.n_rows = 0;
   return mmb::maxsim_fwd_device(P, dtype, impl, static_cast<cudaStream_t>(stream));
 }
 
@@ -561,10 +539,8 @@ extern "C" int mmb200_maxsim_store_fwd(const void* q, const void* store, const i
   MMB_REQUIRE(n_rows < (1ll << 31) - 1024, "at most 2^31 - 1024 store rows per device (TMA row coordinates are int32)");
   MMB_REQUIRE(impl != MMB200_IMPL_TCGEN05_RAGGED, "store mode already fetches only each passage's own rows");
   mmb::MaxsimParams P;
-  P.q = q; P.d = store; P.q_mask = nullptr; P.d_mask = nullptr; P.pair_q = pair_q; P.pair_d = pair_d; P.pair_dmask = nullptr;
-  P.rows_needed = nullptr; P.out = out; P.argmax = nullptr; P.n_q = n_q; P.n_d = n_docs;
-  P.n_pairs = n_pairs; P.pair_base = 0; P.docs_per_query = 1; P.Lq = Lq; P.Ld = max_doc_len; P.dim = dim;
-  P.mask_dtype = MMB200_MASK_NONE;
+  P.q = q; P.d = store; P.pair_q = pair_q; P.pair_d = pair_d; P.out = out; P.n_q = n_q; P.n_d = n_docs;
+  P.n_pairs = n_pairs; P.Lq = Lq; P.Ld = max_doc_len; P.dim = dim;
   P.doc_offsets = doc_offsets; P.n_rows = n_rows;
   return mmb::maxsim_fwd_device(P, dtype, impl, static_cast<cudaStream_t>(stream));
 }

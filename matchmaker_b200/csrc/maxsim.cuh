@@ -4,27 +4,29 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "../../include/matchmaker_b200.h"
+
 namespace mmb {
 
 struct MaxsimParams {
-  const void* q;
-  const void* d;
-  const void* q_mask;
-  const void* d_mask;
-  const int32_t* pair_q;
-  const int32_t* pair_d;
-  const int32_t* pair_dmask;  // row of d_mask used for pair p (default: the document index)
-  const int32_t* rows_needed;  // [n_d] or NULL: rows of document di worth fetching (1 + last unmasked row)
-  float* out;
-  int32_t* argmax;
-  int64_t n_q, n_d, n_pairs;
-  int64_t pair_base;  // query of pair p (when pair_q == NULL) is (p + pair_base) / docs_per_query
-  int32_t docs_per_query, Lq, Ld, dim, mask_dtype;
+  const void* q = nullptr;
+  const void* d = nullptr;
+  const void* q_mask = nullptr;
+  const void* d_mask = nullptr;
+  const int32_t* pair_q = nullptr;
+  const int32_t* pair_d = nullptr;
+  const int32_t* pair_dmask = nullptr;  // row of d_mask used for pair p (default: the document index)
+  const int32_t* rows_needed = nullptr;  // [n_d] or NULL: rows of document di worth fetching (1 + last unmasked row)
+  float* out = nullptr;
+  int32_t* argmax = nullptr;
+  int64_t n_q = 0, n_d = 0, n_pairs = 0;
+  int64_t pair_base = 0;  // query of pair p (when pair_q == NULL) is (p + pair_base) / docs_per_query
+  int32_t docs_per_query = 1, Lq = 0, Ld = 0, dim = 0, mask_dtype = MMB200_MASK_NONE;
   // Store mode (doc_offsets != NULL): d is a ragged token store [n_rows, dim]; document di is rows
   // [doc_offsets[di], doc_offsets[di + 1]), at most Ld of them are read.  No masks; pair_d < 0 and documents without
   // rows score -inf.  NULL: the padded [n_d, Ld, dim] layout above.
-  const int64_t* doc_offsets;
-  int64_t n_rows;
+  const int64_t* doc_offsets = nullptr;
+  int64_t n_rows = 0;
 };
 
 // Rows [*lo, *lo + return value) of document di in store mode; 0 rows for a skipped pair (di < 0).

@@ -6,19 +6,11 @@
 #include <mutex>
 #include <vector>
 
+#include "device_util.cuh"
 #include "host_util.cuh"
 #include "maxsim.cuh"
 
 namespace mmb {
-
-template <typename T>
-__device__ __forceinline__ float ld_as_float(const T* p);
-template <>
-__device__ __forceinline__ float ld_as_float<float>(const float* p) { return *p; }
-template <>
-__device__ __forceinline__ float ld_as_float<__half>(const __half* p) { return __half2float(*p); }
-template <>
-__device__ __forceinline__ float ld_as_float<__nv_bfloat16>(const __nv_bfloat16* p) { return __bfloat162float(*p); }
 
 // Backward of score[p] = sum_i max_j <q_i, d_j> (autograd of matchmaker/models/colbert.py:68-75):
 //   grad_q[qi][i]   = sum over the pairs p of query qi of  g[p] * d[p][j*(p, i)]
@@ -40,7 +32,7 @@ __global__ void __launch_bounds__(128) maxsim_bwd_d_kernel(const T* __restrict__
     for (int i = 0; i < Lq; ++i) {
       const int a = argmax[p * Lq + i];
       if (a < 0) continue;  // uniform across the CTA
-      for (int k = threadIdx.x; k < dim; k += blockDim.x) gd[(int64_t)a * dim + k] += g * ld_as_float(qp + (int64_t)i * dim + k);
+      for (int k = threadIdx.x; k < dim; k += blockDim.x) gd[(int64_t)a * dim + k] += g * to_float(qp[(int64_t)i * dim + k]);
     }
   }
 }
@@ -57,7 +49,7 @@ __global__ void __launch_bounds__(128) maxsim_bwd_q_kernel(const T* __restrict__
       float acc = 0.f;
       for (int64_t p = p0; p < p1; ++p) {
         const int a = argmax[p * Lq + i];
-        if (a >= 0) acc = fmaf(grad_out[p], ld_as_float(d + (p * Ld + a) * (int64_t)dim + k), acc);
+        if (a >= 0) acc = fmaf(grad_out[p], to_float(d[(p * Ld + a) * (int64_t)dim + k]), acc);
       }
       grad_q[(qi * Lq + i) * (int64_t)dim + k] = acc;
     }
@@ -124,11 +116,7 @@ extern "C" int mmb200_maxsim_bwd(const void* q, const void* d, const float* grad
   MMB_REQUIRE(docs_per_query >= 1 && n_pairs <= n_d && (n_pairs + docs_per_query - 1) / docs_per_query <= n_q,
               "pair counts inconsistent");
   DeviceInfo dev;
-  if (int rc = current_device_info(&dev)) return rc;
-  if (!is_sm90(dev)) {
-    set_error("matchmaker_b200 kernels are built for sm_90a only");
-    return MMB200_ERR_UNSUPPORTED;
-  }
+  if (int rc = require_sm90(&dev)) return rc;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   MMB_CHECK_CUDA(cudaMemsetAsync(grad_d, 0, (size_t)n_d * Ld * dim * sizeof(float), stream));
   if (n_pairs == 0) {
@@ -137,18 +125,15 @@ extern "C" int mmb200_maxsim_bwd(const void* q, const void* d, const float* grad
   }
   const int grid_d = (int)std::min<int64_t>((int64_t)dev.sm_count * 16, n_pairs);
   const int grid_q = (int)std::min<int64_t>((int64_t)dev.sm_count * 16, n_q * Lq);
-#define MMB_LAUNCH_BWD(T)                                                                                                       \
-  do {                                                                                                                          \
-    maxsim_bwd_d_kernel<T><<<grid_d, 128, 0, stream>>>((const T*)q, grad_out, argmax, grad_d, n_pairs, docs_per_query, Lq, Ld, dim); \
-    maxsim_bwd_q_kernel<T><<<grid_q, 128, 0, stream>>>((const T*)d, grad_out, argmax, grad_q, n_q, n_pairs, docs_per_query, Lq, Ld, \
-                                                       dim);                                                                    \
-  } while (0)
-  if (dtype == MMB200_F16) MMB_LAUNCH_BWD(__half);
-  else if (dtype == MMB200_BF16) MMB_LAUNCH_BWD(__nv_bfloat16);
-  else MMB_LAUNCH_BWD(float);
-#undef MMB_LAUNCH_BWD
-  MMB_CHECK_CUDA(cudaGetLastError());
-  return MMB200_OK;
+  return dispatch_dtype(dtype, [&](auto t) {
+    using T = decltype(t);
+    maxsim_bwd_d_kernel<T><<<grid_d, 128, 0, stream>>>(static_cast<const T*>(q), grad_out, argmax, grad_d, n_pairs,
+                                                       docs_per_query, Lq, Ld, dim);
+    maxsim_bwd_q_kernel<T><<<grid_q, 128, 0, stream>>>(static_cast<const T*>(d), grad_out, argmax, grad_q, n_q, n_pairs,
+                                                       docs_per_query, Lq, Ld, dim);
+    MMB_CHECK_CUDA(cudaGetLastError());
+    return MMB200_OK;
+  });
 }
 
 extern "C" int mmb200_maxsim_fwd_host(const void* q_host, const void* d_host, const void* q_mask_host,
@@ -207,9 +192,7 @@ extern "C" int mmb200_maxsim_fwd_host(const void* q_host, const void* d_host, co
     MMB_CHECK_CUDA(cudaEventRecord(hp->filled[b], hp->copy));
     MMB_CHECK_CUDA(cudaStreamWaitEvent(hp->compute, hp->filled[b], 0));
     MaxsimParams P;
-    P.q = dq; P.d = slab; P.q_mask = dqm; P.d_mask = d_mask_host ? slab + slab_docs : nullptr;
-    P.pair_q = nullptr; P.pair_d = nullptr; P.pair_dmask = nullptr; P.rows_needed = nullptr; P.out = hp->out + lo; P.argmax = nullptr;
-    P.doc_offsets = nullptr; P.n_rows = 0;
+    P.q = dq; P.d = slab; P.q_mask = dqm; P.d_mask = d_mask_host ? slab + slab_docs : nullptr; P.out = hp->out + lo;
     P.n_q = n_q; P.n_d = n; P.n_pairs = n; P.pair_base = lo; P.docs_per_query = docs_per_query;
     P.Lq = Lq; P.Ld = Ld; P.dim = dim; P.mask_dtype = mask_dtype;
     if (int rc = maxsim_fwd_device(P, dtype, MMB200_IMPL_AUTO, hp->compute)) return rc;

@@ -34,6 +34,7 @@
 
 #include <algorithm>
 
+#include "device_util.cuh"
 #include "host_util.cuh"
 #include "masks.cuh"
 #include "maxsim.cuh"
@@ -182,9 +183,8 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  const int64_t per = P.n_pairs / gridDim.x, rem = P.n_pairs % gridDim.x;
-  const int64_t p_begin = (int64_t)blockIdx.x * per + min((int64_t)blockIdx.x, rem);
-  const int64_t p_end = p_begin + per + ((int64_t)blockIdx.x < rem ? 1 : 0);
+  int64_t p_begin, p_end;
+  cta_share(P.n_pairs, &p_begin, &p_end);
 
   if (threadIdx.x == 0) {
     prefetch_tensormap(&tmap_q);

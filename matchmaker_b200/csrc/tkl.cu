@@ -16,6 +16,7 @@
 #include <cstdio>
 #include <cstdlib>
 
+#include "device_util.cuh"
 #include "host_util.cuh"
 #include "masks.cuh"
 #include "tkl.cuh"
@@ -32,25 +33,7 @@ constexpr int kWinPairs = kWindow / 2;  // 15
 constexpr int kRing = 2 * kPairsPerChunk;  // pairs kept: previous + current chunk
 constexpr int kZStride = kRing + 1;        // odd strides: the window phase walks query rows across lanes
 constexpr int kMaxLq = 40;
-constexpr float kTiny = 1e-13f;
 constexpr float kClamp = 1e-10f;
-
-__device__ __forceinline__ float ex2a(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-__device__ __forceinline__ float lg2a(float x) {
-  float y;
-  asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
-__host__ __device__ inline int tkl_row_stride(int D) {
-  int dp = (D + 3) & ~3;
-  if (((dp >> 2) & 1) == 0) dp += 4;
-  return dp;
-}
 
 // rows -> smem, L2-normalised; one warp per row.  Optionally dots the RAW row with `red_w`.
 __device__ __forceinline__ void load_rows_norm(const float* __restrict__ src, int nrows_valid, int nrows, int D, int dp,
@@ -77,7 +60,7 @@ __device__ __forceinline__ void load_rows_norm(const float* __restrict__ src, in
         ss += __shfl_xor_sync(0xffffffffu, ss, o);
         rd += __shfl_xor_sync(0xffffffffu, rd, o);
       }
-      const float inv = 1.0f / (sqrtf(ss) + kTiny);
+      const float inv = 1.0f / (sqrtf(ss) + kTinyNorm);
       __syncwarp();
       for (int c = lane; c < d4; c += 32) {
         float4 v = *reinterpret_cast<float4*>(drow + 4 * c);
@@ -135,7 +118,7 @@ __global__ void __launch_bounds__(kThreads) tkl_window_kernel(TklParams P, long 
     }
   };
   extern __shared__ __align__(16) float sm[];
-  const int D = P.D, dp = tkl_row_stride(D), Lq = P.Lq, K = P.K;
+  const int D = P.D, dp = padded_row_stride(D), Lq = P.Lq, K = P.K;
   float* qs = sm;                                   // [40][dp]  normalised query rows
   float* ds = qs + (size_t)kMaxLq * dp;             // [40][dp]  normalised chunk rows
   float* cs = ds + (size_t)kChunk * dp;             // [40][41]
@@ -158,7 +141,7 @@ __global__ void __launch_bounds__(kThreads) tkl_window_kernel(TklParams P, long 
   if (t < KB) {
     const bool ok = t < K;
     mu_s[t] = ok ? P.mu[t] : 0.f;
-    a_s[t] = ok ? sqrtf(0.5f * 1.4426950408889634f) / P.sigma[t] : 0.f;
+    a_s[t] = ok ? rbf_scale(P.sigma[t]) : 0.f;
     w_s[t] = ok ? P.dense_w[t] : 0.f;
     km_s[t] = (ok && P.saturation == 1) ? P.sat_params[t] : 1.f;
   }
@@ -202,8 +185,8 @@ __global__ void __launch_bounds__(kThreads) tkl_window_kernel(TklParams P, long 
 #pragma unroll
           for (int k = 0; k < KB; ++k) {
             const float x0 = (c0 - mu_s[k]) * a_s[k], x1 = (c1 - mu_s[k]) * a_s[k];
-            const float v0 = (m0 && k < K) ? ex2a(-x0 * x0) : 0.f;
-            const float v1 = (m1 && k < K) ? ex2a(-x1 * x1) : 0.f;
+            const float v0 = (m0 && k < K) ? ex2_approx(-x0 * x0) : 0.f;
+            const float v1 = (m1 && k < K) ? ex2_approx(-x1 * x1) : 0.f;
             s0 += v0; s1 += v1;
             u[k] = v0 + v1;
           }
@@ -250,7 +233,7 @@ __global__ void __launch_bounds__(kThreads) tkl_window_kernel(TklParams P, long 
           const float sat3 = y0 * sp[10] + y1 * sp[11] + sp[12];
 #pragma unroll
           for (int k = 0; k < KB; ++k) {
-            const float pw = ex2a(sat2 * lg2a(fmaxf(S[k], kClamp)));
+            const float pw = ex2_approx(sat2 * lg2_approx(fmaxf(S[k], kClamp)));
             Tp[k] = (k < K) ? (sat1 * pw - sat3) * gate : 0.f;
           }
         } else {
@@ -420,11 +403,7 @@ extern "C" int mmb200_tkl_window_scores(const float* q, const void* q_mask, cons
   if (q_mask || chunk_mask) MMB_REQUIRE(mask_dtype_size(mask_dtype) != 0, "unknown mask dtype");
   if (B == 0) return MMB200_OK;
   DeviceInfo dev;
-  if (int rc = current_device_info(&dev)) return rc;
-  if (!is_sm90(dev)) {
-    set_error("matchmaker_b200 kernels are built for sm_90a only");
-    return MMB200_ERR_UNSUPPORTED;
-  }
+  if (int rc = require_sm90(&dev)) return rc;
   TklParams P{};
   P.q = q; P.q_mask = q_mask; P.chunks = chunks; P.chunk_mask = chunk_mask; P.slot_to_packed = slot_to_packed;
   P.mu = mu; P.sigma = sigma; P.dense_w = dense_w; P.sat_red_w = sat_red_w; P.sat_params = sat_params;
@@ -438,7 +417,7 @@ extern "C" int mmb200_tkl_window_scores(const float* q, const void* q_mask, cons
   P.chunks_per_seg = (C + segs - 1) / segs;
   P.segs = (C + P.chunks_per_seg - 1) / P.chunks_per_seg;
   const int KB = K <= 12 ? 12 : 16;
-  const int dp = tkl_row_stride(D);
+  const int dp = padded_row_stride(D);
   const size_t need = ((size_t)2 * kMaxLq * dp + kMaxLq * 41 + (size_t)kMaxLq * (kRing * KB + 1) + kMaxLq * kZStride + 3 * kMaxLq +
                        4 * KB + 16 + 20 * KB + (size_t)20 * kMaxLq * KB) * sizeof(float);
   const bool ffma_fits = need <= (size_t)dev.max_smem_optin;
@@ -500,11 +479,7 @@ extern "C" int mmb200_tkl_top_hills(const float* window_score, float* orig_score
   MMB_REQUIRE(W >= 3, "need at least 3 windows");
   if (B == 0) return MMB200_OK;
   DeviceInfo dev;
-  if (int rc = current_device_info(&dev)) return rc;
-  if (!is_sm90(dev)) {
-    set_error("matchmaker_b200 kernels are built for sm_90a only");
-    return MMB200_ERR_UNSUPPORTED;
-  }
+  if (int rc = require_sm90(&dev)) return rc;
   const size_t smem = (size_t)2 * W * sizeof(float);
   MMB_REQUIRE(smem <= (size_t)dev.max_smem_optin, "too many windows for the hills kernel");
   MMB_CHECK_CUDA(cudaFuncSetAttribute(tkl_hills_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

@@ -11,6 +11,7 @@
 // The discrete parts (window "length" counts, the -9900 sentinel, argmax) carry no gradient, as in autograd.
 #include <algorithm>
 
+#include "device_util.cuh"
 #include "host_util.cuh"
 #include "masks.cuh"
 
@@ -20,7 +21,7 @@ namespace {
 
 constexpr int kThreads = 256;
 constexpr int kChunk = 40, kWindow = 30, kMaxLq = 40, kRows = 32;  // 30 window rows padded to 32
-constexpr float kTiny = 1e-13f, kClamp = 1e-10f;
+constexpr float kClamp = 1e-10f;
 constexpr int kNSat = 13;
 
 struct TklBwdParams {
@@ -33,18 +34,10 @@ struct TklBwdParams {
   int32_t Lq, D, C, K, W, mask_dtype, saturation, ws_stride;
 };
 
-__device__ __forceinline__ float ex2a(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
-
-__host__ __device__ inline int row_stride(int D) {
-  int dp = (D + 3) & ~3;
-  if (((dp >> 2) & 1) == 0) dp += 4;
-  return dp;
-}
-
 template <int KB>
 __global__ void __launch_bounds__(kThreads) tkl_bwd_kernel(TklBwdParams P) {
   extern __shared__ __align__(16) float sm[];
-  const int D = P.D, dp = row_stride(D), Lq = P.Lq, K = P.K;
+  const int D = P.D, dp = padded_row_stride(D), Lq = P.Lq, K = P.K;
   const float** rowptr = reinterpret_cast<const float**>(sm);          // [32] source row of each window position
   float** growptr = reinterpret_cast<float**>(sm) + kRows;             // [32] gradient row
   float* qs = sm + 4 * kRows;                  // [40][dp] normalised query rows (after 64 pointers = 512 B)
@@ -82,7 +75,7 @@ __global__ void __launch_bounds__(kThreads) tkl_bwd_kernel(TklBwdParams P) {
     const bool ok = t < K;
     const float sg = ok ? P.sigma[t] : 1.f;
     mu_s[t] = ok ? P.mu[t] : 0.f;
-    a_s[t] = ok ? sqrtf(0.5f * 1.4426950408889634f) / sg : 0.f;
+    a_s[t] = ok ? rbf_scale(sg) : 0.f;
     is2_s[t] = ok ? 1.f / (sg * sg) : 0.f;
     w_s[t] = ok ? P.dense_w[t] : 0.f;
     km_s[t] = (ok && P.saturation == 1) ? P.sat_params[t] : 1.f;
@@ -109,7 +102,7 @@ __global__ void __launch_bounds__(kThreads) tkl_bwd_kernel(TklBwdParams P) {
       }
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) { ss += __shfl_xor_sync(0xffffffffu, ss, o); rd += __shfl_xor_sync(0xffffffffu, rd, o); }
-      const float n = sqrtf(ss), s = n + kTiny;
+      const float n = sqrtf(ss), s = n + kTinyNorm;
       __syncwarp();
       for (int c = lane; c < D; c += 32) { drow[c] *= 1.f / s; gq[(size_t)r * dp + c] = 0.f; }
       if (lane == 0) { nq[r] = n; sq[r] = s; red[r] = rd; da0[r] = 0.f; }
@@ -167,7 +160,7 @@ __global__ void __launch_bounds__(kThreads) tkl_bwd_kernel(TklBwdParams P) {
         else for (int c = lane; c < D; c += 32) drow[c] = 0.f;
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-        const float n = sqrtf(ss), s = n + kTiny;
+        const float n = sqrtf(ss), s = n + kTinyNorm;
         __syncwarp();
         for (int c = lane; c < D; c += 32) drow[c] *= 1.f / s;
         if (lane == 0) { nd[r] = n; sd[r] = s; }
@@ -198,7 +191,7 @@ __global__ void __launch_bounds__(kThreads) tkl_bwd_kernel(TklBwdParams P) {
 #pragma unroll
           for (int k = 0; k < KB; ++k) {
             const float u = (c - mu_s[k]) * a_s[k];
-            const float v = k < K ? ex2a(-u * u) : 0.f;
+            const float v = k < K ? ex2_approx(-u * u) : 0.f;
             S[k] += v; any += v;
           }
           len += any != 0.f ? 1.f : 0.f;
@@ -272,7 +265,7 @@ __global__ void __launch_bounds__(kThreads) tkl_bwd_kernel(TklBwdParams P) {
 #pragma unroll
           for (int k = 0; k < KB; ++k) {
             const float diff = c - mu_s[k], u = diff * a_s[k];
-            G = fmaf(dS[i * KB + k] * ex2a(-u * u), -diff * is2_s[k], G);
+            G = fmaf(dS[i * KB + k] * ex2_approx(-u * u), -diff * is2_s[k], G);
           }
         }
         dc[i * 33 + r] = G;
@@ -368,11 +361,7 @@ extern "C" int mmb200_tkl_bwd(const float* q, const void* q_mask, const float* c
   MMB_REQUIRE(saturation == 0 || saturation == 1, "saturation: 0 = embedding, 1 = log");
   MMB_REQUIRE(saturation == 1 || sat_red_w != nullptr, "embedding saturation needs sat_emb_reduce1 weights");
   DeviceInfo dev;
-  if (int rc = current_device_info(&dev)) return rc;
-  if (!is_sm90(dev)) {
-    set_error("matchmaker_b200 kernels are built for sm_90a only");
-    return MMB200_ERR_UNSUPPORTED;
-  }
+  if (int rc = require_sm90(&dev)) return rc;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   TklBwdParams P{};
   P.q = q; P.q_mask = q_mask; P.chunks = chunks; P.chunk_mask = chunk_mask; P.slot_to_packed = slot_to_packed;
@@ -384,7 +373,7 @@ extern "C" int mmb200_tkl_bwd(const float* q, const void* q_mask, const float* c
   MMB_CHECK_CUDA(cudaMemsetAsync(grad_chunks, 0, (size_t)n_chunks * kChunk * D * sizeof(float), stream));
   if (B == 0) return MMB200_OK;
   const int KB = K <= 12 ? 12 : 16;
-  const int dp = row_stride(D);
+  const int dp = padded_row_stride(D);
   const size_t floats = (size_t)(2 * kMaxLq + 2 * kRows) * dp + 2 * kMaxLq * 33 + 3 * (size_t)kMaxLq * KB +
                         (size_t)kMaxLq * (kNSat + KB) + 6 * kMaxLq + 3 * kRows + 5 * KB + 16 + KB + (kNSat + KB) + 16 + 16;
   const size_t need = floats * sizeof(float) + 4 * kRows * sizeof(float) + 64;

@@ -17,7 +17,7 @@
 // Windows outside every share are exactly 0 and come from one cudaMemsetAsync.
 //
 // Per CTA (768 threads = 6 warpgroups, registers re-dealt with setmaxnreg), same operand scheme as kernel_pool_ts.cu
-// (x = hi + lo with hi = x & 0xffffe000, the document operand split in registers):
+// (x = hi + lo from split_tf32, the document operand split in registers):
 //   warp 0      TMA producer: per 32-column k-chunk up to three [40 x 32] chunk boxes + one [40 x 32] query box
 //   warps 2-3   query convert (Qhi / Qlo B operands, query norms)
 //   warps 4-7   MMA warpgroup: A fragments of the tile's 120 positions (two 64-row halves) from the raw tile, hi / lo in
@@ -36,6 +36,7 @@
 #include <cstdio>
 #include <cstdlib>
 
+#include "device_util.cuh"
 #include "host_util.cuh"
 #include "masks.cuh"
 #include "ptx.cuh"
@@ -70,7 +71,6 @@ constexpr int kCsStride = 122;            // floats per QUERY ROW of the cosine 
                                           // puts the 3-4 query rows a warp reads at once on distinct bank pairs
 constexpr int kSatStride = 33;            // table row stride (token counts 0..30)
 constexpr float kSentinel = 1.0e6f;
-constexpr float kTinyNorm = 1e-13f;
 constexpr float kClamp = 1e-10f;
 
 struct TsShared {
@@ -92,24 +92,6 @@ struct TsShared {
   float part[kEpiWarps][64];  // per-warp partial window scores
   float4 sat[kMaxLq * kSatStride];   // (sat1 * gate, sat2, sat3 * gate, -) per (query row, token count)
 };
-
-__device__ __forceinline__ float ex2f(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-__device__ __forceinline__ float lg2f(float x) {
-  float y;
-  asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
-__device__ __forceinline__ void split4(const float4 v, uint32_t* hi, uint32_t* lo) {
-  hi[0] = __float_as_uint(v.x) & 0xffffe000u; lo[0] = __float_as_uint(v.x - __uint_as_float(hi[0]));
-  hi[1] = __float_as_uint(v.y) & 0xffffe000u; lo[1] = __float_as_uint(v.y - __uint_as_float(hi[1]));
-  hi[2] = __float_as_uint(v.z) & 0xffffe000u; lo[2] = __float_as_uint(v.z - __uint_as_float(hi[2]));
-  hi[3] = __float_as_uint(v.w) & 0xffffe000u; lo[3] = __float_as_uint(v.w - __uint_as_float(hi[3]));
-}
 
 // ---------------------------------------------------------------------------------------------------------------
 // plan: tiles per document (prefix sums), the "cover" test of the kernel set, and the share of every CTA.  One block.
@@ -169,7 +151,7 @@ __global__ void __launch_bounds__(1024) tkl_plan_kernel(const int32_t* __restric
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");   // tkl_ts_kernel may start its prologue now (it waits for this grid's completion before it reads the plan)
   const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
   if (t < K && t < 32) {
-    const float h = 11.0f * sigma[t] / sqrtf(0.5f * 1.4426950408889634f);
+    const float h = 11.0f * sigma[t] / rbf_scale(1.0f);   // 11 / rbf_scale(sigma), rounded as 11 sigma / rbf_scale(1)
     klo[t] = mu[t] - h;
     khi[t] = mu[t] + h;
   }
@@ -248,7 +230,7 @@ __global__ void __launch_bounds__(1024) tkl_plan_kernel(const int32_t* __restric
   }
   if (in_smem)
     for (int64_t i = t; i <= B; i += 1024) { plan[2 + i] = s_tile[i]; plan[3 + B + i] = s_cost[i]; }
-  // Cover: activation k is non-zero (ex2.approx.ftz) for |c - mu_k| * a_k <= sqrt(126); 11.0 leaves a margin.  The union of
+  // Cover: activation k is non-zero (ex2_approx) for |c - mu_k| * a_k <= sqrt(126); 11.0 leaves a margin.  The union of
   // the intervals [klo, khi] covers [-1.01, 1.01] iff the left end and every right end inside the range lie inside an
   // interval that extends beyond them -- one thread per end point instead of a serial sweep.
   __shared__ int uncovered;
@@ -407,7 +389,7 @@ tkl_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant_
           for (int j = 0; j < 5; ++j) {
             const int row = r0 + 8 * j;
             uint32_t hi[4], lo[4];
-            split4(x[j], hi, lo);
+            split_tf32(x[j], hi, lo);
             const int off = row * 128 + ((c ^ (row & 7)) << 4);
             *reinterpret_cast<uint4*>(qo + off) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
             *reinterpret_cast<uint4*>(qo + kMaxLq * 128 + off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
@@ -479,10 +461,7 @@ tkl_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant_
                 const int ch0 = (2 * k) ^ (ra & 7), ch1 = (2 * k + 1) ^ (ra & 7);
                 const float v[4] = {x[ra * 32 + ch0 * 4 + tq], x[rc * 32 + ch0 * 4 + tq], x[ra * 32 + ch1 * 4 + tq], x[rc * 32 + ch1 * 4 + tq]};
 #pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  ah[mb][e] = __float_as_uint(v[e]) & 0xffffe000u;
-                  al[mb][e] = __float_as_uint(v[e] - __uint_as_float(ah[mb][e]));
-                }
+                for (int e = 0; e < 4; ++e) split_tf32(v[e], ah[mb][e], al[mb][e]);
                 ss[2 * mb] = fmaf(v[0], v[0], fmaf(v[2], v[2], ss[2 * mb]));
                 ss[2 * mb + 1] = fmaf(v[1], v[1], fmaf(v[3], v[3], ss[2 * mb + 1]));
               }
@@ -553,7 +532,7 @@ tkl_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant_
       const bool ik_live = et < n_ik;
       const int qi = ik_live ? et / P.K : 0;     // query row of this thread in phase B
       const int kk = ik_live ? et - qi * P.K : 0;
-      const float a_k = sqrtf(0.5f * 1.4426950408889634f) / P.sigma[kk];
+      const float a_k = rbf_scale(P.sigma[kk]);
       const float nma_k = -P.mu[kk] * a_k;        // x = (c - mu) a = c a + nma
       const float w_k = ik_live ? P.dense_w[kk] : 0.f;
       const float km_k = SAT == 1 ? P.sat_params[kk] : 1.f;
@@ -654,7 +633,7 @@ tkl_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant_
             for (int r = 0; r < kBlk; ++r) {
               const float2 c = cblk[r];
               const float x0 = fmaf(c.x, a_k, nma_k), x1 = fmaf(c.y, a_k, nma_k);
-              suf[r] = ex2f(-x0 * x0) + ex2f(-x1 * x1);
+              suf[r] = ex2_approx(-x0 * x0) + ex2_approx(-x1 * x1);
             }
 #pragma unroll
             for (int r = kBlk - 2; r >= 0; --r) suf[r] += suf[r + 1];
@@ -675,17 +654,17 @@ tkl_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant_
               for (int r = 0; r < kBlk; ++r) {
                 const float2 c = cblk[r];
                 const float x0 = fmaf(c.x, a_k, nma_k), x1 = fmaf(c.y, a_k, nma_k);
-                const float u = ex2f(-x0 * x0) + ex2f(-x1 * x1);
+                const float u = ex2_approx(-x0 * x0) + ex2_approx(-x1 * x1);
                 pre = r == 0 ? u : pre + u;
                 const float Ssum = r < kBlk - 1 ? suf[r + 1] + pre : pre;
                 suf[r] = u;   // suf[r] of the previous block was consumed by window r - 1
                 const int lenb = (int)((lw[r >> 1] >> (16 * (r & 1))) & 0xffffu);
                 if (SAT == 0) {
                   const float4 st = *reinterpret_cast<const float4*>(sat_row + lenb);
-                  const float pw = ex2f(st.y * lg2f(fmaxf(Ssum, kClamp)));
+                  const float pw = ex2_approx(st.y * lg2_approx(fmaxf(Ssum, kClamp)));
                   tv[r] = w_k * fmaf(st.x, pw, -st.z);
                 } else {
-                  const float lg = 0.6931471805599453f * lg2f(fmaxf(Ssum * km_k, kClamp));
+                  const float lg = 0.6931471805599453f * lg2_approx(fmaxf(Ssum * km_k, kClamp));
                   tv[r] = (lenb > 0 && qm_i != 0.f) ? w_k * lg : 0.f;
                 }
               }
