@@ -341,6 +341,44 @@ MMB200_API int mmb200_topk_unique(const float* cand_scores, const int64_t* cand_
                                   int64_t* out_ids, int64_t nq, int32_t n_candidates, int32_t k, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Inverted-file (IVF) search: exact top-k over the rows of each query's probed lists
+ *
+ * Replaces: FaissIVFIndexer.search   matchmaker/retrieval/faiss_indices.py:106-145
+ *           (faiss IndexIVFFlat / IndexIVFScalarQuantizer QT_fp16, METRIC_INNER_PRODUCT, GPU).
+ *
+ * rows     [n_rows, dim] (fp16 / bf16) or [n_rows, 2*dim] (MMB200_F32_SPLIT16, as for mmb200_flat_ip_topk): the
+ *          index rows sorted by list; list l is rows [list_offsets[l], list_offsets[l+1]) (int64 [nlist + 1],
+ *          non-decreasing, list_offsets[nlist] <= n_rows).  ids [n_rows] int64 user ids of those rows (any value).
+ * queries  [nq, dim] in the rows' dtype ([nq, 3*dim] for MMB200_F32_SPLIT16; scores are then in the scaled domain).
+ * probes   [nq, nprobe] int64 list ids, distinct within a row; an id outside [0, nlist) (the -1 filler of a coarse
+ *          search over fewer than nprobe lists) probes nothing.
+ * max_list_len: an upper bound of every list's length; a query's candidates from one list are kept in a slot of
+ *          min(k, max_list_len) rounded up to 32 entries.  A list longer than the bound loses candidates (no fault).
+ * out_scores / out_ids [nq, k]: the k best rows of the union of the probed lists under (score desc, id asc); fewer
+ *          than k rows give the (-3.4028235e38, -1) tail.
+ * The probe table is inverted on the device into per-list query sets; every (list, chunk of <= 128 probing queries) is
+ * one work item of the flat-IP tensor-core kernel, which reads the list once per chunk.  No host synchronisation.
+ * Envelope: 1 <= k <= 1024, 1 <= nprobe <= 1024, dim % 64 == 0, n_rows < 2^31 - 128, nq * nprobe < 2^31 - 128,
+ * 16-byte aligned queries and rows.  Outside it: MMB200_ERR_INVALID.  Not sm_90: MMB200_ERR_UNSUPPORTED.
+ * workspace: device scratch of at least mmb200_ivf_workspace_bytes(...) bytes, about nq * nprobe * (2 * qcols + 12 *
+ * slot) bytes (qcols = dim, or 3 * dim for the split); 0 = sizes outside the envelope, -1 = no device.
+ * ------------------------------------------------------------------------------------------ */
+MMB200_API int64_t mmb200_ivf_workspace_bytes(int64_t nq, int32_t nprobe, int64_t nlist, int64_t max_list_len,
+                                              int32_t dim, int32_t k, int32_t dtype);
+MMB200_API int mmb200_ivf_search(const void* queries, const void* rows, const int64_t* ids,
+                                 const int64_t* list_offsets, const int64_t* probes, float* out_scores,
+                                 int64_t* out_ids, void* workspace, int64_t workspace_bytes, int64_t nq,
+                                 int32_t nprobe, int64_t nlist, int64_t n_rows, int64_t max_list_len, int32_t dim,
+                                 int32_t k, int32_t dtype, void* stream);
+
+/* Spherical k-means centroid update: out[l] = normalised mean of rows perm[offsets[l] .. offsets[l+1]) of x
+ * ([n, dim] fp16 / bf16 / fp32, `dtype`).  The sum runs in that order in fp64, so the result is bit-reproducible;
+ * an empty list gives a zero row.  perm [offsets[nlist]] int64, out [nlist, dim] f32.  1 <= dim <= 4096, else
+ * MMB200_ERR_INVALID. */
+MMB200_API int mmb200_ivf_list_means(const void* x, const int64_t* perm, const int64_t* offsets, float* out,
+                                     int64_t nlist, int32_t dim, int32_t dtype, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Storage block loader: byte ranges of files -> one contiguous DEVICE buffer.
  *
  * Replaces: the host path of the encoded collection between matchmaker/dense_retrieval.py:291-302

@@ -33,6 +33,7 @@
 #include <cstdlib>
 #include <type_traits>
 
+#include "device_util.cuh"
 #include "host_util.cuh"
 #include "ptx.cuh"
 
@@ -70,8 +71,18 @@ struct FipParams {
   int32_t n_qblocks, n_ranges, tiles_per_range, n_tiles;
   uint2* lists;             // [grid][BM][cap]  (score bits, position)
   uint32_t* tau_glob;       // [nq] order-preserving image of the per-query threshold
-  float* cand_scores;       // [nq][n_ranges * kpad]
-  int64_t* cand_ids;        // [nq][n_ranges * kpad]
+  float* cand_scores;       // [nq][n_ranges * kpad]; IVF mode: [n_pairs][kpad]
+  int64_t* cand_ids;        // [nq][n_ranges * kpad]; IVF mode: [n_pairs][kpad]
+};
+
+// IVF mode only (flat_ip_tc_kernel<..., true>): a work item is (list, up to BM queries probing it).  A separate kernel
+// parameter, so that the flat-IP instantiations keep their parameter block (compact_row takes FipParams by reference).
+struct IvfParams {
+  const int4* items;        // [*n_items] (list, first row of the gathered queries, query rows, 0)
+  const int32_t* n_items;   // written on the device by ivf_scan_kernel
+  const int64_t* offsets;   // [nlist + 1] row range of every list in the sorted layout
+  const int32_t* pair;      // gathered query row -> its (query, probe) pair q * nprobe + j
+  int32_t nprobe;
 };
 
 // order-preserving map float -> uint32 (larger float <=> larger key)
@@ -197,9 +208,16 @@ __device__ __forceinline__ void wgmma_n128<__nv_bfloat16>(float (&d)[64], uint64
   wgmma_m64n128k16_bf16(d, a, b, acc);
 }
 
-template <typename T, int CL, int EPL = 32>
+// IVF = true: the probed-list scan of mmb200_ivf_search.  A work item is (list, chunk of <= BM probing queries) from
+// V.items; the query tile is the chunk's rows of the pre-gathered queries (TMA cannot gather rows), the passage tiles
+// are the list's row range, and rows past the list end are never candidates.  Each row of the chunk keeps its own list
+// and publishes into its (query, probe) slot; tau_glob stays per query, since the k-th best score a query has in any of
+// its lists bounds all of them.  Runs with CL = 1.  The mode only changes where an item's rows and tiles come from, so it
+// is a template flag: with IVF = false every branch below folds away.
+template <typename T, int CL, int EPL = 32, bool IVF = false>
 __global__ void __launch_bounds__(kThreads, 1)
-flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_p, FipParams P) {
+flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_p, FipParams P,
+                  IvfParams V) {
   extern __shared__ uint8_t smem_raw[];
   // 1024-B alignment for SWIZZLE_128B tiles, derived by pointer arithmetic on the __shared__ array so the
   // compiler keeps the shared address space (LDS/STS instead of generic LD/ST)
@@ -210,7 +228,7 @@ flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int kblocks = P.kblocks;
   const int n_qgroups = (P.n_qblocks + CL - 1) / CL;   // CL consecutive query blocks per cluster work item
-  const int n_items = n_qgroups * P.n_ranges;
+  const int n_items = IVF ? *V.n_items : n_qgroups * P.n_ranges;
   const int rank = CL > 1 ? (int)cluster_ctarank() : 0;
   const int cluster_id = blockIdx.x / CL, n_clusters = gridDim.x / CL;
   constexpr uint16_t kAllCtas = (uint16_t)((1u << CL) - 1u);
@@ -232,8 +250,19 @@ flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
     int stage = 0;
     uint32_t phase = 0;
     for (int item = cluster_id; item < n_items; item += n_clusters) {
-      const int rg = item / n_qgroups, qb = (item % n_qgroups) * CL + rank;  // range-major: co-running CTAs share passages
-      const int t0 = rg * P.tiles_per_range, t1 = min(P.n_tiles, t0 + P.tiles_per_range);
+      int t0, t1, qrow0, prow0 = 0;
+      if constexpr (IVF) {
+        const int4 it = V.items[item];
+        prow0 = (int)V.offsets[it.x];
+        t0 = 0;
+        t1 = (int)((V.offsets[it.x + 1] - prow0 + BN - 1) / BN);
+        qrow0 = it.y;
+      } else {
+        const int rg = item / n_qgroups, qb = (item % n_qgroups) * CL + rank;  // range-major: co-running CTAs share passages
+        t0 = rg * P.tiles_per_range;
+        t1 = min(P.n_tiles, t0 + P.tiles_per_range);
+        qrow0 = qb * BM;
+      }
       for (int t = t0; t < t1; ++t) {
         for (int kb = 0; kb < kblocks; ++kb) {
           mbar_wait(&S->empty[stage], phase ^ 1u);
@@ -241,9 +270,9 @@ flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
           if (elect_one_sync()) {
             mbar_arrive_expect_tx(&S->full[stage], (uint32_t)kStageBytes);
             const int kbp = kb < P.kb_wrap ? kb : kb - P.kb_wrap;   // fp32-split storage: [q_hi|q_lo|q_hi] x [p_hi|p_hi|p_lo]
-            tma_load_2d(&tmap_q, st, &S->full[stage], kb * 64, qb * BM, kEvictLast);
+            tma_load_2d(&tmap_q, st, &S->full[stage], kb * 64, qrow0, kEvictLast);
             if (CL == 1)
-              tma_load_2d(&tmap_p, st + kABytes, &S->full[stage], kbp * 64, t * BN, kEvictFirst);
+              tma_load_2d(&tmap_p, st + kABytes, &S->full[stage], kbp * 64, prow0 + t * BN, kEvictFirst);
             else  // this CTA's slice of the passage tile, written into every CTA of the cluster
               tma_load_2d_multicast(&tmap_p, st + kABytes + rank * (kBBytes / CL), &S->full[stage], kbp * 64,
                                     t * BN + rank * (BN / CL), kAllCtas, kEvictFirst);
@@ -280,10 +309,28 @@ flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
     const int fr0 = 64 * c + 16 * wq + (lane >> 2);   // score-tile rows of this thread's accumulator fragment: fr0, fr0 + 8
     const int fc0 = 2 * (lane & 3);
     for (int item = cluster_id; item < n_items; item += n_clusters) {
-      const int rg = item / n_qgroups, qb = (item % n_qgroups) * CL + rank;  // range-major: co-running CTAs share passages
-      const int t0 = rg * P.tiles_per_range, t1 = min(P.n_tiles, t0 + P.tiles_per_range);
-      const int64_t q = (int64_t)qb * BM + row;
-      const bool live = q < P.nq;
+      int rg, qb, t0, t1;
+      int64_t q, prow0 = 0, row_end = P.n_pass;   // rows [prow0, row_end) of the passages are candidates
+      int32_t pair = -1;
+      bool live;
+      if constexpr (IVF) {
+        const int4 it = V.items[item];
+        rg = qb = 0;
+        prow0 = V.offsets[it.x];
+        row_end = V.offsets[it.x + 1];
+        t0 = 0;
+        t1 = (int)((row_end - prow0 + BN - 1) / BN);
+        live = row < it.z;
+        pair = live ? V.pair[it.y + row] : -1;
+        q = live ? pair / V.nprobe : -1;
+      } else {
+        rg = item / n_qgroups;
+        qb = (item % n_qgroups) * CL + rank;  // range-major: co-running CTAs share passages
+        t0 = rg * P.tiles_per_range;
+        t1 = min(P.n_tiles, t0 + P.tiles_per_range);
+        q = (int64_t)qb * BM + row;
+        live = q < P.nq;
+      }
       uint32_t tau_seen = live ? P.tau_glob[q] : 0xffffffffu;  // dead rows accept nothing
       if (half == 0) { cnt_s[lane] = 0; tau_s[lane] = tau_seen; }
       for (int t = t0; t < t1; ++t) {
@@ -347,18 +394,20 @@ flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
             uint32_t kth;
             const int nc = compact_row<EPL>(P, warp_lists + (size_t)rr * kCap, cnt_s[rr], lane, &kth);
             __syncwarp();
+            int64_t q_rr = -1;   // IVF: the query of row rr
+            if constexpr (IVF) q_rr = __shfl_sync(0xffffffffu, q, rr);
             if (lane == 0) {
               cnt_s[rr] = nc;
               tau_s[rr] = max(tau_s[rr], kth);
-              const int64_t qq = (int64_t)qb * BM + quarter * 32 + rr;
-              if (qq < P.nq) atomicMax(P.tau_glob + qq, kth);
+              const int64_t qq = IVF ? q_rr : (int64_t)qb * BM + quarter * 32 + rr;
+              if (IVF ? qq >= 0 : qq < P.nq) atomicMax(P.tau_glob + qq, kth);
             }
           }
           named_bar_sync(pair_bar, 64);
         }
         const float tau = key2f(tau_s[lane]);
-        const int64_t col0 = (int64_t)t * BN + half * (BN / 2);
-        const bool ragged = (int64_t)t * BN + BN > P.n_pass;
+        const int64_t col0 = prow0 + (int64_t)t * BN + half * (BN / 2);
+        const bool ragged = prow0 + (int64_t)t * BN + BN > row_end;
 #pragma unroll
         for (int cc = 0; cc < BN / 2 / 32; ++cc) {
           uint32_t (&r)[32] = r4[cc];
@@ -385,7 +434,7 @@ flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {
                   bool pass = __uint_as_float(r[8 * i + j]) >= tau;
-                  if (ragged) pass = pass && (int64_t)(pbase + 8 * i + j) < P.n_pass;
+                  if (ragged) pass = pass && (int64_t)(pbase + 8 * i + j) < row_end;
                   e[j] = pass ? (1u << j) : 0u;
                 }
                 uint32_t m = ((e[0] | e[1]) | (e[2] | e[3])) | ((e[4] | e[5]) | (e[6] | e[7]));
@@ -415,12 +464,18 @@ flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
       for (int rr = half; rr < 32; rr += 2) {
         uint32_t kth;
         const int nc = compact_row<EPL>(P, warp_lists + (size_t)rr * kCap, cnt_s[rr], lane, &kth);
-        const int64_t qq = (int64_t)qb * BM + quarter * 32 + rr;
-        if (qq < P.nq) {
+        int64_t q_rr = -1;   // IVF: the query of row rr and its output slot
+        size_t slot_rr = 0;
+        if constexpr (IVF) {
+          q_rr = __shfl_sync(0xffffffffu, q, rr);
+          slot_rr = (size_t)__shfl_sync(0xffffffffu, pair, rr) * P.kpad;
+        }
+        const int64_t qq = IVF ? q_rr : (int64_t)qb * BM + quarter * 32 + rr;
+        if (IVF ? qq >= 0 : qq < P.nq) {
           if (lane == 0 && nc == P.k) atomicMax(P.tau_glob + qq, kth);
           const uint2* lst = warp_lists + (size_t)rr * kCap;
-          float* cso = P.cand_scores + (size_t)qq * P.n_ranges * P.kpad + (size_t)rg * P.kpad;
-          int64_t* ci = P.cand_ids + (size_t)qq * P.n_ranges * P.kpad + (size_t)rg * P.kpad;
+          float* cso = IVF ? P.cand_scores + slot_rr : P.cand_scores + (size_t)qq * P.n_ranges * P.kpad + (size_t)rg * P.kpad;
+          int64_t* ci = IVF ? P.cand_ids + slot_rr : P.cand_ids + (size_t)qq * P.n_ranges * P.kpad + (size_t)rg * P.kpad;
           for (int e = lane; e < P.kpad; e += 32) {
             if (e < nc) {
               const uint2 v = lst[e];
@@ -654,6 +709,122 @@ int launch_merge(const float* cand_scores, const int64_t* cand_ids, int64_t nq, 
   return rc;
 }
 
+// ---------------------------------------------------------------------------------------------
+// IVF probed-list scan: invert the probe table [nq, nprobe] into per-list query sets on the device, gather the probing
+// queries list by list, scan every (list, chunk of <= BM queries) item with flat_ip_tc_kernel<..., IVF = true>, merge
+// the per-(query, probe) slots.  Nothing is read back to the host: the item count stays in device memory.
+// ---------------------------------------------------------------------------------------------
+constexpr int kIvfMaxProbe = 1024;
+
+// probes per list
+__global__ void ivf_count_kernel(const int64_t* __restrict__ probes, int64_t n_pairs, int64_t nlist, int* __restrict__ cnt) {
+  for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < n_pairs; p += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t l = probes[p];
+    if (l >= 0 && l < nlist) atomicAdd(cnt + l, 1);
+  }
+}
+
+// One block of 1024 threads: exclusive scans of the probe counts (first gathered row of each list) and of the item
+// counts ceil(cnt / BM) (first item of each list); the total item count goes to *n_items.  Thread t scans a contiguous
+// segment, so the result does not depend on scheduling.
+__global__ void __launch_bounds__(1024) ivf_scan_kernel(const int* __restrict__ cnt, int64_t nlist,
+                                                        int* __restrict__ row_base, int* __restrict__ item_base,
+                                                        int* __restrict__ n_items) {
+  __shared__ int s_rows[1024], s_items[1024];
+  const int t = threadIdx.x;
+  const int64_t seg = (nlist + 1023) / 1024, lo = min(nlist, t * seg), hi = min(nlist, lo + seg);
+  int rows = 0, items = 0;
+  for (int64_t l = lo; l < hi; ++l) { rows += cnt[l]; items += (cnt[l] + BM - 1) / BM; }
+  s_rows[t] = rows;
+  s_items[t] = items;
+  __syncthreads();
+  for (int o = 1; o < 1024; o <<= 1) {   // inclusive Hillis-Steele scan
+    const int r = t >= o ? s_rows[t - o] : 0, i = t >= o ? s_items[t - o] : 0;
+    __syncthreads();
+    s_rows[t] += r;
+    s_items[t] += i;
+    __syncthreads();
+  }
+  rows = s_rows[t] - rows;
+  items = s_items[t] - items;
+  for (int64_t l = lo; l < hi; ++l) {
+    row_base[l] = rows;
+    item_base[l] = items;
+    rows += cnt[l];
+    items += (cnt[l] + BM - 1) / BM;
+  }
+  if (t == 1023) *n_items = s_items[1023];
+}
+
+// One warp per (query, probe) pair: take the next row of the probed list's query set and copy the query there.  A pair
+// whose list id is out of range (a -1 filler of the coarse search) probes nothing: its slot is filled as empty.
+__global__ void ivf_gather_kernel(const int64_t* __restrict__ probes, int64_t n_pairs, int64_t nlist, int nprobe,
+                                  const int* __restrict__ row_base, int* __restrict__ fill, const uint4* __restrict__ queries,
+                                  int row_vecs, uint4* __restrict__ gathered, int32_t* __restrict__ pair_of_row,
+                                  float* __restrict__ cand_scores, int64_t* __restrict__ cand_ids, int kslot) {
+  const int lane = threadIdx.x & 31;
+  const int64_t warp0 = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5, n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  for (int64_t p = warp0; p < n_pairs; p += n_warps) {
+    const int64_t l = probes[p];
+    const bool ok = l >= 0 && l < nlist;
+    int r = 0;
+    if (ok && lane == 0) r = row_base[l] + atomicAdd(fill + l, 1);
+    r = __shfl_sync(0xffffffffu, r, 0);
+    if (ok) {
+      const uint4* src = queries + (p / nprobe) * row_vecs;
+      uint4* dst = gathered + (int64_t)r * row_vecs;
+      for (int v = lane; v < row_vecs; v += 32) dst[v] = src[v];
+      if (lane == 0) pair_of_row[r] = (int32_t)p;
+    } else {
+      for (int e = lane; e < kslot; e += 32) {
+        cand_scores[p * kslot + e] = -INFINITY;
+        cand_ids[p * kslot + e] = -1;
+      }
+    }
+  }
+}
+
+// The work items of every list: (list, first gathered row, rows), in list order.
+__global__ void ivf_items_kernel(const int* __restrict__ cnt, int64_t nlist, const int* __restrict__ row_base,
+                                 const int* __restrict__ item_base, int4* __restrict__ items) {
+  for (int64_t l = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; l < nlist; l += (int64_t)gridDim.x * blockDim.x) {
+    const int c = cnt[l];
+    for (int j = 0; j * BM < c; ++j)
+      items[item_base[l] + j] = make_int4((int)l, row_base[l] + j * BM, min(BM, c - j * BM), 0);
+  }
+}
+
+struct IvfLayout {
+  size_t tau, lists, cand_s, cand_i, gathered, pair, cnt, fill, row_base, item_base, items, n_items, total;
+  int kslot, grid;
+  int64_t n_pairs, max_items;
+};
+
+// slot = per-(query, probe) candidates: a list of len rows yields at most min(k, len) of them
+IvfLayout ivf_layout(int64_t nq, int nprobe, int64_t nlist, int64_t max_list_len, int qcols, int k, int sm_count) {
+  IvfLayout L{};
+  L.grid = sm_count;
+  L.n_pairs = nq * nprobe;
+  L.kslot = (int)((std::min<int64_t>(k, std::max<int64_t>(1, max_list_len)) + 31) / 32 * 32);
+  L.max_items = std::min<int64_t>(nlist, L.n_pairs) + (L.n_pairs + BM - 1) / BM;
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t o = off; off += align256(bytes); return o; };
+  L.tau = take((size_t)nq * sizeof(uint32_t));
+  L.lists = take((size_t)L.grid * BM * 32 * epl_for_k(k) * sizeof(uint2));
+  L.cand_s = take((size_t)L.n_pairs * L.kslot * sizeof(float));
+  L.cand_i = take((size_t)L.n_pairs * L.kslot * sizeof(int64_t));
+  L.gathered = take((size_t)L.n_pairs * qcols * 2);
+  L.pair = take((size_t)L.n_pairs * sizeof(int32_t));
+  L.cnt = take((size_t)nlist * sizeof(int));
+  L.fill = take((size_t)nlist * sizeof(int));
+  L.row_base = take((size_t)nlist * sizeof(int));
+  L.item_base = take((size_t)nlist * sizeof(int));
+  L.items = take((size_t)L.max_items * sizeof(int4));
+  L.n_items = take(sizeof(int));
+  L.total = off;
+  return L;
+}
+
 }  // namespace
 
 }  // namespace mmb
@@ -752,7 +923,7 @@ extern "C" int mmb200_flat_ip_topk(const void* queries, const void* passages, co
       attr.val.clusterDim.z = 1;
       cfg.attrs = &attr;
       cfg.numAttrs = 1;
-      MMB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel, tq, tp, P));
+      MMB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel, tq, tp, P, IvfParams{}));
       return MMB200_OK;
     };
     if (out_params) *out_params = P;
@@ -800,4 +971,164 @@ extern "C" int mmb200_topk_unique(const float* cand_scores, const int64_t* cand_
   if (int rc = require_sm90(&dev)) return rc;
   return launch_merge(cand_scores, cand_ids, nq, n_candidates, k, out_scores, out_ids, dev, static_cast<cudaStream_t>(stream_),
                       true);
+}
+
+extern "C" int64_t mmb200_ivf_workspace_bytes(int64_t nq, int32_t nprobe, int64_t nlist, int64_t max_list_len, int32_t dim,
+                                              int32_t k, int32_t dtype) {
+  using namespace mmb;
+  if (nq <= 0 || nprobe <= 0 || nprobe > kIvfMaxProbe || nlist <= 0 || k <= 0 || k > kMaxK || dim <= 0 || dim % 64 ||
+      nq * nprobe >= (1ll << 31) - BM)
+    return 0;
+  if (dtype != MMB200_F16 && dtype != MMB200_BF16 && dtype != MMB200_F32_SPLIT16) return 0;
+  DeviceInfo dev;
+  if (current_device_info(&dev)) return -1;
+  const int qcols = dtype == MMB200_F32_SPLIT16 ? 3 * dim : dim;
+  return (int64_t)ivf_layout(nq, nprobe, nlist, max_list_len, qcols, k, dev.sm_count).total;
+}
+
+extern "C" int mmb200_ivf_search(const void* queries, const void* rows, const int64_t* ids, const int64_t* list_offsets,
+                                 const int64_t* probes, float* out_scores, int64_t* out_ids, void* workspace,
+                                 int64_t workspace_bytes_given, int64_t nq, int32_t nprobe, int64_t nlist, int64_t n_rows,
+                                 int64_t max_list_len, int32_t dim, int32_t k, int32_t dtype, void* stream_) {
+  using namespace mmb;
+  MMB_REQUIRE(queries && rows && ids && list_offsets && probes && out_scores && out_ids && workspace, "null pointer");
+  MMB_REQUIRE(nq > 0 && nlist > 0 && n_rows > 0, "need at least one query, one list and one row");
+  MMB_REQUIRE(k >= 1 && k <= kMaxK, "fused top-k supports 1 <= k <= 1024");
+  MMB_REQUIRE(nprobe >= 1 && nprobe <= kIvfMaxProbe, "1 <= nprobe <= 1024");
+  MMB_REQUIRE(dtype == MMB200_F16 || dtype == MMB200_BF16 || dtype == MMB200_F32_SPLIT16,
+              "list storage must be fp16, bf16 or the fp16 hi/lo split of fp32 (MMB200_F32_SPLIT16)");
+  MMB_REQUIRE(dim % 64 == 0 && dim >= 64, "vector dim must be a multiple of 64");
+  MMB_REQUIRE(n_rows < (1ll << 31) - BN, "at most 2^31 - 128 rows per shard");
+  MMB_REQUIRE(max_list_len >= 0 && max_list_len <= n_rows, "max_list_len must bound the list lengths");
+  MMB_REQUIRE(nq * nprobe < (1ll << 31) - BM, "nq * nprobe must stay below 2^31 (search the queries in batches)");
+  MMB_REQUIRE(((reinterpret_cast<uintptr_t>(queries) | reinterpret_cast<uintptr_t>(rows)) & 15) == 0, "16-byte alignment");
+  DeviceInfo dev;
+  if (int rc = require_sm90(&dev)) return rc;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const bool split = dtype == MMB200_F32_SPLIT16;
+  const int qcols = split ? 3 * dim : dim, pcols = split ? 2 * dim : dim;
+  const IvfLayout L = ivf_layout(nq, nprobe, nlist, max_list_len, qcols, k, dev.sm_count);
+  MMB_REQUIRE((size_t)workspace_bytes_given >= L.total, "workspace too small (see mmb200_ivf_workspace_bytes)");
+  uint8_t* w = static_cast<uint8_t*>(workspace);
+  int* cnt = reinterpret_cast<int*>(w + L.cnt);
+  int* fill = reinterpret_cast<int*>(w + L.fill);
+  int* row_base = reinterpret_cast<int*>(w + L.row_base);
+  int* item_base = reinterpret_cast<int*>(w + L.item_base);
+  int4* items = reinterpret_cast<int4*>(w + L.items);
+  int* n_items = reinterpret_cast<int*>(w + L.n_items);
+  int32_t* pair_of_row = reinterpret_cast<int32_t*>(w + L.pair);
+  uint4* gathered = reinterpret_cast<uint4*>(w + L.gathered);
+
+  // probe table -> per-list query sets -> work items
+  MMB_CHECK_CUDA(cudaMemsetAsync(cnt, 0, L.row_base - L.cnt, stream));   // cnt and fill
+  const int g = std::max(1, std::min(dev.sm_count * 8, (int)((L.n_pairs + 255) / 256)));
+  ivf_count_kernel<<<g, 256, 0, stream>>>(probes, L.n_pairs, nlist, cnt);
+  ivf_scan_kernel<<<1, 1024, 0, stream>>>(cnt, nlist, row_base, item_base, n_items);
+  ivf_gather_kernel<<<std::max(1, std::min(dev.sm_count * 8, (int)((L.n_pairs + 7) / 8))), 256, 0, stream>>>(
+      probes, L.n_pairs, nlist, nprobe, row_base, fill, static_cast<const uint4*>(queries), qcols * 2 / 16, gathered,
+      pair_of_row, reinterpret_cast<float*>(w + L.cand_s), reinterpret_cast<int64_t*>(w + L.cand_i), L.kslot);
+  ivf_items_kernel<<<std::max(1, std::min(dev.sm_count * 4, (int)((nlist + 255) / 256))), 256, 0, stream>>>(
+      cnt, nlist, row_base, item_base, items);
+  uint32_t* tau_glob = reinterpret_cast<uint32_t*>(w + L.tau);
+  fill_u32<<<64, 256, 0, stream>>>(tau_glob, nq, kKeyNegInf);
+  MMB_CHECK_CUDA(cudaGetLastError());
+
+  const CUtensorMapDataType tdt = dtype == MMB200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  CUtensorMap tq, tp;
+  {
+    const uint64_t dims[2] = {(uint64_t)qcols, (uint64_t)L.n_pairs};
+    const uint64_t strides[1] = {(uint64_t)qcols * 2};
+    const uint32_t box[2] = {64, BM};
+    if (int rc = encode_tensor_map(&tq, tdt, 2, gathered, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B,
+                                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B))
+      return rc;
+  }
+  {
+    const uint64_t dims[2] = {(uint64_t)pcols, (uint64_t)n_rows};
+    const uint64_t strides[1] = {(uint64_t)pcols * 2};
+    const uint32_t box[2] = {64, BN};
+    if (int rc = encode_tensor_map(&tp, tdt, 2, rows, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B,
+                                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B))
+      return rc;
+  }
+  FipParams P{};
+  P.ids = ids; P.id_base = 0; P.nq = nq; P.n_pass = n_rows; P.dim = dim; P.k = k; P.kpad = L.kslot;
+  P.kblocks = qcols / 64;
+  P.kb_wrap = split ? dim / 64 : P.kblocks;
+  P.n_qblocks = 0; P.n_ranges = 1; P.tiles_per_range = 0; P.n_tiles = 0;
+  P.tau_glob = tau_glob;
+  P.lists = reinterpret_cast<uint2*>(w + L.lists);
+  P.cand_scores = reinterpret_cast<float*>(w + L.cand_s);
+  P.cand_ids = reinterpret_cast<int64_t*>(w + L.cand_i);
+  const IvfParams V{items, n_items, list_offsets, pair_of_row, nprobe};
+  const size_t smem = (size_t)kStages * kStageBytes + (size_t)BM * kCsStride * sizeof(float) + sizeof(FipShared) + 1024;
+  auto launch = [&](auto kernel) -> int {
+    MMB_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<L.grid, kThreads, smem, stream>>>(tq, tp, P, V);
+    MMB_CHECK_CUDA(cudaGetLastError());
+    return MMB200_OK;
+  };
+  int rc;
+  const bool e32 = epl_for_k(k) == 32;
+  if (dtype == MMB200_BF16)
+    rc = e32 ? launch(flat_ip_tc_kernel<__nv_bfloat16, 1, 32, true>) : launch(flat_ip_tc_kernel<__nv_bfloat16, 1, 64, true>);
+  else
+    rc = e32 ? launch(flat_ip_tc_kernel<__half, 1, 32, true>) : launch(flat_ip_tc_kernel<__half, 1, 64, true>);
+  if (rc) return rc;
+  return launch_merge(P.cand_scores, P.cand_ids, nq, nprobe * L.kslot, k, out_scores, out_ids, dev, stream);
+}
+
+// Spherical k-means update: block l averages rows perm[offsets[l] .. offsets[l+1]) of x in that order (fp64
+// accumulation), then divides by the norm.  One fixed order per list: the result is bit-reproducible.
+namespace mmb {
+namespace {
+template <typename T>
+__global__ void __launch_bounds__(256) ivf_list_means_kernel(const T* __restrict__ x, const int64_t* __restrict__ perm,
+                                                             const int64_t* __restrict__ offsets, int64_t nlist, int dim,
+                                                             float* __restrict__ out) {
+  extern __shared__ double acc[];   // [dim]
+  __shared__ double red[8];
+  for (int64_t l = blockIdx.x; l < nlist; l += gridDim.x) {
+    const int64_t lo = offsets[l], hi = offsets[l + 1];
+    for (int c = threadIdx.x; c < dim; c += blockDim.x) {
+      double s = 0.0;
+      for (int64_t r = lo; r < hi; ++r) s += (double)to_float(x[perm[r] * dim + c]);
+      acc[c] = s;
+    }
+    double ss = 0.0;
+    for (int c = threadIdx.x; c < dim; c += blockDim.x) ss += acc[c] * acc[c];
+    for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = ss;
+    __syncthreads();
+    double tot = 0.0;
+    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) tot += red[i];
+    const double inv = tot > 0.0 ? 1.0 / sqrt(tot) : 0.0;   // an empty list gives a zero row
+    for (int c = threadIdx.x; c < dim; c += blockDim.x) out[l * dim + c] = (float)(acc[c] * inv);
+    __syncthreads();
+  }
+}
+}  // namespace
+}  // namespace mmb
+
+extern "C" int mmb200_ivf_list_means(const void* x, const int64_t* perm, const int64_t* offsets, float* out, int64_t nlist,
+                                     int32_t dim, int32_t dtype, void* stream_) {
+  using namespace mmb;
+  MMB_REQUIRE(x && perm && offsets && out, "null pointer");
+  MMB_REQUIRE(nlist >= 1 && dim >= 1 && dim <= 4096, "1 <= dim <= 4096, at least one list");
+  MMB_REQUIRE(dtype == MMB200_F16 || dtype == MMB200_BF16 || dtype == MMB200_F32, "x must be fp16, bf16 or fp32");
+  DeviceInfo dev;
+  if (int rc = require_sm90(&dev)) return rc;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const int grid = (int)std::min<int64_t>(nlist, (int64_t)dev.sm_count * 16);
+  const size_t smem = (size_t)dim * sizeof(double);
+  auto launch = [&](auto t) -> int {
+    using T = decltype(t);
+    MMB_CHECK_CUDA(cudaFuncSetAttribute(ivf_list_means_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    ivf_list_means_kernel<T><<<grid, 256, smem, stream>>>(static_cast<const T*>(x), perm, offsets, nlist, dim, out);
+    MMB_CHECK_CUDA(cudaGetLastError());
+    return MMB200_OK;
+  };
+  if (dtype == MMB200_F16) return launch(__half{});
+  if (dtype == MMB200_BF16) return launch(__nv_bfloat16{});
+  return launch(float{});
 }

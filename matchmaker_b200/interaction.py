@@ -440,6 +440,8 @@ def flat_ip_topk(queries: torch.Tensor, passages: torch.Tensor, k: int, ids: Opt
         unscale = -(sq + split_scale)
         dcode = _lib.F32_SPLIT16
     else:
+        if queries.shape[1] != passages.shape[1]:
+            raise _lib.MatchmakerB200Error(f"flat_ip_topk: queries have dim {queries.shape[1]}, passages {passages.shape[1]}")
         queries = queries.to(passages.dtype).contiguous()
         dim = queries.shape[1]
         dcode = _DTYPES[passages.dtype]
@@ -500,6 +502,101 @@ def topk_unique(cand_scores: torch.Tensor, cand_ids: torch.Tensor, k: int) -> Tu
         rc = lib.mmb200_topk_unique(_ptr(cand_scores), _ptr(cand_ids), _ptr(out_s), _ptr(out_i), nq, L, k, _stream(dev))
     _lib.check(rc, "mmb200_topk_unique")
     return out_s, out_i
+
+
+IVF_MAX_PROBE = 1024
+# Device scratch one ivf_search call may take.  The scratch grows with nq * nprobe (gathered queries, one candidate slot
+# per (query, probe)), so larger query sets are searched in batches that fit.
+IVF_WORKSPACE_CAP = 2 << 30
+
+
+def ivf_query_batch(nq: int, workspace_bytes, cap: int) -> int:
+    """Queries per ivf_search batch: nq halved until `workspace_bytes(batch)` fits `cap` (at least one query).  A size of
+    0 means the batch is outside the envelope (nq * nprobe too large), so it is halved as well."""
+    b = max(1, nq)
+    while b > 1 and not 0 < workspace_bytes(b) <= cap:
+        b = (b + 1) // 2
+    return b
+
+
+def ivf_search(queries: torch.Tensor, rows: torch.Tensor, ids: torch.Tensor, list_offsets: torch.Tensor,
+               probes: torch.Tensor, k: int, max_list_len: int,
+               split_scale: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Exact inner-product top-k over the union of each query's probed lists (faiss IndexIVF search semantics).
+
+    rows [n, dim] fp16 / bf16, sorted by list: list l is rows ``list_offsets[l]:list_offsets[l+1]`` (int64 [nlist+1]);
+    ids [n] int64 user ids; probes [nq, nprobe] int64 list ids, distinct per row (ids outside [0, nlist) probe nothing);
+    max_list_len bounds every list's length.  Returns (scores [nq, k] f32, ids [nq, k] int64) under (score desc, id asc),
+    with a (-3.4028235e38, -1) tail when the probed lists hold fewer than k rows.  fp32 storage: ``rows`` =
+    flat_ip_split_f32(x, "passages")[0] with its scale as ``split_scale``, as for flat_ip_topk.  1 <= k <= 1024,
+    1 <= nprobe <= 1024.  Queries are searched in batches whose scratch fits IVF_WORKSPACE_CAP."""
+    dev = _require_cuda(queries, rows, ids, list_offsets, probes)
+    if rows.dtype not in (torch.float16, torch.bfloat16):
+        raise _lib.MatchmakerB200Error("ivf_search: rows must be fp16 / bf16, or the fp16 split of fp32 (flat_ip_split_f32)")
+    if probes.dim() != 2 or probes.shape[0] != queries.shape[0]:
+        raise _lib.MatchmakerB200Error(f"ivf_search: probes must be [nq, nprobe], got {tuple(probes.shape)}")
+    nq, nprobe = probes.shape
+    nlist = list_offsets.numel() - 1
+    unscale = None
+    if split_scale is not None:
+        if rows.dtype != torch.float16 or rows.shape[1] % 2:
+            raise _lib.MatchmakerB200Error("ivf_search: split storage is [n, 2*dim] fp16")
+        dim = rows.shape[1] // 2
+        if queries.shape[1] != dim:
+            raise _lib.MatchmakerB200Error(f"ivf_search: queries have dim {queries.shape[1]}, split rows {dim}")
+        queries, sq = flat_ip_split_f32(queries, "queries")
+        unscale = -(sq + split_scale)
+        dcode = _lib.F32_SPLIT16
+    else:
+        if queries.shape[1] != rows.shape[1]:
+            raise _lib.MatchmakerB200Error(f"ivf_search: queries have dim {queries.shape[1]}, rows {rows.shape[1]}")
+        queries = queries.to(rows.dtype).contiguous()
+        dim = queries.shape[1]
+        dcode = _DTYPES[rows.dtype]
+    if ids.numel() != rows.shape[0] or list_offsets.dim() != 1 or nlist < 1:
+        raise _lib.MatchmakerB200Error(f"ivf_search: {ids.numel()} ids for {rows.shape[0]} rows, list_offsets "
+                                       f"{tuple(list_offsets.shape)} (need [nlist + 1], nlist >= 1)")
+    rows, probes = rows.contiguous(), probes.to(torch.int64).contiguous()
+    ids, list_offsets = ids.to(torch.int64).contiguous(), list_offsets.to(torch.int64).contiguous()
+    out_s = torch.empty((nq, k), dtype=torch.float32, device=dev)
+    out_i = torch.empty((nq, k), dtype=torch.int64, device=dev)
+    if nq == 0:
+        return out_s, out_i
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        def wsb(b):
+            return lib.mmb200_ivf_workspace_bytes(b, nprobe, nlist, max_list_len, dim, k, dcode)
+        if wsb(1) <= 0:
+            raise _lib.MatchmakerB200Error(f"ivf_search: unsupported sizes nprobe={nprobe} nlist={nlist} dim={dim} k={k} "
+                                           f"(1 <= k <= {FLAT_IP_MAX_K}, 1 <= nprobe <= {IVF_MAX_PROBE}, dim % 64 == 0)")
+        b = ivf_query_batch(nq, wsb, IVF_WORKSPACE_CAP)
+        ws = torch.empty(wsb(b), dtype=torch.uint8, device=dev)
+        for b0 in range(0, nq, b):
+            b1 = min(nq, b0 + b)
+            rc = lib.mmb200_ivf_search(_ptr(queries[b0:b1]), _ptr(rows), _ptr(ids), _ptr(list_offsets), _ptr(probes[b0:b1]),
+                                       _ptr(out_s[b0:b1]), _ptr(out_i[b0:b1]), _ptr(ws), ws.numel(), b1 - b0, nprobe,
+                                       nlist, rows.shape[0], max_list_len, dim, k, dcode, _stream(dev))
+            _lib.check(rc, "mmb200_ivf_search")
+    if unscale is not None:
+        out_s = torch.where(out_s > -3.0e38, torch.ldexp(out_s, torch.tensor(unscale, device=dev)), out_s)
+    return out_s, out_i
+
+
+def ivf_list_means(x: torch.Tensor, perm: torch.Tensor, offsets: torch.Tensor) -> torch.Tensor:
+    """Spherical k-means update: row l = normalised mean of x[perm[offsets[l]:offsets[l+1]]] ([nlist, dim] f32), summed
+    in that order in fp64, so it is bit-reproducible; an empty list gives a zero row.  x [n, dim] fp16 / bf16 / fp32."""
+    dev = _require_cuda(x, perm, offsets)
+    if x.dtype not in _DTYPES:
+        raise _lib.MatchmakerB200Error(f"ivf_list_means: x must be fp16 / bf16 / fp32, got {x.dtype}")
+    x, perm, offsets = x.contiguous(), perm.to(torch.int64).contiguous(), offsets.to(torch.int64).contiguous()
+    nlist = offsets.numel() - 1
+    out = torch.empty((nlist, x.shape[1]), dtype=torch.float32, device=dev)
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        rc = lib.mmb200_ivf_list_means(_ptr(x), _ptr(perm), _ptr(offsets), _ptr(out), nlist, x.shape[1], _DTYPES[x.dtype],
+                                       _stream(dev))
+    _lib.check(rc, "mmb200_ivf_list_means")
+    return out
 
 
 def maxsim_store(q: torch.Tensor, store: torch.Tensor, doc_offsets: torch.Tensor, pair_q: torch.Tensor,

@@ -1,6 +1,7 @@
-"""Index API of matchmaker/retrieval (base_index.py:4-32) for the exact inner-product index
-(`faiss_index_type: "full"`, dense_retrieval.py:310-311) on the H100 kernels."""
+"""Index API of matchmaker/retrieval (base_index.py:4-32) on the H100 kernels: the exact inner-product index
+(`faiss_index_type: "full"`, dense_retrieval.py:310-311) and the inverted-file index (`faiss_index_type: "ivf"`)."""
 from .base_index import BaseNNIndexer  # noqa: F401
 from .flat_ip_index import FlatIPIndexer  # noqa: F401
+from .ivf_index import IVFIndexer  # noqa: F401
 from .colbert_rerank import ColBERTTokenIndex  # noqa: F401
 from .colbert_e2e import ColBERTEndToEndIndexer  # noqa: F401
