@@ -379,6 +379,35 @@ MMB200_API int mmb200_ivf_list_means(const void* x, const int64_t* perm, const i
                                      int64_t nlist, int32_t dim, int32_t dtype, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Graph index: detour pruning of an exact k-NN graph, and a beam search over the graph
+ *
+ * Replaces: FaissHNSWIndexer   matchmaker/retrieval/faiss_indices.py:76-104 (faiss IndexHNSWFlat, CPU only), with one
+ *           flat graph after CAGRA (Ootomo et al., ICDE 2024) instead of faiss's layers.
+ *
+ * mmb200_graph_prune: knn [n, K] int32, the k-NN list of every node in rank order (entries < 0 or >= n are void;
+ *          valid entries of a row distinct).  out [n, R] int32: the R edges of each node with the fewest rank-based
+ *          detours (edge u -> v at rank j has one through w = N(u)[i] when i < j and v = N(w)[p] with p < j), ties by
+ *          rank, stored in rank order; fewer than R valid edges are padded with -1.  Integer work: bit-reproducible.
+ *          1 <= K <= 1023, 1 <= R <= 1024, n < 2^31 - 1.  Outside: MMB200_ERR_INVALID.
+ * mmb200_graph_hash_slots: slots of the search kernel's visited hash for list size L and degree R,
+ *          next_pow2(4 * (L + R)) (0 outside 1 <= L, R <= 1024).  Pure host arithmetic.
+ * mmb200_graph_search: beam search, one CTA per query.  rows [n, dim] fp16 or fp32 (`dtype`, 16-byte aligned), queries
+ *          [nq, dim] in the same dtype, graph [n, R] int32 (-1 = no edge), entries [nq, n_entries] int64 row positions
+ *          that start each query's list, ids [n] int64 user ids (NULL: the row position).  The list keeps the L best
+ *          rows seen under (score desc, position asc); each step expands the best entry not yet expanded, scores its
+ *          unvisited neighbours (fp32, fixed order) and merges them in.  It stops when every entry has been expanded or
+ *          after 2 * L steps.  out_scores / out_ids [nq, k]: the first k entries, then (-3.4028235e38, -1).
+ *          32 <= L <= 1024 (multiple of 32), 1 <= k <= L, 1 <= n_entries <= L, R <= 1024, dim <= 4096 and a multiple
+ *          of 16 bytes.  No host synchronisation.
+ * ------------------------------------------------------------------------------------------ */
+MMB200_API int mmb200_graph_prune(const int32_t* knn, int32_t* out, int64_t n, int32_t K, int32_t R, void* stream);
+MMB200_API int64_t mmb200_graph_hash_slots(int32_t L, int32_t R);
+MMB200_API int mmb200_graph_search(const void* queries, const void* rows, const int64_t* ids, const int32_t* graph,
+                                   const int64_t* entries, float* out_scores, int64_t* out_ids, int64_t nq, int64_t n,
+                                   int32_t dim, int32_t R, int32_t n_entries, int32_t L, int32_t k, int32_t dtype,
+                                   void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Storage block loader: byte ranges of files -> one contiguous DEVICE buffer.
  *
  * Replaces: the host path of the encoded collection between matchmaker/dense_retrieval.py:291-302

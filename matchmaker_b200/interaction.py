@@ -599,6 +599,75 @@ def ivf_list_means(x: torch.Tensor, perm: torch.Tensor, offsets: torch.Tensor) -
     return out
 
 
+GRAPH_MAX_DEGREE = 1024   # R, edges per node
+GRAPH_MAX_KNN = 1023      # K, k-NN degree before pruning
+GRAPH_MAX_LIST = 1024     # L, search list size
+
+
+def graph_hash_slots(L: int, R: int) -> int:
+    """Slots of the search kernel's visited hash for list size L and out-degree R (next_pow2(4 * (L + R)))."""
+    return int(_lib.load().mmb200_graph_hash_slots(int(L), int(R)))
+
+
+def graph_prune(knn: torch.Tensor, R: int) -> torch.Tensor:
+    """Rank-based detour pruning of a k-NN graph: knn [n, K] int32 row positions in rank order (-1 = void) ->
+    [n, R] int32, the R edges of each node with the fewest detours (ties by rank) in rank order, -1 padded.
+    1 <= K <= 1023, 1 <= R <= 1024."""
+    dev = _require_cuda(knn)
+    if knn.dim() != 2:
+        raise _lib.MatchmakerB200Error(f"graph_prune: knn must be [n, K], got {tuple(knn.shape)}")
+    n, K = knn.shape
+    if not (1 <= K <= GRAPH_MAX_KNN and 1 <= R <= GRAPH_MAX_DEGREE):
+        raise _lib.MatchmakerB200Error(f"graph_prune: need 1 <= K <= {GRAPH_MAX_KNN} and 1 <= R <= {GRAPH_MAX_DEGREE}, "
+                                       f"got K={K} R={R}")
+    knn = knn.to(torch.int32).contiguous()
+    out = torch.empty((n, R), dtype=torch.int32, device=dev)
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        rc = lib.mmb200_graph_prune(_ptr(knn), _ptr(out), n, K, int(R), _stream(dev))
+    _lib.check(rc, "mmb200_graph_prune")
+    return out
+
+
+def graph_search(queries: torch.Tensor, rows: torch.Tensor, ids: torch.Tensor, graph: torch.Tensor,
+                 entries: torch.Tensor, k: int, L: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Beam search over a graph index, one CTA per query.
+
+    rows [n, dim] fp16 or fp32 (queries are cast to it); graph [n, R] int32 row positions (-1 = no edge); entries
+    [nq, m] int64 row positions that seed each query's list (1 <= m <= L); ids [n] int64 user ids.  The list keeps the
+    L best rows seen under (score desc, position asc), and every score comes from one fixed-order fp32 formula.
+    Returns (scores [nq, k] f32, ids [nq, k] int64) with a (-3.4028235e38, -1) tail where fewer than k rows were
+    reached.  32 <= L <= 1024 (a multiple of 32), 1 <= k <= L.  No host synchronisation."""
+    dev = _require_cuda(queries, rows, ids, graph, entries)
+    if rows.dtype not in (torch.float16, torch.float32) or rows.dim() != 2:
+        raise _lib.MatchmakerB200Error("graph_search: rows must be [n, dim] fp16 or fp32")
+    n, dim = rows.shape
+    if queries.dim() != 2 or queries.shape[1] != dim:
+        raise _lib.MatchmakerB200Error(f"graph_search: queries have shape {tuple(queries.shape)}, rows dim {dim}")
+    nq = queries.shape[0]
+    if graph.dim() != 2 or graph.shape[0] != n or ids.numel() != n:
+        raise _lib.MatchmakerB200Error(f"graph_search: graph {tuple(graph.shape)} and {ids.numel()} ids for {n} rows")
+    if entries.dim() != 2 or entries.shape[0] != nq:
+        raise _lib.MatchmakerB200Error(f"graph_search: entries must be [nq, m], got {tuple(entries.shape)}")
+    if not (32 <= L <= GRAPH_MAX_LIST and L % 32 == 0 and 1 <= k <= L and 1 <= entries.shape[1] <= L):
+        raise _lib.MatchmakerB200Error(f"graph_search: need 32 <= L <= {GRAPH_MAX_LIST} (a multiple of 32), 1 <= k <= L "
+                                       f"and 1 <= entries <= L, got L={L} k={k} entries={entries.shape[1]}")
+    queries = queries.to(rows.dtype).contiguous()
+    rows, graph = rows.contiguous(), graph.to(torch.int32).contiguous()
+    ids, entries = ids.to(torch.int64).contiguous(), entries.to(torch.int64).contiguous()
+    out_s = torch.empty((nq, k), dtype=torch.float32, device=dev)
+    out_i = torch.empty((nq, k), dtype=torch.int64, device=dev)
+    if nq == 0:
+        return out_s, out_i
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        rc = lib.mmb200_graph_search(_ptr(queries), _ptr(rows), _ptr(ids), _ptr(graph), _ptr(entries), _ptr(out_s),
+                                     _ptr(out_i), nq, n, dim, graph.shape[1], entries.shape[1], int(L), int(k),
+                                     _DTYPES[rows.dtype], _stream(dev))
+    _lib.check(rc, "mmb200_graph_search")
+    return out_s, out_i
+
+
 def maxsim_store(q: torch.Tensor, store: torch.Tensor, doc_offsets: torch.Tensor, pair_q: torch.Tensor,
                  pair_d: torch.Tensor, max_doc_len: int, impl: str = "auto") -> torch.Tensor:
     """ColBERT max-sim against a ragged token store, fp32 [n_pairs] (colbert.py:100-112, no masks).
