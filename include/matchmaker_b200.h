@@ -60,8 +60,9 @@ extern "C" {
 #define MMB200_IMPL_SIMT 1    /* CUDA-core kernel, any shape/dtype */
 #define MMB200_IMPL_TCGEN05 2 /* TMA + wgmma tensor-core kernel (fails if shape unsupported); the name is historical */
 #define MMB200_IMPL_TCGEN05_DOCM 3 /* max-sim only: the "documents on M" tensor-core kernel */
-#define MMB200_IMPL_TCGEN05_RAGGED 4 /* max-sim only: tensor-core kernel that fetches each document only up to its
-                                        last unmasked row (padding rows never leave HBM) */
+#define MMB200_IMPL_TCGEN05_RAGGED 4 /* max-sim only: alias of MMB200_IMPL_TCGEN05, kept for ABI compatibility.  The
+                                        tensor-core max-sim kernel always fetches each document only up to its last
+                                        unmasked row (padding rows never leave HBM) */
 
 MMB200_API int mmb200_version(void);
 MMB200_API const char* mmb200_last_error(void);

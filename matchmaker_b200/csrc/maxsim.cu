@@ -485,22 +485,8 @@ int maxsim_fwd_device(const MaxsimParams& P, int dtype, int impl, cudaStream_t s
   if (P.n_pairs == 0) return MMB200_OK;
   DeviceInfo dev;
   if (int rc = require_sm90(&dev)) return rc;
-  if (impl == MMB200_IMPL_TCGEN05_RAGGED) {
-    // skip-padding variant: fetch only rows up to each document's last unmasked row
-    MMB_REQUIRE(P.pair_dmask == nullptr, "ragged fetch is incompatible with pair_dmask");
-    int32_t* rows = nullptr;
-    MMB_CHECK_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&rows), (size_t)P.n_d * sizeof(int32_t), stream));
-    int rc = maxsim_rows_needed_launch(P.d_mask, P.mask_dtype, rows, P.n_d, P.Ld, stream);
-    bool handled = false;
-    if (rc == MMB200_OK) {
-      MaxsimParams R = P;
-      R.rows_needed = rows;
-      rc = maxsim_qm_launch(R, dtype, dev, stream, &handled);
-    }
-    cudaFreeAsync(rows, stream);
-    if (rc == MMB200_OK && !handled) { set_error("ragged max-sim: shape outside the queries-on-M kernel (Lq <= 32, dim 64/128, f16/bf16)"); rc = MMB200_ERR_UNSUPPORTED; }
-    return rc;
-  }
+  // the live-row fetch is the queries-on-M kernel's only path: the ragged name is an alias of the tensor-core one
+  if (impl == MMB200_IMPL_TCGEN05_RAGGED) impl = MMB200_IMPL_TCGEN05;
   if (impl == MMB200_IMPL_AUTO || impl == MMB200_IMPL_TCGEN05) {
     bool handled = false;
     const int rc = maxsim_qm_launch(P, dtype, dev, stream, &handled);
@@ -537,7 +523,6 @@ extern "C" int mmb200_maxsim_store_fwd(const void* q, const void* store, const i
   MMB_REQUIRE(doc_offsets && pair_q && pair_d, "doc_offsets, pair_q and pair_d must be non-null");
   MMB_REQUIRE(n_rows >= 1 && n_docs >= 1 && max_doc_len >= 1, "the store needs at least one row, one passage, max_doc_len >= 1");
   MMB_REQUIRE(n_rows < (1ll << 31) - 1024, "at most 2^31 - 1024 store rows per device (TMA row coordinates are int32)");
-  MMB_REQUIRE(impl != MMB200_IMPL_TCGEN05_RAGGED, "store mode already fetches only each passage's own rows");
   mmb::MaxsimParams P;
   P.q = q; P.d = store; P.pair_q = pair_q; P.pair_d = pair_d; P.out = out; P.n_q = n_q; P.n_d = n_docs;
   P.n_pairs = n_pairs; P.Lq = Lq; P.Ld = max_doc_len; P.dim = dim;

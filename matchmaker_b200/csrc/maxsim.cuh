@@ -16,7 +16,6 @@ struct MaxsimParams {
   const int32_t* pair_q = nullptr;
   const int32_t* pair_d = nullptr;
   const int32_t* pair_dmask = nullptr;  // row of d_mask used for pair p (default: the document index)
-  const int32_t* rows_needed = nullptr;  // [n_d] or NULL: rows of document di worth fetching (1 + last unmasked row)
   float* out = nullptr;
   int32_t* argmax = nullptr;
   int64_t n_q = 0, n_d = 0, n_pairs = 0;
@@ -40,8 +39,6 @@ __device__ __forceinline__ int store_doc_rows(const MaxsimParams& P, int64_t di,
 struct DeviceInfo;
 // maxsim_qm.cu: "queries on M" wgmma kernel (Lq <= 32, dim 64/128); *handled = false if out of envelope.
 int maxsim_qm_launch(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cudaStream_t stream, bool* handled);
-// rows_needed[di] = 1 + index of the last unmasked row of document di (Ld when d_mask == NULL)
-int maxsim_rows_needed_launch(const void* d_mask, int mask_dtype, int32_t* rows_needed, int64_t n_d, int Ld, cudaStream_t stream);
 
 // Validates, picks the SIMT or a tensor-core kernel and launches on `stream`.
 int maxsim_fwd_device(const MaxsimParams& P, int dtype, int impl, cudaStream_t stream);

@@ -3,32 +3,37 @@
 // Why this orientation: with documents on M (maxsim.cu) the max over document rows is a reduction across the rows of
 // the accumulator, i.e. across threads.  Here the accumulator is transposed:
 //
-//     D[64 x TN] = Qrep[64 x dim] * Doc[TN x dim]^T        (one wgmma chain per document tile)
+//     D[64 x 64] = Qrep[64 x dim] * Chunk[64 x dim]^T        (one wgmma chain per 64-row chunk of a document)
 //
 // row = query token, column = document row, so the max over a document is a per-thread FMNMX chain over the
 // accumulator registers plus two quad shuffles.  Rows 0..31 of Qrep are the query; rows 32..63 of the instruction read
 // whatever follows the query in shared memory and are never looked at.
 //
-// The document mask is applied in the epilogue as an fp32 penalty per document row, added to every query's score of
-// that row: 0 for real tokens, -inf for padding and for the tile's rows past Ld, so masked rows can never win the max.
-// The reference's -1000 fill (matchmaker/models/colbert.py:69) only matters when it IS the max; that is reproduced
-// exactly by one "virtual" document row (the last row of the last tile, index >= Ld, zero data from TMA out-of-bounds
-// fill) whose penalty is -1000 when the document has at least one masked position and -inf otherwise.  Two helper warps
-// write the penalty row per document tile while TMA streams the token vectors.
+// Only live rows are streamed.  A document's live rows are [0, live) with live = 1 + its last unmasked row (Ld without a
+// mask; the passage's length in store mode); it takes max(1, ceil(live / 64)) chunks of the stage ring, and chunks past
+// them are neither fetched, multiplied nor reduced.  Rows of a chunk at or past `live` hold the caller's padding (up to
+// the next 64-row boundary) or TMA's zero fill past Ld: the mask is applied in the epilogue as an fp32 penalty per row,
+// 0 for live unmasked rows and -inf for every other row, so no such row can win the max whatever its data.  The
+// reference's -1000 fill (matchmaker/models/colbert.py:69) only matters when it IS the max; it is one more candidate
+// taken after the last chunk, value -1000 at a column past Ld (so ties go to real rows and the argmax reports -1), when
+// the document has a masked position anywhere in its Ld rows -- live < Ld, or a hole before its last live row.
 //
 // Nothing on a warp's per-document path waits for a global load: the per-pair indices and lengths arrive 32 pairs at a
-// time, a batch ahead (PairStream; the consumers, which only need the query, keep just a batch of pair_q), and the
-// penalty writers keep the mask words of their next two tiles in flight.  setmaxnreg moves registers from the helper
-// warpgroup to the consumers, whose accumulators are the kernel's register peak.
+// time, a batch ahead (PairStream; the consumers, which only need the query, keep just a batch of pair_q), and each
+// penalty writer keeps the mask words of its next document in flight while it writes the current one.  setmaxnreg moves
+// registers from the helper warpgroup to the consumers.
 //
 // Per CTA (persistent, one per SM, 384 threads = 3 warpgroups):
-//   warp 0        TMA producer: query tile (2-slot ring, re-fetched when the query changes), document tiles
-//   warps 1, 2    penalty writers, warp 1 + c for consumer warpgroup c's documents
-//   warpgroups 1, 2  consumers: warpgroup c takes the CTA's documents c, c + 2, ...; per tile 4 * dim / 64 * TN / 64
-//                 wgmma m64n64k16 into registers, then the masked max over the tile in the same registers.  While one
-//                 warpgroup reduces, the other one's MMAs run.  Each warpgroup has its own half of the stage ring, so
-//                 every stage barrier has one consumer that waits for its phases in order.
-// HBM-bound by design: per document one TMA box, one fp32 store.
+//   warp 0        TMA producer: query tile (2-slot ring, re-fetched when the query changes), document chunks: one
+//                 {64, 64 rows, dim / 64} box per chunk (rows past Ld are zero-filled by TMA and cost no HBM traffic)
+//   warps 1, 2    penalty writers, warp 1 + c for consumer warpgroup c's documents: per document they count the live
+//                 rows (a ballot per 32 mask words), hand the count to the producer, and per chunk write the penalty row
+//                 and a header (last chunk of the document, -1000 candidate)
+//   warpgroups 1, 2  consumers: warpgroup c takes the CTA's documents c, c + 2, ...; per chunk 4 * dim / 64 wgmma
+//                 m64n64k16 into registers, then the masked max over the chunk's 64 columns, and the stage goes back at
+//                 once.  While one warpgroup reduces, the other one's MMAs run.  Each warpgroup has its own half of the stage ring, so every stage barrier has one consumer that waits
+//                 for its phases in order.
+// HBM-bound by design: per chunk one TMA box, per document one fp32 store.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -45,37 +50,51 @@ namespace mmb {
 namespace {
 
 constexpr int kThreads = 384;
-constexpr int kMaxStages = 8;                // even: half of the ring per consumer warpgroup
+constexpr int kChunkRows = 64;
+constexpr int kChunkKBlockBytes = kChunkRows * 128;   // one k-block of a chunk (8 KB)
+constexpr int kAuxBytes = 1024;              // per stage after the chunk: penalty row (64 fp32) + header word
+constexpr int kMaxStages = 32;               // even: half of the ring per consumer warpgroup (12 at dim 128, 24 at dim 64)
+constexpr int kLiveSlots = 8;                // live-row counts in flight from each penalty writer to the producer
+constexpr int kMaskWords = 4;                // mask ballots per writer lane: documents of up to 32 * 32 * 4 rows
+constexpr int kMaxLd = 32 * 32 * kMaskWords;
 constexpr int kQSlots = 2;
 constexpr int kQRows = 32;
 constexpr int kQBlockBytes = kQRows * 128;   // one k-block of the query tile (4 KB)
-// setmaxnreg budgets: the helper warpgroup (producer, penalty writers) gives registers to the two consumer warpgroups, whose
-// NCH x 32 accumulators are the kernel's register peak.  128 x 104 + 256 x 200 = 384 x 168 (the launch).
-constexpr int kRegsHelper = 104, kRegsConsumer = 200;
+// chunk header bits
+constexpr int kLastChunk = 1, kFill = 2;
+// setmaxnreg budgets: the helper warpgroup (producer, penalty writers) gives registers to the two consumer warpgroups,
+// whose 32-register accumulator and epilogue are the kernel's register peak.  128 x 120 + 256 x 192 = 384 x 168 (the launch).
+constexpr int kRegsHelper = 120, kRegsConsumer = 192;
 
 struct QmShared {
   uint64_t full[kMaxStages];   // 2 arrivals: TMA producer (with tx bytes) + penalty writer
   uint64_t empty[kMaxStages];  // 4 arrivals: the warps of the warpgroup that owns the stage
   uint64_t qfull[kQSlots];
   uint64_t qempty[kQSlots];    // 8 arrivals: every warp of both consumer warpgroups
+  uint64_t lfull[2][kLiveSlots];    // writer c -> producer: live rows of writer c's next documents (1 arrival)
+  uint64_t lempty[2][kLiveSlots];   // producer -> writer c (1 arrival)
+  int32_t live[2][kLiveSlots];
   float part[2][2];            // [consumer][pair parity]: row sum of query rows 16..31
 };
 
 struct QmLaunch {
   int32_t kblocks;      // dim / 64 (1 or 2)
-  int32_t tn;           // document rows per tile (multiple of 64, <= 256)
-  int32_t tiles;        // tiles per document; tiles * tn >= Ld + 1
   int32_t stages;       // even: stages [0, stages / 2) serve warpgroup 0, the rest warpgroup 1
-  int32_t doc_bytes;    // kblocks * tn * 128
-  int32_t stage_bytes;  // doc_bytes + penalty row (tn fp32, rounded to 1 KB)
+  int32_t chunk_bytes;  // kblocks * 8 KB
+  int32_t stage_bytes;  // chunk_bytes + kAuxBytes
+};
+
+// Tensor maps of the query tile and of the document chunks ({64, 64 rows, kblocks, 1} boxes).
+struct QmMaps {
+  CUtensorMap q;
+  CUtensorMap d;
 };
 
 // One warp's own sequence of pairs p = first, first + step, ... < end and what the warp needs of each: its query, its
-// document, its document-mask row, and (ragged fetch, store mode) its first row and the rows worth fetching.  Lane l
-// holds element l of a batch of 32.  A batch's index arrays are read with one coalesced load per array two batches
-// ahead of use, store mode's doc_offsets of those documents one batch ahead, and elements are handed out by
-// __shfl_sync: the warp never waits on a per-pair global load.  Every lane of the warp calls next() and the accessors
-// together.
+// document, its document-mask row, and (store mode) its first row and length.  Lane l holds element l of a batch of 32.
+// A batch's index arrays are read with one coalesced load per array two batches ahead of use, store mode's doc_offsets
+// of those documents one batch ahead, and elements are handed out by __shfl_sync: the warp never waits on a per-pair
+// global load.  Every lane of the warp calls next() and the accessors together.
 template <bool kStore>
 struct PairStream {
   // Indices are int32 like the pair arrays of the C ABI; the implicit document index p (< n_pairs <= n_d) is one too:
@@ -102,7 +121,7 @@ struct PairStream {
     load1(pre, pre_batch);
     k = -1;
   }
-  // indices: pair_q / pair_d / pair_dmask / rows_needed of this lane's pair
+  // indices: pair_q / pair_d / pair_dmask of this lane's pair
   __device__ __forceinline__ void load1(Batch& b, int64_t bi) {
     const int64_t p = first + (bi * 32 + lane) * step;
     b.q = 0; b.d = -1; b.dm = 0; b.rows = 0; b.row0 = 0; b.row_end = 0;
@@ -110,7 +129,6 @@ struct PairStream {
     b.q = P.pair_q ? P.pair_q[p] : (int32_t)((p + P.pair_base) / P.docs_per_query);
     b.d = P.pair_d ? P.pair_d[p] : (int32_t)p;
     if (P.pair_dmask) b.dm = P.pair_dmask[p];
-    if (!kStore && P.rows_needed) b.rows = P.rows_needed[p];   // ragged fetch has no pair_d: the document is p
   }
   // what depends on the indices (waits for load1's results)
   __device__ __forceinline__ void load2(Batch& b) {
@@ -164,20 +182,29 @@ __device__ __forceinline__ void take(float v, int col, float& m, int& am) {
   }
 }
 
+// element i of a register array indexed by a warp-uniform value (unrolled selects: the array stays in registers)
+template <int N>
+__device__ __forceinline__ uint32_t pick(const uint32_t (&a)[N], int i) {
+  uint32_t v = a[0];
+#pragma unroll
+  for (int j = 1; j < N; ++j) v = i == j ? a[j] : v;
+  return v;
+}
+
 // kArgmax: the training instantiation also tracks WHICH document row won each query token's max (what backward needs,
-// matchmaker/models/colbert.py:71 through autograd).  NCH = tn / 64 accumulator chunks of 32 registers.
-// kStore: store mode (P.doc_offsets != NULL) -- a template parameter so that the padded instantiations compile as before.
-template <typename T, int NCH, bool kArgmax, bool kStore>
+// matchmaker/models/colbert.py:71 through autograd).
+// kStore: store mode (P.doc_offsets != NULL) -- a template parameter so that the padded instantiations carry no
+// doc_offsets loads.
+template <typename T, bool kArgmax, bool kStore>
 __global__ void __launch_bounds__(kThreads, 1)
-maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_d,
-                 const __grid_constant__ CUtensorMap tmap_d16, MaxsimParams P, QmLaunch L) {
+maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
   extern __shared__ uint8_t smem_raw[];
   // 1024-B alignment for SWIZZLE_128B tiles, derived by pointer arithmetic on the __shared__ array so the
   // compiler keeps the shared address space (LDS/STS instead of generic LD/ST)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int qslot_bytes = L.kblocks * kQBlockBytes;
   uint8_t* q_base = smem;                                            // [kQSlots][kblocks][32 rows][128 B]
-  uint8_t* stage_base = q_base + kQSlots * qslot_bytes;              // [stages][doc tile | penalty row]
+  uint8_t* stage_base = q_base + kQSlots * qslot_bytes;              // [stages][chunk | penalty row, header]
   QmShared* S = reinterpret_cast<QmShared*>(stage_base + (size_t)L.stages * L.stage_bytes);
 
   const int warp = threadIdx.x >> 5;
@@ -187,20 +214,13 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   cta_share(P.n_pairs, &p_begin, &p_end);
 
   if (threadIdx.x == 0) {
-    prefetch_tensormap(&tmap_q);
-    prefetch_tensormap(&tmap_d);
+    prefetch_tensormap(&M.q);
+    prefetch_tensormap(&M.d);
     for (int s = 0; s < L.stages; ++s) { mbar_init(&S->full[s], 2); mbar_init(&S->empty[s], 4); }
     for (int s = 0; s < kQSlots; ++s) { mbar_init(&S->qfull[s], 1); mbar_init(&S->qempty[s], 8); }
+    for (int c = 0; c < 2; ++c)
+      for (int s = 0; s < kLiveSlots; ++s) { mbar_init(&S->lfull[c][s], 1); mbar_init(&S->lempty[c][s], 1); }
     fence_barrier_init();
-  }
-  if (P.rows_needed || kStore) {
-    // ragged fetch (and store mode) leaves rows of a stage untouched: start from zeros so that stale rows are always
-    // finite and the virtual row (index >= Ld, only ever written by TMA zero fill) is zero
-    for (int s = 0; s < L.stages; ++s) {
-      uint4* z = reinterpret_cast<uint4*>(stage_base + (size_t)s * L.stage_bytes);
-      for (int e = threadIdx.x; e < L.doc_bytes / 16; e += kThreads) z[e] = make_uint4(0, 0, 0, 0);
-    }
-    fence_proxy_async_smem();
   }
   __syncthreads();
 
@@ -211,7 +231,7 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     // the whole warp walks the pairs (it shares out their metadata); lane 0 waits on the barriers and issues the TMA
     PairStream<kStore> meta(P, p_begin, p_end, 1, lane);
     const int ring = L.stages >> 1;
-    int64_t seq0 = 0, seq1 = 0;   // tiles filled so far into each warpgroup's half of the ring
+    int64_t seq0 = 0, seq1 = 0;   // chunks filled so far into each warpgroup's half of the ring
     int64_t prev_q = -1;
     uint32_t qcount = 0;
     for (int64_t p = p_begin; p < p_end; ++p) {
@@ -220,43 +240,40 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
       const int64_t di = meta.d();
       // store mode: the passage's rows start at row `row0` of the [n_rows, dim] store (tensor-map dim 3 has extent 1)
       const int64_t row0 = kStore ? meta.row0() : 0;
-      const int need_rows = meta.rows();
       if (lane == 0) {
         if (qi != prev_q) {
           const uint32_t slot = qcount & 1u, use = qcount >> 1;
           mbar_wait(&S->qempty[slot], (use & 1u) ^ 1u);
           mbar_arrive_expect_tx(&S->qfull[slot], (uint32_t)(L.kblocks * kQBlockBytes));
           for (int kb = 0; kb < L.kblocks; ++kb)
-            tma_load_4d(&tmap_q, q_base + (size_t)slot * qslot_bytes + kb * kQBlockBytes, &S->qfull[slot], 0, 0, kb, (int)qi,
+            tma_load_4d(&M.q, q_base + (size_t)slot * qslot_bytes + kb * kQBlockBytes, &S->qfull[slot], 0, 0, kb, (int)qi,
                         kEvictLast);
           ++qcount;
           prev_q = qi;
         }
-        const int dcoord = kStore ? 0 : (int)di;
         const int c = (int)((p - p_begin) & 1);
-        for (int t = 0; t < L.tiles; ++t) {
+        // live rows of this document, from its penalty writer
+        const int64_t i = (p - p_begin) >> 1;
+        const int ls = (int)(i % kLiveSlots);
+        mbar_wait(&S->lfull[c][ls], (uint32_t)((i / kLiveSlots) & 1));
+        const int live = S->live[c][ls];
+        mbar_arrive(&S->lempty[c][ls]);
+        const int dcoord = kStore ? 0 : (int)di;
+        const int nch = max(1, (live + kChunkRows - 1) / kChunkRows);
+        for (int ch = 0; ch < nch; ++ch) {
           const int64_t j = c ? seq1++ : seq0++;
           const int stage = c * ring + (int)(j % ring);
           const uint32_t phase = (uint32_t)((j / ring) & 1);
           mbar_wait(&S->empty[stage], phase ^ 1u);
           uint8_t* dst = stage_base + (size_t)stage * L.stage_bytes;
-          if (!P.rows_needed && !kStore) {
-            mbar_arrive_expect_tx(&S->full[stage], (uint32_t)L.doc_bytes);
-            tma_load_4d(&tmap_d, dst, &S->full[stage], 0, t * L.tn, 0, (int)di, kEvictFirst);
+          const int row = (int)row0 + ch * kChunkRows;
+          if (live == 0) {
+            mbar_arrive(&S->full[stage]);
           } else {
-            // 16-row blocks up to the document's last unmasked row (store mode: its last row); the rest of the stage
-            // keeps stale (finite) rows, which the penalty row masks with -inf
-            const int rows_here = min(max(need_rows - t * L.tn, 0), L.tn);
-            const int nb = (rows_here + 15) >> 4;
-            if (nb == 0) {
-              mbar_arrive(&S->full[stage]);
-            } else {
-              mbar_arrive_expect_tx(&S->full[stage], (uint32_t)(nb * L.kblocks * 2048));
-              for (int kb = 0; kb < L.kblocks; ++kb)
-                for (int b16 = 0; b16 < nb; ++b16)
-                  tma_load_4d(&tmap_d16, dst + kb * L.tn * 128 + b16 * 2048, &S->full[stage], 0,
-                              (int)row0 + t * L.tn + b16 * 16, kb, dcoord, kEvictFirst);
-            }
+            // one box per chunk, also for the last one: the rows it reads past the last live row (at most 63, zero
+            // fill past Ld) cost less than the extra TMA issues and handshakes of 16-row boxes
+            mbar_arrive_expect_tx(&S->full[stage], (uint32_t)L.chunk_bytes);
+            tma_load_4d(&M.d, dst, &S->full[stage], 0, row, 0, dcoord, kEvictFirst);
           }
         }
       }
@@ -265,76 +282,107 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   } else if (warp == 1 || warp == 2) {
     setmaxnreg_dec<kRegsHelper>();
     // ------------------------------- penalty writers -----------------------------
-    // writer c fills the penalty rows of consumer warpgroup c's half of the ring (pairs p_begin + c, + 2, ...), so every
-    // stage has one writer that sees its uses in order (a second writer could pass a parity wait one phase early).  The
-    // mask words of the writer's next two tiles (four documents of the CTA at one tile per document) are in flight in
-    // two register sets that take turns; a copy between them would wait for the load.
-    constexpr int kW = 2 * NCH;          // rows of a tile per lane (TN = 64 NCH)
+    // writer c serves consumer warpgroup c's half of the ring (pairs p_begin + c, + 2, ...), so every stage has one
+    // writer that sees its uses in order (a second writer could pass a parity wait one phase early).  Per document:
+    // ballot the mask words of its rows (lane l of the warp keeps ballot words l, l + 32, ...), count the live rows,
+    // hand the count to the producer, load the mask words of the writer's next document, then write one penalty row per
+    // chunk.  The first 256 rows' words of the next document are in flight in registers while this one is written.
+    constexpr int kW = 8;                // mask words per lane prefetched: rows [0, 256) of a document
     const int c = warp - 1;
     const int dmt = P.d_mask ? P.mask_dtype : MMB200_MASK_NONE;
     const int ring = L.stages >> 1;
+    const int nwin = (P.Ld + 32 * kW - 1) / (32 * kW);
     PairStream<kStore> meta(P, p_begin + c, p_end, 2, lane);
-    int64_t seq = 0;                    // tiles written into this half of the ring
-    int64_t wp = p_begin + c;           // pair and tile being written
-    int wt = 0;
-    bool any_masked = false;
-    int64_t fp = wp;                    // pair and tile being fetched
-    int ft = 0;
-    int64_t f_dm = 0;                   // mask row and row limit of pair fp
-    int f_lim = 0;
-    auto fetch = [&](uint64_t (&raw)[kW], int& lim) {
-      if (fp < p_end && ft == 0) {
-        meta.next();
-        f_dm = meta.dm();
-        f_lim = kStore ? meta.rows() : P.Ld;   // store mode: the passage's length, 0 for a skipped pair
-      }
+    int64_t seq = 0;                    // chunks written into this half of the ring
+    int64_t ndoc = 0;                   // documents whose live count was handed to the producer
+    int64_t fp = p_begin + c;           // next pair whose mask words are loaded
+    // mask words folded to 32 bits (an int64 word's halves OR-ed: only zero / nonzero matters; fp32 keeps its bits)
+    auto load_win = [&](uint32_t (&raw)[kW], int64_t dm, int w) {
 #pragma unroll
       for (int k = 0; k < kW; ++k) {
-        const int r = lane + 32 * k, g = ft * L.tn + r;
+        const int g = w * 32 * kW + 32 * k + lane;
         raw[k] = 1;
-        if (dmt != MMB200_MASK_NONE && fp < p_end && r < L.tn && g < P.Ld)
-          raw[k] = mask_raw(P.d_mask, dmt, f_dm * (int64_t)P.Ld + g);
+        if (dmt != MMB200_MASK_NONE && g < P.Ld) {
+          const uint64_t v = mask_raw(P.d_mask, dmt, dm * (int64_t)P.Ld + g);
+          raw[k] = (uint32_t)(v | (v >> 32));
+        }
       }
-      lim = f_lim;
-      if (++ft == L.tiles) { ft = 0; fp += 2; }
     };
-    auto write = [&](const uint64_t (&raw)[kW], int lim) {
-      float pen[kW];
-      bool masked_here = false;
-#pragma unroll
-      for (int k = 0; k < kW; ++k) {
-        const int r = lane + 32 * k, g = wt * L.tn + r;
-        const bool in_doc = r < L.tn && g < lim;
-        const bool ok = in_doc && mask_test(raw[k], dmt);
-        masked_here |= in_doc && !ok;
-        pen[k] = ok ? 0.f : -INFINITY;
+    auto fetch = [&](uint32_t (&raw)[kW], int64_t& dm, int& lim) {
+      if (fp < p_end) {
+        meta.next();
+        dm = meta.dm();
+        lim = kStore ? meta.rows() : P.Ld;   // store mode: the passage's length, 0 for a skipped pair
+        load_win(raw, dm, 0);
       }
-      any_masked |= __any_sync(0xffffffffu, masked_here);
-      const int stage = c * ring + (int)(seq % ring);
-      const uint32_t phase = (uint32_t)((seq / ring) & 1);
-      ++seq;
-      mbar_wait(&S->empty[stage], phase ^ 1u);
-      float* pt = reinterpret_cast<float*>(stage_base + (size_t)stage * L.stage_bytes + L.doc_bytes);
-#pragma unroll
-      for (int k = 0; k < kW; ++k) {
-        const int r = lane + 32 * k, g = wt * L.tn + r;
-        // the virtual -1000 row exists only in the masked (padded) layout
-        if (r < L.tn) pt[r] = (!kStore && g == L.tiles * L.tn - 1) ? (any_masked ? -1000.f : -INFINITY) : pen[k];
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&S->full[stage]);
-      if (++wt == L.tiles) { wt = 0; wp += 2; any_masked = false; }
+      fp += 2;
     };
-    uint64_t ra[kW], rb[kW];
-    int la, lb;
-    fetch(ra, la);
-    fetch(rb, lb);
-    while (wp < p_end) {
-      write(ra, la);
-      fetch(ra, la);
-      if (wp >= p_end) break;
-      write(rb, lb);
-      fetch(rb, lb);
+    // one document: scan its mask, hand its live count to the producer, prefetch the writer's next document into `raw`,
+    // write its chunks' penalty rows
+    auto doc = [&](uint32_t (&raw)[kW], int64_t& dm, int& lim) {
+      uint32_t bits[kMaskWords];
+#pragma unroll
+      for (int i = 0; i < kMaskWords; ++i) bits[i] = 0;
+      bool masked = false;
+      for (int w = 0; w < nwin; ++w) {
+        if (w > 0) load_win(raw, dm, w);   // documents longer than 256 rows: the later words are loaded here
+#pragma unroll
+        for (int k = 0; k < kW; ++k) {
+          const int g = w * 32 * kW + 32 * k + lane;
+          const bool in_doc = g < lim;
+          const bool ok = in_doc && mask_test(raw[k], dmt);
+          masked |= in_doc && !ok;
+          const uint32_t b = __ballot_sync(0xffffffffu, ok);
+          const int wi = w * kW + k;       // ballot word of rows [32 wi, 32 wi + 32)
+#pragma unroll
+          for (int i = 0; i < kMaskWords; ++i)
+            if (wi == 32 * i + lane) bits[i] = b;
+        }
+      }
+      int last = 0;   // 1 + last live row among this lane's words
+#pragma unroll
+      for (int i = 0; i < kMaskWords; ++i)
+        if (bits[i]) last = 32 * (32 * i + lane) + 32 - __clz(bits[i]);
+      const int live = (int)__reduce_max_sync(0xffffffffu, (unsigned)last);
+      // the reference fills every masked position with -1000, including the trailing ones that are never visited
+      const bool fill = !kStore && __any_sync(0xffffffffu, masked);
+      {
+        const int ls = (int)(ndoc % kLiveSlots);
+        mbar_wait(&S->lempty[c][ls], (uint32_t)(((ndoc / kLiveSlots) & 1) ^ 1));
+        if (lane == 0) {
+          S->live[c][ls] = live;
+          mbar_arrive(&S->lfull[c][ls]);
+        }
+        ++ndoc;
+      }
+      fetch(raw, dm, lim);
+      const int nch = max(1, (live + kChunkRows - 1) / kChunkRows);
+      for (int ch = 0; ch < nch; ++ch) {
+        const int stage = c * ring + (int)(seq % ring);
+        const uint32_t phase = (uint32_t)((seq / ring) & 1);
+        ++seq;
+        const uint32_t b0 = __shfl_sync(0xffffffffu, pick(bits, ch >> 4), (2 * ch) & 31);
+        const uint32_t b1 = __shfl_sync(0xffffffffu, pick(bits, ch >> 4), (2 * ch + 1) & 31);
+        mbar_wait(&S->empty[stage], phase ^ 1u);
+        float* pt = reinterpret_cast<float*>(stage_base + (size_t)stage * L.stage_bytes + L.chunk_bytes);
+        pt[lane] = (b0 >> lane) & 1u ? 0.f : -INFINITY;
+        pt[32 + lane] = (b1 >> lane) & 1u ? 0.f : -INFINITY;
+        if (lane == 0)
+          reinterpret_cast<int32_t*>(pt)[kChunkRows] = ch == nch - 1 ? (kLastChunk | (fill ? kFill : 0)) : 0;
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&S->full[stage]);
+      }
+    };
+    uint32_t ra[kW], rb[kW];
+    int64_t dma = 0, dmb = 0;
+    int la = 0, lb = 0;
+    fetch(ra, dma, la);
+    fetch(rb, dmb, lb);
+    for (int64_t wp = p_begin + c; wp < p_end;) {
+      doc(ra, dma, la);
+      if ((wp += 2) >= p_end) break;
+      doc(rb, dmb, lb);
+      wp += 2;
     }
   } else if (warp == 3) {
     setmaxnreg_dec<kRegsHelper>();   // idle: its registers go to the consumers
@@ -347,7 +395,7 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     const int cq = 2 * (lane & 3);        // this thread's first column inside an 8-column group
     const int qmt = P.q_mask ? P.mask_dtype : MMB200_MASK_NONE;
     const int ring = L.stages >> 1;
-    int64_t seq = 0;   // tiles consumed from this warpgroup's half of the ring
+    int64_t seq = 0;   // chunks consumed from this warpgroup's half of the ring
     int64_t prev_q = -1;
     uint32_t qcount = 0;
     int cur_slot = 0;
@@ -383,46 +431,61 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
       }
       float m0 = -INFINITY, m1 = -INFINITY;
       int a0 = -1, a1 = -1;   // row of the running maximum (first one on ties); stays -1 when nothing beats -inf
-      for (int t = 0; t < L.tiles; ++t) {
+      // waits for the next chunk of this warpgroup's ring and starts its MMAs (the first K-step overwrites: scale-d = 0)
+      auto issue = [&](float (&acc)[32]) -> int {
         const int stage = c * ring + (int)(seq % ring);
         mbar_wait(&S->full[stage], (uint32_t)((seq / ring) & 1));
         ++seq;
         const uint32_t daddr = smem_u32(stage_base + (size_t)stage * L.stage_bytes);
-        float acc[NCH][32];   // the first K-step overwrites (scale-d = 0): no zeroing inside the wgmma pipeline
         wgmma_fence();
         for (int kb = 0; kb < L.kblocks; ++kb) {
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint64_t adesc = make_wgmma_sw128_desc(qaddr + kb * kQBlockBytes + k * 32);
-#pragma unroll
-            for (int h = 0; h < NCH; ++h)
-              wgmma_n64<T>(acc[h], adesc, make_wgmma_sw128_desc(daddr + kb * L.tn * 128 + h * 64 * 128 + k * 32), (kb | k) != 0);
-          }
+          for (int k = 0; k < 4; ++k)
+            wgmma_n64<T>(acc, make_wgmma_sw128_desc(qaddr + kb * kQBlockBytes + k * 32),
+                         make_wgmma_sw128_desc(daddr + kb * kChunkKBlockBytes + k * 32), (kb | k) != 0);
         }
         wgmma_commit();
-        wgmma_wait<0>();
-#pragma unroll
-        for (int h = 0; h < NCH; ++h) wgmma_fence_regs(acc[h]);
+        wgmma_fence_regs(acc);
+        return stage;
+      };
+      // masked max over a finished chunk's 64 columns (columns col0 ..), then the stage goes back to the producer
+      auto reduce = [&](float (&acc)[32], int stage, int col0) {
+        wgmma_fence_regs(acc);
         if (wq < 2) {
-          const float* pen = reinterpret_cast<const float*>(stage_base + (size_t)stage * L.stage_bytes + L.doc_bytes);
+          const float* pen = reinterpret_cast<const float*>(stage_base + (size_t)stage * L.stage_bytes + L.chunk_bytes);
 #pragma unroll
-          for (int h = 0; h < NCH; ++h) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const int col = h * 64 + 8 * j + cq;
-              const float2 pv = *reinterpret_cast<const float2*>(pen + col);
-              const int gcol = t * L.tn + col;
-              take<kArgmax>(acc[h][4 * j + 0] + pv.x, gcol, m0, a0);
-              take<kArgmax>(acc[h][4 * j + 1] + pv.y, gcol + 1, m0, a0);
-              take<kArgmax>(acc[h][4 * j + 2] + pv.x, gcol, m1, a1);
-              take<kArgmax>(acc[h][4 * j + 3] + pv.y, gcol + 1, m1, a1);
-            }
+          for (int j = 0; j < 8; ++j) {
+            const int col = 8 * j + cq;
+            const float2 pv = *reinterpret_cast<const float2*>(pen + col);
+            take<kArgmax>(acc[4 * j + 0] + pv.x, col0 + col, m0, a0);
+            take<kArgmax>(acc[4 * j + 1] + pv.y, col0 + col + 1, m0, a0);
+            take<kArgmax>(acc[4 * j + 2] + pv.x, col0 + col, m1, a1);
+            take<kArgmax>(acc[4 * j + 3] + pv.y, col0 + col + 1, m1, a1);
           }
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(&S->empty[stage]);
+      };
+      auto header = [&](int stage) {
+        return *reinterpret_cast<const volatile int32_t*>(stage_base + (size_t)stage * L.stage_bytes + L.chunk_bytes +
+                                                          kChunkRows * 4);
+      };
+      // one chunk at a time: its stage goes back to the producer as soon as it is reduced, and the other warpgroup's
+      // MMAs fill the tensor cores meanwhile
+      float acc[32];
+      int hdr = 0;
+      for (int col0 = 0; !(hdr & kLastChunk); col0 += kChunkRows) {
+        const int st = issue(acc);
+        hdr = header(st);
+        wgmma_wait<0>();
+        reduce(acc, st, col0);
       }
       if (wq < 2) {
+        // the reference's -1000 fill, after every real row (ties keep the real row); column Ld reports -1 below
+        if (hdr & kFill) {
+          take<kArgmax>(-1000.f, P.Ld, m0, a0);
+          take<kArgmax>(-1000.f, P.Ld, m1, a1);
+        }
         // the four threads of a quad hold the same two rows: combine (larger value, then first column)
 #pragma unroll
         for (int o = 1; o <= 2; o <<= 1) {
@@ -438,7 +501,7 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
         }
         const bool ok0 = mask_test(qraw0, qmt), ok1 = mask_test(qraw1, qmt);   // qraw = 0 for rows >= Lq
         if constexpr (kArgmax) {
-          // rows >= Ld are the -inf padding and the virtual -1000 row: a max taken there carries no gradient (-1), like a
+          // rows >= Ld are the -inf padding and the -1000 fill: a max taken there carries no gradient (-1), like a
           // masked query token
           if ((lane & 3) == 0) {
             if (r0 < P.Lq) P.argmax[p * (int64_t)P.Lq + r0] = (ok0 && a0 < P.Ld) ? a0 : -1;
@@ -458,80 +521,41 @@ maxsim_qm_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
 }
 
 template <typename T, bool kArgmax, bool kStore>
-int launch_qm(int nch, int grid, size_t smem_bytes, cudaStream_t stream, const CUtensorMap& tq, const CUtensorMap& td,
-              const CUtensorMap& td16, const MaxsimParams& P, const QmLaunch& L) {
-#define MMB_QM_CASE(N)                                                                                                  \
-  case N:                                                                                                               \
-    MMB_CHECK_CUDA(cudaFuncSetAttribute(maxsim_qm_kernel<T, N, kArgmax, kStore>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                        (int)smem_bytes));                                                              \
-    maxsim_qm_kernel<T, N, kArgmax, kStore><<<grid, kThreads, smem_bytes, stream>>>(tq, td, td16, P, L);                \
-    break;
-  switch (nch) {
-    MMB_QM_CASE(1)
-    MMB_QM_CASE(2)
-    MMB_QM_CASE(3)
-    MMB_QM_CASE(4)
-    default:
-      set_error("maxsim queries-on-M: tile width out of range");
-      return MMB200_ERR_INVALID;
-  }
-#undef MMB_QM_CASE
+int launch_qm(int grid, size_t smem_bytes, cudaStream_t stream, const QmMaps& M, const MaxsimParams& P,
+              const QmLaunch& L) {
+  MMB_CHECK_CUDA(cudaFuncSetAttribute(maxsim_qm_kernel<T, kArgmax, kStore>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)smem_bytes));
+  maxsim_qm_kernel<T, kArgmax, kStore><<<grid, kThreads, smem_bytes, stream>>>(M, P, L);
   MMB_CHECK_CUDA(cudaGetLastError());
   return MMB200_OK;
 }
 
 }  // namespace
 
-// rows_needed[di] = 1 + last unmasked row (one warp per document)
-__global__ void __launch_bounds__(256) rows_needed_kernel(const void* __restrict__ d_mask, int mask_dtype,
-                                                          int32_t* __restrict__ rows_needed, int64_t n_d, int Ld) {
-  const int lane = threadIdx.x & 31;
-  const int64_t w = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
-  if (w >= n_d) return;
-  int last = 0;
-  if (!d_mask) last = Ld;
-  else
-    for (int j = lane; j < Ld; j += 32)
-      if (mask_at(d_mask, mask_dtype, w * Ld + j)) last = j + 1;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) last = max(last, __shfl_xor_sync(0xffffffffu, last, o));
-  if (lane == 0) rows_needed[w] = last;
-}
-
-int maxsim_rows_needed_launch(const void* d_mask, int mask_dtype, int32_t* rows_needed, int64_t n_d, int Ld,
-                              cudaStream_t stream) {
-  if (n_d == 0) return MMB200_OK;
-  rows_needed_kernel<<<(unsigned)((n_d + 7) / 8), 256, 0, stream>>>(d_mask, d_mask ? mask_dtype : MMB200_MASK_NONE, rows_needed, n_d, Ld);
-  MMB_CHECK_CUDA(cudaGetLastError());
-  return MMB200_OK;
-}
-
 // Returns MMB200_OK with *handled = false when the shape is outside this kernel's envelope.
 int maxsim_qm_launch(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cudaStream_t stream, bool* handled) {
   *handled = false;
   if (dtype != MMB200_F16 && dtype != MMB200_BF16) return MMB200_OK;
-  if (P.Lq > kQRows || (P.dim != 64 && P.dim != 128)) return MMB200_OK;
-  if (P.rows_needed && (P.pair_d || P.pair_dmask)) return MMB200_OK;  // rows_needed is indexed by the implicit doc id
+  if (P.Lq > kQRows || (P.dim != 64 && P.dim != 128) || P.Ld > kMaxLd) return MMB200_OK;
   if ((reinterpret_cast<uintptr_t>(P.q) | reinterpret_cast<uintptr_t>(P.d)) & 15) return MMB200_OK;
+  if (P.doc_offsets && P.argmax) return MMB200_OK;   // store mode never asks for argmax
   QmLaunch L;
   L.kblocks = P.dim / 64;
-  const int rows = P.Ld + (P.doc_offsets ? 0 : 1);  // + the virtual row that carries the reference's -1000 fill
-  L.tiles = (rows + 255) / 256;
-  L.tn = (((rows + L.tiles - 1) / L.tiles) + 63) / 64 * 64;
-  L.doc_bytes = L.kblocks * L.tn * 128;
-  L.stage_bytes = L.doc_bytes + (L.tn * 4 + 1023) / 1024 * 1024;
+  L.chunk_bytes = L.kblocks * kChunkKBlockBytes;
+  L.stage_bytes = L.chunk_bytes + kAuxBytes;
   const int fixed = kQSlots * L.kblocks * kQBlockBytes + (int)sizeof(QmShared) + 1024;
   L.stages = std::min(kMaxStages, (dev.max_smem_optin - fixed) / L.stage_bytes) & ~1;
-  if (L.stages < 2) return MMB200_OK;
+  // at least two stages per half of the ring, so that a chunk loads while the previous one is reduced
+  if (L.stages < 4) return MMB200_OK;
   const size_t smem_bytes = (size_t)L.stages * L.stage_bytes + fixed;
 
   const CUtensorMapDataType tdt = dtype == MMB200_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-  CUtensorMap tq, td;
+  QmMaps M;
   {
     const uint64_t dims[4] = {64, (uint64_t)P.Lq, (uint64_t)L.kblocks, (uint64_t)P.n_q};
     const uint64_t strides[3] = {(uint64_t)P.dim * 2, 128, (uint64_t)P.Lq * P.dim * 2};
     const uint32_t box[4] = {64, (uint32_t)kQRows, 1, 1};
-    if (int rc = encode_tensor_map(&tq, tdt, 4, P.q, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B,
+    if (int rc = encode_tensor_map(&M.q, tdt, 4, P.q, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B,
                                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B))
       return rc;
   }
@@ -542,33 +566,21 @@ int maxsim_qm_launch(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cu
   {
     const uint64_t dims[4] = {64, d_rows, (uint64_t)L.kblocks, d_count};
     const uint64_t strides[3] = {(uint64_t)P.dim * 2, 128, d_rows * P.dim * 2};
-    const uint32_t box[4] = {64, (uint32_t)L.tn, (uint32_t)L.kblocks, 1};
-    if (int rc = encode_tensor_map(&td, tdt, 4, P.d, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B,
-                                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B))
-      return rc;
-  }
-  CUtensorMap td16;
-  {
-    const uint64_t dims[4] = {64, d_rows, (uint64_t)L.kblocks, d_count};
-    const uint64_t strides[3] = {(uint64_t)P.dim * 2, 128, d_rows * P.dim * 2};
-    const uint32_t box[4] = {64, 16, 1, 1};
-    if (int rc = encode_tensor_map(&td16, tdt, 4, P.d, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B,
+    const uint32_t box[4] = {64, (uint32_t)kChunkRows, (uint32_t)L.kblocks, 1};
+    if (int rc = encode_tensor_map(&M.d, tdt, 4, P.d, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B,
                                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B))
       return rc;
   }
   *handled = true;
   const int grid = (int)std::min<int64_t>(dev.sm_count, P.n_pairs);
-  const int nch = L.tn / 64;
-  if (P.doc_offsets) {   // store mode never asks for argmax
-    if (P.argmax) { *handled = false; return MMB200_OK; }
-    return dtype == MMB200_F16 ? launch_qm<__half, false, true>(nch, grid, smem_bytes, stream, tq, td, td16, P, L)
-                               : launch_qm<__nv_bfloat16, false, true>(nch, grid, smem_bytes, stream, tq, td, td16, P, L);
-  }
+  if (P.doc_offsets)
+    return dtype == MMB200_F16 ? launch_qm<__half, false, true>(grid, smem_bytes, stream, M, P, L)
+                               : launch_qm<__nv_bfloat16, false, true>(grid, smem_bytes, stream, M, P, L);
   if (dtype == MMB200_F16)
-    return P.argmax ? launch_qm<__half, true, false>(nch, grid, smem_bytes, stream, tq, td, td16, P, L)
-                    : launch_qm<__half, false, false>(nch, grid, smem_bytes, stream, tq, td, td16, P, L);
-  return P.argmax ? launch_qm<__nv_bfloat16, true, false>(nch, grid, smem_bytes, stream, tq, td, td16, P, L)
-                  : launch_qm<__nv_bfloat16, false, false>(nch, grid, smem_bytes, stream, tq, td, td16, P, L);
+    return P.argmax ? launch_qm<__half, true, false>(grid, smem_bytes, stream, M, P, L)
+                    : launch_qm<__half, false, false>(grid, smem_bytes, stream, M, P, L);
+  return P.argmax ? launch_qm<__nv_bfloat16, true, false>(grid, smem_bytes, stream, M, P, L)
+                  : launch_qm<__nv_bfloat16, false, false>(grid, smem_bytes, stream, M, P, L);
 }
 
 }  // namespace mmb

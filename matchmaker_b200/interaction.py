@@ -14,6 +14,8 @@ from . import _lib
 _DTYPES = {torch.float16: _lib.F16, torch.bfloat16: _lib.BF16, torch.float32: _lib.F32}
 _MASK_DTYPES = {torch.bool: _lib.MASK_U8, torch.uint8: _lib.MASK_U8, torch.int32: _lib.MASK_I32,
                 torch.int64: _lib.MASK_I64, torch.float32: _lib.MASK_F32}
+# "tcgen05_ragged" is an alias of "tcgen05": the max-sim tensor-core kernel fetches only each document's live rows
+# (up to its last unmasked one) whichever name selects it; the name stays accepted for existing callers.
 _IMPLS = {"auto": _lib.IMPL_AUTO, "simt": _lib.IMPL_SIMT, "tcgen05": _lib.IMPL_TCGEN05,
           "tcgen05_docm": _lib.IMPL_TCGEN05_DOCM, "tcgen05_ragged": _lib.IMPL_TCGEN05_RAGGED}
 
