@@ -409,6 +409,48 @@ MMB200_API int mmb200_graph_search(const void* queries, const void* rows, const 
                                    void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Anisotropic-hashing (AH) index: a scan of 4-bit residual codes through per-query lookup tables, then exact reorder
+ *
+ * Replaces: ScaNNIndexer   matchmaker/retrieval/scann_index.py:10-53 (scann tree + score_ah(2, ...) + reorder, CPU only).
+ *
+ * mmb200_ah_search: the kr best rows by approximate score over each query's probed leaves.
+ *          codes    [n_rows, dim / 4] uint8 sorted by leaf: leaf l is rows [list_offsets[l], list_offsets[l+1]) (int64
+ *                   [nlist + 1], non-decreasing).  Byte j of a row holds the codeword of block 2j in its low nibble and
+ *                   that of block 2j + 1 in its high nibble (M = dim / 2 blocks of 2 dimensions, 16 codewords each).
+ *          luts     [nq, M, 16] fp32: luts[q][m][c] = <query q, codeword c of block m>.
+ *          probes   [nq, nprobe] int64 leaf ids, distinct within a row; an id outside [0, nlist) probes nothing.
+ *          bias     [nq, nprobe] fp32: <query, centroid of the probed leaf>.
+ *          Approximate score of row r of leaf l for query q = bias + sum over m ascending of luts[q][m][code_m(r)], fp32.
+ *          Each (query, probe) keeps its best min(kr, leaf length) rows in a slot of min(kr, max_list_len) rounded up
+ *          to 32 entries (max_list_len should bound every leaf's length: a longer leaf keeps only its slot's worth of
+ *          best rows, no fault), and the slots of a query are merged.
+ *          out_scores / out_pos [nq, kr]: approximate scores and ROW POSITIONS under (score desc, position asc), with a
+ *          (-3.4028235e38, -1) tail when the probed leaves hold fewer than kr rows.  Work items (leaf, chunk of <= 128
+ *          probing queries) are built on the device; each reads the leaf's codes once per 8 resident lookup tables
+ *          (fewer when the tables are large).  No host synchronisation.
+ * mmb200_ah_workspace_bytes: device scratch of one mmb200_ah_search call, about nq * nprobe * 12 * slot bytes; 0 =
+ *          sizes outside the envelope (checked without a device), -1 = no device.
+ *          Envelope: 1 <= kr <= 1024, 1 <= nprobe <= 1024, dim % 64 == 0 with one lookup table (32 * dim bytes) and the
+ *          code ring (32 * dim bytes) in 227 KB of shared memory (dim <= 3584), nq * nprobe < 2^31 - 128,
+ *          n_rows < 2^31, 16-byte aligned luts and codes.  Outside it: MMB200_ERR_INVALID.  Not sm_90:
+ *          MMB200_ERR_UNSUPPORTED.
+ * mmb200_ah_reorder: exact re-scoring of a shortlist.  rows [n_rows, dim] fp16 or fp32 (`dtype`, 16-byte aligned),
+ *          queries [nq, dim] in the same dtype, shortlist [nq, kr] int64 row positions (entries outside [0, n_rows) are
+ *          void), ids [n_rows] int64 user ids (NULL: the position).  Every score is one fixed-order fp32 formula (lane
+ *          teams over 16-byte chunks, xor butterfly).  out_scores / out_ids [nq, top_n]: the best top_n under (score
+ *          desc, id asc), then (-3.4028235e38, -1).  1 <= top_n <= kr <= 1024, dim % 64 == 0, dim <= 4096.
+ * ------------------------------------------------------------------------------------------ */
+MMB200_API int64_t mmb200_ah_workspace_bytes(int64_t nq, int32_t nprobe, int64_t nlist, int64_t max_list_len,
+                                             int32_t dim, int32_t kr);
+MMB200_API int mmb200_ah_search(const float* luts, const uint8_t* codes, const int64_t* list_offsets,
+                                const int64_t* probes, const float* bias, float* out_scores, int64_t* out_pos,
+                                void* workspace, int64_t workspace_bytes, int64_t nq, int32_t nprobe, int64_t nlist,
+                                int64_t n_rows, int64_t max_list_len, int32_t dim, int32_t kr, void* stream);
+MMB200_API int mmb200_ah_reorder(const void* queries, const void* rows, const int64_t* ids, const int64_t* shortlist,
+                                 float* out_scores, int64_t* out_ids, int64_t nq, int64_t n_rows, int32_t dim,
+                                 int32_t kr, int32_t top_n, int32_t dtype, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Storage block loader: byte ranges of files -> one contiguous DEVICE buffer.
  *
  * Replaces: the host path of the encoded collection between matchmaker/dense_retrieval.py:291-302

@@ -47,6 +47,9 @@ SIGNATURES = {
     "mmb200_ivf_workspace_bytes": (_i64, [_i64, _i32, _i64, _i64, _i32, _i32, _i32]),
     "mmb200_ivf_search": (_c.c_int, [_vp] * 8 + [_i64, _i64, _i32, _i64, _i64, _i64, _i32, _i32, _i32, _vp]),
     "mmb200_ivf_list_means": (_c.c_int, [_vp] * 4 + [_i64, _i32, _i32, _vp]),
+    "mmb200_ah_workspace_bytes": (_i64, [_i64, _i32, _i64, _i64, _i32, _i32]),
+    "mmb200_ah_search": (_c.c_int, [_vp] * 8 + [_i64, _i64, _i32, _i64, _i64, _i64, _i32, _i32, _vp]),
+    "mmb200_ah_reorder": (_c.c_int, [_vp] * 6 + [_i64, _i64, _i32, _i32, _i32, _i32, _vp]),
     "mmb200_graph_prune": (_c.c_int, [_vp, _vp, _i64, _i32, _i32, _vp]),
     "mmb200_graph_hash_slots": (_i64, [_i32, _i32]),
     "mmb200_graph_search": (_c.c_int, [_vp] * 7 + [_i64, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),

@@ -55,6 +55,30 @@ __device__ __forceinline__ float to_float<__half>(__half v) { return __half2floa
 template <>
 __device__ __forceinline__ float to_float<__nv_bfloat16>(__nv_bfloat16 v) { return __bfloat162float(v); }
 
+// acc + <q[0..n), row chunk v> with one fma per element in element order: n = 8 fp16 (dot_chunk) or 4 fp32
+// (dot_chunk_f32) values packed in 16 bytes.  The scoring loops of the graph search and the AH reorder use them.
+__device__ __forceinline__ float dot_half2(uint32_t w, const float* q, float acc) {
+  float lo, hi;
+  asm("{\n\t.reg .f16 a, b;\n\tmov.b32 {a, b}, %2;\n\tcvt.f32.f16 %0, a;\n\tcvt.f32.f16 %1, b;\n\t}"
+      : "=f"(lo), "=f"(hi)
+      : "r"(w));
+  acc = fmaf(q[0], lo, acc);
+  return fmaf(q[1], hi, acc);
+}
+__device__ __forceinline__ float dot_chunk(const uint4 v, const float* q, float acc) {
+  acc = dot_half2(v.x, q, acc);
+  acc = dot_half2(v.y, q + 2, acc);
+  acc = dot_half2(v.z, q + 4, acc);
+  return dot_half2(v.w, q + 6, acc);
+}
+__device__ __forceinline__ float dot_chunk_f32(const uint4 v, const float* q, float acc) {
+  acc = fmaf(q[0], __uint_as_float(v.x), acc);
+  acc = fmaf(q[1], __uint_as_float(v.y), acc);
+  acc = fmaf(q[2], __uint_as_float(v.z), acc);
+  acc = fmaf(q[3], __uint_as_float(v.w), acc);
+  return acc;
+}
+
 // Contiguous share [*begin, *end) of n items for this CTA of a persistent grid; the first n % gridDim.x CTAs take one more.
 __device__ __forceinline__ void cta_share(int64_t n, int64_t* begin, int64_t* end) {
   const int64_t per = n / gridDim.x, rem = n % gridDim.x;

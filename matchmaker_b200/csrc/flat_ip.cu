@@ -35,6 +35,7 @@
 
 #include "device_util.cuh"
 #include "host_util.cuh"
+#include "ivf_items.cuh"
 #include "ptx.cuh"
 
 namespace mmb {
@@ -714,47 +715,7 @@ int launch_merge(const float* cand_scores, const int64_t* cand_ids, int64_t nq, 
 // queries list by list, scan every (list, chunk of <= BM queries) item with flat_ip_tc_kernel<..., IVF = true>, merge
 // the per-(query, probe) slots.  Nothing is read back to the host: the item count stays in device memory.
 // ---------------------------------------------------------------------------------------------
-constexpr int kIvfMaxProbe = 1024;
-
-// probes per list
-__global__ void ivf_count_kernel(const int64_t* __restrict__ probes, int64_t n_pairs, int64_t nlist, int* __restrict__ cnt) {
-  for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < n_pairs; p += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t l = probes[p];
-    if (l >= 0 && l < nlist) atomicAdd(cnt + l, 1);
-  }
-}
-
-// One block of 1024 threads: exclusive scans of the probe counts (first gathered row of each list) and of the item
-// counts ceil(cnt / BM) (first item of each list); the total item count goes to *n_items.  Thread t scans a contiguous
-// segment, so the result does not depend on scheduling.
-__global__ void __launch_bounds__(1024) ivf_scan_kernel(const int* __restrict__ cnt, int64_t nlist,
-                                                        int* __restrict__ row_base, int* __restrict__ item_base,
-                                                        int* __restrict__ n_items) {
-  __shared__ int s_rows[1024], s_items[1024];
-  const int t = threadIdx.x;
-  const int64_t seg = (nlist + 1023) / 1024, lo = min(nlist, t * seg), hi = min(nlist, lo + seg);
-  int rows = 0, items = 0;
-  for (int64_t l = lo; l < hi; ++l) { rows += cnt[l]; items += (cnt[l] + BM - 1) / BM; }
-  s_rows[t] = rows;
-  s_items[t] = items;
-  __syncthreads();
-  for (int o = 1; o < 1024; o <<= 1) {   // inclusive Hillis-Steele scan
-    const int r = t >= o ? s_rows[t - o] : 0, i = t >= o ? s_items[t - o] : 0;
-    __syncthreads();
-    s_rows[t] += r;
-    s_items[t] += i;
-    __syncthreads();
-  }
-  rows = s_rows[t] - rows;
-  items = s_items[t] - items;
-  for (int64_t l = lo; l < hi; ++l) {
-    row_base[l] = rows;
-    item_base[l] = items;
-    rows += cnt[l];
-    items += (cnt[l] + BM - 1) / BM;
-  }
-  if (t == 1023) *n_items = s_items[1023];
-}
+static_assert(BM == kIvfChunk, "an IVF work item is one query block");
 
 // One warp per (query, probe) pair: take the next row of the probed list's query set and copy the query there.  A pair
 // whose list id is out of range (a -1 filler of the coarse search) probes nothing: its slot is filled as empty.
@@ -781,16 +742,6 @@ __global__ void ivf_gather_kernel(const int64_t* __restrict__ probes, int64_t n_
         cand_ids[p * kslot + e] = -1;
       }
     }
-  }
-}
-
-// The work items of every list: (list, first gathered row, rows), in list order.
-__global__ void ivf_items_kernel(const int* __restrict__ cnt, int64_t nlist, const int* __restrict__ row_base,
-                                 const int* __restrict__ item_base, int4* __restrict__ items) {
-  for (int64_t l = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; l < nlist; l += (int64_t)gridDim.x * blockDim.x) {
-    const int c = cnt[l];
-    for (int j = 0; j * BM < c; ++j)
-      items[item_base[l] + j] = make_int4((int)l, row_base[l] + j * BM, min(BM, c - j * BM), 0);
   }
 }
 

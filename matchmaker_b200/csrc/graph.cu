@@ -129,28 +129,6 @@ __device__ __forceinline__ float key_score(uint64_t k) {
   return __uint_as_float((o & 0x80000000u) ? (o & 0x7fffffffu) : ~o);
 }
 
-__device__ __forceinline__ float dot_half2(uint32_t w, const float* q, float acc) {
-  float lo, hi;
-  asm("{\n\t.reg .f16 a, b;\n\tmov.b32 {a, b}, %2;\n\tcvt.f32.f16 %0, a;\n\tcvt.f32.f16 %1, b;\n\t}"
-      : "=f"(lo), "=f"(hi)
-      : "r"(w));
-  acc = fmaf(q[0], lo, acc);
-  return fmaf(q[1], hi, acc);
-}
-__device__ __forceinline__ float dot_chunk(const uint4 v, const float* q, float acc) {
-  acc = dot_half2(v.x, q, acc);
-  acc = dot_half2(v.y, q + 2, acc);
-  acc = dot_half2(v.z, q + 4, acc);
-  return dot_half2(v.w, q + 6, acc);
-}
-__device__ __forceinline__ float dot_chunk_f32(const uint4 v, const float* q, float acc) {
-  acc = fmaf(q[0], __uint_as_float(v.x), acc);
-  acc = fmaf(q[1], __uint_as_float(v.y), acc);
-  acc = fmaf(q[2], __uint_as_float(v.z), acc);
-  acc = fmaf(q[3], __uint_as_float(v.w), acc);
-  return acc;
-}
-
 // keys[r] = key(<q, row ids[r]>, ids[r]) for r < c.  A team of `team` lanes (a power of two <= 32) scores one row with
 // 16-byte loads: lane t sums chunks t, t + team, ... in order, then the team adds its lanes by an xor butterfly.
 template <typename T>

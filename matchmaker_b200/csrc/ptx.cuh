@@ -125,6 +125,14 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, void* smem_d
       : "memory");
 }
 
+// Plain bulk copy (no tensor map): `bytes` (a multiple of 16) from 16-byte aligned global memory to 16-byte aligned shared
+// memory; completion is signalled as transaction bytes on `bar`.
+__device__ __forceinline__ void bulk_load(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(gmem_src)), "r"(bytes), "r"(smem_u32(bar))
+               : "memory");
+}
+
 // ---------------------------------------------------------------------------------------------
 // wgmma (sm_90a): D[64 x N] (+)= A[64 x K] * B[N x K]^T, issued by all 128 threads of a warpgroup (4 consecutive
 // warps starting at a multiple of 4), accumulator in registers.  Fragment of thread (warp w of the warpgroup, lane l),

@@ -601,6 +601,89 @@ def ivf_list_means(x: torch.Tensor, perm: torch.Tensor, offsets: torch.Tensor) -
     return out
 
 
+AH_MAX_KR = 1024
+# Device scratch one ah_search call may take; it grows with nq * nprobe (one candidate slot per (query, probe)), so
+# larger query sets are searched in batches that fit.
+AH_WORKSPACE_CAP = 2 << 30
+
+
+def ah_search(luts: torch.Tensor, codes: torch.Tensor, list_offsets: torch.Tensor, probes: torch.Tensor,
+              bias: torch.Tensor, kr: int, max_list_len: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Approximate top-kr over each query's probed leaves from 4-bit AH codes (mmb200_ah_search).
+
+    luts [nq, dim/2, 16] f32 lookup tables; codes [n, dim/4] uint8 sorted by leaf (leaf l is rows
+    ``list_offsets[l]:list_offsets[l+1]``, block 2j in the low nibble of byte j, block 2j+1 in the high one); probes
+    [nq, nprobe] int64 leaf ids (ids outside [0, nlist) probe nothing); bias [nq, nprobe] f32, each probed leaf's
+    <query, centroid>.  Score = bias + sum over blocks ascending of luts[q, m, code], fp32.  Returns (approximate scores
+    [nq, kr] f32, row positions [nq, kr] int64) under (score desc, position asc) with a (-3.4028235e38, -1) tail.
+    1 <= kr <= 1024, 1 <= nprobe <= 1024, dim % 64 == 0.  Queries are searched in batches whose scratch fits
+    AH_WORKSPACE_CAP.  No host synchronisation."""
+    dev = _require_cuda(luts, codes, list_offsets, probes, bias)
+    if codes.dtype != torch.uint8 or codes.dim() != 2:
+        raise _lib.MatchmakerB200Error("ah_search: codes must be [n, dim/4] uint8")
+    n, dim = codes.shape[0], codes.shape[1] * 4
+    if probes.dim() != 2 or luts.shape != (probes.shape[0], dim // 2, 16) or bias.shape != probes.shape:
+        raise _lib.MatchmakerB200Error(f"ah_search: luts {tuple(luts.shape)}, probes {tuple(probes.shape)} and bias "
+                                       f"{tuple(bias.shape)} do not fit codes for dim {dim}")
+    nq, nprobe = probes.shape
+    nlist = list_offsets.numel() - 1
+    luts, codes = luts.to(torch.float32).contiguous(), codes.contiguous()
+    probes, bias = probes.to(torch.int64).contiguous(), bias.to(torch.float32).contiguous()
+    list_offsets = list_offsets.to(torch.int64).contiguous()
+    out_s = torch.empty((nq, kr), dtype=torch.float32, device=dev)
+    out_p = torch.empty((nq, kr), dtype=torch.int64, device=dev)
+    if nq == 0:
+        return out_s, out_p
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        def wsb(b):
+            return lib.mmb200_ah_workspace_bytes(b, nprobe, nlist, max_list_len, dim, kr)
+        if wsb(1) <= 0:
+            raise _lib.MatchmakerB200Error(f"ah_search: unsupported sizes nprobe={nprobe} nlist={nlist} dim={dim} kr={kr} "
+                                           f"(1 <= kr <= {AH_MAX_KR}, 1 <= nprobe <= {IVF_MAX_PROBE}, dim % 64 == 0)")
+        b = ivf_query_batch(nq, wsb, AH_WORKSPACE_CAP)
+        ws = torch.empty(wsb(b), dtype=torch.uint8, device=dev)
+        for b0 in range(0, nq, b):
+            b1 = min(nq, b0 + b)
+            rc = lib.mmb200_ah_search(_ptr(luts[b0:b1]), _ptr(codes), _ptr(list_offsets), _ptr(probes[b0:b1]),
+                                      _ptr(bias[b0:b1]), _ptr(out_s[b0:b1]), _ptr(out_p[b0:b1]), _ptr(ws), ws.numel(),
+                                      b1 - b0, nprobe, nlist, n, max_list_len, dim, kr, _stream(dev))
+            _lib.check(rc, "mmb200_ah_search")
+    return out_s, out_p
+
+
+def ah_reorder(queries: torch.Tensor, rows: torch.Tensor, ids: Optional[torch.Tensor], shortlist: torch.Tensor,
+               top_n: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Exact re-scoring of a shortlist (mmb200_ah_reorder): rows [n, dim] fp16 or fp32 (queries are cast to it),
+    shortlist [nq, kr] int64 row positions (-1 = void), ids [n] int64 user ids.  Every score is one fixed-order fp32
+    formula.  Returns (scores [nq, top_n] f32, ids [nq, top_n] int64) under (score desc, id asc) with a
+    (-3.4028235e38, -1) tail.  1 <= top_n <= kr <= 1024.  No host synchronisation."""
+    dev = _require_cuda(queries, rows, ids, shortlist)
+    if rows.dtype not in (torch.float16, torch.float32) or rows.dim() != 2:
+        raise _lib.MatchmakerB200Error("ah_reorder: rows must be [n, dim] fp16 or fp32")
+    n, dim = rows.shape
+    if queries.dim() != 2 or queries.shape[1] != dim or shortlist.dim() != 2 or shortlist.shape[0] != queries.shape[0]:
+        raise _lib.MatchmakerB200Error(f"ah_reorder: queries {tuple(queries.shape)}, shortlist {tuple(shortlist.shape)} "
+                                       f"for rows of dim {dim}")
+    nq, kr = shortlist.shape
+    if not 1 <= top_n <= kr <= AH_MAX_KR:
+        raise _lib.MatchmakerB200Error(f"ah_reorder: need 1 <= top_n <= kr <= {AH_MAX_KR}, got top_n={top_n} kr={kr}")
+    queries, rows = queries.to(rows.dtype).contiguous(), rows.contiguous()
+    shortlist = shortlist.to(torch.int64).contiguous()
+    if ids is not None:
+        ids = ids.to(torch.int64).contiguous()
+    out_s = torch.empty((nq, top_n), dtype=torch.float32, device=dev)
+    out_i = torch.empty((nq, top_n), dtype=torch.int64, device=dev)
+    if nq == 0:
+        return out_s, out_i
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        rc = lib.mmb200_ah_reorder(_ptr(queries), _ptr(rows), _ptr(ids), _ptr(shortlist), _ptr(out_s), _ptr(out_i), nq, n,
+                                   dim, kr, int(top_n), _DTYPES[rows.dtype], _stream(dev))
+    _lib.check(rc, "mmb200_ah_reorder")
+    return out_s, out_i
+
+
 GRAPH_MAX_DEGREE = 1024   # R, edges per node
 GRAPH_MAX_KNN = 1023      # K, k-NN degree before pruning
 GRAPH_MAX_LIST = 1024     # L, search list size
