@@ -227,8 +227,9 @@ __global__ void __launch_bounds__(kThreads) tkl_bwd_kernel(TklBwdParams P) {
           const float dy0 = dsat1 * sp[4] + dz2 * sp[7] + dsat3 * sp[10];
           const float dy1 = dsat1 * sp[5] + dz2 * sp[8] + dsat3 * sp[11];
           const float dn0 = dy0 * sp[0], dn1 = dy1 * sp[1];
-          const float mdn = (dn0 + dn1) * 0.5f, mdnn = (dn0 * n0 + dn1 * n1) * 0.5f;
-          da0[i] += rstd * (dn0 - mdn - n0 * mdnn);  // the length input (index 1) is a count: no gradient
+          // LayerNorm over two values: n1 = -n0, so d a0 = rstd (dn0 - dn1) / 2 (1 - n0^2) with 1 - n0^2 = eps rstd^2.  The
+          // last form keeps full precision when |a0 - a1| >> sqrt(eps), where 1 - n0 * n0 is fp32 rounding noise.
+          da0[i] += rstd * (dn0 - dn1) * 0.5f * (1e-5f * rstd * rstd);  // the length input (index 1) is a count: no gradient
           pp[0] = dy0 * n0; pp[1] = dy1 * n1; pp[2] = dy0; pp[3] = dy1;            // sat_normer weight, bias
           pp[4] = dsat1 * y0; pp[5] = dsat1 * y1; pp[6] = dsat1;                   // saturation_linear
           pp[7] = dz2 * y0; pp[8] = dz2 * y1; pp[9] = dz2;                         // saturation_linear2
@@ -344,6 +345,22 @@ __global__ void tkl_reduce_batch(const float* __restrict__ ws, float* __restrict
   out[j] = s;
 }
 
+// dynamic shared memory of tkl_bwd_kernel<KB> at embedding dim D: the carve-up at the top of the kernel
+size_t bwd_smem_bytes(int D, int KB) {
+  const size_t dp = padded_row_stride(D);
+  const size_t floats = (size_t)(2 * kMaxLq + 2 * kRows) * dp + 2 * kMaxLq * 33 + 3 * (size_t)kMaxLq * KB +
+                        (size_t)kMaxLq * (kNSat + KB) + 6 * kMaxLq + 3 * kRows + 5 * KB + 16 + KB + (kNSat + KB) + 16 + 16;
+  return floats * sizeof(float) + 4 * kRows * sizeof(float) + 64;
+}
+
+// the largest embedding dim (a multiple of 4) whose plan fits in `limit` bytes: 356 with either KB under the H100's
+// 227 KB opt-in limit
+int bwd_max_dim(int KB, size_t limit) {
+  int d = 0;
+  while (bwd_smem_bytes(d + 4, KB) <= limit) d += 4;
+  return d;
+}
+
 }  // namespace
 }  // namespace mmb
 
@@ -357,7 +374,9 @@ extern "C" int mmb200_tkl_bwd(const float* q, const void* q_mask, const float* c
   using namespace mmb;
   MMB_REQUIRE(q && chunks && slot_to_packed && mu && sigma && dense_w && sat_params && chunk_scoring && top_idx &&
                   orig_score && grad_score && grad_q && grad_chunks && grad_params && workspace, "null pointer");
-  MMB_REQUIRE(Lq >= 1 && Lq <= kMaxLq && D > 0 && D % 4 == 0 && D <= 512 && K >= 1 && K <= 16 && C >= 1, "shape outside the TKL backward envelope");
+  // the bound on D comes from the shared-memory plan below (it depends on K and on the device)
+  MMB_REQUIRE(Lq >= 1 && Lq <= kMaxLq && D > 0 && D % 4 == 0 && K >= 1 && K <= 16 && C >= 1,
+              "shape outside the TKL backward envelope (1 <= Lq <= 40, D a multiple of 4, 1 <= K <= 16)");
   MMB_REQUIRE(saturation == 0 || saturation == 1, "saturation: 0 = embedding, 1 = log");
   MMB_REQUIRE(saturation == 1 || sat_red_w != nullptr, "embedding saturation needs sat_emb_reduce1 weights");
   DeviceInfo dev;
@@ -370,17 +389,17 @@ extern "C" int mmb200_tkl_bwd(const float* q, const void* q_mask, const float* c
   P.grad_q = grad_q; P.grad_chunks = grad_chunks; P.ws = workspace; P.B = B; P.Lq = Lq; P.D = D; P.C = C; P.K = K;
   P.W = (C * kChunk - kWindow) / 2 + 1; P.mask_dtype = mask_dtype; P.saturation = saturation;
   P.ws_stride = K + 15 + (saturation == 0 ? kNSat + D : K);
-  MMB_CHECK_CUDA(cudaMemsetAsync(grad_chunks, 0, (size_t)n_chunks * kChunk * D * sizeof(float), stream));
-  if (B == 0) return MMB200_OK;
   const int KB = K <= 12 ? 12 : 16;
-  const int dp = padded_row_stride(D);
-  const size_t floats = (size_t)(2 * kMaxLq + 2 * kRows) * dp + 2 * kMaxLq * 33 + 3 * (size_t)kMaxLq * KB +
-                        (size_t)kMaxLq * (kNSat + KB) + 6 * kMaxLq + 3 * kRows + 5 * KB + 16 + KB + (kNSat + KB) + 16 + 16;
-  const size_t need = floats * sizeof(float) + 4 * kRows * sizeof(float) + 64;
+  const size_t need = bwd_smem_bytes(D, KB);
   if (need > (size_t)dev.max_smem_optin) {
-    set_error("TKL backward: shared-memory plan does not fit");
+    const size_t limit = (size_t)dev.max_smem_optin;
+    set_error("TKL backward: D=" + std::to_string(D) + " with K=" + std::to_string(K) + " needs " + std::to_string(need) +
+              " bytes of shared memory, the device allows " + std::to_string(limit) + " (D <= " +
+              std::to_string(bwd_max_dim(KB, limit)) + " fits with K <= " + std::to_string(KB) + ")");
     return MMB200_ERR_UNSUPPORTED;
   }
+  MMB_CHECK_CUDA(cudaMemsetAsync(grad_chunks, 0, (size_t)n_chunks * kChunk * D * sizeof(float), stream));
+  if (B == 0) return MMB200_OK;
   const int grid = (int)std::min<int64_t>(B, (int64_t)dev.sm_count * 2);
   if (KB == 12) {
     MMB_CHECK_CUDA(cudaFuncSetAttribute(tkl_bwd_kernel<12>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)need));

@@ -801,7 +801,11 @@ def _tkl_slot_map(packed_indices: torch.Tensor) -> torch.Tensor:
 def tkl_bwd(q_ctx, q_mask, doc_chunks, chunk_mask, packed_indices, chunk_pieces, mu, sigma, dense_weight, saturation,
             sat_params, sat_red_weight, chunk_scoring, top_idx, orig_score, grad_score):
     """Gradients of the TKL interaction stage: returns (grad_q_ctx, grad_doc_chunks, grad_dense_weight [K],
-    grad_chunk_scoring [15], grad_sat_params, grad_sat_red_weight or None)."""
+    grad_chunk_scoring [15], grad_sat_params, grad_sat_red_weight or None).
+
+    Envelope: 1 <= Lq <= 40, 1 <= K <= 16, D a multiple of 4 up to what the kernel's shared-memory plan holds, D <= 356
+    on an H100 (227 KB per block); outside it the call raises MatchmakerB200Error before any launch.  The forward accepts
+    wider D through the tensor-core kernel, so a model with D > 356 can score but not train."""
     dev = _require_cuda(q_ctx, doc_chunks, grad_score)
     q_ctx = q_ctx.float().contiguous()
     doc_chunks = doc_chunks.float().contiguous()
