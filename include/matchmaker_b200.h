@@ -372,6 +372,18 @@ MMB200_API int mmb200_ivf_search(const void* queries, const void* rows, const in
                                  int32_t nprobe, int64_t nlist, int64_t n_rows, int64_t max_list_len, int32_t dim,
                                  int32_t k, int32_t dtype, void* stream);
 
+/* The same search over rows that are NOT sorted by list: list position p (list l is positions
+ * [list_offsets[l], list_offsets[l+1])) is row row_index[p] of `rows`.  row_index [list_offsets[nlist]] int64, each
+ * entry in [0, n_rows); ids [n_rows] are indexed by row, not by list position.  Every other argument, the result and
+ * the envelope are those of mmb200_ivf_search, including the workspace (mmb200_ivf_workspace_bytes).  This lets one
+ * passage-ordered copy of the rows (ColBERT's token store) serve an inverted-file scan and per-passage scoring: the
+ * scan gathers each tile's rows with 16-byte cp.async copies instead of one TMA box. */
+MMB200_API int mmb200_ivf_search_gather(const void* queries, const void* rows, const int64_t* ids,
+                                        const int64_t* row_index, const int64_t* list_offsets, const int64_t* probes,
+                                        float* out_scores, int64_t* out_ids, void* workspace, int64_t workspace_bytes,
+                                        int64_t nq, int32_t nprobe, int64_t nlist, int64_t n_rows,
+                                        int64_t max_list_len, int32_t dim, int32_t k, int32_t dtype, void* stream);
+
 /* Spherical k-means centroid update: out[l] = normalised mean of rows perm[offsets[l] .. offsets[l+1]) of x
  * ([n, dim] fp16 / bf16 / fp32, `dtype`).  The sum runs in that order in fp64, so the result is bit-reproducible;
  * an empty list gives a zero row.  perm [offsets[nlist]] int64, out [nlist, dim] f32.  1 <= dim <= 4096, else

@@ -46,6 +46,7 @@ SIGNATURES = {
     "mmb200_topk_unique": (_c.c_int, [_vp] * 4 + [_i64, _i32, _i32, _vp]),
     "mmb200_ivf_workspace_bytes": (_i64, [_i64, _i32, _i64, _i64, _i32, _i32, _i32]),
     "mmb200_ivf_search": (_c.c_int, [_vp] * 8 + [_i64, _i64, _i32, _i64, _i64, _i64, _i32, _i32, _i32, _vp]),
+    "mmb200_ivf_search_gather": (_c.c_int, [_vp] * 9 + [_i64, _i64, _i32, _i64, _i64, _i64, _i32, _i32, _i32, _vp]),
     "mmb200_ivf_list_means": (_c.c_int, [_vp] * 4 + [_i64, _i32, _i32, _vp]),
     "mmb200_ah_workspace_bytes": (_i64, [_i64, _i32, _i64, _i64, _i32, _i32]),
     "mmb200_ah_search": (_c.c_int, [_vp] * 8 + [_i64, _i64, _i32, _i64, _i64, _i64, _i32, _i32, _vp]),

@@ -86,6 +86,14 @@ struct IvfParams {
   int32_t nprobe;
 };
 
+// Gather mode only (flat_ip_tc_gather_kernel): list position p of the layout is store row row_index[p].  The rows stay
+// where they are (in the order stage 2 of ColBERT retrieval reads them); `FipParams::ids` is indexed by store row.
+struct GatherParams {
+  const uint8_t* rows;        // the store, rows `row_pitch` bytes apart (16-byte aligned)
+  const int64_t* row_index;   // [list_offsets[nlist]] store row of every list position
+  int64_t row_pitch;
+};
+
 // order-preserving map float -> uint32 (larger float <=> larger key)
 __device__ __forceinline__ uint32_t f2key(float f) {
   const uint32_t b = __float_as_uint(f);
@@ -103,10 +111,10 @@ __device__ __forceinline__ int64_t pos_to_id(const FipParams& P, uint32_t pos) {
 // Warp-cooperative compaction of one row's candidate list to its top-k under (score desc, id asc).
 // `list` has `cnt` valid entries (cnt <= 32 * EPL).  Returns the new count (min(cnt, k)) and the key of
 // the k-th best entry in *kth_key (kKeyNegInf if fewer than k entries).
-// __noinline__: the epilogue's per-tile loop has to stay inside the instruction cache.  With this routine inlined (and
-// the column loop unrolled) the loop body streamed ~100 KB of code per tile and ran at IPC 0.03.
-template <int EPL>
-__device__ __noinline__ int compact_row(const FipParams& P, uint2* list, int cnt, int lane, uint32_t* kth_key) {
+// GATHER: a list entry's position is a list position, its id that of store row row_index[position].
+template <int EPL, bool GATHER>
+__device__ __forceinline__ int compact_row_impl(const FipParams& P, const int64_t* row_index, uint2* list, int cnt,
+                                                int lane, uint32_t* kth_key) {
   uint32_t key[EPL], pos[EPL];
 #pragma unroll
   for (int j = 0; j < EPL; ++j) {
@@ -168,7 +176,8 @@ __device__ __noinline__ int compact_row(const FipParams& P, uint2* list, int cnt
 #pragma unroll
       for (int j = 0; j < EPL; ++j)
         if (key[j] == T && !(taken & (1ull << j))) {
-          const unsigned long long id = (unsigned long long)(pos_to_id(P, pos[j]) ^ (1ll << 63));  // signed order
+          const int64_t sid = GATHER ? P.ids[row_index[pos[j]]] : pos_to_id(P, pos[j]);
+          const unsigned long long id = (unsigned long long)(sid ^ (1ll << 63));  // signed order
           if (id < best) { best = id; bj = j; }
         }
       unsigned long long wbest = best;
@@ -194,6 +203,18 @@ __device__ __noinline__ int compact_row(const FipParams& P, uint2* list, int cnt
   return P.k;
 }
 
+// __noinline__: the epilogue's per-tile loop has to stay inside the instruction cache.  With this routine inlined (and
+// the column loop unrolled) the loop body streamed ~100 KB of code per tile and ran at IPC 0.03.
+template <int EPL>
+__device__ __noinline__ int compact_row(const FipParams& P, uint2* list, int cnt, int lane, uint32_t* kth_key) {
+  return compact_row_impl<EPL, false>(P, nullptr, list, cnt, lane, kth_key);
+}
+template <int EPL>
+__device__ __noinline__ int compact_row_gather(const FipParams& P, const int64_t* row_index, uint2* list, int cnt,
+                                               int lane, uint32_t* kth_key) {
+  return compact_row_impl<EPL, true>(P, row_index, list, cnt, lane, kth_key);
+}
+
 // CL = thread-block cluster size.  The CL CTAs of a cluster work on CL consecutive query blocks against the SAME passage
 // tiles: each CTA fetches 1/CL of every passage tile and multicasts it to the whole cluster, so the L2 -> SM traffic per
 // CTA drops from 32 KB to (16 + 16 / CL) KB per k-block.  A stage may be refilled only when EVERY CTA of the cluster has
@@ -215,10 +236,16 @@ __device__ __forceinline__ void wgmma_n128<__nv_bfloat16>(float (&d)[64], uint64
 // and publishes into its (query, probe) slot; tau_glob stays per query, since the k-th best score a query has in any of
 // its lists bounds all of them.  Runs with CL = 1.  The mode only changes where an item's rows and tiles come from, so it
 // is a template flag: with IVF = false every branch below folds away.
-template <typename T, int CL, int EPL = 32, bool IVF = false>
-__global__ void __launch_bounds__(kThreads, 1)
-flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_p, FipParams P,
-                  IvfParams V) {
+//
+// GATHER = true (IVF mode, flat_ip_tc_gather_kernel): list position p is store row G.row_index[p], so the passage tile
+// of an item is a gather that TMA cannot do.  The producer warp fills each stage's passage half with 16-byte cp.async
+// copies in the SWIZZLE_128B layout TMA would write (rows past the list end zero-filled) and signals them on the stage's
+// `full` barrier with one cp.async arrival per lane; the query half stays TMA.  List entries keep list positions, ids
+// are P.ids[row_index[position]].  The consumers fence the async proxy before their wgmma reads the cp.async data.
+template <typename T, int CL, int EPL, bool IVF, bool GATHER>
+__device__ __forceinline__ void flat_ip_tc_body(const CUtensorMap& tmap_q, const CUtensorMap* tmap_p,
+                                                FipParams P, IvfParams V, GatherParams G) {
+  static_assert(!GATHER || (IVF && CL == 1), "the gather mode is a variant of the IVF scan");
   extern __shared__ uint8_t smem_raw[];
   // 1024-B alignment for SWIZZLE_128B tiles, derived by pointer arithmetic on the __shared__ array so the
   // compiler keeps the shared address space (LDS/STS instead of generic LD/ST)
@@ -234,10 +261,12 @@ flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
   const int cluster_id = blockIdx.x / CL, n_clusters = gridDim.x / CL;
   constexpr uint16_t kAllCtas = (uint16_t)((1u << CL) - 1u);
 
+  int64_t* tile_rows = reinterpret_cast<int64_t*>(S + 1);   // GATHER: [BN] store rows of the producer's current tile
   if (threadIdx.x == 0) {
     prefetch_tensormap(&tmap_q);
-    prefetch_tensormap(&tmap_p);
-    for (int s = 0; s < kStages; ++s) { mbar_init(&S->full[s], 1); mbar_init(&S->empty[s], 8 * CL); }
+    if constexpr (!GATHER) prefetch_tensormap(tmap_p);
+    // GATHER: the producer's expect_tx arrival + one cp.async arrival per lane
+    for (int s = 0; s < kStages; ++s) { mbar_init(&S->full[s], GATHER ? 33 : 1); mbar_init(&S->empty[s], 8 * CL); }
     fence_barrier_init();
   }
   if (CL > 1) cluster_sync_all(); else __syncthreads();   // peers signal our barriers: their init must be visible cluster-wide
@@ -252,11 +281,13 @@ flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
     uint32_t phase = 0;
     for (int item = cluster_id; item < n_items; item += n_clusters) {
       int t0, t1, qrow0, prow0 = 0;
+      int64_t prow_end = 0;
       if constexpr (IVF) {
         const int4 it = V.items[item];
         prow0 = (int)V.offsets[it.x];
+        prow_end = V.offsets[it.x + 1];
         t0 = 0;
-        t1 = (int)((V.offsets[it.x + 1] - prow0 + BN - 1) / BN);
+        t1 = (int)((prow_end - prow0 + BN - 1) / BN);
         qrow0 = it.y;
       } else {
         const int rg = item / n_qgroups, qb = (item % n_qgroups) * CL + rank;  // range-major: co-running CTAs share passages
@@ -265,18 +296,44 @@ flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
         qrow0 = qb * BM;
       }
       for (int t = t0; t < t1; ++t) {
+        if constexpr (GATHER) {   // the tile's store rows, -1 past the list end (the previous tile's copies are issued)
+          __syncwarp();
+#pragma unroll
+          for (int j = 0; j < BN / 32; ++j) {
+            const int64_t p = prow0 + (int64_t)t * BN + lane + 32 * j;
+            tile_rows[lane + 32 * j] = p < prow_end ? G.row_index[p] : -1;
+          }
+          __syncwarp();
+        }
         for (int kb = 0; kb < kblocks; ++kb) {
           mbar_wait(&S->empty[stage], phase ^ 1u);
           uint8_t* st = smem + (size_t)stage * kStageBytes;
           if (elect_one_sync()) {
-            mbar_arrive_expect_tx(&S->full[stage], (uint32_t)kStageBytes);
+            mbar_arrive_expect_tx(&S->full[stage], (uint32_t)(GATHER ? kABytes : kStageBytes));
             const int kbp = kb < P.kb_wrap ? kb : kb - P.kb_wrap;   // fp32-split storage: [q_hi|q_lo|q_hi] x [p_hi|p_hi|p_lo]
             tma_load_2d(&tmap_q, st, &S->full[stage], kb * 64, qrow0, kEvictLast);
-            if (CL == 1)
-              tma_load_2d(&tmap_p, st + kABytes, &S->full[stage], kbp * 64, prow0 + t * BN, kEvictFirst);
-            else  // this CTA's slice of the passage tile, written into every CTA of the cluster
-              tma_load_2d_multicast(&tmap_p, st + kABytes + rank * (kBBytes / CL), &S->full[stage], kbp * 64,
-                                    t * BN + rank * (BN / CL), kAllCtas, kEvictFirst);
+            if constexpr (!GATHER) {
+              if (CL == 1)
+                tma_load_2d(tmap_p, st + kABytes, &S->full[stage], kbp * 64, prow0 + t * BN, kEvictFirst);
+              else  // this CTA's slice of the passage tile, written into every CTA of the cluster
+                tma_load_2d_multicast(tmap_p, st + kABytes + rank * (kBBytes / CL), &S->full[stage], kbp * 64,
+                                      t * BN + rank * (BN / CL), kAllCtas, kEvictFirst);
+            }
+          }
+          if constexpr (GATHER) {
+            // lane = 16-byte chunk (lane & 7) of rows lane / 8 + 4 i: eight lanes read one row's 128 bytes of the k-block
+            const int kbp = kb < P.kb_wrap ? kb : kb - P.kb_wrap;
+            const int chunk = lane & 7;
+            const uint8_t* src0 = G.rows + (size_t)kbp * 128 + chunk * 16;
+            const uint32_t dst0 = smem_u32(st + kABytes);
+#pragma unroll 8
+            for (int i = 0; i < BN / 4; ++i) {
+              const int r = (lane >> 3) + 4 * i;
+              const int64_t row = tile_rows[r];
+              const uint32_t dst = dst0 + r * 128 + ((chunk ^ (r & 7)) << 4);   // SWIZZLE_128B: chunk c of row r
+              cp_async_16_zfill(dst, row >= 0 ? src0 + row * G.row_pitch : src0, row >= 0 ? 16u : 0u);
+            }
+            cp_async_mbar_arrive_noinc(&S->full[stage]);
           }
           __syncwarp();
           if (++stage == kStages) { stage = 0; phase ^= 1u; }
@@ -351,6 +408,7 @@ flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
           int prev = -1;
           for (int kb = 0; kb < kblocks; ++kb) {
             mbar_wait(&S->full[stage], phase);
+            if constexpr (GATHER) fence_proxy_async_smem();   // cp.async wrote the passage half: generic -> async proxy
             const uint32_t a = smem_u32(smem + (size_t)stage * kStageBytes);
             wgmma_fence();
 #pragma unroll
@@ -393,7 +451,9 @@ flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
             if ((idx & 1) != half) continue;
             const int rr = __ffs(m) - 1;
             uint32_t kth;
-            const int nc = compact_row<EPL>(P, warp_lists + (size_t)rr * kCap, cnt_s[rr], lane, &kth);
+            int nc;
+            if constexpr (GATHER) nc = compact_row_gather<EPL>(P, G.row_index, warp_lists + (size_t)rr * kCap, cnt_s[rr], lane, &kth);
+            else nc = compact_row<EPL>(P, warp_lists + (size_t)rr * kCap, cnt_s[rr], lane, &kth);
             __syncwarp();
             int64_t q_rr = -1;   // IVF: the query of row rr
             if constexpr (IVF) q_rr = __shfl_sync(0xffffffffu, q, rr);
@@ -464,7 +524,9 @@ flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
       named_bar_sync(pair_bar, 64);
       for (int rr = half; rr < 32; rr += 2) {
         uint32_t kth;
-        const int nc = compact_row<EPL>(P, warp_lists + (size_t)rr * kCap, cnt_s[rr], lane, &kth);
+        int nc;
+        if constexpr (GATHER) nc = compact_row_gather<EPL>(P, G.row_index, warp_lists + (size_t)rr * kCap, cnt_s[rr], lane, &kth);
+        else nc = compact_row<EPL>(P, warp_lists + (size_t)rr * kCap, cnt_s[rr], lane, &kth);
         int64_t q_rr = -1;   // IVF: the query of row rr and its output slot
         size_t slot_rr = 0;
         if constexpr (IVF) {
@@ -481,7 +543,7 @@ flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
             if (e < nc) {
               const uint2 v = lst[e];
               cso[e] = __uint_as_float(v.x);
-              ci[e] = pos_to_id(P, v.y);
+              ci[e] = GATHER ? P.ids[G.row_index[v.y]] : pos_to_id(P, v.y);
             } else {
               cso[e] = -INFINITY;
               ci[e] = -1;
@@ -495,6 +557,21 @@ flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
   }
 
   if (CL > 1) cluster_sync_all(); else __syncthreads();   // no CTA may exit while peers still multicast into it
+}
+
+template <typename T, int CL, int EPL = 32, bool IVF = false>
+__global__ void __launch_bounds__(kThreads, 1)
+flat_ip_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_p, FipParams P,
+                  IvfParams V) {
+  flat_ip_tc_body<T, CL, EPL, IVF, false>(tmap_q, &tmap_p, P, V, GatherParams{});
+}
+
+// A kernel of its own rather than one more flag on flat_ip_tc_kernel: the flat and IVF instantiations keep their names
+// and parameter blocks, and this one takes no passage tensor map.
+template <typename T, int EPL>
+__global__ void __launch_bounds__(kThreads, 1)
+flat_ip_tc_gather_kernel(const __grid_constant__ CUtensorMap tmap_q, FipParams P, IvfParams V, GatherParams G) {
+  flat_ip_tc_body<T, 1, EPL, true, true>(tmap_q, nullptr, P, V, G);
 }
 
 
@@ -937,11 +1014,14 @@ extern "C" int64_t mmb200_ivf_workspace_bytes(int64_t nq, int32_t nprobe, int64_
   return (int64_t)ivf_layout(nq, nprobe, nlist, max_list_len, qcols, k, dev.sm_count).total;
 }
 
-extern "C" int mmb200_ivf_search(const void* queries, const void* rows, const int64_t* ids, const int64_t* list_offsets,
-                                 const int64_t* probes, float* out_scores, int64_t* out_ids, void* workspace,
-                                 int64_t workspace_bytes_given, int64_t nq, int32_t nprobe, int64_t nlist, int64_t n_rows,
-                                 int64_t max_list_len, int32_t dim, int32_t k, int32_t dtype, void* stream_) {
-  using namespace mmb;
+namespace mmb {
+namespace {
+// mmb200_ivf_search (row_index == nullptr: list position = row) and mmb200_ivf_search_gather (list position p = row
+// row_index[p] of the rows as given).
+int ivf_search_impl(const void* queries, const void* rows, const int64_t* ids, const int64_t* row_index,
+                    const int64_t* list_offsets, const int64_t* probes, float* out_scores, int64_t* out_ids, void* workspace,
+                    int64_t workspace_bytes_given, int64_t nq, int32_t nprobe, int64_t nlist, int64_t n_rows,
+                    int64_t max_list_len, int32_t dim, int32_t k, int32_t dtype, void* stream_) {
   MMB_REQUIRE(queries && rows && ids && list_offsets && probes && out_scores && out_ids && workspace, "null pointer");
   MMB_REQUIRE(nq > 0 && nlist > 0 && n_rows > 0, "need at least one query, one list and one row");
   MMB_REQUIRE(k >= 1 && k <= kMaxK, "fused top-k supports 1 <= k <= 1024");
@@ -985,6 +1065,7 @@ extern "C" int mmb200_ivf_search(const void* queries, const void* rows, const in
   MMB_CHECK_CUDA(cudaGetLastError());
 
   const CUtensorMapDataType tdt = dtype == MMB200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  const bool gather = row_index != nullptr;
   CUtensorMap tq, tp;
   {
     const uint64_t dims[2] = {(uint64_t)qcols, (uint64_t)L.n_pairs};
@@ -994,7 +1075,7 @@ extern "C" int mmb200_ivf_search(const void* queries, const void* rows, const in
                                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B))
       return rc;
   }
-  {
+  if (!gather) {
     const uint64_t dims[2] = {(uint64_t)pcols, (uint64_t)n_rows};
     const uint64_t strides[1] = {(uint64_t)pcols * 2};
     const uint32_t box[2] = {64, BN};
@@ -1012,21 +1093,57 @@ extern "C" int mmb200_ivf_search(const void* queries, const void* rows, const in
   P.cand_scores = reinterpret_cast<float*>(w + L.cand_s);
   P.cand_ids = reinterpret_cast<int64_t*>(w + L.cand_i);
   const IvfParams V{items, n_items, list_offsets, pair_of_row, nprobe};
-  const size_t smem = (size_t)kStages * kStageBytes + (size_t)BM * kCsStride * sizeof(float) + sizeof(FipShared) + 1024;
+  // the gather mode keeps its tile's store rows behind FipShared
+  const size_t smem = (size_t)kStages * kStageBytes + (size_t)BM * kCsStride * sizeof(float) + sizeof(FipShared) + 1024 +
+                      (gather ? BN * sizeof(int64_t) : 0);
   auto launch = [&](auto kernel) -> int {
     MMB_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kernel<<<L.grid, kThreads, smem, stream>>>(tq, tp, P, V);
     MMB_CHECK_CUDA(cudaGetLastError());
     return MMB200_OK;
   };
+  const GatherParams G{static_cast<const uint8_t*>(rows), row_index, (int64_t)pcols * 2};
+  auto launch_gather = [&](auto kernel) -> int {
+    MMB_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<L.grid, kThreads, smem, stream>>>(tq, P, V, G);
+    MMB_CHECK_CUDA(cudaGetLastError());
+    return MMB200_OK;
+  };
   int rc;
   const bool e32 = epl_for_k(k) == 32;
-  if (dtype == MMB200_BF16)
+  if (gather) {
+    if (dtype == MMB200_BF16)
+      rc = e32 ? launch_gather(flat_ip_tc_gather_kernel<__nv_bfloat16, 32>) : launch_gather(flat_ip_tc_gather_kernel<__nv_bfloat16, 64>);
+    else
+      rc = e32 ? launch_gather(flat_ip_tc_gather_kernel<__half, 32>) : launch_gather(flat_ip_tc_gather_kernel<__half, 64>);
+  } else if (dtype == MMB200_BF16) {
     rc = e32 ? launch(flat_ip_tc_kernel<__nv_bfloat16, 1, 32, true>) : launch(flat_ip_tc_kernel<__nv_bfloat16, 1, 64, true>);
-  else
+  } else {
     rc = e32 ? launch(flat_ip_tc_kernel<__half, 1, 32, true>) : launch(flat_ip_tc_kernel<__half, 1, 64, true>);
+  }
   if (rc) return rc;
   return launch_merge(P.cand_scores, P.cand_ids, nq, nprobe * L.kslot, k, out_scores, out_ids, dev, stream);
+}
+}  // namespace
+}  // namespace mmb
+
+extern "C" int mmb200_ivf_search(const void* queries, const void* rows, const int64_t* ids, const int64_t* list_offsets,
+                                 const int64_t* probes, float* out_scores, int64_t* out_ids, void* workspace,
+                                 int64_t workspace_bytes_given, int64_t nq, int32_t nprobe, int64_t nlist, int64_t n_rows,
+                                 int64_t max_list_len, int32_t dim, int32_t k, int32_t dtype, void* stream_) {
+  return mmb::ivf_search_impl(queries, rows, ids, nullptr, list_offsets, probes, out_scores, out_ids, workspace,
+                              workspace_bytes_given, nq, nprobe, nlist, n_rows, max_list_len, dim, k, dtype, stream_);
+}
+
+extern "C" int mmb200_ivf_search_gather(const void* queries, const void* rows, const int64_t* ids, const int64_t* row_index,
+                                        const int64_t* list_offsets, const int64_t* probes, float* out_scores,
+                                        int64_t* out_ids, void* workspace, int64_t workspace_bytes_given, int64_t nq,
+                                        int32_t nprobe, int64_t nlist, int64_t n_rows, int64_t max_list_len, int32_t dim,
+                                        int32_t k, int32_t dtype, void* stream_) {
+  using namespace mmb;
+  MMB_REQUIRE(row_index != nullptr, "null pointer");
+  return ivf_search_impl(queries, rows, ids, row_index, list_offsets, probes, out_scores, out_ids, workspace,
+                         workspace_bytes_given, nq, nprobe, nlist, n_rows, max_list_len, dim, k, dtype, stream_);
 }
 
 // Spherical k-means update: block l averages rows perm[offsets[l] .. offsets[l+1]) of x in that order (fp64

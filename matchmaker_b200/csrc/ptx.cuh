@@ -125,6 +125,19 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, void* smem_d
       : "memory");
 }
 
+// 16-byte cp.async (L2 only) of which the first `src_bytes` (16 or 0) are read; the rest of the 16 bytes is zero-filled.
+__device__ __forceinline__ void cp_async_16_zfill(uint32_t smem_dst, const void* gmem_src, uint32_t src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(gmem_src)),
+               "r"(src_bytes)
+               : "memory");
+}
+
+// One arrival on `bar` once every cp.async this thread issued so far has landed.  .noinc: the arrival counts against
+// the barrier's expected count, which has to include it.
+__device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint64_t* bar) {
+  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+
 // Plain bulk copy (no tensor map): `bytes` (a multiple of 16) from 16-byte aligned global memory to 16-byte aligned shared
 // memory; completion is signalled as transaction bytes on `bar`.
 __device__ __forceinline__ void bulk_load(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {

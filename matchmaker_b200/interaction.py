@@ -522,8 +522,8 @@ def ivf_query_batch(nq: int, workspace_bytes, cap: int) -> int:
 
 
 def ivf_search(queries: torch.Tensor, rows: torch.Tensor, ids: torch.Tensor, list_offsets: torch.Tensor,
-               probes: torch.Tensor, k: int, max_list_len: int,
-               split_scale: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+               probes: torch.Tensor, k: int, max_list_len: int, split_scale: Optional[int] = None,
+               row_index: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
     """Exact inner-product top-k over the union of each query's probed lists (faiss IndexIVF search semantics).
 
     rows [n, dim] fp16 / bf16, sorted by list: list l is rows ``list_offsets[l]:list_offsets[l+1]`` (int64 [nlist+1]);
@@ -531,8 +531,12 @@ def ivf_search(queries: torch.Tensor, rows: torch.Tensor, ids: torch.Tensor, lis
     max_list_len bounds every list's length.  Returns (scores [nq, k] f32, ids [nq, k] int64) under (score desc, id asc),
     with a (-3.4028235e38, -1) tail when the probed lists hold fewer than k rows.  fp32 storage: ``rows`` =
     flat_ip_split_f32(x, "passages")[0] with its scale as ``split_scale``, as for flat_ip_topk.  1 <= k <= 1024,
-    1 <= nprobe <= 1024.  Queries are searched in batches whose scratch fits IVF_WORKSPACE_CAP."""
-    dev = _require_cuda(queries, rows, ids, list_offsets, probes)
+    1 <= nprobe <= 1024.  Queries are searched in batches whose scratch fits IVF_WORKSPACE_CAP.
+
+    row_index (int64 [list_offsets[-1]], optional): the rows are NOT sorted by list; list position p is row
+    ``row_index[p]`` of ``rows``, and ``ids`` is indexed by row (mmb200_ivf_search_gather).  The result equals the call
+    without row_index over ``rows[row_index]`` with ids ``ids[row_index]``, without that copy of the rows."""
+    dev = _require_cuda(queries, rows, ids, list_offsets, probes, row_index)
     if rows.dtype not in (torch.float16, torch.bfloat16):
         raise _lib.MatchmakerB200Error("ivf_search: rows must be fp16 / bf16, or the fp16 split of fp32 (flat_ip_split_f32)")
     if probes.dim() != 2 or probes.shape[0] != queries.shape[0]:
@@ -558,6 +562,11 @@ def ivf_search(queries: torch.Tensor, rows: torch.Tensor, ids: torch.Tensor, lis
     if ids.numel() != rows.shape[0] or list_offsets.dim() != 1 or nlist < 1:
         raise _lib.MatchmakerB200Error(f"ivf_search: {ids.numel()} ids for {rows.shape[0]} rows, list_offsets "
                                        f"{tuple(list_offsets.shape)} (need [nlist + 1], nlist >= 1)")
+    if row_index is not None:
+        if row_index.dim() != 1 or row_index.numel() > rows.shape[0]:
+            raise _lib.MatchmakerB200Error(f"ivf_search: row_index must be [list_offsets[-1]] (at most one entry per row), "
+                                           f"got {tuple(row_index.shape)} for {rows.shape[0]} rows")
+        row_index = row_index.to(torch.int64).contiguous()
     rows, probes = rows.contiguous(), probes.to(torch.int64).contiguous()
     ids, list_offsets = ids.to(torch.int64).contiguous(), list_offsets.to(torch.int64).contiguous()
     out_s = torch.empty((nq, k), dtype=torch.float32, device=dev)
@@ -575,10 +584,15 @@ def ivf_search(queries: torch.Tensor, rows: torch.Tensor, ids: torch.Tensor, lis
         ws = torch.empty(wsb(b), dtype=torch.uint8, device=dev)
         for b0 in range(0, nq, b):
             b1 = min(nq, b0 + b)
-            rc = lib.mmb200_ivf_search(_ptr(queries[b0:b1]), _ptr(rows), _ptr(ids), _ptr(list_offsets), _ptr(probes[b0:b1]),
-                                       _ptr(out_s[b0:b1]), _ptr(out_i[b0:b1]), _ptr(ws), ws.numel(), b1 - b0, nprobe,
-                                       nlist, rows.shape[0], max_list_len, dim, k, dcode, _stream(dev))
-            _lib.check(rc, "mmb200_ivf_search")
+            tail = (_ptr(probes[b0:b1]), _ptr(out_s[b0:b1]), _ptr(out_i[b0:b1]), _ptr(ws), ws.numel(), b1 - b0, nprobe,
+                    nlist, rows.shape[0], max_list_len, dim, k, dcode, _stream(dev))
+            if row_index is None:
+                rc = lib.mmb200_ivf_search(_ptr(queries[b0:b1]), _ptr(rows), _ptr(ids), _ptr(list_offsets), *tail)
+                _lib.check(rc, "mmb200_ivf_search")
+            else:
+                rc = lib.mmb200_ivf_search_gather(_ptr(queries[b0:b1]), _ptr(rows), _ptr(ids), _ptr(row_index),
+                                                  _ptr(list_offsets), *tail)
+                _lib.check(rc, "mmb200_ivf_search_gather")
     if unscale is not None:
         out_s = torch.where(out_s > -3.0e38, torch.ldexp(out_s, torch.tensor(unscale, device=dev)), out_s)
     return out_s, out_i

@@ -8,3 +8,4 @@ from .graph_index import GraphIndexer  # noqa: F401
 from .scann_index import ScaNNIndexer  # noqa: F401
 from .colbert_rerank import ColBERTTokenIndex  # noqa: F401
 from .colbert_e2e import ColBERTEndToEndIndexer  # noqa: F401
+from .colbert_ivf import ColBERTIVFIndexer  # noqa: F401
