@@ -151,7 +151,8 @@ MMB200_API int mmb200_maxsim_store_fwd(const void* q, const void* store, const i
  *
  * q [B,Lq,D] f32, d [B,Ld,D] f32 (D % 4 == 0, 16-byte aligned); q_mask [B,Lq], d_mask [B,Ld] of
  * `mask_dtype` (matchmaker passes float masks: MMB200_MASK_F32); mu, sigma, weight [K] f32 device
- * arrays, alpha [K] or NULL (= 1); K <= 32.
+ * arrays, alpha [K] or NULL (= 1); K <= 32.  B == 0 is valid (the per-pair pointers may then be NULL): nothing runs,
+ * and every backward of this family sets grad_weight / grad_alpha to 0.
  * Outputs (any of per_kernel / per_kernel_query / cosine may be NULL):
  *   score [B]; per_kernel [B,K] (= P); per_kernel_query [B,Lq,K] (= S, what backward needs);
  *   cosine [B,Lq,Ld] = c_ij * q_mask[i] * d_mask[j] (the reference's secondary output).

@@ -445,8 +445,11 @@ __global__ void __launch_bounds__(256) kp_reduce_batch(const float* __restrict__
 // host
 // ---------------------------------------------------------------------------------------------
 
+// An empty batch (B == 0) is valid: its per-pair tensors are empty, so their pointers may be null (torch hands out a null
+// data pointer for an empty tensor).
 static int kp_validate(const KpParams& P) {
-  MMB_REQUIRE(P.q && P.d && P.mu && P.sigma && P.weight, "null pointer");
+  MMB_REQUIRE(P.mu && P.sigma && P.weight, "null pointer");
+  MMB_REQUIRE(P.B == 0 || (P.q && P.d), "null pointer");
   MMB_REQUIRE(P.B >= 0 && P.Lq > 0 && P.Ld > 0 && P.D > 0, "bad shape");
   MMB_REQUIRE(P.D % 4 == 0, "embedding dim must be a multiple of 4 floats (16-byte rows)");
   MMB_REQUIRE(P.K >= 1 && P.K <= 32, "1 <= K <= 32 kernels supported");
@@ -503,7 +506,7 @@ static int kp_fwd_impl(const float* q, const float* d, const void* q_mask, const
   P.B = B; P.Lq = Lq; P.Ld = Ld; P.D = D; P.K = K; P.mask_dtype = mask_dtype; P.log_scale = log_scale;
   P.score = score; P.per_kernel = per_kernel; P.per_kernel_query = per_kernel_query; P.cosine = cosine;
   if (int rc = kp_validate(P)) return rc;
-  MMB_REQUIRE(score != nullptr, "score must be non-null");
+  MMB_REQUIRE(score != nullptr || B == 0, "score must be non-null");
   if (B == 0) return MMB200_OK;
   DeviceInfo dev;
   if (int rc = require_sm90(&dev)) return rc;
@@ -543,14 +546,18 @@ static int kp_bwd_impl(const float* q, const float* d, const void* q_mask, const
   P.B = B; P.Lq = Lq; P.Ld = Ld; P.D = D; P.K = K; P.mask_dtype = mask_dtype; P.log_scale = log_scale;
   P.S = per_kernel_query; P.grad_score = grad_score; P.grad_q = grad_q; P.grad_d = grad_d;
   if (int rc = kp_validate(P)) return rc;
-  MMB_REQUIRE(per_kernel_query && grad_score && grad_q && grad_d && workspace, "null pointer");
+  MMB_REQUIRE(B == 0 || (per_kernel_query && grad_score && grad_q && grad_d && workspace), "null pointer");
   MMB_REQUIRE(D <= 512, "kernel_pool backward supports embedding dim <= 512");
   P.ws_weight = workspace;
   P.ws_alpha = workspace + B * K;
-  if (B == 0) return MMB200_OK;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (B == 0) {   // the weight and alpha gradients are sums over no pairs
+    if (grad_weight) MMB_CHECK_CUDA(cudaMemsetAsync(grad_weight, 0, (size_t)K * sizeof(float), stream));
+    if (grad_alpha) MMB_CHECK_CUDA(cudaMemsetAsync(grad_alpha, 0, (size_t)K * sizeof(float), stream));
+    return MMB200_OK;
+  }
   DeviceInfo dev;
   if (int rc = require_sm90(&dev)) return rc;
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   int rc;
   if (saved) {
     bool handled = false;
@@ -613,7 +620,7 @@ extern "C" int mmb200_kernel_pool_fwd_train(const float* q, const float* d, cons
                                             int64_t B, int32_t Lq, int32_t Ld, int32_t D, int32_t K, float log_scale,
                                             float clamp_min, float score_bias, int32_t mask_dtype, void* stream_) {
   using namespace mmb;
-  MMB_REQUIRE(saved != nullptr && per_kernel_query != nullptr, "saved and per_kernel_query must be non-null");
+  MMB_REQUIRE((saved != nullptr && per_kernel_query != nullptr) || B == 0, "saved and per_kernel_query must be non-null");
   if (!kp_train_tc_shape_ok(Lq, Ld, D, K)) {
     set_error("kernel_pool_fwd_train: shape outside the tensor-core training envelope (Lq <= 32, K <= 32, D % 4 == 0, D <= 320)");
     return MMB200_ERR_UNSUPPORTED;
@@ -630,7 +637,7 @@ extern "C" int mmb200_kernel_pool_bwd_saved(const float* q, const float* d, cons
                                             float* workspace, int64_t B, int32_t Lq, int32_t Ld, int32_t D, int32_t K,
                                             float log_scale, float clamp_min, int32_t mask_dtype, void* stream_) {
   using namespace mmb;
-  MMB_REQUIRE(saved != nullptr, "saved must be non-null");
+  MMB_REQUIRE(saved != nullptr || B == 0, "saved must be non-null");
   if (!kp_train_tc_shape_ok(Lq, Ld, D, K)) {
     set_error("kernel_pool_bwd_saved: shape outside the tensor-core training envelope (Lq <= 32, K <= 32, D % 4 == 0, D <= 320)");
     return MMB200_ERR_UNSUPPORTED;
