@@ -92,6 +92,8 @@ MMB200_API int mmb200_device_info(int device, int* sm_count, int* cc_major, int*
  * out    [n_pairs] float32
  * argmax [n_pairs, Lq] int32 or NULL: index j* of the max per query token (-1 when the query
  *        token is masked or every document position is masked) -- what backward needs.
+ * A tensor with no elements may be passed as NULL: an empty batch (n_q = n_d = n_pairs = 0) returns 0 and launches
+ * nothing.
  * ------------------------------------------------------------------------------------------ */
 MMB200_API int mmb200_maxsim_fwd(const void* q, const void* d, const void* q_mask, const void* d_mask,
                       const int32_t* pair_q, const int32_t* pair_d, const int32_t* pair_dmask,
@@ -104,7 +106,8 @@ MMB200_API int mmb200_maxsim_fwd(const void* q, const void* d, const void* q_mas
  * grad_out [n_pairs] f32; argmax from the forward; grad_q [n_q, Lq, dim] f32 and
  * grad_d [n_d, Ld, dim] f32 are OVERWRITTEN (zero-filled then accumulated).
  * Mirrors what autograd derives from colbert.py:68-75 (gradient flows only through the max
- * element; masked query tokens and fully masked documents get none). */
+ * element; masked query tokens and fully masked documents get none).  A tensor with no elements may be NULL; with
+ * n_q = n_d = 0 nothing is written. */
 MMB200_API int mmb200_maxsim_bwd(const void* q, const void* d, const float* grad_out, const int32_t* argmax,
                       float* grad_q, float* grad_d, int64_t n_q, int64_t n_d, int64_t n_pairs,
                       int32_t docs_per_query, int32_t Lq, int32_t Ld, int32_t dim, int32_t dtype,

@@ -8,7 +8,8 @@
 // over it; here one persistent kernel streams the document token matrices through shared
 // memory once and never writes the score matrix.
 //
-// Kernel `maxsim_tc_kernel` (documents on M; any Lq <= 128, dim % 64 == 0):
+// Kernel `maxsim_tc_kernel` (documents on M; Lq <= 128, dim % 64 == 0, 64 <= dim <= 1024, and the query tile must leave
+// room for two document stages: up to Lq 96 at dim 640 / 768 / 832 / 960, Lq 64 at dim 896 / 1024 on an H100; DESIGN 3.1):
 //   * one CTA per SM, persistent over a contiguous range of pairs;
 //   * warp 0 (one lane): TMA producer.  A document tile is 128 token rows x dim, fetched as
 //     [KBS k-blocks][128 rows][64 halfs] with SWIZZLE_128B by ONE 4-D cp.async.bulk.tensor
@@ -107,10 +108,12 @@ __global__ void __launch_bounds__(kSimtThreads) maxsim_simt_kernel(MaxsimParams 
           }
         }
       }
+      // rows in ascending order: the first maximal real row wins, and a real row wins an exact tie against the -1000
+      // fill of a masked row before it (the rule of the warp combine below and of the queries-on-M kernel)
 #pragma unroll
       for (int t = 0; t < kSimtMaxQPerLane; ++t) {
         const float v = ok ? acc[t] : kMaskedScore;
-        if (v > best[t]) { best[t] = v; barg[t] = ok ? j : -1; }
+        if (v > best[t] || (v == best[t] && ok && barg[t] < 0)) { best[t] = v; barg[t] = ok ? j : -1; }
       }
     }
 #pragma unroll
@@ -473,10 +476,12 @@ static int launch_simt(const MaxsimParams& P, int dtype, const DeviceInfo& dev, 
   });
 }
 
+// A tensor with no elements may come with a null pointer (torch hands one out for an empty tensor): an empty batch
+// (n_q = n_d = n_pairs = 0) is valid and launches nothing.
 int maxsim_fwd_device(const MaxsimParams& P, int dtype, int impl, cudaStream_t stream) {
-  MMB_REQUIRE(P.q && P.d && P.out, "q, d, out must be non-null");
+  MMB_REQUIRE((P.q || P.n_q == 0) && (P.d || P.n_d == 0) && (P.out || P.n_pairs == 0), "null pointer: q, d, out must be non-null");
   MMB_REQUIRE(dtype_size(dtype) != 0, "unknown dtype");
-  MMB_REQUIRE(P.n_pairs >= 0 && P.n_q > 0 && P.n_d > 0, "bad counts");
+  MMB_REQUIRE(P.n_pairs >= 0 && P.n_q >= 0 && P.n_d >= 0 && (P.n_pairs == 0 || (P.n_q > 0 && P.n_d > 0)), "bad counts");
   MMB_REQUIRE(P.Lq > 0 && P.Ld > 0 && P.dim > 0, "bad shape");
   MMB_REQUIRE(P.docs_per_query >= 1, "docs_per_query must be >= 1");
   if ((P.q_mask || P.d_mask)) MMB_REQUIRE(mask_dtype_size(P.mask_dtype) != 0, "unknown mask dtype");

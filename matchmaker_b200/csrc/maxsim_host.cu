@@ -111,10 +111,14 @@ extern "C" int mmb200_maxsim_bwd(const void* q, const void* d, const float* grad
                                  int32_t docs_per_query, int32_t Lq, int32_t Ld, int32_t dim, int32_t dtype,
                                  void* stream_) {
   using namespace mmb;
-  MMB_REQUIRE(q && d && grad_out && argmax && grad_q && grad_d, "null pointer");
+  // a tensor with no elements may come with a null pointer (torch hands one out for an empty tensor)
+  MMB_REQUIRE((n_q == 0 || (q && grad_q)) && (n_d == 0 || (d && grad_d)) && (n_pairs == 0 || (grad_out && argmax)),
+              "null pointer");
   MMB_REQUIRE(dtype_size(dtype) != 0, "unknown dtype");
-  MMB_REQUIRE(docs_per_query >= 1 && n_pairs <= n_d && (n_pairs + docs_per_query - 1) / docs_per_query <= n_q,
+  MMB_REQUIRE(n_q >= 0 && n_pairs >= 0 && docs_per_query >= 1 && n_pairs <= n_d &&
+              (n_pairs + docs_per_query - 1) / docs_per_query <= n_q,
               "pair counts inconsistent");
+  if (n_q == 0 && n_d == 0) return MMB200_OK;   // empty batch: no gradient to write
   DeviceInfo dev;
   if (int rc = require_sm90(&dev)) return rc;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
