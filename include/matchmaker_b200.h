@@ -396,6 +396,43 @@ MMB200_API int mmb200_ivf_list_means(const void* x, const int64_t* perm, const i
                                      int64_t nlist, int32_t dim, int32_t dtype, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Residual token codes (ColBERT IVF retrieval over a compressed store)
+ *
+ * Row r of list l = list_ids[r] is kept as `bits` (1 or 2) bits per dimension:
+ *   code[d]  = #{i : cutoff[d][i] <= float(x[d]) - float(base[l][d])}     (fp32 arithmetic)
+ *   value[d] = fp16_rn(float(base[l][d]) + float(weight[d][code[d]]))
+ * base [nlist][dim] fp16, weight [dim][2^bits] fp16, cutoff [dim][2^bits - 1] fp32 ascending.  Dimension d is bits
+ * [bits * (d % (8 / bits)), +bits) of byte d * bits / 8 of the row; codes [n_rows][dim * bits / 8] uint8.
+ * dim % 64 == 0, 64 <= dim <= 1024; list_ids must lie in [0, nlist).  Every function decodes exactly `value`. */
+MMB200_API int mmb200_residual_encode(const void* rows, const int32_t* list_ids, const void* base, const float* cutoff,
+                                      uint8_t* codes, int64_t n_rows, int32_t dim, int32_t bits, void* stream);
+
+/* out [n_rows][dim] fp16 = the decoded rows. */
+MMB200_API int mmb200_residual_decode(const uint8_t* codes, const int32_t* list_ids, const void* base,
+                                      const void* weight, void* out, int64_t n_rows, int32_t dim, int32_t bits,
+                                      void* stream);
+
+/* mmb200_ivf_search_gather (fp16) over the decoded rows of `codes` without materialising them: list position p is
+ * code row row_index[p], which belongs to list l for every p in [list_offsets[l], list_offsets[l+1]).  The result is
+ * bit-identical to mmb200_ivf_search_gather over mmb200_residual_decode(codes); workspace as mmb200_ivf_workspace_bytes
+ * with dtype MMB200_F16. */
+MMB200_API int mmb200_ivf_search_residual(const void* queries, const uint8_t* codes, const void* base,
+                                          const void* weight, int32_t bits, const int64_t* ids,
+                                          const int64_t* row_index, const int64_t* list_offsets, const int64_t* probes,
+                                          float* out_scores, int64_t* out_ids, void* workspace,
+                                          int64_t workspace_bytes, int64_t nq, int32_t nprobe, int64_t nlist,
+                                          int64_t n_rows, int64_t max_list_len, int32_t dim, int32_t k, void* stream);
+
+/* mmb200_maxsim_store_fwd with impl MMB200_IMPL_TCGEN05_DOCM over the decoded rows of `codes` (fp16 queries
+ * [n_q, Lq, dim], 1 <= Lq <= 128), bit-identical to it over mmb200_residual_decode(codes). */
+MMB200_API int mmb200_maxsim_store_residual_fwd(const void* q, const uint8_t* codes, const int32_t* list_ids,
+                                                const void* base, const void* weight, int32_t bits,
+                                                const int64_t* doc_offsets, const int32_t* pair_q,
+                                                const int32_t* pair_d, float* out, int64_t n_q, int64_t n_rows,
+                                                int64_t n_docs, int64_t n_pairs, int32_t Lq, int32_t max_doc_len,
+                                                int32_t dim, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Graph index: detour pruning of an exact k-NN graph, and a beam search over the graph
  *
  * Replaces: FaissHNSWIndexer   matchmaker/retrieval/faiss_indices.py:76-104 (faiss IndexHNSWFlat, CPU only), with one

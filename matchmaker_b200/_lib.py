@@ -48,6 +48,12 @@ SIGNATURES = {
     "mmb200_ivf_search": (_c.c_int, [_vp] * 8 + [_i64, _i64, _i32, _i64, _i64, _i64, _i32, _i32, _i32, _vp]),
     "mmb200_ivf_search_gather": (_c.c_int, [_vp] * 9 + [_i64, _i64, _i32, _i64, _i64, _i64, _i32, _i32, _i32, _vp]),
     "mmb200_ivf_list_means": (_c.c_int, [_vp] * 4 + [_i64, _i32, _i32, _vp]),
+    "mmb200_residual_encode": (_c.c_int, [_vp] * 5 + [_i64, _i32, _i32, _vp]),
+    "mmb200_residual_decode": (_c.c_int, [_vp] * 5 + [_i64, _i32, _i32, _vp]),
+    "mmb200_ivf_search_residual": (_c.c_int, [_vp] * 4 + [_i32] + [_vp] * 7 + [_i64, _i64, _i32, _i64, _i64, _i64, _i32,
+                                                                                _i32, _vp]),
+    "mmb200_maxsim_store_residual_fwd": (_c.c_int, [_vp] * 5 + [_i32] + [_vp] * 4 + [_i64, _i64, _i64, _i64, _i32, _i32,
+                                                                                        _i32, _vp]),
     "mmb200_ah_workspace_bytes": (_i64, [_i64, _i32, _i64, _i64, _i32, _i32]),
     "mmb200_ah_search": (_c.c_int, [_vp] * 8 + [_i64, _i64, _i32, _i64, _i64, _i64, _i32, _i32, _vp]),
     "mmb200_ah_reorder": (_c.c_int, [_vp] * 6 + [_i64, _i64, _i32, _i32, _i32, _i32, _vp]),

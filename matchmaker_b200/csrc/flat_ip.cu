@@ -37,6 +37,7 @@
 #include "host_util.cuh"
 #include "ivf_items.cuh"
 #include "ptx.cuh"
+#include "residual.cuh"
 
 namespace mmb {
 
@@ -242,10 +243,18 @@ __device__ __forceinline__ void wgmma_n128<__nv_bfloat16>(float (&d)[64], uint64
 // copies in the SWIZZLE_128B layout TMA would write (rows past the list end zero-filled) and signals them on the stage's
 // `full` barrier with one cp.async arrival per lane; the query half stays TMA.  List entries keep list positions, ids
 // are P.ids[row_index[position]].  The consumers fence the async proxy before their wgmma reads the cp.async data.
-template <typename T, int CL, int EPL, bool IVF, bool GATHER>
+//
+// RB > 0 (gather mode over residual codes, flat_ip_tc_residual_kernel): the store holds RB-bit residual codes
+// (residual.cuh) and the producer is the whole warpgroup 8-11.  An item is one list, so every value of a dimension
+// depends only on its code: at the start of an item the producers build the list's table of decoded values
+// ([dim][2^RB] fp16 behind the tile's store rows) and thread p then decodes row p of every passage tile with one table
+// lookup per value, writing the same SWIZZLE_128B layout (zeros past the list end) with 16-byte shared stores.  Each
+// producer thread fences the async proxy and arrives on `full` (1 + 128 arrivals); the query half stays TMA.
+template <typename T, int CL, int EPL, bool IVF, bool GATHER, int RB = 0>
 __device__ __forceinline__ void flat_ip_tc_body(const CUtensorMap& tmap_q, const CUtensorMap* tmap_p,
-                                                FipParams P, IvfParams V, GatherParams G) {
+                                                FipParams P, IvfParams V, GatherParams G, ResidualCodes R = {}) {
   static_assert(!GATHER || (IVF && CL == 1), "the gather mode is a variant of the IVF scan");
+  static_assert(RB == 0 || (GATHER && (RB == 1 || RB == 2)), "residual codes are read in gather mode, 1 or 2 bits");
   extern __shared__ uint8_t smem_raw[];
   // 1024-B alignment for SWIZZLE_128B tiles, derived by pointer arithmetic on the __shared__ array so the
   // compiler keeps the shared address space (LDS/STS instead of generic LD/ST)
@@ -266,7 +275,8 @@ __device__ __forceinline__ void flat_ip_tc_body(const CUtensorMap& tmap_q, const
     prefetch_tensormap(&tmap_q);
     if constexpr (!GATHER) prefetch_tensormap(tmap_p);
     // GATHER: the producer's expect_tx arrival + one cp.async arrival per lane
-    for (int s = 0; s < kStages; ++s) { mbar_init(&S->full[s], GATHER ? 33 : 1); mbar_init(&S->empty[s], 8 * CL); }
+    // RB > 0: the expect_tx arrival + one arrival per producer thread
+    for (int s = 0; s < kStages; ++s) { mbar_init(&S->full[s], RB ? 129 : GATHER ? 33 : 1); mbar_init(&S->empty[s], 8 * CL); }
     fence_barrier_init();
   }
   if (CL > 1) cluster_sync_all(); else __syncthreads();   // peers signal our barriers: their init must be visible cluster-wide
@@ -274,7 +284,50 @@ __device__ __forceinline__ void flat_ip_tc_body(const CUtensorMap& tmap_q, const
   if (warp >= 8) {
     setmaxnreg_dec<kRegsProducer>();
   }
-  if (warp == 8) {
+  if (RB > 0 && warp >= 8) {
+    if constexpr (RB > 0) {
+      const int p = threadIdx.x - 256;   // tile row decoded by this thread
+      uint16_t* rtab = reinterpret_cast<uint16_t*>(tile_rows + BN);
+      const uint16_t* b16 = reinterpret_cast<const uint16_t*>(R.base);
+      const uint16_t* w16 = reinterpret_cast<const uint16_t*>(R.weight);
+      const int pitch = P.dim * RB / 8, ntab = P.dim << RB;
+      uint32_t fill = 0;   // stages filled so far: stage fill % kStages, phase (fill / kStages) & 1
+      for (int item = blockIdx.x; item < n_items; item += gridDim.x) {   // CL = 1: cluster_id = blockIdx.x
+        const int4 it = V.items[item];
+        const int64_t prow0 = V.offsets[it.x];
+        const int len = (int)(V.offsets[it.x + 1] - prow0);
+        const int64_t* ri = G.row_index + prow0 + p;
+        named_bar_sync(7, 128);   // every producer thread is done with the previous item's table
+        for (int e = p; e < ntab; e += 128) rtab[e] = residual_value(b16[(int64_t)it.x * P.dim + (e >> RB)], w16[e]);
+        named_bar_sync(7, 128);
+        for (int t0 = 0; t0 < len; t0 += BN) {
+          const bool live = t0 + p < len;
+          const uint8_t* crow = R.codes + (live ? ri[t0] : 0) * pitch;
+          for (int kb = 0; kb < kblocks; ++kb, ++fill) {
+            const uint32_t stage = fill % kStages, phase = (fill / kStages) & 1u;
+            uint4 words = make_uint4(0u, 0u, 0u, 0u);
+            if (live) words = residual_kblock_bits<RB>(crow, kb);   // in flight during the wait
+            mbar_wait(&S->empty[stage], phase ^ 1u);
+            uint8_t* st = smem + (size_t)stage * kStageBytes;
+            if (warp == 8 && elect_one_sync()) {
+              mbar_arrive_expect_tx(&S->full[stage], (uint32_t)kABytes);
+              tma_load_2d(&tmap_q, st, &S->full[stage], kb * 64, it.y, kEvictLast);
+            }
+            uint8_t* dst = st + kABytes + p * 128;
+            const uint16_t* tab = rtab + ((kb * 64) << RB);
+#pragma unroll
+            for (int c = 0; c < 8; ++c) {
+              const uint4 v = live ? residual_chunk_from_table<RB>(residual_chunk_bits<RB>(words, c), tab + ((8 * c) << RB))
+                                   : make_uint4(0u, 0u, 0u, 0u);
+              *reinterpret_cast<uint4*>(dst + ((c ^ (p & 7)) << 4)) = v;   // SWIZZLE_128B: chunk c of row p
+            }
+            fence_proxy_async_smem();   // generic-proxy writes -> the consumers' wgmma (async proxy)
+            mbar_arrive(&S->full[stage]);
+          }
+        }
+      }
+    }
+  } else if (warp == 8) {
     // the whole warp walks the loop (uniform control flow and operands); one elected lane issues the TMA: inside an
     // `if (lane == 0)` region the compiler wraps every TMA in an ELECT / R2UR waterfall loop (ptx.cuh)
     int stage = 0;
@@ -572,6 +625,14 @@ template <typename T, int EPL>
 __global__ void __launch_bounds__(kThreads, 1)
 flat_ip_tc_gather_kernel(const __grid_constant__ CUtensorMap tmap_q, FipParams P, IvfParams V, GatherParams G) {
   flat_ip_tc_body<T, 1, EPL, true, true>(tmap_q, nullptr, P, V, G);
+}
+
+// The gather mode over RB-bit residual codes (mmb200_ivf_search_residual): G.rows is unused, G.row_index as above.
+template <int EPL, int RB>
+__global__ void __launch_bounds__(kThreads, 1)
+flat_ip_tc_residual_kernel(const __grid_constant__ CUtensorMap tmap_q, FipParams P, IvfParams V, GatherParams G,
+                           ResidualCodes R) {
+  flat_ip_tc_body<__half, 1, EPL, true, true, RB>(tmap_q, nullptr, P, V, G, R);
 }
 
 
@@ -1016,12 +1077,13 @@ extern "C" int64_t mmb200_ivf_workspace_bytes(int64_t nq, int32_t nprobe, int64_
 
 namespace mmb {
 namespace {
-// mmb200_ivf_search (row_index == nullptr: list position = row) and mmb200_ivf_search_gather (list position p = row
-// row_index[p] of the rows as given).
+// mmb200_ivf_search (row_index == nullptr: list position = row), mmb200_ivf_search_gather (list position p = row
+// row_index[p] of the rows as given) and mmb200_ivf_search_residual (the same over residual codes R, rows = R->codes).
 int ivf_search_impl(const void* queries, const void* rows, const int64_t* ids, const int64_t* row_index,
                     const int64_t* list_offsets, const int64_t* probes, float* out_scores, int64_t* out_ids, void* workspace,
                     int64_t workspace_bytes_given, int64_t nq, int32_t nprobe, int64_t nlist, int64_t n_rows,
-                    int64_t max_list_len, int32_t dim, int32_t k, int32_t dtype, void* stream_) {
+                    int64_t max_list_len, int32_t dim, int32_t k, int32_t dtype, void* stream_,
+                    const ResidualCodes* R = nullptr) {
   MMB_REQUIRE(queries && rows && ids && list_offsets && probes && out_scores && out_ids && workspace, "null pointer");
   MMB_REQUIRE(nq > 0 && nlist > 0 && n_rows > 0, "need at least one query, one list and one row");
   MMB_REQUIRE(k >= 1 && k <= kMaxK, "fused top-k supports 1 <= k <= 1024");
@@ -1093,9 +1155,9 @@ int ivf_search_impl(const void* queries, const void* rows, const int64_t* ids, c
   P.cand_scores = reinterpret_cast<float*>(w + L.cand_s);
   P.cand_ids = reinterpret_cast<int64_t*>(w + L.cand_i);
   const IvfParams V{items, n_items, list_offsets, pair_of_row, nprobe};
-  // the gather mode keeps its tile's store rows behind FipShared
+  // the gather mode keeps its tile's store rows behind FipShared, the residual mode its list's decoded values after them
   const size_t smem = (size_t)kStages * kStageBytes + (size_t)BM * kCsStride * sizeof(float) + sizeof(FipShared) + 1024 +
-                      (gather ? BN * sizeof(int64_t) : 0);
+                      (gather ? BN * sizeof(int64_t) : 0) + (R ? ((size_t)dim << R->bits) * sizeof(__half) : 0);
   auto launch = [&](auto kernel) -> int {
     MMB_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kernel<<<L.grid, kThreads, smem, stream>>>(tq, tp, P, V);
@@ -1111,7 +1173,18 @@ int ivf_search_impl(const void* queries, const void* rows, const int64_t* ids, c
   };
   int rc;
   const bool e32 = epl_for_k(k) == 32;
-  if (gather) {
+  if (R) {
+    auto launch_residual = [&](auto kernel) -> int {
+      MMB_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      kernel<<<L.grid, kThreads, smem, stream>>>(tq, P, V, G, *R);
+      MMB_CHECK_CUDA(cudaGetLastError());
+      return MMB200_OK;
+    };
+    if (R->bits == 1)
+      rc = e32 ? launch_residual(flat_ip_tc_residual_kernel<32, 1>) : launch_residual(flat_ip_tc_residual_kernel<64, 1>);
+    else
+      rc = e32 ? launch_residual(flat_ip_tc_residual_kernel<32, 2>) : launch_residual(flat_ip_tc_residual_kernel<64, 2>);
+  } else if (gather) {
     if (dtype == MMB200_BF16)
       rc = e32 ? launch_gather(flat_ip_tc_gather_kernel<__nv_bfloat16, 32>) : launch_gather(flat_ip_tc_gather_kernel<__nv_bfloat16, 64>);
     else
@@ -1144,6 +1217,21 @@ extern "C" int mmb200_ivf_search_gather(const void* queries, const void* rows, c
   MMB_REQUIRE(row_index != nullptr, "null pointer");
   return ivf_search_impl(queries, rows, ids, row_index, list_offsets, probes, out_scores, out_ids, workspace,
                          workspace_bytes_given, nq, nprobe, nlist, n_rows, max_list_len, dim, k, dtype, stream_);
+}
+
+extern "C" int mmb200_ivf_search_residual(const void* queries, const uint8_t* codes, const void* base, const void* weight,
+                                          int32_t bits, const int64_t* ids, const int64_t* row_index,
+                                          const int64_t* list_offsets, const int64_t* probes, float* out_scores,
+                                          int64_t* out_ids, void* workspace, int64_t workspace_bytes_given, int64_t nq,
+                                          int32_t nprobe, int64_t nlist, int64_t n_rows, int64_t max_list_len,
+                                          int32_t dim, int32_t k, void* stream_) {
+  using namespace mmb;
+  MMB_REQUIRE(codes && base && weight && row_index, "null pointer");
+  MMB_REQUIRE(bits == 1 || bits == 2, "residual codes have 1 or 2 bits per dimension");
+  MMB_REQUIRE(dim >= kResidualMinDim && dim <= kResidualMaxDim, "residual codes need 64 <= dim <= 1024");
+  const ResidualCodes R{codes, static_cast<const __half*>(base), static_cast<const __half*>(weight), bits};
+  return ivf_search_impl(queries, codes, ids, row_index, list_offsets, probes, out_scores, out_ids, workspace,
+                         workspace_bytes_given, nq, nprobe, nlist, n_rows, max_list_len, dim, k, MMB200_F16, stream_, &R);
 }
 
 // Spherical k-means update: block l averages rows perm[offsets[l] .. offsets[l+1]) of x in that order (fp64

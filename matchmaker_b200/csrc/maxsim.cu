@@ -43,6 +43,7 @@
 #include "masks.cuh"
 #include "maxsim.cuh"
 #include "ptx.cuh"
+#include "residual.cuh"
 
 namespace mmb {
 
@@ -184,10 +185,17 @@ __device__ __forceinline__ void wgmma_n32<__nv_bfloat16>(float (&d)[16], uint64_
 }
 
 // NC = npad / 32 accumulator chunks of 16 registers per thread.
-template <typename T, int KBS, int NC>
-__global__ void __launch_bounds__(kTcThreads, 1)
-maxsim_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_d,
-                 MaxsimParams P, TcLaunch L) {
+//
+// RB > 0 (maxsim_tc_residual_kernel, store mode only): the store holds RB-bit residual codes (residual.cuh) with one
+// list id per row, and warps 0-3 all produce: thread p decodes row p of every document tile (its codes from HBM, its
+// list's base row from L2, the per-dimension weights from a shared-memory copy placed after TcShared) into the same
+// SWIZZLE_128B layout the TMA writes, with 16-byte shared stores.  Rows past the passage are not written (the consumers
+// exclude them).  Each producer thread fences the async proxy and arrives on `full` (128 arrivals); warp 0 still
+// fetches the query tiles by TMA.
+template <typename T, int KBS, int NC, int RB = 0>
+__device__ __forceinline__ void maxsim_tc_body(const CUtensorMap& tmap_q, const CUtensorMap* tmap_d, MaxsimParams P,
+                                               TcLaunch L, ResidualCodes R = {}, const int32_t* list_ids = nullptr) {
+  static_assert(RB == 0 || RB == 1 || RB == 2, "residual codes have 1 or 2 bits");
   extern __shared__ uint8_t smem_raw[];
   // 1024-B alignment for SWIZZLE_128B tiles, derived by pointer arithmetic on the __shared__ array so the
   // compiler keeps the shared address space (LDS/STS instead of generic LD/ST)
@@ -205,8 +213,8 @@ maxsim_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
 
   if (threadIdx.x == 0) {
     prefetch_tensormap(&tmap_q);
-    prefetch_tensormap(&tmap_d);
-    for (int s = 0; s < L.stages; ++s) { mbar_init(&S->full[s], 1); mbar_init(&S->empty[s], 8); }
+    if constexpr (RB == 0) prefetch_tensormap(tmap_d);
+    for (int s = 0; s < L.stages; ++s) { mbar_init(&S->full[s], RB ? 128 : 1); mbar_init(&S->empty[s], 8); }
     for (int s = 0; s < kQSlots; ++s) { mbar_init(&S->qfull[s], 1); mbar_init(&S->qempty[s], 8); }
     fence_barrier_init();
   }
@@ -214,7 +222,62 @@ maxsim_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
 
   const int ksteps = L.kblocks / KBS;
 
-  if (warp == 0) {
+  if (RB > 0 && warp < 4) {
+    if constexpr (RB > 0) {
+      const int p = threadIdx.x;   // tile row decoded by this thread
+      const int dim = P.dim, pitch = dim * RB / 8;
+      uint16_t* wtab = reinterpret_cast<uint16_t*>(S + 1);   // [dim][2^RB] weights
+      const uint16_t* w16 = reinterpret_cast<const uint16_t*>(R.weight);
+      for (int e = p; e < (dim << RB); e += 128) wtab[e] = w16[e];
+      named_bar_sync(2, 128);
+      int stage = 0;
+      uint32_t phase = 0;
+      int64_t prev_q = -1;
+      uint32_t qcount = 0;
+      for (int64_t pp = p_begin; pp < p_end; ++pp) {
+        const int64_t qi = pair_query(P, pp), di = pair_doc(P, pp);
+        if (qi != prev_q) {
+          if (p == 0) {
+            const uint32_t slot = L.qslots == 2 ? (qcount & 1u) : 0u, use = L.qslots == 2 ? (qcount >> 1) : qcount;
+            mbar_wait(&S->qempty[slot], (use & 1u) ^ 1u);
+            mbar_arrive_expect_tx(&S->qfull[slot], (uint32_t)L.qslot_bytes);
+            tma_load_4d(&tmap_q, q_base + (size_t)slot * L.qslot_bytes, &S->qfull[slot], 0, 0, 0, (int)qi, kEvictLast);
+          }
+          ++qcount;
+          prev_q = qi;
+        }
+        int64_t row0 = 0;
+        const int nrows = store_doc_rows(P, di, &row0);
+        for (int t = 0; t < L.tiles; ++t) {
+          const bool mine = t * kTileRows + p < nrows;
+          const int64_t row = row0 + t * kTileRows + p;
+          const uint8_t* crow = R.codes + (mine ? row : 0) * pitch;
+          const uint16_t* brow = reinterpret_cast<const uint16_t*>(R.base) + (mine ? (int64_t)list_ids[row] * dim : 0);
+          for (int ks = 0; ks < ksteps; ++ks) {
+            mbar_wait(&S->empty[stage], phase ^ 1u);
+            if (mine) {
+#pragma unroll
+              for (int kb = 0; kb < KBS; ++kb) {
+                const int kbi = ks * KBS + kb;
+                const uint4 words = residual_kblock_bits<RB>(crow, kbi);
+                uint4 b8[8];
+#pragma unroll
+                for (int c = 0; c < 8; ++c) b8[c] = __ldg(reinterpret_cast<const uint4*>(brow + kbi * 64 + 8 * c));
+                uint8_t* dst = stage_base + (size_t)stage * kStageBytes + kb * kKBlockBytes + p * 128;
+#pragma unroll
+                for (int c = 0; c < 8; ++c)
+                  *reinterpret_cast<uint4*>(dst + ((c ^ (p & 7)) << 4)) =
+                      residual_chunk<RB>(residual_chunk_bits<RB>(words, c), b8[c], wtab + ((kbi * 64 + 8 * c) << RB));
+              }
+              fence_proxy_async_smem();   // generic-proxy writes -> the consumers' wgmma (async proxy)
+            }
+            mbar_arrive(&S->full[stage]);
+            if (++stage == L.stages) { stage = 0; phase ^= 1u; }
+          }
+        }
+      }
+    }
+  } else if (warp == 0) {
     // ------------------------------- TMA producer -------------------------------
     if (lane == 0) {
       int stage = 0;
@@ -242,7 +305,7 @@ maxsim_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
             mbar_wait(&S->empty[stage], phase ^ 1u);
             if (t * kTileRows < nrows) {
               mbar_arrive_expect_tx(&S->full[stage], (uint32_t)kStageBytes);
-              tma_load_4d(&tmap_d, stage_base + (size_t)stage * kStageBytes, &S->full[stage], 0, (int)row0 + t * kTileRows,
+              tma_load_4d(tmap_d, stage_base + (size_t)stage * kStageBytes, &S->full[stage], 0, (int)row0 + t * kTileRows,
                           ks * KBS, dcoord, kEvictFirst);
             } else {
               mbar_arrive(&S->full[stage]);
@@ -374,6 +437,21 @@ maxsim_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   }
 }
 
+template <typename T, int KBS, int NC>
+__global__ void __launch_bounds__(kTcThreads, 1)
+maxsim_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_d,
+                 MaxsimParams P, TcLaunch L) {
+  maxsim_tc_body<T, KBS, NC>(tmap_q, &tmap_d, P, L);
+}
+
+// Store-mode max-sim over RB-bit residual codes (mmb200_maxsim_store_residual_fwd); row r belongs to list list_ids[r].
+template <int KBS, int NC, int RB>
+__global__ void __launch_bounds__(kTcThreads, 1)
+maxsim_tc_residual_kernel(const __grid_constant__ CUtensorMap tmap_q, MaxsimParams P, TcLaunch L, ResidualCodes R,
+                          const int32_t* list_ids) {
+  maxsim_tc_body<__half, KBS, NC, RB>(tmap_q, nullptr, P, L, R, list_ids);
+}
+
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
@@ -410,7 +488,8 @@ static int launch_tc_nc(int nc, int grid, size_t smem_bytes, cudaStream_t stream
   return MMB200_OK;
 }
 
-static int launch_tc(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cudaStream_t stream) {
+// Tile plan of the documents-on-M kernel; `extra` bytes of shared memory follow TcShared.
+static int plan_tc(const MaxsimParams& P, const DeviceInfo& dev, int extra, TcLaunch* out, size_t* smem_out) {
   TcLaunch L;
   L.npad = ((P.Lq + 31) / 32) * 32;
   L.kblocks = P.dim / 64;
@@ -422,7 +501,7 @@ static int launch_tc(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cu
   // re-fetched after the consumers release it
   int fixed = 0;
   for (L.qslots = kQSlots; L.qslots >= 1; --L.qslots) {
-    fixed = L.qslots * L.qslot_bytes + (int)sizeof(TcShared) + 1024 /* alignment slack */;
+    fixed = L.qslots * L.qslot_bytes + (int)sizeof(TcShared) + extra + 1024 /* alignment slack */;
     L.stages = std::min(kMaxStages, (dev.max_smem_optin - fixed) / stage_bytes);
     if (L.stages >= 2) break;
   }
@@ -430,18 +509,27 @@ static int launch_tc(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cu
     set_error("maxsim documents-on-M: query tile too large for shared memory");
     return MMB200_ERR_UNSUPPORTED;
   }
-  const size_t smem_bytes = (size_t)L.stages * stage_bytes + fixed;
+  *out = L;
+  *smem_out = (size_t)L.stages * stage_bytes + fixed;
+  return MMB200_OK;
+}
 
+// TMA map of the query tiles of the documents-on-M kernel: [NPAD rows][64 halfs] per k-block, all k-blocks of a query.
+static int encode_tc_query_map(CUtensorMap* tq, const MaxsimParams& P, const TcLaunch& L, CUtensorMapDataType tdt) {
+  const uint64_t dims[4] = {64, (uint64_t)P.Lq, (uint64_t)L.kblocks, (uint64_t)P.n_q};
+  const uint64_t strides[3] = {(uint64_t)P.dim * 2, 128, (uint64_t)P.Lq * P.dim * 2};
+  const uint32_t box[4] = {64, (uint32_t)L.npad, (uint32_t)L.kblocks, 1};
+  return encode_tensor_map(tq, tdt, 4, P.q, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B,
+                           CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
+}
+
+static int launch_tc(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cudaStream_t stream) {
+  TcLaunch L;
+  size_t smem_bytes;
+  if (int rc = plan_tc(P, dev, 0, &L, &smem_bytes)) return rc;
   const CUtensorMapDataType tdt = dtype == MMB200_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   CUtensorMap tq, td;
-  {
-    const uint64_t dims[4] = {64, (uint64_t)P.Lq, (uint64_t)L.kblocks, (uint64_t)P.n_q};
-    const uint64_t strides[3] = {(uint64_t)P.dim * 2, 128, (uint64_t)P.Lq * P.dim * 2};
-    const uint32_t box[4] = {64, (uint32_t)L.npad, (uint32_t)L.kblocks, 1};
-    if (int rc = encode_tensor_map(&tq, tdt, 4, P.q, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B,
-                                   CU_TENSOR_MAP_L2_PROMOTION_L2_128B))
-      return rc;
-  }
+  if (int rc = encode_tc_query_map(&tq, P, L, tdt)) return rc;
   {
     // store mode: the [n_rows, dim] store is one "document"; a passage's tile starts at its first row
     const uint64_t d_rows = P.doc_offsets ? (uint64_t)P.n_rows : (uint64_t)P.Ld;
@@ -533,4 +621,67 @@ extern "C" int mmb200_maxsim_store_fwd(const void* q, const void* store, const i
   P.n_pairs = n_pairs; P.Lq = Lq; P.Ld = max_doc_len; P.dim = dim;
   P.doc_offsets = doc_offsets; P.n_rows = n_rows;
   return mmb::maxsim_fwd_device(P, dtype, impl, static_cast<cudaStream_t>(stream));
+}
+
+namespace mmb {
+template <int KBS, int RB>
+static int launch_tc_residual_nc(int nc, int grid, size_t smem_bytes, cudaStream_t stream, const CUtensorMap& tq,
+                                 const MaxsimParams& P, const TcLaunch& L, const ResidualCodes& R,
+                                 const int32_t* list_ids) {
+#define MMB_TCR_CASE(N)                                                                                              \
+  case N:                                                                                                            \
+    MMB_CHECK_CUDA(cudaFuncSetAttribute(maxsim_tc_residual_kernel<KBS, N, RB>,                                        \
+                                        cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));              \
+    maxsim_tc_residual_kernel<KBS, N, RB><<<grid, kTcThreads, smem_bytes, stream>>>(tq, P, L, R, list_ids);          \
+    break;
+  switch (nc) {
+    MMB_TCR_CASE(1)
+    MMB_TCR_CASE(2)
+    MMB_TCR_CASE(3)
+    MMB_TCR_CASE(4)
+    default:
+      set_error("residual max-sim: query tile out of range");
+      return MMB200_ERR_INVALID;
+  }
+#undef MMB_TCR_CASE
+  MMB_CHECK_CUDA(cudaGetLastError());
+  return MMB200_OK;
+}
+}  // namespace mmb
+
+extern "C" int mmb200_maxsim_store_residual_fwd(const void* q, const uint8_t* codes, const int32_t* list_ids,
+                                                const void* base, const void* weight, int32_t bits,
+                                                const int64_t* doc_offsets, const int32_t* pair_q, const int32_t* pair_d,
+                                                float* out, int64_t n_q, int64_t n_rows, int64_t n_docs, int64_t n_pairs,
+                                                int32_t Lq, int32_t max_doc_len, int32_t dim, void* stream_) {
+  using namespace mmb;
+  MMB_REQUIRE(n_pairs >= 0 && n_q >= 0, "bad counts");
+  if (n_pairs == 0) return MMB200_OK;
+  MMB_REQUIRE(q && codes && list_ids && base && weight && doc_offsets && pair_q && pair_d && out, "null pointer");
+  MMB_REQUIRE(n_q >= 1 && n_rows >= 1 && n_docs >= 1 && max_doc_len >= 1,
+              "need a query, one stored row, one passage and max_doc_len >= 1");
+  MMB_REQUIRE(bits == 1 || bits == 2, "residual codes have 1 or 2 bits per dimension");
+  MMB_REQUIRE(dim % 64 == 0 && dim >= kResidualMinDim && dim <= kResidualMaxDim, "residual codes need dim % 64 == 0, 64 <= dim <= 1024");
+  MMB_REQUIRE(Lq >= 1 && Lq <= 128, "1 <= Lq <= 128");
+  MMB_REQUIRE(((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(codes) | reinterpret_cast<uintptr_t>(base)) & 15) == 0,
+              "16-byte alignment");
+  DeviceInfo dev;
+  if (int rc = require_sm90(&dev)) return rc;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  MaxsimParams P;
+  P.q = q; P.pair_q = pair_q; P.pair_d = pair_d; P.out = out; P.n_q = n_q; P.n_d = n_docs; P.n_pairs = n_pairs;
+  P.Lq = Lq; P.Ld = max_doc_len; P.dim = dim; P.doc_offsets = doc_offsets; P.n_rows = n_rows;
+  TcLaunch L;
+  size_t smem_bytes;
+  if (int rc = plan_tc(P, dev, (dim << bits) * (int)sizeof(__half), &L, &smem_bytes)) return rc;
+  CUtensorMap tq;
+  if (int rc = encode_tc_query_map(&tq, P, L, CU_TENSOR_MAP_DATA_TYPE_FLOAT16)) return rc;
+  const ResidualCodes R{codes, static_cast<const __half*>(base), static_cast<const __half*>(weight), bits};
+  const int grid = (int)std::min<int64_t>(dev.sm_count, n_pairs);
+  const int nc = L.npad / 32;
+  if (bits == 1)
+    return L.kbs == 2 ? launch_tc_residual_nc<2, 1>(nc, grid, smem_bytes, stream, tq, P, L, R, list_ids)
+                      : launch_tc_residual_nc<1, 1>(nc, grid, smem_bytes, stream, tq, P, L, R, list_ids);
+  return L.kbs == 2 ? launch_tc_residual_nc<2, 2>(nc, grid, smem_bytes, stream, tq, P, L, R, list_ids)
+                    : launch_tc_residual_nc<1, 2>(nc, grid, smem_bytes, stream, tq, P, L, R, list_ids);
 }

@@ -615,6 +615,163 @@ def ivf_list_means(x: torch.Tensor, perm: torch.Tensor, offsets: torch.Tensor) -
     return out
 
 
+RESIDUAL_BITS = (1, 2)
+
+
+def _residual_tables(base: torch.Tensor, weight: torch.Tensor, bits: int, dim: int, what: str):
+    if bits not in RESIDUAL_BITS:
+        raise _lib.MatchmakerB200Error(f"{what}: bits must be 1 or 2, got {bits}")
+    if dim % 64 or not 64 <= dim <= 1024:
+        raise _lib.MatchmakerB200Error(f"{what}: residual codes need dim % 64 == 0 and 64 <= dim <= 1024, got {dim}")
+    if base.dtype != torch.float16 or base.dim() != 2 or base.shape[1] != dim:
+        raise _lib.MatchmakerB200Error(f"{what}: base must be [nlist, {dim}] fp16, got {tuple(base.shape)} {base.dtype}")
+    if weight is not None and (weight.dtype != torch.float16 or tuple(weight.shape) != (dim, 1 << bits)):
+        raise _lib.MatchmakerB200Error(f"{what}: weight must be [{dim}, {1 << bits}] fp16, got {tuple(weight.shape)} "
+                                       f"{weight.dtype}")
+    return base.contiguous(), None if weight is None else weight.contiguous()
+
+
+def _residual_codes(codes: torch.Tensor, dim: int, bits: int, what: str) -> torch.Tensor:
+    if codes.dtype != torch.uint8 or codes.dim() != 2 or codes.shape[1] != dim * bits // 8:
+        raise _lib.MatchmakerB200Error(f"{what}: codes must be [n_rows, {dim * bits // 8}] uint8, got "
+                                       f"{tuple(codes.shape)} {codes.dtype}")
+    return codes.contiguous()
+
+
+def _residual_list_ids(list_ids: torch.Tensor, n_rows: int, nlist: int, what: str) -> torch.Tensor:
+    if list_ids.dim() != 1 or list_ids.numel() != n_rows:
+        raise _lib.MatchmakerB200Error(f"{what}: list_ids must be [{n_rows}], got {tuple(list_ids.shape)}")
+    list_ids = list_ids.to(torch.int32).contiguous()
+    if n_rows and not (0 <= int(list_ids.min()) and int(list_ids.max()) < nlist):
+        raise _lib.MatchmakerB200Error(f"{what}: list ids must lie in [0, {nlist})")
+    return list_ids
+
+
+def residual_encode(rows: torch.Tensor, list_ids: torch.Tensor, base: torch.Tensor, cutoff: torch.Tensor,
+                    bits: int) -> torch.Tensor:
+    """Residual codes [n, dim * bits / 8] uint8 of fp16 rows [n, dim] of lists ``list_ids`` (int [n], in [0, nlist)):
+    code[d] = #{i : cutoff[d][i] <= float(x[d]) - float(base[l][d])} in fp32, ``bits`` (1 or 2) bits per dimension,
+    dimension d in bits [bits * (d % (8 / bits)), +bits) of byte d * bits / 8.  base [nlist, dim] fp16, cutoff
+    [dim, 2^bits - 1] fp32 ascending.  dim % 64 == 0, 64 <= dim <= 1024."""
+    dev = _require_cuda(rows, list_ids, base, cutoff)
+    if rows.dtype != torch.float16 or rows.dim() != 2:
+        raise _lib.MatchmakerB200Error(f"residual_encode: rows must be [n, dim] fp16, got {tuple(rows.shape)} {rows.dtype}")
+    n, dim = rows.shape
+    base, _ = _residual_tables(base, None, bits, dim, "residual_encode")
+    if cutoff.dtype != torch.float32 or tuple(cutoff.shape) != (dim, (1 << bits) - 1):
+        raise _lib.MatchmakerB200Error(f"residual_encode: cutoff must be [{dim}, {(1 << bits) - 1}] fp32")
+    list_ids = _residual_list_ids(list_ids, n, base.shape[0], "residual_encode")
+    rows, cutoff = rows.contiguous(), cutoff.contiguous()
+    out = torch.empty((n, dim * bits // 8), dtype=torch.uint8, device=dev)
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        rc = lib.mmb200_residual_encode(_ptr(rows), _ptr(list_ids), _ptr(base), _ptr(cutoff), _ptr(out), n, dim, bits,
+                                        _stream(dev))
+    _lib.check(rc, "mmb200_residual_encode")
+    return out
+
+
+def residual_decode(codes: torch.Tensor, list_ids: torch.Tensor, base: torch.Tensor, weight: torch.Tensor,
+                    bits: int) -> torch.Tensor:
+    """fp16 rows [n, dim] of residual codes (:func:`residual_encode`): value[d] = fp16_rn(float(base[l][d]) +
+    float(weight[d][code[d]])), weight [dim, 2^bits] fp16."""
+    dev = _require_cuda(codes, list_ids, base, weight)
+    dim = base.shape[1] if base.dim() == 2 else -1
+    base, weight = _residual_tables(base, weight, bits, dim, "residual_decode")
+    codes = _residual_codes(codes, dim, bits, "residual_decode")
+    n = codes.shape[0]
+    list_ids = _residual_list_ids(list_ids, n, base.shape[0], "residual_decode")
+    out = torch.empty((n, dim), dtype=torch.float16, device=dev)
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        rc = lib.mmb200_residual_decode(_ptr(codes), _ptr(list_ids), _ptr(base), _ptr(weight), _ptr(out), n, dim, bits,
+                                        _stream(dev))
+    _lib.check(rc, "mmb200_residual_decode")
+    return out
+
+
+def ivf_search_residual(queries: torch.Tensor, codes: torch.Tensor, base: torch.Tensor, weight: torch.Tensor,
+                        bits: int, ids: torch.Tensor, row_index: torch.Tensor, list_offsets: torch.Tensor,
+                        probes: torch.Tensor, k: int, max_list_len: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """:func:`ivf_search` with ``row_index`` over residual codes instead of fp16 rows: list position p is code row
+    ``row_index[p]``, which must belong to the list whose positions hold p.  Bit-identical to
+    ``ivf_search(queries, residual_decode(codes, ...), ids, list_offsets, probes, k, max_list_len, row_index=row_index)``
+    without materialising the decoded rows.  queries [nq, dim] (cast to fp16)."""
+    dev = _require_cuda(queries, codes, base, weight, ids, row_index, list_offsets, probes)
+    dim = base.shape[1] if base.dim() == 2 else -1
+    base, weight = _residual_tables(base, weight, bits, dim, "ivf_search_residual")
+    codes = _residual_codes(codes, dim, bits, "ivf_search_residual")
+    nlist = list_offsets.numel() - 1
+    if queries.dim() != 2 or queries.shape[1] != dim:
+        raise _lib.MatchmakerB200Error(f"ivf_search_residual: queries must be [nq, {dim}], got {tuple(queries.shape)}")
+    if probes.dim() != 2 or probes.shape[0] != queries.shape[0]:
+        raise _lib.MatchmakerB200Error(f"ivf_search_residual: probes must be [nq, nprobe], got {tuple(probes.shape)}")
+    if ids.numel() != codes.shape[0] or list_offsets.dim() != 1 or nlist != base.shape[0]:
+        raise _lib.MatchmakerB200Error(f"ivf_search_residual: {ids.numel()} ids for {codes.shape[0]} rows, "
+                                       f"list_offsets {tuple(list_offsets.shape)} for {base.shape[0]} bases")
+    if row_index.dim() != 1 or row_index.numel() > codes.shape[0]:
+        raise _lib.MatchmakerB200Error(f"ivf_search_residual: row_index must be [list_offsets[-1]], got "
+                                       f"{tuple(row_index.shape)} for {codes.shape[0]} rows")
+    nq, nprobe = probes.shape
+    queries = queries.to(torch.float16).contiguous()
+    probes, ids = probes.to(torch.int64).contiguous(), ids.to(torch.int64).contiguous()
+    row_index, list_offsets = row_index.to(torch.int64).contiguous(), list_offsets.to(torch.int64).contiguous()
+    out_s = torch.empty((nq, k), dtype=torch.float32, device=dev)
+    out_i = torch.empty((nq, k), dtype=torch.int64, device=dev)
+    if nq == 0:
+        return out_s, out_i
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        def wsb(b):
+            return lib.mmb200_ivf_workspace_bytes(b, nprobe, nlist, max_list_len, dim, k, _lib.F16)
+        if wsb(1) <= 0:
+            raise _lib.MatchmakerB200Error(f"ivf_search_residual: unsupported sizes nprobe={nprobe} nlist={nlist} k={k} "
+                                           f"(1 <= k <= {FLAT_IP_MAX_K}, 1 <= nprobe <= {IVF_MAX_PROBE})")
+        b = ivf_query_batch(nq, wsb, IVF_WORKSPACE_CAP)
+        ws = torch.empty(wsb(b), dtype=torch.uint8, device=dev)
+        for b0 in range(0, nq, b):
+            b1 = min(nq, b0 + b)
+            rc = lib.mmb200_ivf_search_residual(_ptr(queries[b0:b1]), _ptr(codes), _ptr(base), _ptr(weight), bits,
+                                                _ptr(ids), _ptr(row_index), _ptr(list_offsets), _ptr(probes[b0:b1]),
+                                                _ptr(out_s[b0:b1]), _ptr(out_i[b0:b1]), _ptr(ws), ws.numel(), b1 - b0,
+                                                nprobe, nlist, codes.shape[0], max_list_len, dim, k, _stream(dev))
+            _lib.check(rc, "mmb200_ivf_search_residual")
+    return out_s, out_i
+
+
+def maxsim_store_residual(q: torch.Tensor, codes: torch.Tensor, list_ids: torch.Tensor, base: torch.Tensor,
+                          weight: torch.Tensor, bits: int, doc_offsets: torch.Tensor, pair_q: torch.Tensor,
+                          pair_d: torch.Tensor, max_doc_len: int) -> torch.Tensor:
+    """:func:`maxsim_store` over residual codes (row r of list ``list_ids[r]``), fp32 [n_pairs]: bit-identical to
+    ``maxsim_store(q, residual_decode(codes, ...), doc_offsets, pair_q, pair_d, max_doc_len, impl="tcgen05_docm")``.
+    q [n_q, Lq, dim] (cast to fp16), 1 <= Lq <= 128."""
+    dev = _require_cuda(q, codes, list_ids, base, weight, doc_offsets, pair_q, pair_d)
+    dim = base.shape[1] if base.dim() == 2 else -1
+    base, weight = _residual_tables(base, weight, bits, dim, "maxsim_store_residual")
+    codes = _residual_codes(codes, dim, bits, "maxsim_store_residual")
+    if q.dim() != 3 or q.shape[-1] != dim:
+        raise _lib.MatchmakerB200Error(f"maxsim_store_residual: q must be [n_q, Lq, {dim}], got {tuple(q.shape)}")
+    if list_ids.dim() != 1 or list_ids.numel() != codes.shape[0]:
+        raise _lib.MatchmakerB200Error("maxsim_store_residual: one list id per code row")
+    q = q.to(torch.float16).contiguous()
+    list_ids = list_ids.to(torch.int32).contiguous()
+    doc_offsets = doc_offsets.to(torch.int64).contiguous()
+    pair_q = pair_q.to(torch.int32).contiguous().view(-1)
+    pair_d = pair_d.to(torch.int32).contiguous().view(-1)
+    if pair_q.numel() != pair_d.numel():
+        raise _lib.MatchmakerB200Error("pair_q / pair_d length mismatch")
+    n_q, Lq, _ = q.shape
+    out = torch.empty(pair_q.numel(), dtype=torch.float32, device=dev)
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        rc = lib.mmb200_maxsim_store_residual_fwd(_ptr(q), _ptr(codes), _ptr(list_ids), _ptr(base), _ptr(weight), bits,
+                                                  _ptr(doc_offsets), _ptr(pair_q), _ptr(pair_d), _ptr(out), n_q,
+                                                  codes.shape[0], doc_offsets.numel() - 1, pair_q.numel(), Lq,
+                                                  int(max_doc_len), dim, _stream(dev))
+    _lib.check(rc, "mmb200_maxsim_store_residual_fwd")
+    return out
+
+
 AH_MAX_KR = 1024
 # Device scratch one ah_search call may take; it grows with nq * nprobe (one candidate slot per (query, probe)), so
 # larger query sets are searched in batches that fit.

@@ -9,3 +9,4 @@ from .scann_index import ScaNNIndexer  # noqa: F401
 from .colbert_rerank import ColBERTTokenIndex  # noqa: F401
 from .colbert_e2e import ColBERTEndToEndIndexer  # noqa: F401
 from .colbert_ivf import ColBERTIVFIndexer  # noqa: F401
+from .colbert_residual import ColBERTResidualIndexer  # noqa: F401

@@ -104,6 +104,11 @@ class IVFIndexer(BaseNNIndexer):
         """Spherical k-means: `niter` rounds of (assign every point to its argmax-inner-product centroid, replace each
         centroid by the normalised mean of its points).  Deterministic: the same data gives bit-identical centroids."""
         x, init = self._training_points(data_chunks)
+        return self.train_points(x, init, niter, init_centroids)
+
+    def train_points(self, x: torch.Tensor, init: torch.Tensor, niter: int = KMEANS_ITERATIONS,
+                     init_centroids: Optional[torch.Tensor] = None):
+        """`train` on the points `_training_points` returned, for callers that use the sample again."""
         if init_centroids is None:
             c = torch.nn.functional.normalize(x[init].float(), dim=1)
         else:
