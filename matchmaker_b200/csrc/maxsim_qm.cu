@@ -12,27 +12,32 @@
 // Only live rows are streamed.  A document's live rows are [0, live) with live = 1 + its last unmasked row (Ld without a
 // mask; the passage's length in store mode); it takes max(1, ceil(live / 64)) chunks of the stage ring, and chunks past
 // them are neither fetched, multiplied nor reduced.  Rows of a chunk at or past `live` hold the caller's padding (up to
-// the next 64-row boundary) or TMA's zero fill past Ld: the mask is applied in the epilogue as an fp32 penalty per row,
-// 0 for live unmasked rows and -inf for every other row, so no such row can win the max whatever its data.  The
-// reference's -1000 fill (matchmaker/models/colbert.py:69) only matters when it IS the max; it is one more candidate
-// taken after the last chunk, value -1000 at a column past Ld (so ties go to real rows and the argmax reports -1), when
-// the document has a masked position anywhere in its Ld rows -- live < Ld, or a hole before its last live row.
+// the next 64-row boundary), TMA's zero fill past Ld, or (a document with no live row) whatever the stage held before:
+// the mask is applied in the epilogue as an fp32 penalty per row, 0 for live unmasked rows and -inf for every other row,
+// so no such row can win the max whatever its data.  The reference's -1000 fill (matchmaker/models/colbert.py:69) only
+// matters when it IS the max; it is one more candidate taken after the last chunk, value -1000 at a column past Ld (so
+// ties go to real rows and the argmax reports -1), when the document has a masked position anywhere in its Ld rows --
+// live < Ld, or a hole before its last live row.
 //
-// Nothing on a warp's per-document path waits for a global load: the per-pair indices and lengths arrive 32 pairs at a
-// time, a batch ahead (PairStream; the consumers, which only need the query, keep just a batch of pair_q), and each
-// penalty writer keeps the mask words of its next document in flight while it writes the current one.  setmaxnreg moves
+// Everything a document's chunks need from its mask is summed up in a per-document RECORD in shared memory, written by
+// scout warps up to a ring's depth of documents ahead: the live-row count, the fill flag and one bit per row (1 = live
+// and unmasked).  The producer takes the chunk count from it and the consumers take the penalty of every column from its
+// bits, so the mask loads' latency sits entirely in the scouts, which wait on nothing but a free record slot.  Nothing
+// on a warp's per-document path waits for a global load: the per-pair indices and lengths arrive 32 pairs at a time, a
+// batch ahead (PairStream; the consumers, which only need the query, keep just a batch of pair_q).  setmaxnreg moves
 // registers from the helper warpgroup to the consumers.
 //
 // Per CTA (persistent, one per SM, 384 threads = 3 warpgroups):
 //   warp 0        TMA producer: query tile (2-slot ring, re-fetched when the query changes), document chunks: one
 //                 {64, 64 rows, dim / 64} box per chunk (rows past Ld are zero-filled by TMA and cost no HBM traffic)
-//   warps 1, 2    penalty writers, warp 1 + c for consumer warpgroup c's documents: per document they count the live
-//                 rows (a ballot per 32 mask words), hand the count to the producer, and per chunk write the penalty row
-//                 and a header (last chunk of the document, -1000 candidate)
+//   warps 1-3     mask scouts: scout s takes the CTA's documents s, s + 3, ...; per document it ballots the mask words
+//                 of its rows (keeping its next two documents' words in flight) and fills the document's record
 //   warpgroups 1, 2  consumers: warpgroup c takes the CTA's documents c, c + 2, ...; per chunk 4 * dim / 64 wgmma
 //                 m64n64k16 into registers, then the masked max over the chunk's 64 columns, and the stage goes back at
-//                 once.  While one warpgroup reduces, the other one's MMAs run.  Each warpgroup has its own half of the stage ring, so every stage barrier has one consumer that waits
-//                 for its phases in order.
+//                 once.  While one warpgroup reduces, the other one's MMAs run.  Each warpgroup has its own half of the
+//                 stage ring, so every stage barrier has one consumer that waits for its phases in order.
+// Record slot n % records holds the CTA's document n; the slot count is a multiple of 6, so every slot has one scout
+// and one consumer warpgroup, and each of them (and the producer) passes through the slot's phases in order.
 // HBM-bound by design: per chunk one TMA box, per document one fp32 store.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -52,28 +57,29 @@ namespace {
 constexpr int kThreads = 384;
 constexpr int kChunkRows = 64;
 constexpr int kChunkKBlockBytes = kChunkRows * 128;   // one k-block of a chunk (8 KB)
-constexpr int kAuxBytes = 1024;              // per stage after the chunk: penalty row (64 fp32) + header word
 constexpr int kMaxStages = 32;               // even: half of the ring per consumer warpgroup (12 at dim 128, 24 at dim 64)
-constexpr int kLiveSlots = 8;                // live-row counts in flight from each penalty writer to the producer
-constexpr int kMaskWords = 4;                // mask ballots per writer lane: documents of up to 32 * 32 * 4 rows
-constexpr int kMaxLd = 32 * 32 * kMaskWords;
+constexpr int kMaxLd = 4096;
+constexpr int kScouts = 3;                   // warps 1..3 (one scout falls behind the documents; two or three keep up)
+constexpr int kRecordStep = 6;               // record slots come in multiples of kScouts and of the 2 consumer warpgroups
+constexpr int kMaxRecords = 48;
+constexpr int kRecordReserve = 12 * 1024;    // shared memory kept for records before the stage count is chosen
 constexpr int kQSlots = 2;
 constexpr int kQRows = 32;
 constexpr int kQBlockBytes = kQRows * 128;   // one k-block of the query tile (4 KB)
-// chunk header bits
-constexpr int kLastChunk = 1, kFill = 2;
-// setmaxnreg budgets: the helper warpgroup (producer, penalty writers) gives registers to the two consumer warpgroups,
-// whose 32-register accumulator and epilogue are the kernel's register peak.  128 x 120 + 256 x 192 = 384 x 168 (the launch).
+// record word 0: live rows | kFill; word 1 unused (keeps the bit words 8-byte aligned); words 2 + 2 ch, 3 + 2 ch: the
+// bits of chunk ch's rows [64 ch, 64 ch + 32) and [64 ch + 32, 64 ch + 64)
+constexpr uint32_t kFill = 1u << 16, kLiveMask = kFill - 1;
+// setmaxnreg budgets: the helper warpgroup (producer, scouts) gives registers to the two consumer warpgroups, whose
+// 32-register accumulator and epilogue are the kernel's register peak.  128 x 120 + 256 x 192 = 384 x 168 (the launch).
 constexpr int kRegsHelper = 120, kRegsConsumer = 192;
 
 struct QmShared {
-  uint64_t full[kMaxStages];   // 2 arrivals: TMA producer (with tx bytes) + penalty writer
+  uint64_t full[kMaxStages];   // 1 arrival: TMA producer (with tx bytes)
   uint64_t empty[kMaxStages];  // 4 arrivals: the warps of the warpgroup that owns the stage
   uint64_t qfull[kQSlots];
   uint64_t qempty[kQSlots];    // 8 arrivals: every warp of both consumer warpgroups
-  uint64_t lfull[2][kLiveSlots];    // writer c -> producer: live rows of writer c's next documents (1 arrival)
-  uint64_t lempty[2][kLiveSlots];   // producer -> writer c (1 arrival)
-  int32_t live[2][kLiveSlots];
+  uint64_t rfull[kMaxRecords];    // 1 arrival: the scout that filled the record
+  uint64_t rempty[kMaxRecords];   // 5 arrivals: the producer and the 4 warps of the consuming warpgroup
   float part[2][2];            // [consumer][pair parity]: row sum of query rows 16..31
 };
 
@@ -81,7 +87,18 @@ struct QmLaunch {
   int32_t kblocks;      // dim / 64 (1 or 2)
   int32_t stages;       // even: stages [0, stages / 2) serve warpgroup 0, the rest warpgroup 1
   int32_t chunk_bytes;  // kblocks * 8 KB
-  int32_t stage_bytes;  // chunk_bytes + kAuxBytes
+  int32_t records;      // record slots, a multiple of kRecordStep
+  int32_t rec_words;    // record stride: 2 + 2 * ceil(Ld / 64) words
+};
+
+// Slot and phase parity of one role's walk through the record ring: every step-th document from the role's first one.
+struct RecCursor {
+  int slot;
+  uint32_t phase;
+  __device__ __forceinline__ void advance(int step, int records) {
+    slot += step;
+    if (slot >= records) { slot -= records; phase ^= 1u; }
+  }
 };
 
 // Tensor maps of the query tile and of the document chunks ({64, 64 rows, kblocks, 1} boxes).
@@ -182,15 +199,6 @@ __device__ __forceinline__ void take(float v, int col, float& m, int& am) {
   }
 }
 
-// element i of a register array indexed by a warp-uniform value (unrolled selects: the array stays in registers)
-template <int N>
-__device__ __forceinline__ uint32_t pick(const uint32_t (&a)[N], int i) {
-  uint32_t v = a[0];
-#pragma unroll
-  for (int j = 1; j < N; ++j) v = i == j ? a[j] : v;
-  return v;
-}
-
 // kArgmax: the training instantiation also tracks WHICH document row won each query token's max (what backward needs,
 // matchmaker/models/colbert.py:71 through autograd).
 // kStore: store mode (P.doc_offsets != NULL) -- a template parameter so that the padded instantiations carry no
@@ -204,8 +212,9 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int qslot_bytes = L.kblocks * kQBlockBytes;
   uint8_t* q_base = smem;                                            // [kQSlots][kblocks][32 rows][128 B]
-  uint8_t* stage_base = q_base + kQSlots * qslot_bytes;              // [stages][chunk | penalty row, header]
-  QmShared* S = reinterpret_cast<QmShared*>(stage_base + (size_t)L.stages * L.stage_bytes);
+  uint8_t* stage_base = q_base + kQSlots * qslot_bytes;              // [stages][chunk]
+  uint32_t* rec_base = reinterpret_cast<uint32_t*>(stage_base + (size_t)L.stages * L.chunk_bytes);   // [records][rec_words]
+  QmShared* S = reinterpret_cast<QmShared*>(rec_base + (size_t)L.records * L.rec_words);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -216,10 +225,9 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
   if (threadIdx.x == 0) {
     prefetch_tensormap(&M.q);
     prefetch_tensormap(&M.d);
-    for (int s = 0; s < L.stages; ++s) { mbar_init(&S->full[s], 2); mbar_init(&S->empty[s], 4); }
+    for (int s = 0; s < L.stages; ++s) { mbar_init(&S->full[s], 1); mbar_init(&S->empty[s], 4); }
     for (int s = 0; s < kQSlots; ++s) { mbar_init(&S->qfull[s], 1); mbar_init(&S->qempty[s], 8); }
-    for (int c = 0; c < 2; ++c)
-      for (int s = 0; s < kLiveSlots; ++s) { mbar_init(&S->lfull[c][s], 1); mbar_init(&S->lempty[c][s], 1); }
+    for (int r = 0; r < L.records; ++r) { mbar_init(&S->rfull[r], 1); mbar_init(&S->rempty[r], 5); }
     fence_barrier_init();
   }
   __syncthreads();
@@ -234,6 +242,7 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
     int64_t seq0 = 0, seq1 = 0;   // chunks filled so far into each warpgroup's half of the ring
     int64_t prev_q = -1;
     uint32_t qcount = 0;
+    RecCursor rc{0, 0};
     for (int64_t p = p_begin; p < p_end; ++p) {
       meta.next();
       const int64_t qi = meta.q();
@@ -252,12 +261,11 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
           prev_q = qi;
         }
         const int c = (int)((p - p_begin) & 1);
-        // live rows of this document, from its penalty writer
-        const int64_t i = (p - p_begin) >> 1;
-        const int ls = (int)(i % kLiveSlots);
-        mbar_wait(&S->lfull[c][ls], (uint32_t)((i / kLiveSlots) & 1));
-        const int live = S->live[c][ls];
-        mbar_arrive(&S->lempty[c][ls]);
+        // live rows of this document, from its record (filled by its scout long before)
+        mbar_wait(&S->rfull[rc.slot], rc.phase);
+        const int live = (int)(rec_base[(size_t)rc.slot * L.rec_words] & kLiveMask);
+        mbar_arrive(&S->rempty[rc.slot]);
+        rc.advance(1, L.records);
         const int dcoord = kStore ? 0 : (int)di;
         const int nch = max(1, (live + kChunkRows - 1) / kChunkRows);
         for (int ch = 0; ch < nch; ++ch) {
@@ -265,7 +273,7 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
           const int stage = c * ring + (int)(j % ring);
           const uint32_t phase = (uint32_t)((j / ring) & 1);
           mbar_wait(&S->empty[stage], phase ^ 1u);
-          uint8_t* dst = stage_base + (size_t)stage * L.stage_bytes;
+          uint8_t* dst = stage_base + (size_t)stage * L.chunk_bytes;
           const int row = (int)row0 + ch * kChunkRows;
           if (live == 0) {
             mbar_arrive(&S->full[stage]);
@@ -279,23 +287,21 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
       }
       __syncwarp();
     }
-  } else if (warp == 1 || warp == 2) {
+  } else if (warp <= kScouts) {
     setmaxnreg_dec<kRegsHelper>();
-    // ------------------------------- penalty writers -----------------------------
-    // writer c serves consumer warpgroup c's half of the ring (pairs p_begin + c, + 2, ...), so every stage has one
-    // writer that sees its uses in order (a second writer could pass a parity wait one phase early).  Per document:
-    // ballot the mask words of its rows (lane l of the warp keeps ballot words l, l + 32, ...), count the live rows,
-    // hand the count to the producer, load the mask words of the writer's next document, then write one penalty row per
-    // chunk.  The first 256 rows' words of the next document are in flight in registers while this one is written.
+    // ------------------------------- mask scouts -----------------------------
+    // scout s fills the records of the CTA's documents s, s + kScouts, ...  Per document: ballot the mask words of its
+    // rows (lane l loads the words of rows l, l + 32, ...), which gives the row bits, the live count and the fill flag.
+    // The first 256 rows' words of the scout's next two documents are in flight in registers while one is scanned, and
+    // the only wait is for the document's record slot to come free.
     constexpr int kW = 8;                // mask words per lane prefetched: rows [0, 256) of a document
-    const int c = warp - 1;
+    const int s = warp - 1;
     const int dmt = P.d_mask ? P.mask_dtype : MMB200_MASK_NONE;
-    const int ring = L.stages >> 1;
     const int nwin = (P.Ld + 32 * kW - 1) / (32 * kW);
-    PairStream<kStore> meta(P, p_begin + c, p_end, 2, lane);
-    int64_t seq = 0;                    // chunks written into this half of the ring
-    int64_t ndoc = 0;                   // documents whose live count was handed to the producer
-    int64_t fp = p_begin + c;           // next pair whose mask words are loaded
+    const int bit_words = L.rec_words - 2;
+    PairStream<kStore> meta(P, p_begin + s, p_end, kScouts, lane);
+    RecCursor rc{s, 0};
+    int64_t fp = p_begin + s;           // next pair whose mask words are loaded
     // mask words folded to 32 bits (an int64 word's halves OR-ed: only zero / nonzero matters; fp32 keeps its bits)
     auto load_win = [&](uint32_t (&raw)[kW], int64_t dm, int w) {
 #pragma unroll
@@ -315,14 +321,14 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
         lim = kStore ? meta.rows() : P.Ld;   // store mode: the passage's length, 0 for a skipped pair
         load_win(raw, dm, 0);
       }
-      fp += 2;
+      fp += kScouts;
     };
-    // one document: scan its mask, hand its live count to the producer, prefetch the writer's next document into `raw`,
-    // write its chunks' penalty rows
+    // one document: wait for its record slot, scan its mask into the record, prefetch the scout's document after next
+    // into `raw`, hand the record over
     auto doc = [&](uint32_t (&raw)[kW], int64_t& dm, int& lim) {
-      uint32_t bits[kMaskWords];
-#pragma unroll
-      for (int i = 0; i < kMaskWords; ++i) bits[i] = 0;
+      mbar_wait(&S->rempty[rc.slot], rc.phase ^ 1u);
+      uint32_t* rec = rec_base + (size_t)rc.slot * L.rec_words;
+      int live = 0;
       bool masked = false;
       for (int w = 0; w < nwin; ++w) {
         if (w > 0) load_win(raw, dm, w);   // documents longer than 256 rows: the later words are loaded here
@@ -334,58 +340,30 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
           masked |= in_doc && !ok;
           const uint32_t b = __ballot_sync(0xffffffffu, ok);
           const int wi = w * kW + k;       // ballot word of rows [32 wi, 32 wi + 32)
-#pragma unroll
-          for (int i = 0; i < kMaskWords; ++i)
-            if (wi == 32 * i + lane) bits[i] = b;
+          if (b) live = 32 * wi + 32 - __clz(b);
+          if (lane == 0 && wi < bit_words) rec[2 + wi] = b;
         }
       }
-      int last = 0;   // 1 + last live row among this lane's words
-#pragma unroll
-      for (int i = 0; i < kMaskWords; ++i)
-        if (bits[i]) last = 32 * (32 * i + lane) + 32 - __clz(bits[i]);
-      const int live = (int)__reduce_max_sync(0xffffffffu, (unsigned)last);
       // the reference fills every masked position with -1000, including the trailing ones that are never visited
       const bool fill = !kStore && __any_sync(0xffffffffu, masked);
-      {
-        const int ls = (int)(ndoc % kLiveSlots);
-        mbar_wait(&S->lempty[c][ls], (uint32_t)(((ndoc / kLiveSlots) & 1) ^ 1));
-        if (lane == 0) {
-          S->live[c][ls] = live;
-          mbar_arrive(&S->lfull[c][ls]);
-        }
-        ++ndoc;
-      }
       fetch(raw, dm, lim);
-      const int nch = max(1, (live + kChunkRows - 1) / kChunkRows);
-      for (int ch = 0; ch < nch; ++ch) {
-        const int stage = c * ring + (int)(seq % ring);
-        const uint32_t phase = (uint32_t)((seq / ring) & 1);
-        ++seq;
-        const uint32_t b0 = __shfl_sync(0xffffffffu, pick(bits, ch >> 4), (2 * ch) & 31);
-        const uint32_t b1 = __shfl_sync(0xffffffffu, pick(bits, ch >> 4), (2 * ch + 1) & 31);
-        mbar_wait(&S->empty[stage], phase ^ 1u);
-        float* pt = reinterpret_cast<float*>(stage_base + (size_t)stage * L.stage_bytes + L.chunk_bytes);
-        pt[lane] = (b0 >> lane) & 1u ? 0.f : -INFINITY;
-        pt[32 + lane] = (b1 >> lane) & 1u ? 0.f : -INFINITY;
-        if (lane == 0)
-          reinterpret_cast<int32_t*>(pt)[kChunkRows] = ch == nch - 1 ? (kLastChunk | (fill ? kFill : 0)) : 0;
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&S->full[stage]);
+      if (lane == 0) {
+        rec[0] = (uint32_t)live | (fill ? kFill : 0u);
+        mbar_arrive(&S->rfull[rc.slot]);
       }
+      rc.advance(kScouts, L.records);
     };
     uint32_t ra[kW], rb[kW];
     int64_t dma = 0, dmb = 0;
     int la = 0, lb = 0;
     fetch(ra, dma, la);
     fetch(rb, dmb, lb);
-    for (int64_t wp = p_begin + c; wp < p_end;) {
+    for (int64_t sp = p_begin + s; sp < p_end;) {
       doc(ra, dma, la);
-      if ((wp += 2) >= p_end) break;
+      if ((sp += kScouts) >= p_end) break;
       doc(rb, dmb, lb);
-      wp += 2;
+      sp += kScouts;
     }
-  } else if (warp == 3) {
-    setmaxnreg_dec<kRegsHelper>();   // idle: its registers go to the consumers
   } else {
     setmaxnreg_inc<kRegsConsumer>();
     // ------------------------------- consumers: wgmma + masked max ------------------------
@@ -399,6 +377,7 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
     int64_t prev_q = -1;
     uint32_t qcount = 0;
     int cur_slot = 0;
+    RecCursor rc{c, 0};   // records of this warpgroup's documents
     // pair_q mode: pair_q of this lane's pair in the current and the next batch of 32 pairs (one coalesced load per batch,
     // a batch ahead of use); the consumers need nothing else per pair, so they carry no PairStream (register budget)
     auto load_q = [&](int64_t n0) -> int32_t { return p_begin + n0 + lane < p_end ? P.pair_q[p_begin + n0 + lane] : 0; };
@@ -429,6 +408,11 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
         if (r0 < P.Lq) qraw0 = (qmt != MMB200_MASK_NONE) ? mask_raw(P.q_mask, qmt, qi * (int64_t)P.Lq + r0) : 1;
         if (r1 < P.Lq) qraw1 = (qmt != MMB200_MASK_NONE) ? mask_raw(P.q_mask, qmt, qi * (int64_t)P.Lq + r1) : 1;
       }
+      // this document's record: live rows, fill flag, row bits (filled by its scout long before)
+      mbar_wait(&S->rfull[rc.slot], rc.phase);
+      const uint32_t* rec = rec_base + (size_t)rc.slot * L.rec_words;
+      const uint32_t head = rec[0];
+      const int nch = max(1, (int)((head & kLiveMask) + kChunkRows - 1) / kChunkRows);
       float m0 = -INFINITY, m1 = -INFINITY;
       int a0 = -1, a1 = -1;   // row of the running maximum (first one on ties); stays -1 when nothing beats -inf
       // waits for the next chunk of this warpgroup's ring and starts its MMAs (the first K-step overwrites: scale-d = 0)
@@ -436,7 +420,7 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
         const int stage = c * ring + (int)(seq % ring);
         mbar_wait(&S->full[stage], (uint32_t)((seq / ring) & 1));
         ++seq;
-        const uint32_t daddr = smem_u32(stage_base + (size_t)stage * L.stage_bytes);
+        const uint32_t daddr = smem_u32(stage_base + (size_t)stage * L.chunk_bytes);
         wgmma_fence();
         for (int kb = 0; kb < L.kblocks; ++kb) {
 #pragma unroll
@@ -448,41 +432,43 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
         wgmma_fence_regs(acc);
         return stage;
       };
-      // masked max over a finished chunk's 64 columns (columns col0 ..), then the stage goes back to the producer
-      auto reduce = [&](float (&acc)[32], int stage, int col0) {
+      // masked max over a finished chunk's 64 columns (chunk ch: columns 64 ch ..), then the stage goes back to the
+      // producer.  The penalty of a column is 0 for a live unmasked row and -inf otherwise, ADDED to the product (not a
+      // select), so that scores and argmax are those of the full-tile kernel also for NaN / inf padding.
+      auto reduce = [&](float (&acc)[32], int stage, int ch) {
         wgmma_fence_regs(acc);
         if (wq < 2) {
-          const float* pen = reinterpret_cast<const float*>(stage_base + (size_t)stage * L.stage_bytes + L.chunk_bytes);
+          const uint2 bw = *reinterpret_cast<const uint2*>(rec + 2 + 2 * ch);
+          const uint32_t b0 = bw.x >> cq, b1 = bw.y >> cq;
+          const int col0 = ch * kChunkRows;
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
             const int col = 8 * j + cq;
-            const float2 pv = *reinterpret_cast<const float2*>(pen + col);
-            take<kArgmax>(acc[4 * j + 0] + pv.x, col0 + col, m0, a0);
-            take<kArgmax>(acc[4 * j + 1] + pv.y, col0 + col + 1, m0, a0);
-            take<kArgmax>(acc[4 * j + 2] + pv.x, col0 + col, m1, a1);
-            take<kArgmax>(acc[4 * j + 3] + pv.y, col0 + col + 1, m1, a1);
+            const uint32_t b = (j < 4 ? b0 : b1) >> (8 * (j & 3));
+            const float px = (b & 1u) ? 0.f : -INFINITY, py = (b & 2u) ? 0.f : -INFINITY;
+            take<kArgmax>(acc[4 * j + 0] + px, col0 + col, m0, a0);
+            take<kArgmax>(acc[4 * j + 1] + py, col0 + col + 1, m0, a0);
+            take<kArgmax>(acc[4 * j + 2] + px, col0 + col, m1, a1);
+            take<kArgmax>(acc[4 * j + 3] + py, col0 + col + 1, m1, a1);
           }
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(&S->empty[stage]);
       };
-      auto header = [&](int stage) {
-        return *reinterpret_cast<const volatile int32_t*>(stage_base + (size_t)stage * L.stage_bytes + L.chunk_bytes +
-                                                          kChunkRows * 4);
-      };
       // one chunk at a time: its stage goes back to the producer as soon as it is reduced, and the other warpgroup's
       // MMAs fill the tensor cores meanwhile
       float acc[32];
-      int hdr = 0;
-      for (int col0 = 0; !(hdr & kLastChunk); col0 += kChunkRows) {
+      for (int ch = 0; ch < nch; ++ch) {
         const int st = issue(acc);
-        hdr = header(st);
         wgmma_wait<0>();
-        reduce(acc, st, col0);
+        reduce(acc, st, ch);
       }
+      // the record goes back (every read of it is above)
+      if (lane == 0) mbar_arrive(&S->rempty[rc.slot]);
+      rc.advance(2, L.records);
       if (wq < 2) {
         // the reference's -1000 fill, after every real row (ties keep the real row); column Ld reports -1 below
-        if (hdr & kFill) {
+        if (head & kFill) {
           take<kArgmax>(-1000.f, P.Ld, m0, a0);
           take<kArgmax>(-1000.f, P.Ld, m1, a1);
         }
@@ -542,12 +528,16 @@ int maxsim_qm_launch(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cu
   QmLaunch L;
   L.kblocks = P.dim / 64;
   L.chunk_bytes = L.kblocks * kChunkKBlockBytes;
-  L.stage_bytes = L.chunk_bytes + kAuxBytes;
+  L.rec_words = 2 + 2 * ((P.Ld + kChunkRows - 1) / kChunkRows);
   const int fixed = kQSlots * L.kblocks * kQBlockBytes + (int)sizeof(QmShared) + 1024;
-  L.stages = std::min(kMaxStages, (dev.max_smem_optin - fixed) / L.stage_bytes) & ~1;
+  L.stages = std::min(kMaxStages, (dev.max_smem_optin - fixed - kRecordReserve) / L.chunk_bytes) & ~1;
+  // the records take what is left: 48 slots up to Ld 256 or so, 30 at dim 128 and Ld 4096
+  const int rec_bytes = L.rec_words * 4;
+  L.records = std::min(kMaxRecords, (dev.max_smem_optin - fixed - L.stages * L.chunk_bytes) / rec_bytes);
+  L.records -= L.records % kRecordStep;
   // at least two stages per half of the ring, so that a chunk loads while the previous one is reduced
-  if (L.stages < 4) return MMB200_OK;
-  const size_t smem_bytes = (size_t)L.stages * L.stage_bytes + fixed;
+  if (L.stages < 4 || L.records < kRecordStep) return MMB200_OK;
+  const size_t smem_bytes = (size_t)L.stages * L.chunk_bytes + (size_t)L.records * rec_bytes + fixed;
 
   const CUtensorMapDataType tdt = dtype == MMB200_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   QmMaps M;

@@ -8,6 +8,8 @@
     dense_full   impl="tcgen05" on that same mask: equal bytes, so the difference is the cost of the ragged bookkeeping
     compact      impl="tcgen05" on a copy of the documents re-laid out at Ld = --compact-ld (about the mean fetched rows),
                  masks cut to match: the same kernel over about the live bytes.  Scores differ; it is a ceiling for timing
+    compact_nomask  that copy with q_mask = d_mask = None: the same bytes with no mask loads, so the difference to
+                 `compact` is what the mask path costs
     train        impl="tcgen05" with return_argmax=True, the training instantiation
     read         a plain full read of the 2.95 GB document tensor (an fp32-accumulated sum): a rough attainable-bandwidth
                  reference, not the kernel's roof
@@ -16,7 +18,9 @@
 
 Prints one JSON line per variant and a markdown table; --out also writes the JSON.  The SM clock is sampled through NVML
 read-only queries while the timed rounds run, as in bench.py.  `live_gb_per_s` counts the document bytes a live-row fetch
-reads (each document up to its last unmasked row, rounded up to 16 rows).  --profile runs a separate torch.profiler pass
+reads (each document up to its last unmasked row, rounded up to 16 rows); `fetched_gb_per_s` the bytes the kernel
+actually fetches (max(1, ceil(live / 64)) 64-row chunks per document, rows past the padded length not counted: TMA
+zero-fills them without reading HBM).  --profile runs a separate torch.profiler pass
 afterwards (a few launches of each max-sim variant) and prints every kernel each variant launches with its device time
 and the gap between consecutive kernels of one call.
 """
@@ -77,6 +81,16 @@ def main():
     idx = torch.arange(1, bench.LD + 1, device=dev)
     live = (wl.cdm.to(torch.int64) * idx).amax(dim=1)
     live_bytes = int(((live + 15) // 16 * 16).clamp(max=bench.LD).sum().item()) * bench.DIM * 2
+
+    def fetched_bytes(dm, ld):
+        """Document bytes the kernel fetches: max(1, ceil(live / 64)) 64-row chunks per document, rows past the padded
+        length excluded (TMA zero-fills them without reading HBM); live = ld without a mask."""
+        if dm is None:
+            return wl.cd.shape[0] * ld * bench.DIM * 2
+        lv = (dm.to(torch.int64) * torch.arange(1, ld + 1, device=dev)).amax(dim=1)
+        rows = ((lv + 63) // 64).clamp(min=1) * 64
+        return int(rows.clamp(max=ld).sum().item()) * bench.DIM * 2
+
     variants = {
         "masked": lambda: interaction.maxsim(wl.cq, wl.cd, wl.cqm, wl.cdm, docs_per_query=dpq, impl="tcgen05"),
         "nomask": lambda: interaction.maxsim(wl.cq, wl.cd, None, None, docs_per_query=dpq, impl="tcgen05"),
@@ -84,6 +98,7 @@ def main():
         "ragged_full": lambda: interaction.maxsim(wl.cq, wl.cd, wl.cqm, full_dm, docs_per_query=dpq, impl="tcgen05_ragged"),
         "dense_full": lambda: interaction.maxsim(wl.cq, wl.cd, wl.cqm, full_dm, docs_per_query=dpq, impl="tcgen05"),
         "compact": lambda: interaction.maxsim(wl.cq, compact_d, wl.cqm, compact_dm, docs_per_query=dpq, impl="tcgen05"),
+        "compact_nomask": lambda: interaction.maxsim(wl.cq, compact_d, None, None, docs_per_query=dpq, impl="tcgen05"),
         "train": lambda: interaction.maxsim(wl.cq, wl.cd, wl.cqm, wl.cdm, docs_per_query=dpq, impl="tcgen05",
                                             return_argmax=True),
         "read": lambda: wl.cd.sum(dtype=torch.float32),
@@ -93,7 +108,12 @@ def main():
     # document bytes each variant reads from HBM
     var_bytes = {"masked": wl.cd.numel() * 2, "nomask": wl.cd.numel() * 2, "ragged": live_bytes,
                  "ragged_full": wl.cd.numel() * 2, "dense_full": wl.cd.numel() * 2, "compact": compact_d.numel() * 2,
-                 "train": wl.cd.numel() * 2, "read": wl.cd.numel() * 2}
+                 "compact_nomask": compact_d.numel() * 2, "train": wl.cd.numel() * 2, "read": wl.cd.numel() * 2}
+    # document bytes each max-sim variant actually fetches (the live-row chunks of its masks)
+    var_fetched = {"masked": fetched_bytes(wl.cdm, bench.LD), "nomask": fetched_bytes(None, bench.LD),
+                   "ragged": fetched_bytes(wl.cdm, bench.LD), "ragged_full": fetched_bytes(full_dm, bench.LD),
+                   "dense_full": fetched_bytes(full_dm, bench.LD), "compact": fetched_bytes(compact_dm, cl),
+                   "compact_nomask": fetched_bytes(None, cl), "train": fetched_bytes(wl.cdm, bench.LD)}
     for f in variants.values():
         for _ in range(3):
             f()
@@ -130,6 +150,8 @@ def main():
             rec["alg_gb_per_s"] = wl.alg_bytes / (med * 1e-3) / 1e9
             rec["us_per_doc_per_sm"] = med * 1e3 / (wl.pairs / torch.cuda.get_device_properties(dev).multi_processor_count)
             rec["doc_gb_per_s"] = var_bytes[name] / (med * 1e-3) / 1e9
+            rec["fetched_gb"] = var_fetched[name] / 1e9
+            rec["fetched_gb_per_s"] = var_fetched[name] / (med * 1e-3) / 1e9
             if name in ("masked", "ragged", "train"):   # bytes a live-row fetch needs, over this variant's time
                 rec["live_gb_per_s"] = live_bytes / (med * 1e-3) / 1e9
         res["variants"][name] = rec
@@ -139,14 +161,16 @@ def main():
         res["card"], res["power_limit_w"], clocks.get("sm_mhz"), clocks.get("sm_max_mhz"), bench.LD))
     print("live-row bytes %.3f GB of %.3f GB; compact copy %.3f GB (Ld %d)" % (
         live_bytes / 1e9, doc_bytes / 1e9, compact_d.numel() * 2 / 1e9, cl))
-    print("| variant | median ms | min | max | pairs/s | GB/s (algorithmic; `read`: tensor bytes) | document GB/s read |")
-    print("|---|---|---|---|---|---|---|")
+    print("| variant | median ms | min | max | pairs/s | GB/s (algorithmic; `read`: tensor bytes) | document GB/s read "
+          "| GB fetched | fetched GB/s |")
+    print("|---|---|---|---|---|---|---|---|---|")
     for name, rec in res["variants"].items():
         gbs = rec.get("alg_gb_per_s", rec.get("gb_per_s"))
         pps = "%.3g" % rec["pairs_per_s"] if "pairs_per_s" in rec else "-"
         dgb = rec.get("doc_gb_per_s", rec.get("gb_per_s"))
-        print("| %s | %.3f | %.3f | %.3f | %s | %.0f | %.0f |" % (name, rec["median_ms"], rec["min_ms"], rec["max_ms"], pps,
-                                                                gbs, dgb))
+        fgb = "%.3f | %.0f" % (rec["fetched_gb"], rec["fetched_gb_per_s"]) if "fetched_gb" in rec else "- | -"
+        print("| %s | %.3f | %.3f | %.3f | %s | %.0f | %.0f | %s |" % (name, rec["median_ms"], rec["min_ms"],
+                                                                     rec["max_ms"], pps, gbs, dgb, fgb))
     if args.profile:
         res["profile"] = profile(variants, args.profile)
     if args.out:
