@@ -9,12 +9,14 @@
 // accumulator registers plus two quad shuffles.  Rows 0..31 of Qrep are the query; rows 32..63 of the instruction read
 // whatever follows the query in shared memory and are never looked at.
 //
-// Only live rows are streamed.  A document's live rows are [0, live) with live = 1 + its last unmasked row (Ld without a
-// mask; the passage's length in store mode); it takes max(1, ceil(live / 64)) chunks of the stage ring, and chunks past
-// them are neither fetched, multiplied nor reduced.  Rows of a chunk at or past `live` hold the caller's padding (up to
-// the next 64-row boundary), TMA's zero fill past Ld, or (a document with no live row) whatever the stage held before:
-// the mask is applied in the epilogue as an fp32 penalty per row, 0 for live unmasked rows and -inf for every other row,
-// so no such row can win the max whatever its data.  The reference's -1000 fill (matchmaker/models/colbert.py:69) only
+// Only live rows are fetched.  A document's live rows are [0, live) with live = 1 + its last unmasked row (Ld without a
+// mask; the passage's length in store mode); it takes nch = max(1, ceil(live / 64)) chunks of the stage ring.  In the
+// padded layout the chunks are END-aligned: chunk ch starts at row live - 64 (nch - ch), so the first one may start
+// below row 0, where TMA zero-fills without reading HBM, and no padding row is read.  Store mode stays start-aligned
+// (below a passage's first row lie the previous passage's rows), so its last chunk holds rows past `live`.  A document
+// with no live row takes one chunk that is not fetched (the stage holds whatever it held before).  The mask is applied
+// in the reduction as an fp32 penalty per row, 0 for live unmasked rows and -inf for every other row (rows below 0
+// included), so no such row can win the max whatever its data.  The reference's -1000 fill (matchmaker/models/colbert.py:69) only
 // matters when it IS the max; it is one more candidate taken after the last chunk, value -1000 at a column past Ld (so
 // ties go to real rows and the argmax reports -1), when the document has a masked position anywhere in its Ld rows --
 // live < Ld, or a hole before its last live row.
@@ -29,7 +31,8 @@
 //
 // Per CTA (persistent, one per SM, 384 threads = 3 warpgroups):
 //   warp 0        TMA producer: query tile (2-slot ring, re-fetched when the query changes), document chunks: one
-//                 {64, 64 rows, dim / 64} box per chunk (rows past Ld are zero-filled by TMA and cost no HBM traffic)
+//                 {64, 64 rows, dim / 64} box per chunk (rows below 0 and past Ld are zero-filled by TMA and cost no
+//                 HBM traffic), issued by one elected lane of the converged warp
 //   warps 1-3     mask scouts: scout s takes the CTA's documents s, s + 3, ...; per document it ballots the mask words
 //                 of its rows (keeping its next two documents' words in flight) and fills the document's record
 //   warpgroups 1, 2  consumers: warpgroup c takes the CTA's documents c, c + 2, ...; per chunk 4 * dim / 64 wgmma
@@ -66,12 +69,30 @@ constexpr int kRecordReserve = 12 * 1024;    // shared memory kept for records b
 constexpr int kQSlots = 2;
 constexpr int kQRows = 32;
 constexpr int kQBlockBytes = kQRows * 128;   // one k-block of the query tile (4 KB)
-// record word 0: live rows | kFill; word 1 unused (keeps the bit words 8-byte aligned); words 2 + 2 ch, 3 + 2 ch: the
-// bits of chunk ch's rows [64 ch, 64 ch + 32) and [64 ch + 32, 64 ch + 64)
+// record word 0: live rows | kFill; word 1 unused (keeps the bit words 8-byte aligned); words 2, 3: zero, the bits of
+// rows [-64, 0) (an end-aligned first chunk reads them: rows below 0 are never live); words 4 + 2 k, 5 + 2 k: the bits
+// of rows [64 k, 64 k + 32) and [64 k + 32, 64 k + 64)
 constexpr uint32_t kFill = 1u << 16, kLiveMask = kFill - 1;
+constexpr int kRecBits = 4;   // first word of row 0's bits
 // setmaxnreg budgets: the helper warpgroup (producer, scouts) gives registers to the two consumer warpgroups, whose
 // 32-register accumulator and epilogue are the kernel's register peak.  128 x 120 + 256 x 192 = 384 x 168 (the launch).
 constexpr int kRegsHelper = 120, kRegsConsumer = 192;
+
+// Debugging build only (-DMMB200_ENABLE_PROF, MMB200_MAXSIM_PROF=1): clock64 cycles of each role and of each of its
+// waits, summed over the CTAs into g_qm_prof and printed by the host after the launch.  The product build compiles
+// every QM_PROF statement out.
+#ifdef MMB200_ENABLE_PROF
+enum QmProf {
+  kPrTotal, kPrQEmpty, kPrRFull, kPrEmpty, kPrTma, kPrChunks,                 // producer (warp 0, lane 0)
+  kCoTotal, kCoRFull, kCoFull, kCoMma, kCoReduce, kCoEpilogue, kCoDocs,       // consumers (lane 0 of warps 4 and 8)
+  kScTotal, kScREmpty,                                                        // scouts (lane 0 of warps 1..3)
+  kProfCount
+};
+__device__ unsigned long long g_qm_prof[kProfCount];
+#define QM_PROF(...) __VA_ARGS__
+#else
+#define QM_PROF(...)
+#endif
 
 struct QmShared {
   uint64_t full[kMaxStages];   // 1 arrival: TMA producer (with tx bytes)
@@ -88,7 +109,7 @@ struct QmLaunch {
   int32_t stages;       // even: stages [0, stages / 2) serve warpgroup 0, the rest warpgroup 1
   int32_t chunk_bytes;  // kblocks * 8 KB
   int32_t records;      // record slots, a multiple of kRecordStep
-  int32_t rec_words;    // record stride: 2 + 2 * ceil(Ld / 64) words
+  int32_t rec_words;    // record stride: 4 + 2 * ceil(Ld / 64) words
 };
 
 // Slot and phase parity of one role's walk through the record ring: every step-th document from the role's first one.
@@ -227,7 +248,12 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
     prefetch_tensormap(&M.d);
     for (int s = 0; s < L.stages; ++s) { mbar_init(&S->full[s], 1); mbar_init(&S->empty[s], 4); }
     for (int s = 0; s < kQSlots; ++s) { mbar_init(&S->qfull[s], 1); mbar_init(&S->qempty[s], 8); }
-    for (int r = 0; r < L.records; ++r) { mbar_init(&S->rfull[r], 1); mbar_init(&S->rempty[r], 5); }
+    for (int r = 0; r < L.records; ++r) {
+      mbar_init(&S->rfull[r], 1);
+      mbar_init(&S->rempty[r], 5);
+      rec_base[(size_t)r * L.rec_words + kRecBits - 2] = 0;
+      rec_base[(size_t)r * L.rec_words + kRecBits - 1] = 0;
+    }
     fence_barrier_init();
   }
   __syncthreads();
@@ -236,57 +262,78 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
   if (warp == 0) {
     setmaxnreg_dec<kRegsHelper>();
     // ------------------------------- TMA producer -------------------------------
-    // the whole warp walks the pairs (it shares out their metadata); lane 0 waits on the barriers and issues the TMA
+    // The whole warp walks the pairs (it shares out their metadata) and waits on the barriers; one elected lane
+    // arrives and issues the TMA, so every coordinate stays warp-uniform and the issue needs no per-lane loop.  Each
+    // warpgroup's half of the stage ring is walked with a running stage index and phase (no division per chunk).
     PairStream<kStore> meta(P, p_begin, p_end, 1, lane);
     const int ring = L.stages >> 1;
-    int64_t seq0 = 0, seq1 = 0;   // chunks filled so far into each warpgroup's half of the ring
+    int st_cur = 0, st_oth = 0;            // next stage inside the half of the current / the other document's warpgroup
+    uint32_t ph_cur = 0, ph_oth = 0;       // and its phase parity
     int64_t prev_q = -1;
     uint32_t qcount = 0;
     RecCursor rc{0, 0};
+    QM_PROF(unsigned long long prof[kProfCount] = {}; const long long t_start = clock64(); long long t_;)
     for (int64_t p = p_begin; p < p_end; ++p) {
       meta.next();
       const int64_t qi = meta.q();
       const int64_t di = meta.d();
       // store mode: the passage's rows start at row `row0` of the [n_rows, dim] store (tensor-map dim 3 has extent 1)
       const int64_t row0 = kStore ? meta.row0() : 0;
-      if (lane == 0) {
-        if (qi != prev_q) {
-          const uint32_t slot = qcount & 1u, use = qcount >> 1;
-          mbar_wait(&S->qempty[slot], (use & 1u) ^ 1u);
+      if (qi != prev_q) {
+        const uint32_t slot = qcount & 1u, use = qcount >> 1;
+        QM_PROF(t_ = clock64();)
+        mbar_wait(&S->qempty[slot], (use & 1u) ^ 1u);
+        QM_PROF(prof[kPrQEmpty] += clock64() - t_;)
+        if (elect_one_sync()) {
           mbar_arrive_expect_tx(&S->qfull[slot], (uint32_t)(L.kblocks * kQBlockBytes));
           for (int kb = 0; kb < L.kblocks; ++kb)
             tma_load_4d(&M.q, q_base + (size_t)slot * qslot_bytes + kb * kQBlockBytes, &S->qfull[slot], 0, 0, kb, (int)qi,
                         kEvictLast);
-          ++qcount;
-          prev_q = qi;
         }
-        const int c = (int)((p - p_begin) & 1);
-        // live rows of this document, from its record (filled by its scout long before)
-        mbar_wait(&S->rfull[rc.slot], rc.phase);
-        const int live = (int)(rec_base[(size_t)rc.slot * L.rec_words] & kLiveMask);
-        mbar_arrive(&S->rempty[rc.slot]);
-        rc.advance(1, L.records);
-        const int dcoord = kStore ? 0 : (int)di;
-        const int nch = max(1, (live + kChunkRows - 1) / kChunkRows);
-        for (int ch = 0; ch < nch; ++ch) {
-          const int64_t j = c ? seq1++ : seq0++;
-          const int stage = c * ring + (int)(j % ring);
-          const uint32_t phase = (uint32_t)((j / ring) & 1);
-          mbar_wait(&S->empty[stage], phase ^ 1u);
-          uint8_t* dst = stage_base + (size_t)stage * L.chunk_bytes;
-          const int row = (int)row0 + ch * kChunkRows;
+        __syncwarp();
+        ++qcount;
+        prev_q = qi;
+      }
+      const int c = (int)((p - p_begin) & 1);
+      // live rows of this document, from its record (filled by its scout long before)
+      QM_PROF(t_ = clock64();)
+      mbar_wait(&S->rfull[rc.slot], rc.phase);
+      QM_PROF(prof[kPrRFull] += clock64() - t_;)
+      const int live = (int)(rec_base[(size_t)rc.slot * L.rec_words] & kLiveMask);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&S->rempty[rc.slot]);
+      rc.advance(1, L.records);
+      const int dcoord = kStore ? 0 : (int)di;
+      const int nch = max(1, (live + kChunkRows - 1) / kChunkRows);
+      // padded layout: the chunks are END-aligned, chunk ch starts at row live - 64 (nch - ch), so they cover exactly
+      // [live - 64 nch, live); rows below 0 are outside the tensor map's row extent and TMA zero-fills them without
+      // reading HBM.  Store mode stays start-aligned: a negative offset there would read the previous passage's rows.
+      int row = kStore ? (int)row0 : live - kChunkRows * nch;
+      for (int ch = 0; ch < nch; ++ch, row += kChunkRows) {
+        const int stage = c * ring + st_cur;
+        QM_PROF(t_ = clock64();)
+        mbar_wait(&S->empty[stage], ph_cur ^ 1u);
+        QM_PROF(prof[kPrEmpty] += clock64() - t_; t_ = clock64(); ++prof[kPrChunks];)
+        if (elect_one_sync()) {
           if (live == 0) {
             mbar_arrive(&S->full[stage]);
           } else {
-            // one box per chunk, also for the last one: the rows it reads past the last live row (at most 63, zero
-            // fill past Ld) cost less than the extra TMA issues and handshakes of 16-row boxes
+            // one full box per chunk: the zero fill below row 0 and past Ld costs no HBM traffic, and short boxes
+            // cost more TMA issues and handshakes than they save
             mbar_arrive_expect_tx(&S->full[stage], (uint32_t)L.chunk_bytes);
-            tma_load_4d(&M.d, dst, &S->full[stage], 0, row, 0, dcoord, kEvictFirst);
+            tma_load_4d(&M.d, stage_base + (size_t)stage * L.chunk_bytes, &S->full[stage], 0, row, 0, dcoord, kEvictFirst);
           }
         }
+        __syncwarp();
+        QM_PROF(prof[kPrTma] += clock64() - t_;)
+        if (++st_cur == ring) { st_cur = 0; ph_cur ^= 1u; }
       }
-      __syncwarp();
+      // the next document belongs to the other warpgroup
+      const int st = st_cur; st_cur = st_oth; st_oth = st;
+      const uint32_t ph = ph_cur; ph_cur = ph_oth; ph_oth = ph;
     }
+    QM_PROF(prof[kPrTotal] = clock64() - t_start;
+            if (lane == 0) for (int i = kPrTotal; i <= kPrChunks; ++i) atomicAdd(&g_qm_prof[i], prof[i]);)
   } else if (warp <= kScouts) {
     setmaxnreg_dec<kRegsHelper>();
     // ------------------------------- mask scouts -----------------------------
@@ -298,7 +345,7 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
     const int s = warp - 1;
     const int dmt = P.d_mask ? P.mask_dtype : MMB200_MASK_NONE;
     const int nwin = (P.Ld + 32 * kW - 1) / (32 * kW);
-    const int bit_words = L.rec_words - 2;
+    const int bit_words = L.rec_words - kRecBits;
     PairStream<kStore> meta(P, p_begin + s, p_end, kScouts, lane);
     RecCursor rc{s, 0};
     int64_t fp = p_begin + s;           // next pair whose mask words are loaded
@@ -325,8 +372,11 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
     };
     // one document: wait for its record slot, scan its mask into the record, prefetch the scout's document after next
     // into `raw`, hand the record over
+    QM_PROF(unsigned long long prof_re = 0; const long long t_start = clock64();)
     auto doc = [&](uint32_t (&raw)[kW], int64_t& dm, int& lim) {
+      QM_PROF(const long long t_ = clock64();)
       mbar_wait(&S->rempty[rc.slot], rc.phase ^ 1u);
+      QM_PROF(prof_re += clock64() - t_;)
       uint32_t* rec = rec_base + (size_t)rc.slot * L.rec_words;
       int live = 0;
       bool masked = false;
@@ -341,7 +391,7 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
           const uint32_t b = __ballot_sync(0xffffffffu, ok);
           const int wi = w * kW + k;       // ballot word of rows [32 wi, 32 wi + 32)
           if (b) live = 32 * wi + 32 - __clz(b);
-          if (lane == 0 && wi < bit_words) rec[2 + wi] = b;
+          if (lane == 0 && wi < bit_words) rec[kRecBits + wi] = b;
         }
       }
       // the reference fills every masked position with -1000, including the trailing ones that are never visited
@@ -364,6 +414,10 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
       doc(rb, dmb, lb);
       sp += kScouts;
     }
+    QM_PROF(if (lane == 0) {
+      atomicAdd(&g_qm_prof[kScTotal], (unsigned long long)(clock64() - t_start));
+      atomicAdd(&g_qm_prof[kScREmpty], prof_re);
+    })
   } else {
     setmaxnreg_inc<kRegsConsumer>();
     // ------------------------------- consumers: wgmma + masked max ------------------------
@@ -373,7 +427,6 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
     const int cq = 2 * (lane & 3);        // this thread's first column inside an 8-column group
     const int qmt = P.q_mask ? P.mask_dtype : MMB200_MASK_NONE;
     const int ring = L.stages >> 1;
-    int64_t seq = 0;   // chunks consumed from this warpgroup's half of the ring
     int64_t prev_q = -1;
     uint32_t qcount = 0;
     int cur_slot = 0;
@@ -383,92 +436,129 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
     auto load_q = [&](int64_t n0) -> int32_t { return p_begin + n0 + lane < p_end ? P.pair_q[p_begin + n0 + lane] : 0; };
     int32_t qb_cur = 0, qb_nxt = 0;
     if (P.pair_q) { qb_cur = load_q(0); qb_nxt = load_q(32); }
-    for (int64_t n = 0; p_begin + n < p_end; ++n) {
-      const int64_t p = p_begin + n;
-      int64_t qi;
-      if (P.pair_q) {
-        if ((n & 31) == 0 && n > 0) { qb_cur = qb_nxt; qb_nxt = load_q(n + 32); }
-        qi = __shfl_sync(0xffffffffu, qb_cur, (int)(n & 31));
-      } else {
-        qi = (p + P.pair_base) / P.docs_per_query;
+    // implicit queries: (p + pair_base) / docs_per_query, divided once and then counted along
+    int64_t q_run = 0;
+    int32_t q_rem = 0;
+    if (!P.pair_q) {
+      q_run = (p_begin + P.pair_base) / P.docs_per_query;
+      q_rem = (int32_t)((p_begin + P.pair_base) - q_run * P.docs_per_query);
+    }
+    QM_PROF(unsigned long long prof[kProfCount] = {}; const long long t_start = clock64(); long long t_;)
+    // Query tiles: walks the CTA's pairs up to pair n (every warp of both warpgroups passes through every query change,
+    // so each query slot's empty barrier gets its 8 arrivals in order).  A slot goes back after every MMA of this
+    // warpgroup that read it has completed (each chunk's MMAs are waited for before it is reduced).
+    int64_t n_walk = 0;
+    auto walk_to = [&](int64_t n) {
+      for (; n_walk <= n; ++n_walk) {
+        int64_t qi;
+        if (P.pair_q) {
+          if ((n_walk & 31) == 0 && n_walk > 0) { qb_cur = qb_nxt; qb_nxt = load_q(n_walk + 32); }
+          qi = __shfl_sync(0xffffffffu, qb_cur, (int)(n_walk & 31));
+        } else {
+          qi = q_run;
+          if (++q_rem == P.docs_per_query) { q_rem = 0; ++q_run; }
+        }
+        if (qi != prev_q) {
+          if (prev_q >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&S->qempty[cur_slot]); }
+          cur_slot = (int)(qcount & 1u);
+          mbar_wait(&S->qfull[cur_slot], (qcount >> 1) & 1u);
+          ++qcount;
+          prev_q = qi;
+        }
       }
-      if (qi != prev_q) {
-        // every MMA of this warpgroup that read the old query tile has completed (wgmma_wait below)
-        if (prev_q >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&S->qempty[cur_slot]); }
-        cur_slot = (int)(qcount & 1u);
-        mbar_wait(&S->qfull[cur_slot], (qcount >> 1) & 1u);
-        ++qcount;
-        prev_q = qi;
-      }
-      if ((int)(n & 1) != c) continue;
-      const uint32_t qaddr = smem_u32(q_base + (size_t)cur_slot * qslot_bytes);
-      // query-mask words: first needed in the epilogue, after this document's MMAs (L1 hits after the query's first pair)
-      uint64_t qraw0 = 0, qraw1 = 0;
+      return prev_q;
+    };
+    // what a document's chunks and epilogue need
+    struct Doc {
+      int64_t n;              // pair p_begin + n
+      uint32_t qaddr;         // its query tile
+      uint64_t qraw0, qraw1;  // query-mask words of this thread's rows (0 for rows >= Lq)
+      int slot;               // its record slot
+      uint32_t head;          // record word 0
+      int live, nch;
+    };
+    auto begin = [&](Doc& D, int64_t n) {
+      const int64_t qi = walk_to(n);
+      D.n = n;
+      D.qaddr = smem_u32(q_base + (size_t)cur_slot * qslot_bytes);
+      // query-mask words: first needed in the epilogue (L1 hits after the query's first pair)
+      D.qraw0 = 0;
+      D.qraw1 = 0;
       if (wq < 2) {
-        if (r0 < P.Lq) qraw0 = (qmt != MMB200_MASK_NONE) ? mask_raw(P.q_mask, qmt, qi * (int64_t)P.Lq + r0) : 1;
-        if (r1 < P.Lq) qraw1 = (qmt != MMB200_MASK_NONE) ? mask_raw(P.q_mask, qmt, qi * (int64_t)P.Lq + r1) : 1;
+        if (r0 < P.Lq) D.qraw0 = (qmt != MMB200_MASK_NONE) ? mask_raw(P.q_mask, qmt, qi * (int64_t)P.Lq + r0) : 1;
+        if (r1 < P.Lq) D.qraw1 = (qmt != MMB200_MASK_NONE) ? mask_raw(P.q_mask, qmt, qi * (int64_t)P.Lq + r1) : 1;
       }
-      // this document's record: live rows, fill flag, row bits (filled by its scout long before)
+      // the document's record: live rows, fill flag, row bits (filled by its scout long before)
+      QM_PROF(t_ = clock64();)
       mbar_wait(&S->rfull[rc.slot], rc.phase);
-      const uint32_t* rec = rec_base + (size_t)rc.slot * L.rec_words;
-      const uint32_t head = rec[0];
-      const int nch = max(1, (int)((head & kLiveMask) + kChunkRows - 1) / kChunkRows);
-      float m0 = -INFINITY, m1 = -INFINITY;
-      int a0 = -1, a1 = -1;   // row of the running maximum (first one on ties); stays -1 when nothing beats -inf
-      // waits for the next chunk of this warpgroup's ring and starts its MMAs (the first K-step overwrites: scale-d = 0)
-      auto issue = [&](float (&acc)[32]) -> int {
-        const int stage = c * ring + (int)(seq % ring);
-        mbar_wait(&S->full[stage], (uint32_t)((seq / ring) & 1));
-        ++seq;
-        const uint32_t daddr = smem_u32(stage_base + (size_t)stage * L.chunk_bytes);
-        wgmma_fence();
-        for (int kb = 0; kb < L.kblocks; ++kb) {
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            wgmma_n64<T>(acc, make_wgmma_sw128_desc(qaddr + kb * kQBlockBytes + k * 32),
-                         make_wgmma_sw128_desc(daddr + kb * kChunkKBlockBytes + k * 32), (kb | k) != 0);
-        }
-        wgmma_commit();
-        wgmma_fence_regs(acc);
-        return stage;
-      };
-      // masked max over a finished chunk's 64 columns (chunk ch: columns 64 ch ..), then the stage goes back to the
-      // producer.  The penalty of a column is 0 for a live unmasked row and -inf otherwise, ADDED to the product (not a
-      // select), so that scores and argmax are those of the full-tile kernel also for NaN / inf padding.
-      auto reduce = [&](float (&acc)[32], int stage, int ch) {
-        wgmma_fence_regs(acc);
-        if (wq < 2) {
-          const uint2 bw = *reinterpret_cast<const uint2*>(rec + 2 + 2 * ch);
-          const uint32_t b0 = bw.x >> cq, b1 = bw.y >> cq;
-          const int col0 = ch * kChunkRows;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const int col = 8 * j + cq;
-            const uint32_t b = (j < 4 ? b0 : b1) >> (8 * (j & 3));
-            const float px = (b & 1u) ? 0.f : -INFINITY, py = (b & 2u) ? 0.f : -INFINITY;
-            take<kArgmax>(acc[4 * j + 0] + px, col0 + col, m0, a0);
-            take<kArgmax>(acc[4 * j + 1] + py, col0 + col + 1, m0, a0);
-            take<kArgmax>(acc[4 * j + 2] + px, col0 + col, m1, a1);
-            take<kArgmax>(acc[4 * j + 3] + py, col0 + col + 1, m1, a1);
-          }
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&S->empty[stage]);
-      };
-      // one chunk at a time: its stage goes back to the producer as soon as it is reduced, and the other warpgroup's
-      // MMAs fill the tensor cores meanwhile
-      float acc[32];
-      for (int ch = 0; ch < nch; ++ch) {
-        const int st = issue(acc);
-        wgmma_wait<0>();
-        reduce(acc, st, ch);
-      }
-      // the record goes back (every read of it is above)
-      if (lane == 0) mbar_arrive(&S->rempty[rc.slot]);
+      QM_PROF(prof[kCoRFull] += clock64() - t_; ++prof[kCoDocs];)
+      D.slot = rc.slot;
       rc.advance(2, L.records);
+      D.head = rec_base[(size_t)D.slot * L.rec_words];
+      D.live = (int)(D.head & kLiveMask);
+      D.nch = max(1, (D.live + kChunkRows - 1) / kChunkRows);
+    };
+    // waits for the next chunk of this warpgroup's ring and starts its MMAs against query tile qaddr (the first K-step
+    // overwrites: scale-d = 0); returns the stage
+    int st_next = 0;
+    uint32_t ph_next = 0;
+    auto issue = [&](float (&acc)[32], uint32_t qaddr) -> int {
+      const int stage = c * ring + st_next;
+      QM_PROF(t_ = clock64();)
+      mbar_wait(&S->full[stage], ph_next);
+      QM_PROF(prof[kCoFull] += clock64() - t_;)
+      if (++st_next == ring) { st_next = 0; ph_next ^= 1u; }
+      const uint32_t daddr = smem_u32(stage_base + (size_t)stage * L.chunk_bytes);
+      wgmma_fence();
+      for (int kb = 0; kb < L.kblocks; ++kb) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          wgmma_n64<T>(acc, make_wgmma_sw128_desc(qaddr + kb * kQBlockBytes + k * 32),
+                       make_wgmma_sw128_desc(daddr + kb * kChunkKBlockBytes + k * 32), (kb | k) != 0);
+      }
+      wgmma_commit();
+      wgmma_fence_regs(acc);
+      return stage;
+    };
+    float m0 = -INFINITY, m1 = -INFINITY;
+    int a0 = -1, a1 = -1;   // row of the running maximum (first one on ties); stays -1 when nothing beats -inf
+    // masked max over chunk ch of document D (finished MMAs in acc), then the stage goes back to the producer.  Column
+    // j of the chunk is row start + j: start = 64 ch in store mode, live - 64 (nch - ch) for the end-aligned padded
+    // layout (only the first chunk can start below row 0).  The penalty of a column is 0 for a live unmasked row and
+    // -inf otherwise (rows below 0 included), ADDED to the product (not a select), so that scores and argmax are those
+    // of the full-tile kernel also for NaN / inf padding.
+    auto reduce = [&](float (&acc)[32], int stage, const Doc& D, int ch) {
+      wgmma_fence_regs(acc);
       if (wq < 2) {
+        const int col0 = kStore ? kChunkRows * ch : D.live - kChunkRows * (D.nch - ch);
+        // the chunk's 64 row bits: a funnel shift of the two 64-row words its rows straddle ([-1] is the zero guard)
+        const uint64_t* row_bits = reinterpret_cast<const uint64_t*>(rec_base + (size_t)D.slot * L.rec_words + kRecBits);
+        const int wi = col0 >> 6, sh = col0 & 63;
+        uint64_t bw = row_bits[wi];
+        if (sh) bw = (bw >> sh) | (row_bits[wi + 1] << (64 - sh));
+        const uint32_t b0 = (uint32_t)bw >> cq, b1 = (uint32_t)(bw >> 32) >> cq;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int col = 8 * j + cq;
+          const uint32_t b = (j < 4 ? b0 : b1) >> (8 * (j & 3));
+          const float px = (b & 1u) ? 0.f : -INFINITY, py = (b & 2u) ? 0.f : -INFINITY;
+          take<kArgmax>(acc[4 * j + 0] + px, col0 + col, m0, a0);
+          take<kArgmax>(acc[4 * j + 1] + py, col0 + col + 1, m0, a0);
+          take<kArgmax>(acc[4 * j + 2] + px, col0 + col, m1, a1);
+          take<kArgmax>(acc[4 * j + 3] + py, col0 + col + 1, m1, a1);
+        }
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&S->empty[stage]);
+    };
+    // after document D's last chunk: the -1000 fill, the query mask, the row sum and the store; the record goes back
+    auto epilogue = [&](const Doc& D) {
+      QM_PROF(t_ = clock64();)
+      if (lane == 0) mbar_arrive(&S->rempty[D.slot]);   // every read of the record is above
+      if (wq < 2) {
+        const int64_t p = p_begin + D.n;
         // the reference's -1000 fill, after every real row (ties keep the real row); column Ld reports -1 below
-        if (head & kFill) {
+        if (D.head & kFill) {
           take<kArgmax>(-1000.f, P.Ld, m0, a0);
           take<kArgmax>(-1000.f, P.Ld, m1, a1);
         }
@@ -485,7 +575,7 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
             m1 = fmaxf(m1, om1);
           }
         }
-        const bool ok0 = mask_test(qraw0, qmt), ok1 = mask_test(qraw1, qmt);   // qraw = 0 for rows >= Lq
+        const bool ok0 = mask_test(D.qraw0, qmt), ok1 = mask_test(D.qraw1, qmt);   // qraw = 0 for rows >= Lq
         if constexpr (kArgmax) {
           // rows >= Ld are the -inf padding and the -1000 fill: a max taken there carries no gradient (-1), like a
           // masked query token
@@ -497,12 +587,34 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
         float total = (lane & 3) == 0 ? (ok0 ? m0 : 0.f) + (ok1 ? m1 : 0.f) : 0.f;
 #pragma unroll
         for (int o = 4; o < 32; o <<= 1) total += __shfl_xor_sync(0xffffffffu, total, o);
-        const int buf = (int)((n >> 1) & 1);
+        const int buf = (int)((D.n >> 1) & 1);
         if (wq == 1 && lane == 0) S->part[c][buf] = total;
         named_bar_sync(1 + c, 64);
         if (wq == 0 && lane == 0) P.out[p] = total + S->part[c][buf];
       }
+      m0 = -INFINITY; m1 = -INFINITY;
+      a0 = -1; a1 = -1;
+      QM_PROF(prof[kCoEpilogue] += clock64() - t_;)
+    };
+    // one chunk at a time: its stage goes back to the producer as soon as it is reduced, and the other warpgroup's
+    // MMAs fill the tensor cores meanwhile
+    const int64_t n_pairs = p_end - p_begin;
+    float acc[32];
+    for (int64_t n = c; n < n_pairs; n += 2) {
+      Doc D;
+      begin(D, n);
+      for (int ch = 0; ch < D.nch; ++ch) {
+        const int st = issue(acc, D.qaddr);
+        QM_PROF(t_ = clock64();)
+        wgmma_wait<0>();
+        QM_PROF(prof[kCoMma] += clock64() - t_; t_ = clock64();)
+        reduce(acc, st, D, ch);
+        QM_PROF(prof[kCoReduce] += clock64() - t_;)
+      }
+      epilogue(D);
     }
+    QM_PROF(prof[kCoTotal] = clock64() - t_start;
+            if (wq == 0 && lane == 0) for (int i = kCoTotal; i <= kCoDocs; ++i) atomicAdd(&g_qm_prof[i], prof[i]);)
   }
 }
 
@@ -514,6 +626,18 @@ int launch_qm(int grid, size_t smem_bytes, cudaStream_t stream, const QmMaps& M,
   maxsim_qm_kernel<T, kArgmax, kStore><<<grid, kThreads, smem_bytes, stream>>>(M, P, L);
   MMB_CHECK_CUDA(cudaGetLastError());
   return MMB200_OK;
+}
+
+int launch_qm_dispatch(int grid, size_t smem_bytes, cudaStream_t stream, const QmMaps& M, const MaxsimParams& P,
+                       const QmLaunch& L, int dtype) {
+  if (P.doc_offsets)
+    return dtype == MMB200_F16 ? launch_qm<__half, false, true>(grid, smem_bytes, stream, M, P, L)
+                               : launch_qm<__nv_bfloat16, false, true>(grid, smem_bytes, stream, M, P, L);
+  if (dtype == MMB200_F16)
+    return P.argmax ? launch_qm<__half, true, false>(grid, smem_bytes, stream, M, P, L)
+                    : launch_qm<__half, false, false>(grid, smem_bytes, stream, M, P, L);
+  return P.argmax ? launch_qm<__nv_bfloat16, true, false>(grid, smem_bytes, stream, M, P, L)
+                  : launch_qm<__nv_bfloat16, false, false>(grid, smem_bytes, stream, M, P, L);
 }
 
 }  // namespace
@@ -528,7 +652,7 @@ int maxsim_qm_launch(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cu
   QmLaunch L;
   L.kblocks = P.dim / 64;
   L.chunk_bytes = L.kblocks * kChunkKBlockBytes;
-  L.rec_words = 2 + 2 * ((P.Ld + kChunkRows - 1) / kChunkRows);
+  L.rec_words = kRecBits + 2 * ((P.Ld + kChunkRows - 1) / kChunkRows);
   const int fixed = kQSlots * L.kblocks * kQBlockBytes + (int)sizeof(QmShared) + 1024;
   L.stages = std::min(kMaxStages, (dev.max_smem_optin - fixed - kRecordReserve) / L.chunk_bytes) & ~1;
   // the records take what is left: 48 slots up to Ld 256 or so, 30 at dim 128 and Ld 4096
@@ -563,14 +687,35 @@ int maxsim_qm_launch(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cu
   }
   *handled = true;
   const int grid = (int)std::min<int64_t>(dev.sm_count, P.n_pairs);
-  if (P.doc_offsets)
-    return dtype == MMB200_F16 ? launch_qm<__half, false, true>(grid, smem_bytes, stream, M, P, L)
-                               : launch_qm<__nv_bfloat16, false, true>(grid, smem_bytes, stream, M, P, L);
-  if (dtype == MMB200_F16)
-    return P.argmax ? launch_qm<__half, true, false>(grid, smem_bytes, stream, M, P, L)
-                    : launch_qm<__half, false, false>(grid, smem_bytes, stream, M, P, L);
-  return P.argmax ? launch_qm<__nv_bfloat16, true, false>(grid, smem_bytes, stream, M, P, L)
-                  : launch_qm<__nv_bfloat16, false, false>(grid, smem_bytes, stream, M, P, L);
+#ifdef MMB200_ENABLE_PROF
+  const bool prof = getenv("MMB200_MAXSIM_PROF") != nullptr;
+  if (prof) {
+    const unsigned long long zero[kProfCount] = {};
+    MMB_CHECK_CUDA(cudaMemcpyToSymbolAsync(g_qm_prof, zero, sizeof(zero), 0, cudaMemcpyHostToDevice, stream));
+  }
+  const int rc = launch_qm_dispatch(grid, smem_bytes, stream, M, P, L, dtype);
+  if (prof && rc == MMB200_OK) {
+    unsigned long long h[kProfCount];
+    MMB_CHECK_CUDA(cudaMemcpyFromSymbolAsync(h, g_qm_prof, sizeof(h), 0, cudaMemcpyDeviceToHost, stream));
+    MMB_CHECK_CUDA(cudaStreamSynchronize(stream));
+    // per CTA (producer), per consumer warpgroup, per scout; cycles, and cycles per chunk / per document
+    const double ctas = grid, wgs = 2.0 * grid, scouts = (double)kScouts * grid;
+    const double chunks = (double)h[kPrChunks], docs = (double)h[kCoDocs];
+    fprintf(stderr,
+            "maxsim_prof pairs %lld Ld %d chunks %.0f | cycles per CTA: producer total %.0f qempty %.0f rfull %.0f "
+            "empty %.0f tma %.0f | per consumer warpgroup: total %.0f rfull %.0f full %.0f mma %.0f reduce %.0f "
+            "epilogue %.0f | per scout: total %.0f rempty %.0f | per chunk: producer %.0f (empty %.0f, tma %.0f), "
+            "warpgroup full %.0f mma %.0f reduce %.0f | per document per warpgroup: total %.0f epilogue %.0f rfull %.0f\n",
+            (long long)P.n_pairs, P.Ld, chunks, h[kPrTotal] / ctas, h[kPrQEmpty] / ctas, h[kPrRFull] / ctas,
+            h[kPrEmpty] / ctas, h[kPrTma] / ctas, h[kCoTotal] / wgs, h[kCoRFull] / wgs, h[kCoFull] / wgs, h[kCoMma] / wgs,
+            h[kCoReduce] / wgs, h[kCoEpilogue] / wgs, h[kScTotal] / scouts, h[kScREmpty] / scouts,
+            h[kPrTotal] / chunks, h[kPrEmpty] / chunks, h[kPrTma] / chunks, h[kCoFull] / chunks,
+            h[kCoMma] / chunks, h[kCoReduce] / chunks, h[kCoTotal] / docs, h[kCoEpilogue] / docs, h[kCoRFull] / docs);
+  }
+  return rc;
+#else
+  return launch_qm_dispatch(grid, smem_bytes, stream, M, P, L, dtype);
+#endif
 }
 
 }  // namespace mmb

@@ -19,8 +19,10 @@
 Prints one JSON line per variant and a markdown table; --out also writes the JSON.  The SM clock is sampled through NVML
 read-only queries while the timed rounds run, as in bench.py.  `live_gb_per_s` counts the document bytes a live-row fetch
 reads (each document up to its last unmasked row, rounded up to 16 rows); `fetched_gb_per_s` the bytes the kernel
-actually fetches (max(1, ceil(live / 64)) 64-row chunks per document, rows past the padded length not counted: TMA
-zero-fills them without reading HBM).  --profile runs a separate torch.profiler pass
+actually fetches: each document's rows [0, live), its end-aligned 64-row chunks zero-filling the rows below 0 without
+reading HBM.  Against the debugging build (`python -m matchmaker_b200.build --prof`) with
+MMB200_MAXSIM_PROF=1, the library prints the kernel's per-role cycle counters after every launch (`--rounds 1 --steps 1`
+keeps that to four launches per variant).  --profile runs a separate torch.profiler pass
 afterwards (a few launches of each max-sim variant) and prints every kernel each variant launches with its device time
 and the gap between consecutive kernels of one call.
 """
@@ -83,13 +85,12 @@ def main():
     live_bytes = int(((live + 15) // 16 * 16).clamp(max=bench.LD).sum().item()) * bench.DIM * 2
 
     def fetched_bytes(dm, ld):
-        """Document bytes the kernel fetches: max(1, ceil(live / 64)) 64-row chunks per document, rows past the padded
-        length excluded (TMA zero-fills them without reading HBM); live = ld without a mask."""
+        """Document bytes the kernel fetches: rows [0, live) of each document (its end-aligned chunks zero-fill the rows
+        below 0 without reading HBM); live = ld without a mask."""
         if dm is None:
             return wl.cd.shape[0] * ld * bench.DIM * 2
         lv = (dm.to(torch.int64) * torch.arange(1, ld + 1, device=dev)).amax(dim=1)
-        rows = ((lv + 63) // 64).clamp(min=1) * 64
-        return int(rows.clamp(max=ld).sum().item()) * bench.DIM * 2
+        return int(lv.sum().item()) * bench.DIM * 2
 
     variants = {
         "masked": lambda: interaction.maxsim(wl.cq, wl.cd, wl.cqm, wl.cdm, docs_per_query=dpq, impl="tcgen05"),
@@ -114,7 +115,9 @@ def main():
                    "ragged": fetched_bytes(wl.cdm, bench.LD), "ragged_full": fetched_bytes(full_dm, bench.LD),
                    "dense_full": fetched_bytes(full_dm, bench.LD), "compact": fetched_bytes(compact_dm, cl),
                    "compact_nomask": fetched_bytes(None, cl), "train": fetched_bytes(wl.cdm, bench.LD)}
-    for f in variants.values():
+    for name, f in variants.items():
+        if os.environ.get("MMB200_MAXSIM_PROF"):   # a debugging build prints its counters after each launch
+            print("maxsim_prof variant %s" % name, file=sys.stderr, flush=True)
         for _ in range(3):
             f()
     torch.cuda.synchronize()
