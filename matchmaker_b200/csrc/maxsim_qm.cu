@@ -1,13 +1,17 @@
-// ColBERT max-sim, "queries on M" wgmma kernel: the hot path for Lq <= 32.
+// ColBERT max-sim, the headline wgmma kernel: the hot path for Lq <= 32.  ("qm", queries on M, is its historical name:
+// the MMA once put the query on M and the documents on N.)
 //
-// Why this orientation: with documents on M (maxsim.cu) the max over document rows is a reduction across the rows of
-// the accumulator, i.e. across threads.  Here the accumulator is transposed:
+// Orientation: document rows on M, query tokens on N.  Per 64-row chunk of a document
 //
-//     D[64 x 64] = Qrep[64 x dim] * Chunk[64 x dim]^T        (one wgmma chain per 64-row chunk of a document)
+//     D[64 x 32] = Chunk[64 x dim] * Q[32 x dim]^T        (4 * dim / 64 wgmma m64n32k16)
 //
-// row = query token, column = document row, so the max over a document is a per-thread FMNMX chain over the
-// accumulator registers plus two quad shuffles.  Rows 0..31 of Qrep are the query; rows 32..63 of the instruction read
-// whatever follows the query in shared memory and are never looked at.
+// A is the chunk in its stage, B the 32-row query tile: nothing is padded (N = 32 is Lq's ceiling), where a query on
+// M = 64 wasted half of every instruction.  Thread (warp w, lane l) of a consumer warpgroup holds chunk rows
+// 16 w + l / 4 and that + 8 for query tokens 8 j + 2 (l % 4) + {0, 1}, j < 4: 16 accumulators, 2 rows x 8 tokens.  The
+// max over a document's rows crosses threads, so it is deferred: each thread keeps a running maximum per token over
+// its rows of every chunk of the document (per chunk 2 penalties and 8 independent 2-deep chains, in every warp), and
+// the rows meet once per document, after its last chunk: shuffles over lane bits 2..4, then the four warps through
+// shared memory, where warp 0 finishes the document while warps 1-3 go on to the next one.
 //
 // Only live rows are fetched.  A document's live rows are [0, live) with live = 1 + its last unmasked row (Ld without a
 // mask; the passage's length in store mode); it takes nch = max(1, ceil(live / 64)) chunks of the stage ring.  In the
@@ -17,13 +21,13 @@
 // with no live row takes one chunk that is not fetched (the stage holds whatever it held before).  The mask is applied
 // in the reduction as an fp32 penalty per row, 0 for live unmasked rows and -inf for every other row (rows below 0
 // included), so no such row can win the max whatever its data.  The reference's -1000 fill (matchmaker/models/colbert.py:69) only
-// matters when it IS the max; it is one more candidate taken after the last chunk, value -1000 at a column past Ld (so
-// ties go to real rows and the argmax reports -1), when the document has a masked position anywhere in its Ld rows --
+// matters when it IS the max; it is one more candidate taken after the whole document, value -1000 at row Ld (so ties
+// go to real rows and the argmax reports -1), when the document has a masked position anywhere in its Ld rows --
 // live < Ld, or a hole before its last live row.
 //
 // Everything a document's chunks need from its mask is summed up in a per-document RECORD in shared memory, written by
 // scout warps up to a ring's depth of documents ahead: the live-row count, the fill flag and one bit per row (1 = live
-// and unmasked).  The producer takes the chunk count from it and the consumers take the penalty of every column from its
+// and unmasked).  The producer takes the chunk count from it and the consumers take the penalty of every row from its
 // bits, so the mask loads' latency sits entirely in the scouts, which wait on nothing but a free record slot.  Nothing
 // on a warp's per-document path waits for a global load: the per-pair indices and lengths arrive 32 pairs at a time, a
 // batch ahead (PairStream; the consumers, which only need the query, keep just a batch of pair_q).  setmaxnreg moves
@@ -36,9 +40,10 @@
 //   warps 1-3     mask scouts: scout s takes the CTA's documents s, s + 3, ...; per document it ballots the mask words
 //                 of its rows (keeping its next two documents' words in flight) and fills the document's record
 //   warpgroups 1, 2  consumers: warpgroup c takes the CTA's documents c, c + 2, ...; per chunk 4 * dim / 64 wgmma
-//                 m64n64k16 into registers, then the masked max over the chunk's 64 columns, and the stage goes back at
-//                 once.  While one warpgroup reduces, the other one's MMAs run.  Each warpgroup has its own half of the
-//                 stage ring, so every stage barrier has one consumer that waits for its phases in order.
+//                 m64n32k16 into registers, then the masked running maxima of the chunk's rows, and the stage goes
+//                 back at once; per document one combine of the rows.  While one warpgroup reduces, the other one's
+//                 MMAs run.  Each warpgroup has its own half of the stage ring, so every stage barrier has one consumer
+//                 that waits for its phases in order.
 // Record slot n % records holds the CTA's document n; the slot count is a multiple of 6, so every slot has one scout
 // and one consumer warpgroup, and each of them (and the producer) passes through the slot's phases in order.
 // HBM-bound by design: per chunk one TMA box, per document one fp32 store.
@@ -75,7 +80,8 @@ constexpr int kQBlockBytes = kQRows * 128;   // one k-block of the query tile (4
 constexpr uint32_t kFill = 1u << 16, kLiveMask = kFill - 1;
 constexpr int kRecBits = 4;   // first word of row 0's bits
 // setmaxnreg budgets: the helper warpgroup (producer, scouts) gives registers to the two consumer warpgroups, whose
-// 32-register accumulator and epilogue are the kernel's register peak.  128 x 120 + 256 x 192 = 384 x 168 (the launch).
+// accumulator, running maxima and epilogue are the kernel's register peak.  128 x 120 + 256 x 192 = 384 x 168 (the
+// launch).
 constexpr int kRegsHelper = 120, kRegsConsumer = 192;
 
 // Debugging build only (-DMMB200_ENABLE_PROF, MMB200_MAXSIM_PROF=1): clock64 cycles of each role and of each of its
@@ -84,7 +90,7 @@ constexpr int kRegsHelper = 120, kRegsConsumer = 192;
 #ifdef MMB200_ENABLE_PROF
 enum QmProf {
   kPrTotal, kPrQEmpty, kPrRFull, kPrEmpty, kPrTma, kPrChunks,                 // producer (warp 0, lane 0)
-  kCoTotal, kCoRFull, kCoFull, kCoMma, kCoReduce, kCoEpilogue, kCoDocs,       // consumers (lane 0 of warps 4 and 8)
+  kCoTotal, kCoRFull, kCoFull, kCoIssue, kCoMma, kCoReduce, kCoEpilogue, kCoDocs,   // consumers (lane 0 of warps 4, 8)
   kScTotal, kScREmpty,                                                        // scouts (lane 0 of warps 1..3)
   kProfCount
 };
@@ -101,7 +107,9 @@ struct QmShared {
   uint64_t qempty[kQSlots];    // 8 arrivals: every warp of both consumer warpgroups
   uint64_t rfull[kMaxRecords];    // 1 arrival: the scout that filled the record
   uint64_t rempty[kMaxRecords];   // 5 arrivals: the producer and the 4 warps of the consuming warpgroup
-  float part[2][2];            // [consumer][pair parity]: row sum of query rows 16..31
+  // [consumer][document parity][warp][query token]: each warp's maxima over its rows of the document, and their rows
+  float xm[2][2][4][32];
+  int32_t xa[2][2][4][32];
 };
 
 struct QmLaunch {
@@ -198,23 +206,23 @@ struct PairStream {
 };
 
 template <typename T>
-__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc);
+__device__ __forceinline__ void wgmma_n32(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc);
 template <>
-__device__ __forceinline__ void wgmma_n64<__half>(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
-  wgmma_m64n64k16_f16(d, a, b, acc);
+__device__ __forceinline__ void wgmma_n32<__half>(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc) {
+  wgmma_m64n32k16_f16(d, a, b, acc);
 }
 template <>
-__device__ __forceinline__ void wgmma_n64<__nv_bfloat16>(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
-  wgmma_m64n64k16_bf16(d, a, b, acc);
+__device__ __forceinline__ void wgmma_n32<__nv_bfloat16>(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc) {
+  wgmma_m64n32k16_bf16(d, a, b, acc);
 }
 
-// running maximum of (v, column) in column order; ties keep the first column
+// running maximum of (v, row) in row order; ties keep the first row
 template <bool kArgmax>
-__device__ __forceinline__ void take(float v, int col, float& m, int& am) {
+__device__ __forceinline__ void take(float v, int row, float& m, int& am) {
   if constexpr (kArgmax) {
     const bool gt = v > m;
     m = gt ? v : m;
-    am = gt ? col : am;
+    am = gt ? row : am;
   } else {
     m = fmaxf(m, v);
   }
@@ -422,9 +430,8 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
     setmaxnreg_inc<kRegsConsumer>();
     // ------------------------------- consumers: wgmma + masked max ------------------------
     const int c = (warp >> 2) - 1;        // consumer warpgroup 0 / 1
-    const int wq = warp & 3;              // warp inside the warpgroup: rows 16 wq .. 16 wq + 15
-    const int r0 = 16 * wq + (lane >> 2), r1 = r0 + 8;   // this thread's query rows (< 32 for wq < 2)
-    const int cq = 2 * (lane & 3);        // this thread's first column inside an 8-column group
+    const int wq = warp & 3;              // warp inside the warpgroup: chunk rows 16 wq .. 16 wq + 15
+    const int r0 = 16 * wq + (lane >> 2); // this thread's chunk rows: r0 and r0 + 8
     const int qmt = P.q_mask ? P.mask_dtype : MMB200_MASK_NONE;
     const int ring = L.stages >> 1;
     int64_t prev_q = -1;
@@ -471,8 +478,8 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
     // what a document's chunks and epilogue need
     struct Doc {
       int64_t n;              // pair p_begin + n
-      uint32_t qaddr;         // its query tile
-      uint64_t qraw0, qraw1;  // query-mask words of this thread's rows (0 for rows >= Lq)
+      uint32_t qlo;           // low word of its query tile's B descriptor
+      uint64_t qraw;          // warp 0: query-mask word of token `lane` (0 for tokens >= Lq)
       int slot;               // its record slot
       uint32_t head;          // record word 0
       int live, nch;
@@ -480,14 +487,11 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
     auto begin = [&](Doc& D, int64_t n) {
       const int64_t qi = walk_to(n);
       D.n = n;
-      D.qaddr = smem_u32(q_base + (size_t)cur_slot * qslot_bytes);
-      // query-mask words: first needed in the epilogue (L1 hits after the query's first pair)
-      D.qraw0 = 0;
-      D.qraw1 = 0;
-      if (wq < 2) {
-        if (r0 < P.Lq) D.qraw0 = (qmt != MMB200_MASK_NONE) ? mask_raw(P.q_mask, qmt, qi * (int64_t)P.Lq + r0) : 1;
-        if (r1 < P.Lq) D.qraw1 = (qmt != MMB200_MASK_NONE) ? mask_raw(P.q_mask, qmt, qi * (int64_t)P.Lq + r1) : 1;
-      }
+      D.qlo = (uint32_t)make_wgmma_sw128_desc(smem_u32(q_base + (size_t)cur_slot * qslot_bytes));
+      // query-mask word: first needed in warp 0's epilogue (L1 hits after the query's first pair)
+      D.qraw = 0;
+      if (wq == 0 && lane < P.Lq)
+        D.qraw = (qmt != MMB200_MASK_NONE) ? mask_raw(P.q_mask, qmt, qi * (int64_t)P.Lq + lane) : 1;
       // the document's record: live rows, fill flag, row bits (filled by its scout long before)
       QM_PROF(t_ = clock64();)
       mbar_wait(&S->rfull[rc.slot], rc.phase);
@@ -498,113 +502,142 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
       D.live = (int)(D.head & kLiveMask);
       D.nch = max(1, (D.live + kChunkRows - 1) / kChunkRows);
     };
-    // waits for the next chunk of this warpgroup's ring and starts its MMAs against query tile qaddr (the first K-step
-    // overwrites: scale-d = 0); returns the stage
+    // waits for the next chunk of this warpgroup's ring and starts its MMAs, D[64 rows x 32 tokens] = Chunk * Q^T (the
+    // first K-step overwrites: scale-d = 0); returns the stage.  A descriptor's high word is the same for every SW128
+    // tile; its low word is built once, from a warp-uniform (shuffled) address so that it stays in a uniform register,
+    // and stepped by immediates: +2 (32 B) per K-step, one k-block of the chunk / of the query tile per k-block.
     int st_next = 0;
     uint32_t ph_next = 0;
-    auto issue = [&](float (&acc)[32], uint32_t qaddr) -> int {
+    constexpr uint64_t kDescHi = (uint64_t)(1024 >> 4) << 32 | (uint64_t)1 << 62;   // make_wgmma_sw128_desc's
+    auto issue = [&](float (&acc)[16], uint32_t qlo_doc) -> int {
       const int stage = c * ring + st_next;
       QM_PROF(t_ = clock64();)
       mbar_wait(&S->full[stage], ph_next);
-      QM_PROF(prof[kCoFull] += clock64() - t_;)
+      QM_PROF(prof[kCoFull] += clock64() - t_; t_ = clock64();)
       if (++st_next == ring) { st_next = 0; ph_next ^= 1u; }
       const uint32_t daddr = smem_u32(stage_base + (size_t)stage * L.chunk_bytes);
+      const uint32_t dlo = (uint32_t)make_wgmma_sw128_desc(__shfl_sync(0xffffffffu, daddr, 0));
+      const uint32_t qlo = __shfl_sync(0xffffffffu, qlo_doc, 0);
       wgmma_fence();
-      for (int kb = 0; kb < L.kblocks; ++kb) {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) wgmma_n32<T>(acc, kDescHi | (dlo + 2 * k), kDescHi | (qlo + 2 * k), k != 0);
+      if (L.kblocks > 1) {
 #pragma unroll
         for (int k = 0; k < 4; ++k)
-          wgmma_n64<T>(acc, make_wgmma_sw128_desc(qaddr + kb * kQBlockBytes + k * 32),
-                       make_wgmma_sw128_desc(daddr + kb * kChunkKBlockBytes + k * 32), (kb | k) != 0);
+          wgmma_n32<T>(acc, kDescHi | (dlo + (kChunkKBlockBytes >> 4) + 2 * k),
+                       kDescHi | (qlo + (kQBlockBytes >> 4) + 2 * k), 1);
       }
       wgmma_commit();
       wgmma_fence_regs(acc);
+      QM_PROF(prof[kCoIssue] += clock64() - t_;)
       return stage;
     };
-    float m0 = -INFINITY, m1 = -INFINITY;
-    int a0 = -1, a1 = -1;   // row of the running maximum (first one on ties); stays -1 when nothing beats -inf
-    // masked max over chunk ch of document D (finished MMAs in acc), then the stage goes back to the producer.  Column
-    // j of the chunk is row start + j: start = 64 ch in store mode, live - 64 (nch - ch) for the end-aligned padded
-    // layout (only the first chunk can start below row 0).  The penalty of a column is 0 for a live unmasked row and
-    // -inf otherwise (rows below 0 included), ADDED to the product (not a select), so that scores and argmax are those
-    // of the full-tile kernel also for NaN / inf padding.
-    auto reduce = [&](float (&acc)[32], int stage, const Doc& D, int ch) {
-      wgmma_fence_regs(acc);
-      if (wq < 2) {
-        const int col0 = kStore ? kChunkRows * ch : D.live - kChunkRows * (D.nch - ch);
-        // the chunk's 64 row bits: a funnel shift of the two 64-row words its rows straddle ([-1] is the zero guard)
-        const uint64_t* row_bits = reinterpret_cast<const uint64_t*>(rec_base + (size_t)D.slot * L.rec_words + kRecBits);
-        const int wi = col0 >> 6, sh = col0 & 63;
-        uint64_t bw = row_bits[wi];
-        if (sh) bw = (bw >> sh) | (row_bits[wi + 1] << (64 - sh));
-        const uint32_t b0 = (uint32_t)bw >> cq, b1 = (uint32_t)(bw >> 32) >> cq;
+    // Running maxima of this thread's 8 query tokens 8 j + 2 (lane % 4) + {0, 1} (e = 2 j + {0, 1}) over the rows it
+    // holds of every chunk of the document so far, and with kArgmax the row of each (the first one on ties: a thread
+    // visits its rows in increasing order); -1 while nothing beats -inf.
+    float mx[8];
+    int ax[8];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const int col = 8 * j + cq;
-          const uint32_t b = (j < 4 ? b0 : b1) >> (8 * (j & 3));
-          const float px = (b & 1u) ? 0.f : -INFINITY, py = (b & 2u) ? 0.f : -INFINITY;
-          take<kArgmax>(acc[4 * j + 0] + px, col0 + col, m0, a0);
-          take<kArgmax>(acc[4 * j + 1] + py, col0 + col + 1, m0, a0);
-          take<kArgmax>(acc[4 * j + 2] + px, col0 + col, m1, a1);
-          take<kArgmax>(acc[4 * j + 3] + py, col0 + col + 1, m1, a1);
-        }
+    for (int e = 0; e < 8; ++e) { mx[e] = -INFINITY; ax[e] = -1; }
+    // masked max over chunk ch of document D (finished MMAs in acc), then the stage goes back to the producer.  Row r
+    // of the chunk is document row col0 + r: col0 = 64 ch in store mode, live - 64 (nch - ch) for the end-aligned padded
+    // layout (only the first chunk can start below row 0, whose bits are the record's zero guard words).  The penalty
+    // of a row is 0 for a live unmasked row and -inf otherwise, ADDED to the product (not a select), so that scores and
+    // argmax are those of the full-tile kernel also for NaN / inf padding.
+    auto reduce = [&](float (&acc)[16], int stage, const Doc& D, int ch) {
+      wgmma_fence_regs(acc);
+      const int col0 = kStore ? kChunkRows * ch : D.live - kChunkRows * (D.nch - ch);
+      const int x0 = col0 + r0, x1 = x0 + 8;   // >= -64
+      const uint32_t* bits = rec_base + (size_t)D.slot * L.rec_words + kRecBits;
+      const float p0 = (bits[x0 >> 5] >> (x0 & 31)) & 1u ? 0.f : -INFINITY;
+      const float p1 = (bits[x1 >> 5] >> (x1 & 31)) & 1u ? 0.f : -INFINITY;
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const int i = 4 * (e >> 1) + (e & 1);
+        take<kArgmax>(acc[i] + p0, x0, mx[e], ax[e]);
+        take<kArgmax>(acc[i + 2] + p1, x1, mx[e], ax[e]);
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(&S->empty[stage]);
     };
-    // after document D's last chunk: the -1000 fill, the query mask, the row sum and the store; the record goes back
+    // (value, row) pairs: the larger value, then the first row (a row index -1 goes with -inf and loses every tie)
+    auto combine = [&](float om, int oa, float& m, int& a) {
+      if constexpr (kArgmax) {
+        if (om > m || (om == m && (unsigned)oa < (unsigned)a)) { m = om; a = oa; }
+      } else {
+        m = fmaxf(m, om);
+      }
+    };
+    // after document D's last chunk: the maxima over the warpgroup's rows, the -1000 fill, the query mask, the row sum
+    // and the store; the record goes back
     auto epilogue = [&](const Doc& D) {
       QM_PROF(t_ = clock64();)
       if (lane == 0) mbar_arrive(&S->rempty[D.slot]);   // every read of the record is above
-      if (wq < 2) {
-        const int64_t p = p_begin + D.n;
-        // the reference's -1000 fill, after every real row (ties keep the real row); column Ld reports -1 below
-        if (D.head & kFill) {
-          take<kArgmax>(-1000.f, P.Ld, m0, a0);
-          take<kArgmax>(-1000.f, P.Ld, m1, a1);
-        }
-        // the four threads of a quad hold the same two rows: combine (larger value, then first column)
+      // the 8 lanes of a warp that share lane % 4 hold the same tokens for different rows (lane bits 2..4)
 #pragma unroll
-        for (int o = 1; o <= 2; o <<= 1) {
-          const float om0 = __shfl_xor_sync(0xffffffffu, m0, o), om1 = __shfl_xor_sync(0xffffffffu, m1, o);
-          if constexpr (kArgmax) {
-            const int oa0 = __shfl_xor_sync(0xffffffffu, a0, o), oa1 = __shfl_xor_sync(0xffffffffu, a1, o);
-            if (om0 > m0 || (om0 == m0 && (unsigned)oa0 < (unsigned)a0)) { m0 = om0; a0 = oa0; }
-            if (om1 > m1 || (om1 == m1 && (unsigned)oa1 < (unsigned)a1)) { m1 = om1; a1 = oa1; }
-          } else {
-            m0 = fmaxf(m0, om0);
-            m1 = fmaxf(m1, om1);
-          }
+      for (int o = 4; o < 32; o <<= 1) {
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+          const float om = __shfl_xor_sync(0xffffffffu, mx[e], o);
+          const int oa = kArgmax ? __shfl_xor_sync(0xffffffffu, ax[e], o) : 0;
+          combine(om, oa, mx[e], ax[e]);
         }
-        const bool ok0 = mask_test(D.qraw0, qmt), ok1 = mask_test(D.qraw1, qmt);   // qraw = 0 for rows >= Lq
+      }
+      // the four warps' maxima meet in shared memory, [warp][token]; warp 0 finishes the document while warps 1-3 go
+      // on.  The warpgroup's next document writes the other buffer; the one after writes this one again only once
+      // the MMAs of the document between have completed, and warp 0 issues its part of them after reading this one.
+      const int buf = (int)((D.n >> 1) & 1);
+      float* xm = S->xm[c][buf][0];
+      int32_t* xa = S->xa[c][buf][0];
+      if (lane < 4) {
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+          const int t = 8 * (e >> 1) + 2 * lane + (e & 1);
+          xm[32 * wq + t] = mx[e];
+          if constexpr (kArgmax) xa[32 * wq + t] = ax[e];
+        }
+      }
+#pragma unroll
+      for (int e = 0; e < 8; ++e) { mx[e] = -INFINITY; ax[e] = -1; }
+      if (wq != 0) {
+        named_bar_arrive(1 + c, 128);
+      } else {
+        named_bar_sync(1 + c, 128);
+        // lane t: query token t
+        float m = xm[lane];
+        int a = kArgmax ? xa[lane] : -1;
+#pragma unroll
+        for (int w = 1; w < 4; ++w) combine(xm[32 * w + lane], kArgmax ? xa[32 * w + lane] : 0, m, a);
+        // the reference's -1000 fill, after every real row (ties keep the real row); row Ld reports -1 below
+        if (D.head & kFill) take<kArgmax>(-1000.f, P.Ld, m, a);
+        const bool ok = mask_test(D.qraw, qmt);   // qraw = 0 for tokens >= Lq
+        const int64_t p = p_begin + D.n;
         if constexpr (kArgmax) {
           // rows >= Ld are the -inf padding and the -1000 fill: a max taken there carries no gradient (-1), like a
           // masked query token
-          if ((lane & 3) == 0) {
-            if (r0 < P.Lq) P.argmax[p * (int64_t)P.Lq + r0] = (ok0 && a0 < P.Ld) ? a0 : -1;
-            if (r1 < P.Lq) P.argmax[p * (int64_t)P.Lq + r1] = (ok1 && a1 < P.Ld) ? a1 : -1;
-          }
+          if (lane < P.Lq) P.argmax[p * (int64_t)P.Lq + lane] = (ok && a < P.Ld) ? a : -1;
         }
-        float total = (lane & 3) == 0 ? (ok0 ? m0 : 0.f) + (ok1 ? m1 : 0.f) : 0.f;
+        // the score sums the tokens as ((t0 + t1) + (t2 + t3)) + ((t4 + t5) + (t6 + t7)) over t_i = q[i] + q[i + 8]
+        // for tokens 0..15, the same over tokens 16..31, and then the two halves: a fixed association, so that the
+        // score does not depend on how the rows were split among threads
+        float s = ok ? m : 0.f;
+        s += __shfl_down_sync(0xffffffffu, s, 8);
 #pragma unroll
-        for (int o = 4; o < 32; o <<= 1) total += __shfl_xor_sync(0xffffffffu, total, o);
-        const int buf = (int)((D.n >> 1) & 1);
-        if (wq == 1 && lane == 0) S->part[c][buf] = total;
-        named_bar_sync(1 + c, 64);
-        if (wq == 0 && lane == 0) P.out[p] = total + S->part[c][buf];
+        for (int o = 1; o < 8; o <<= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+        const float hi = __shfl_sync(0xffffffffu, s, 16);
+        if (lane == 0) P.out[p] = s + hi;
       }
-      m0 = -INFINITY; m1 = -INFINITY;
-      a0 = -1; a1 = -1;
       QM_PROF(prof[kCoEpilogue] += clock64() - t_;)
     };
     // one chunk at a time: its stage goes back to the producer as soon as it is reduced, and the other warpgroup's
     // MMAs fill the tensor cores meanwhile
     const int64_t n_pairs = p_end - p_begin;
-    float acc[32];
+    float acc[16];
     for (int64_t n = c; n < n_pairs; n += 2) {
       Doc D;
       begin(D, n);
       for (int ch = 0; ch < D.nch; ++ch) {
-        const int st = issue(acc, D.qaddr);
+        const int st = issue(acc, D.qlo);
         QM_PROF(t_ = clock64();)
         wgmma_wait<0>();
         QM_PROF(prof[kCoMma] += clock64() - t_; t_ = clock64();)
@@ -655,7 +688,7 @@ int maxsim_qm_launch(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cu
   L.rec_words = kRecBits + 2 * ((P.Ld + kChunkRows - 1) / kChunkRows);
   const int fixed = kQSlots * L.kblocks * kQBlockBytes + (int)sizeof(QmShared) + 1024;
   L.stages = std::min(kMaxStages, (dev.max_smem_optin - fixed - kRecordReserve) / L.chunk_bytes) & ~1;
-  // the records take what is left: 48 slots up to Ld 256 or so, 30 at dim 128 and Ld 4096
+  // the records take what is left: 48 slots up to Ld 256 or so, 24 at dim 128 and Ld 4096
   const int rec_bytes = L.rec_words * 4;
   L.records = std::min(kMaxRecords, (dev.max_smem_optin - fixed - L.stages * L.chunk_bytes) / rec_bytes);
   L.records -= L.records % kRecordStep;
@@ -703,14 +736,16 @@ int maxsim_qm_launch(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cu
     const double chunks = (double)h[kPrChunks], docs = (double)h[kCoDocs];
     fprintf(stderr,
             "maxsim_prof pairs %lld Ld %d chunks %.0f | cycles per CTA: producer total %.0f qempty %.0f rfull %.0f "
-            "empty %.0f tma %.0f | per consumer warpgroup: total %.0f rfull %.0f full %.0f mma %.0f reduce %.0f "
-            "epilogue %.0f | per scout: total %.0f rempty %.0f | per chunk: producer %.0f (empty %.0f, tma %.0f), "
-            "warpgroup full %.0f mma %.0f reduce %.0f | per document per warpgroup: total %.0f epilogue %.0f rfull %.0f\n",
+            "empty %.0f tma %.0f | per consumer warpgroup: total %.0f rfull %.0f full %.0f issue %.0f mma %.0f "
+            "reduce %.0f epilogue %.0f | per scout: total %.0f rempty %.0f | per chunk: producer %.0f (empty %.0f, "
+            "tma %.0f), warpgroup full %.0f issue %.0f mma %.0f reduce %.0f | per document per warpgroup: total %.0f "
+            "epilogue %.0f rfull %.0f\n",
             (long long)P.n_pairs, P.Ld, chunks, h[kPrTotal] / ctas, h[kPrQEmpty] / ctas, h[kPrRFull] / ctas,
-            h[kPrEmpty] / ctas, h[kPrTma] / ctas, h[kCoTotal] / wgs, h[kCoRFull] / wgs, h[kCoFull] / wgs, h[kCoMma] / wgs,
-            h[kCoReduce] / wgs, h[kCoEpilogue] / wgs, h[kScTotal] / scouts, h[kScREmpty] / scouts,
-            h[kPrTotal] / chunks, h[kPrEmpty] / chunks, h[kPrTma] / chunks, h[kCoFull] / chunks,
-            h[kCoMma] / chunks, h[kCoReduce] / chunks, h[kCoTotal] / docs, h[kCoEpilogue] / docs, h[kCoRFull] / docs);
+            h[kPrEmpty] / ctas, h[kPrTma] / ctas, h[kCoTotal] / wgs, h[kCoRFull] / wgs, h[kCoFull] / wgs,
+            h[kCoIssue] / wgs, h[kCoMma] / wgs, h[kCoReduce] / wgs, h[kCoEpilogue] / wgs, h[kScTotal] / scouts,
+            h[kScREmpty] / scouts, h[kPrTotal] / chunks, h[kPrEmpty] / chunks, h[kPrTma] / chunks, h[kCoFull] / chunks,
+            h[kCoIssue] / chunks, h[kCoMma] / chunks, h[kCoReduce] / chunks, h[kCoTotal] / docs, h[kCoEpilogue] / docs,
+            h[kCoRFull] / docs);
   }
   return rc;
 #else

@@ -287,6 +287,11 @@ __device__ __forceinline__ bool elect_one_sync() {
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+// Arrives without waiting: the shared-memory writes before it are visible to the threads that bar.sync on the same
+// barrier (nthreads counts both sides).
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
 
 // ---------------------------------------------------------------------------------------------
 // streaming global loads
