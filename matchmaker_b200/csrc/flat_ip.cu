@@ -943,14 +943,15 @@ extern "C" int mmb200_flat_ip_topk(const void* queries, const void* passages, co
                                    int64_t n_pass, int32_t dim, int32_t k, int32_t dtype, int64_t id_base,
                                    void* stream_) {
   using namespace mmb;
-  MMB_REQUIRE(queries && passages && out_scores && out_ids && workspace, "null pointer");
-  MMB_REQUIRE(nq > 0 && n_pass > 0, "need at least one query and one passage");
+  MMB_REQUIRE(nq >= 0 && n_pass > 0, "need at least one passage");
   MMB_REQUIRE(k >= 1 && k <= kMaxK, "fused top-k supports 1 <= k <= 1024");
   MMB_REQUIRE(dtype == MMB200_F16 || dtype == MMB200_BF16 || dtype == MMB200_F32_SPLIT16,
               "passage storage must be fp16, bf16 or the fp16 hi/lo split of fp32 (MMB200_F32_SPLIT16)");
-  const bool split = dtype == MMB200_F32_SPLIT16;
   MMB_REQUIRE(dim % 64 == 0 && dim >= 64, "vector dim must be a multiple of 64");
   MMB_REQUIRE(n_pass < (1ll << 32) - 512, "at most 2^32 passages per shard");
+  if (nq == 0) return MMB200_OK;   // an empty batch: nothing to read or write (its tensors may be null), no device needed
+  MMB_REQUIRE(queries && passages && out_scores && out_ids && workspace, "null pointer");
+  const bool split = dtype == MMB200_F32_SPLIT16;
   MMB_REQUIRE(((reinterpret_cast<uintptr_t>(queries) | reinterpret_cast<uintptr_t>(passages)) & 15) == 0, "16-byte alignment");
   DeviceInfo dev;
   if (int rc = require_sm90(&dev)) return rc;

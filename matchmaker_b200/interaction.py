@@ -451,6 +451,9 @@ def flat_ip_topk(queries: torch.Tensor, passages: torch.Tensor, k: int, ids: Opt
     nq = queries.shape[0]
     if ids is not None:
         ids = ids.to(torch.int64).contiguous()
+    if nq == 0 and 1 <= k <= FLAT_IP_MAX_K:   # as ivf_search: an empty batch has an empty result
+        return (torch.empty((0, k), dtype=torch.float32, device=dev),
+                torch.empty((0, k), dtype=torch.int64, device=dev))
     lib = _lib.load()
     with torch.cuda.device(dev):
         wsb = lib.mmb200_flat_ip_workspace_bytes(nq, n, k)
