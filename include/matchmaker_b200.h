@@ -78,8 +78,8 @@ MMB200_API int mmb200_device_info(int device, int* sm_count, int* cc_major, int*
  * Replaces: ColBERT.forward scoring            matchmaker/models/colbert.py:68-75   (masks given)
  *           ColBERT.forward_aggregation        matchmaker/models/colbert.py:100-112 (masks NULL)
  *           ColBERT.forward_inbatch_aggregation matchmaker/models/colbert.py:154-162
- *               (all pairs: n_pairs = n_q * n_d, pair_q[p] = p / n_d, pair_d[p] = p % n_d, or
- *                mmb200_maxsim_allpairs_fwd below)
+ *               (all pairs: n_pairs = n_q * n_d, pair_q[p] = p / n_d, pair_d[p] = p % n_d; its
+ *                backward is mmb200_maxsim_allpairs_bwd below)
  *
  * q      [n_q, Lq, dim]  dtype `dtype`
  * d      [n_d, Ld, dim]  dtype `dtype`
@@ -112,6 +112,19 @@ MMB200_API int mmb200_maxsim_bwd(const void* q, const void* d, const float* grad
                       float* grad_q, float* grad_d, int64_t n_q, int64_t n_d, int64_t n_pairs,
                       int32_t docs_per_query, int32_t Lq, int32_t Ld, int32_t dim, int32_t dtype,
                       void* stream);
+
+/* Backward of all-pairs scoring: mmb200_maxsim_fwd with n_pairs = n_q * n_d, pair_q[p] = p / n_d, pair_d[p] = p % n_d
+ * (any pair_dmask), so pair p = a * n_d + b is query a against document b and every document is shared by all queries.
+ * grad_out [n_q, n_d] f32; argmax [n_q * n_d, Lq] int32 from that forward (-1: no gradient);
+ *   grad_q[a][i] = sum_b g[a,b] * d[b][argmax[a,b,i]]                       (ascending b)
+ *   grad_d[b][r] = sum over (a, i) with argmax[a,b,i] = r of g[a,b] * q[a][i]  (ascending (a, i))
+ * grad_q [n_q, Lq, dim] and grad_d [n_d, Ld, dim] f32 are OVERWRITTEN; a row no argmax points at is 0.  No atomics:
+ * two runs give the same bits, and with n_q = 1 they are those of mmb200_maxsim_bwd(docs_per_query = n_d).
+ * n_q * n_d < 2^31.  A tensor with no elements may be NULL; with n_q = 0 or n_d = 0 the other side's gradient is
+ * zero-filled and no kernel runs. */
+MMB200_API int mmb200_maxsim_allpairs_bwd(const void* q, const void* d, const float* grad_out, const int32_t* argmax,
+                                          float* grad_q, float* grad_d, int64_t n_q, int64_t n_d, int32_t Lq,
+                                          int32_t Ld, int32_t dim, int32_t dtype, void* stream);
 
 /* Host-buffer variant (the end-to-end call): all pointers are HOST pointers (pinned memory
  * gives full PCIe bandwidth, pageable works).  Documents are streamed to the device in chunks

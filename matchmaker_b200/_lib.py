@@ -32,6 +32,7 @@ SIGNATURES = {
                                      _i32, _i32, _i32, _i32, _vp]),
     "mmb200_maxsim_bwd": (_c.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _i32, _i32, _i32, _i32, _i32,
                                      _vp]),
+    "mmb200_maxsim_allpairs_bwd": (_c.c_int, [_vp] * 6 + [_i64, _i64, _i32, _i32, _i32, _i32, _vp]),
     "mmb200_maxsim_fwd_host": (_c.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _i32, _i32, _i32, _i32, _i32, _i32,
                                           _i64]),
     "mmb200_kernel_pool_fwd": (_c.c_int, [_vp] * 12 + [_i64, _i32, _i32, _i32, _i32, _f32, _i32, _i32, _vp]),

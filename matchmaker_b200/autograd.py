@@ -12,7 +12,8 @@ from . import interaction
 class _MaxSim(torch.autograd.Function):
     @staticmethod
     def forward(ctx, q, d, q_mask, d_mask, docs_per_query):
-        # ctx.needs_input_grad is all False under torch.no_grad() / for detached inputs: nothing is saved then
+        # ctx.needs_input_grad follows the inputs' requires_grad, not the grad mode: it is all False for detached inputs
+        # (nothing is saved then), but under torch.no_grad() inputs that require grad still take the argmax forward
         need_grad = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
         if need_grad:
             out, argmax = interaction.maxsim(q, d, q_mask, d_mask, docs_per_query=docs_per_query, return_argmax=True)
@@ -33,6 +34,39 @@ def maxsim(q: torch.Tensor, d: torch.Tensor, q_mask: Optional[torch.Tensor] = No
            d_mask: Optional[torch.Tensor] = None, docs_per_query: int = 1) -> torch.Tensor:
     """Differentiable ColBERT max-sim (pairs mode); see :func:`matchmaker_b200.interaction.maxsim`."""
     return _MaxSim.apply(q, d, q_mask, d_mask, docs_per_query)
+
+
+class _MaxSimAllPairs(torch.autograd.Function):
+    """Only entered when a gradient is wanted (see maxsim_allpairs below): the argmax forward, then its backward."""
+
+    @staticmethod
+    def forward(ctx, q, q_mask, d, d_mask, reference_mask_indexing):
+        out, argmax = interaction.maxsim_allpairs(q, q_mask, d, d_mask, reference_mask_indexing=reference_mask_indexing,
+                                                  return_argmax=True)
+        ctx.save_for_backward(q, d, argmax)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        q, d, argmax = ctx.saved_tensors
+        gq, gd = interaction.maxsim_allpairs_bwd(q, d, grad_out, argmax)
+        return (gq.to(q.dtype) if ctx.needs_input_grad[0] else None, None,
+                gd.to(d.dtype) if ctx.needs_input_grad[2] else None, None, None)
+
+
+def maxsim_allpairs(q: torch.Tensor, q_mask: Optional[torch.Tensor], d: torch.Tensor, d_mask: Optional[torch.Tensor],
+                    reference_mask_indexing: bool = False) -> torch.Tensor:
+    """Differentiable all-pairs max-sim [n_q, n_d] (in-batch negatives); see
+    :func:`matchmaker_b200.interaction.maxsim_allpairs`.  The gradient follows the forward's argmax, so with
+    ``reference_mask_indexing=True`` it is what autograd of colbert.py:154-162 gives, masks and all.
+
+    Without a gradient to compute (grad mode off, e.g. under ``torch.no_grad()``, or neither q nor d requiring grad)
+    this is exactly :func:`interaction.maxsim_allpairs`: no argmax, nothing saved, the inference kernels' bits.  The
+    decision is taken here, outside the Function, because inside ``Function.forward`` grad mode is always off and
+    ``ctx.needs_input_grad`` reflects only the inputs' ``requires_grad``."""
+    if torch.is_grad_enabled() and (q.requires_grad or d.requires_grad):
+        return _MaxSimAllPairs.apply(q, q_mask, d, d_mask, reference_mask_indexing)
+    return interaction.maxsim_allpairs(q, q_mask, d, d_mask, reference_mask_indexing=reference_mask_indexing)
 
 
 # "auto": forward that saves its cosines + tensor-core backward where the shape allows; "simt": always the FFMA backward

@@ -1,4 +1,4 @@
-// Max-sim: backward kernel and the host-buffer (end-to-end) entry point.
+// Max-sim: backward kernels (pairs and in-batch all-pairs) and the host-buffer (end-to-end) entry point.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -52,6 +52,137 @@ __global__ void __launch_bounds__(128) maxsim_bwd_q_kernel(const T* __restrict__
         if (a >= 0) acc = fmaf(grad_out[p], to_float(d[(p * Ld + a) * (int64_t)dim + k]), acc);
       }
       grad_q[(qi * Lq + i) * (int64_t)dim + k] = acc;
+    }
+  }
+}
+
+// Backward of all-pairs scoring (colbert.py:154-162): pair p = a * n_d + b is query a against document b, so every
+// document is shared by all n_q queries and its gradient is a sum over them:
+//   grad_q[a][i] = sum_b                          g[a,b] * d[b][argmax[a,b,i]]     (ascending b)
+//   grad_d[b][r] = sum_{(a, i) : argmax[a,b,i] = r}  g[a,b] * q[a][i]              (ascending (a, i))
+// Same rules as above: no atomics, each output element owned by one thread, fmaf from 0 in that order; with n_q = 1 the
+// bits are those of maxsim_bwd_{d,q}_kernel with docs_per_query = n_d.
+//   maxsim_allpairs_bwd_d_kernel  one CTA per (document, block of 64 rows, slice of 128 features): an in-batch call has
+//                                 few documents (32 at TAS-B's batch), and this split still gives every SM a CTA.  Per
+//                                 chunk of 1024 (a, i) the warps compact, in order, the entries whose argmax falls in
+//                                 the CTA's rows; thread k then walks that list into its own column of a shared-memory
+//                                 accumulator, and writes the column (zeros where no argmax points) at the end
+//   maxsim_allpairs_bwd_q_kernel  one CTA per (query, token), like maxsim_bwd_q_kernel with document b = p % n_d; the
+//                                 argmax and gradient of 1024 documents at a time are staged in shared memory so that
+//                                 the document rows of four pairs are in flight at once
+constexpr int kAllBwdThreads = 128;   // the feature slice of a grad_d CTA
+constexpr int kAllBwdRows = 64;
+constexpr int kAllBwdChunk = 1024;
+constexpr int kAllBwdUnroll = 4;
+
+template <typename T>
+__global__ void __launch_bounds__(kAllBwdThreads)
+maxsim_allpairs_bwd_d_kernel(const T* __restrict__ q, const float* __restrict__ grad_out, const int32_t* __restrict__ argmax,
+                             float* __restrict__ grad_d, int64_t n_q, int64_t n_d, int Lq, int Ld, int dim) {
+  constexpr int kPerWarp = kAllBwdChunk / (kAllBwdThreads / 32);
+  __shared__ float acc[kAllBwdRows][kAllBwdThreads];   // column threadIdx.x belongs to thread threadIdx.x alone
+  __shared__ int hit_e[kAllBwdChunk];                  // entry - chunk base | (row - r0) << 16
+  __shared__ float hit_g[kAllBwdChunk];
+  __shared__ int hit_n[kAllBwdThreads / 32];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int rblocks = (Ld + kAllBwdRows - 1) / kAllBwdRows, slices = (dim + kAllBwdThreads - 1) / kAllBwdThreads;
+  const int64_t n_items = n_d * rblocks * slices, n_e = n_q * Lq;
+  for (int64_t item = blockIdx.x; item < n_items; item += gridDim.x) {
+    const int64_t b = item / (rblocks * slices);
+    const int rem = (int)(item % (rblocks * slices));
+    const int r0 = (rem / slices) * kAllBwdRows, nr = min(kAllBwdRows, Ld - r0);
+    const int k = (rem % slices) * kAllBwdThreads + threadIdx.x;
+    const bool kok = k < dim;
+    for (int r = 0; r < kAllBwdRows; ++r) acc[r][threadIdx.x] = 0.f;
+    for (int64_t c0 = 0; c0 < n_e; c0 += kAllBwdChunk) {
+      int cnt = 0;
+      for (int t = 0; t < kPerWarp; t += 32) {
+        const int er = warp * kPerWarp + t + lane;
+        const int64_t e = c0 + er;   // e = a * Lq + i
+        int r = -1;
+        float g = 0.f;
+        if (e < n_e) {
+          const int64_t a = e / Lq, p = a * n_d + b;
+          r = argmax[p * Lq + (e - a * Lq)];
+          if (r >= r0 && r < r0 + nr) g = grad_out[p];
+        }
+        const bool hit = r >= r0 && r < r0 + nr;
+        const unsigned m = __ballot_sync(0xffffffffu, hit);
+        if (hit) {
+          const int slot = warp * kPerWarp + cnt + __popc(m & ((1u << lane) - 1u));
+          hit_e[slot] = er | ((r - r0) << 16);
+          hit_g[slot] = g;
+        }
+        cnt += __popc(m);
+      }
+      if (lane == 0) hit_n[warp] = cnt;
+      __syncthreads();
+      if (kok) {
+        for (int w = 0; w < kAllBwdThreads / 32; ++w) {   // the warps' lists in order: ascending (a, i)
+          const int n = hit_n[w];
+          const int* he = hit_e + w * kPerWarp;
+          const float* hg = hit_g + w * kPerWarp;
+          for (int h = 0; h < n; h += kAllBwdUnroll) {
+            float v[kAllBwdUnroll];
+            int rr[kAllBwdUnroll];
+#pragma unroll
+            for (int u = 0; u < kAllBwdUnroll; ++u) {
+              rr[u] = -1;
+              v[u] = 0.f;
+              if (h + u < n) {
+                const int x = he[h + u];
+                rr[u] = x >> 16;
+                v[u] = to_float(q[(c0 + (x & 0xffff)) * dim + k]);   // q[a][i][k]
+              }
+            }
+#pragma unroll
+            for (int u = 0; u < kAllBwdUnroll; ++u)
+              if (rr[u] >= 0) acc[rr[u]][threadIdx.x] = fmaf(hg[h + u], v[u], acc[rr[u]][threadIdx.x]);
+          }
+        }
+      }
+      __syncthreads();   // the hit lists are rewritten by the next chunk
+    }
+    if (kok)
+      for (int r = 0; r < nr; ++r) grad_d[(b * Ld + r0 + r) * (int64_t)dim + k] = acc[r][threadIdx.x];
+  }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kAllBwdThreads)
+maxsim_allpairs_bwd_q_kernel(const T* __restrict__ d, const float* __restrict__ grad_out, const int32_t* __restrict__ argmax,
+                             float* __restrict__ grad_q, int64_t n_q, int64_t n_d, int Lq, int Ld, int dim) {
+  __shared__ int s_r[kAllBwdChunk];
+  __shared__ float s_g[kAllBwdChunk];
+  for (int64_t item = blockIdx.x; item < n_q * Lq; item += gridDim.x) {
+    const int64_t a = item / Lq;
+    const int i = (int)(item % Lq);
+    float* gq = grad_q + item * (int64_t)dim;
+    for (int64_t b0 = 0; b0 < n_d; b0 += kAllBwdChunk) {
+      const int nb = (int)min((int64_t)kAllBwdChunk, n_d - b0);
+      __syncthreads();
+      for (int j = threadIdx.x; j < nb; j += blockDim.x) {
+        const int64_t p = a * n_d + b0 + j;
+        s_r[j] = argmax[p * Lq + i];
+        s_g[j] = grad_out[p];
+      }
+      __syncthreads();
+      for (int k = threadIdx.x; k < dim; k += blockDim.x) {
+        float acc = b0 == 0 ? 0.f : gq[k];   // a document count beyond one chunk continues the same chain
+        for (int j = 0; j < nb; j += kAllBwdUnroll) {
+          float v[kAllBwdUnroll];
+          int rr[kAllBwdUnroll];
+#pragma unroll
+          for (int u = 0; u < kAllBwdUnroll; ++u) {
+            rr[u] = j + u < nb ? s_r[j + u] : -1;
+            v[u] = rr[u] >= 0 ? to_float(d[((b0 + j + u) * Ld + rr[u]) * (int64_t)dim + k]) : 0.f;
+          }
+#pragma unroll
+          for (int u = 0; u < kAllBwdUnroll; ++u)
+            if (rr[u] >= 0) acc = fmaf(s_g[j + u], v[u], acc);
+        }
+        gq[k] = acc;
+      }
     }
   }
 }
@@ -135,6 +266,40 @@ extern "C" int mmb200_maxsim_bwd(const void* q, const void* d, const float* grad
                                                        docs_per_query, Lq, Ld, dim);
     maxsim_bwd_q_kernel<T><<<grid_q, 128, 0, stream>>>(static_cast<const T*>(d), grad_out, argmax, grad_q, n_q, n_pairs,
                                                        docs_per_query, Lq, Ld, dim);
+    MMB_CHECK_CUDA(cudaGetLastError());
+    return MMB200_OK;
+  });
+}
+
+extern "C" int mmb200_maxsim_allpairs_bwd(const void* q, const void* d, const float* grad_out, const int32_t* argmax,
+                                          float* grad_q, float* grad_d, int64_t n_q, int64_t n_d, int32_t Lq,
+                                          int32_t Ld, int32_t dim, int32_t dtype, void* stream_) {
+  using namespace mmb;
+  MMB_REQUIRE(n_q >= 0 && n_d >= 0 && Lq >= 1 && Ld >= 1 && dim >= 1, "bad shape");
+  MMB_REQUIRE(n_d == 0 || n_q <= ((int64_t(1) << 31) - 1) / n_d,
+              "n_q * n_d must be below 2^31 (the forward's pair indices are int32)");
+  // a tensor with no elements may come with a null pointer (torch hands one out for an empty tensor)
+  MMB_REQUIRE((n_q == 0 || (q && grad_q)) && (n_d == 0 || (d && grad_d)) && (n_q * n_d == 0 || (grad_out && argmax)),
+              "null pointer");
+  MMB_REQUIRE(dtype_size(dtype) != 0, "unknown dtype");
+  if (n_q == 0 && n_d == 0) return MMB200_OK;
+  DeviceInfo dev;
+  if (int rc = require_sm90(&dev)) return rc;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (n_q == 0 || n_d == 0) {   // no pairs: the side that has rows gets a zero gradient
+    if (n_q) MMB_CHECK_CUDA(cudaMemsetAsync(grad_q, 0, (size_t)n_q * Lq * dim * sizeof(float), stream));
+    if (n_d) MMB_CHECK_CUDA(cudaMemsetAsync(grad_d, 0, (size_t)n_d * Ld * dim * sizeof(float), stream));
+    return MMB200_OK;
+  }
+  const int64_t d_items = n_d * ((Ld + kAllBwdRows - 1) / kAllBwdRows) * ((dim + kAllBwdThreads - 1) / kAllBwdThreads);
+  const int grid_d = (int)std::min<int64_t>((int64_t)dev.sm_count * 16, d_items);
+  const int grid_q = (int)std::min<int64_t>((int64_t)dev.sm_count * 16, n_q * Lq);
+  return dispatch_dtype(dtype, [&](auto t) {
+    using T = decltype(t);
+    maxsim_allpairs_bwd_d_kernel<T><<<grid_d, kAllBwdThreads, 0, stream>>>(static_cast<const T*>(q), grad_out, argmax,
+                                                                           grad_d, n_q, n_d, Lq, Ld, dim);
+    maxsim_allpairs_bwd_q_kernel<T><<<grid_q, kAllBwdThreads, 0, stream>>>(static_cast<const T*>(d), grad_out, argmax,
+                                                                           grad_q, n_q, n_d, Lq, Ld, dim);
     MMB_CHECK_CUDA(cudaGetLastError());
     return MMB200_OK;
   });

@@ -116,13 +116,14 @@ def maxsim(q: torch.Tensor, d: torch.Tensor, q_mask: Optional[torch.Tensor] = No
 
 def maxsim_allpairs(q: torch.Tensor, q_mask: Optional[torch.Tensor], d: torch.Tensor,
                     d_mask: Optional[torch.Tensor], impl: str = "auto",
-                    reference_mask_indexing: bool = False) -> torch.Tensor:
+                    reference_mask_indexing: bool = False, return_argmax: bool = False):
     """All query x document max-sim scores [n_q, n_d] (colbert.py:154-162).
 
     ``reference_mask_indexing=True`` reproduces the reference bit-for-bit: colbert.py:158 expands
     ``document_mask`` [n_d, Ld] along the *query* axis of the [n_q, n_d, Lq, Ld] score tensor, i.e. pair
     (a, b) is masked with the mask of document ``a`` (only defined for n_q == n_d, the in-batch case).
-    The default applies each document's own mask."""
+    The default applies each document's own mask.  ``return_argmax=True`` also returns the argmax
+    [n_q * n_d, Lq] int32 of pair a * n_d + b, what :func:`maxsim_allpairs_bwd` takes."""
     n_q, n_d = q.shape[0], d.shape[0]
     idx = torch.arange(n_q * n_d, device=q.device, dtype=torch.int32)
     pq = torch.div(idx, n_d, rounding_mode="floor").to(torch.int32)
@@ -132,7 +133,40 @@ def maxsim_allpairs(q: torch.Tensor, q_mask: Optional[torch.Tensor], d: torch.Te
         if n_q != n_d:
             raise _lib.MatchmakerB200Error("reference mask indexing (colbert.py:158) needs n_q == n_d")
         pdm = pq
-    return maxsim(q, d, q_mask, d_mask, pair_q=pq, pair_d=pd, impl=impl, pair_dmask=pdm).view(n_q, n_d)
+    res = maxsim(q, d, q_mask, d_mask, pair_q=pq, pair_d=pd, impl=impl, pair_dmask=pdm, return_argmax=return_argmax)
+    if return_argmax:
+        return res[0].view(n_q, n_d), res[1]
+    return res.view(n_q, n_d)
+
+
+def maxsim_allpairs_bwd(q: torch.Tensor, d: torch.Tensor, grad_out: torch.Tensor,
+                        argmax: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Gradients of :func:`maxsim_allpairs` w.r.t. q [n_q, Lq, dim] and d [n_d, Ld, dim], fp32, from
+    grad_out [n_q, n_d] and the forward's argmax [n_q * n_d, Lq] (either mask indexing: the gradient
+    follows the argmax)."""
+    dev = _require_cuda(q, d, grad_out, argmax)
+    if q.dtype != d.dtype or q.dtype not in _DTYPES:
+        raise _lib.MatchmakerB200Error(f"q/d must share a dtype in fp16/bf16/fp32, got {q.dtype}, {d.dtype}")
+    if q.dim() != 3 or d.dim() != 3 or q.shape[-1] != d.shape[-1]:
+        raise _lib.MatchmakerB200Error(f"expected q [n_q,Lq,dim], d [n_d,Ld,dim]; got {tuple(q.shape)}, {tuple(d.shape)}")
+    q = q.contiguous()
+    d = d.contiguous()
+    n_q, Lq, dim = q.shape
+    n_d, Ld, _ = d.shape
+    if grad_out.numel() != n_q * n_d:
+        raise _lib.MatchmakerB200Error(f"grad_out has {grad_out.numel()} elements, expected n_q * n_d = {n_q * n_d}")
+    if argmax.dtype != torch.int32 or tuple(argmax.shape) != (n_q * n_d, Lq):
+        raise _lib.MatchmakerB200Error(f"argmax must be int32 [{n_q * n_d}, {Lq}], got {argmax.dtype} "
+                                       f"{tuple(argmax.shape)}")
+    grad_out = grad_out.to(torch.float32).contiguous()
+    gq = torch.empty((n_q, Lq, dim), dtype=torch.float32, device=dev)
+    gd = torch.empty((n_d, Ld, dim), dtype=torch.float32, device=dev)
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        rc = lib.mmb200_maxsim_allpairs_bwd(_ptr(q), _ptr(d), _ptr(grad_out), _ptr(argmax.contiguous()), _ptr(gq),
+                                            _ptr(gd), n_q, n_d, Lq, Ld, dim, _DTYPES[q.dtype], _stream(dev))
+    _lib.check(rc, "mmb200_maxsim_allpairs_bwd")
+    return gq, gd
 
 
 def maxsim_bwd(q: torch.Tensor, d: torch.Tensor, grad_out: torch.Tensor, argmax: torch.Tensor,

@@ -96,11 +96,12 @@ class ColBERT(nn.Module):
                                     reference_mask_indexing: bool = True):
         """All-pairs scores [Nq, Nd] (colbert.py:154-162).  By default bit-compatible with the reference,
         including its indexing of ``document_mask`` by the query position (colbert.py:158; see DESIGN.md);
-        pass ``reference_mask_indexing=False`` to mask every document with its own mask."""
+        pass ``reference_mask_indexing=False`` to mask every document with its own mask.  Differentiable: the
+        scores train the encoder (in-batch negatives)."""
         if query_vecs.dtype != document_vecs.dtype:
             document_vecs = document_vecs.to(query_vecs.dtype)
-        return interaction.maxsim_allpairs(query_vecs, query_mask, document_vecs, document_mask,
-                                           reference_mask_indexing=reference_mask_indexing)
+        return autograd.maxsim_allpairs(query_vecs, query_mask, document_vecs, document_mask,
+                                        reference_mask_indexing=reference_mask_indexing)
 
     def get_param_stats(self):
         return "ColBERT: / "
