@@ -47,6 +47,12 @@ extern "C" {
 #define MMB200_BF16 1
 #define MMB200_F32 2
 #define MMB200_F32_SPLIT16 3 /* mmb200_flat_ip_topk only: fp32 vectors held as fp16 hi / lo halves (see there) */
+/* OCP E4M3 "fn" (torch.float8_e4m3fn: max +-448, no infinity), one byte per value.  Accepted by mmb200_flat_ip_topk,
+ * mmb200_ivf_search_gather (and mmb200_ivf_workspace_bytes) and mmb200_maxsim_store_fwd, with both operands in it and
+ * 128 <= dim <= 1024, dim % 128 == 0.  The products run on the FP8 tensor cores with fp32 accumulation and the
+ * results are the plain sums of products of the stored values: with values stored as e4m3(x * 2^s), the caller
+ * multiplies a score by 2^-(s_query + s_store) to return to the unscaled domain (exact; void scores stay as they are). */
+#define MMB200_F8E4M3 4
 
 /* element types of mask tensors (nonzero = real token, zero = padding) */
 #define MMB200_MASK_NONE 0
@@ -147,7 +153,10 @@ MMB200_API int mmb200_maxsim_fwd_host(const void* q_host, const void* d_host, co
  * q [n_q, Lq, dim]; pair_q / pair_d [n_pairs] int32; pair_d[p] < 0 skips the pair (nothing is fetched) and, like a
  * passage without rows, scores -inf.  dtype / impl as mmb200_maxsim_fwd (AUTO picks the kernel it would pick for
  * the padded [n_docs, max_doc_len, dim] layout; scores are bit-identical to that layout with masks).  The tensor-core
- * kernels address the store with the passage's first row as the TMA row coordinate: n_rows < 2^31 - 1024. */
+ * kernels address the store with the passage's first row as the TMA row coordinate: n_rows < 2^31 - 1024.
+ * dtype MMB200_F8E4M3 (q and store): the documents-on-M tensor-core kernel only (impl AUTO or
+ * MMB200_IMPL_TCGEN05_DOCM; any other impl is MMB200_ERR_UNSUPPORTED), 1 <= Lq <= 128, dim % 128 == 0,
+ * 128 <= dim <= 1024 (outside: MMB200_ERR_INVALID); scores in the scaled domain (see MMB200_F8E4M3). */
 MMB200_API int mmb200_maxsim_store_fwd(const void* q, const void* store, const int64_t* doc_offsets,
                                        const int32_t* pair_q, const int32_t* pair_d, float* out, int64_t n_q,
                                        int64_t n_rows, int64_t n_docs, int64_t n_pairs, int32_t Lq, int32_t max_doc_len,
@@ -330,6 +339,8 @@ MMB200_API int mmb200_tkl_bwd(const float* q, const void* q_mask, const float* c
  *          tie order unspecified); when n_pass < k the tail is (-3.4028235e38, -1) as in faiss.
  * workspace: device scratch of at least mmb200_flat_ip_workspace_bytes(nq, n_pass, k) bytes.
  * 1 <= k <= 1024 (k <= 256: 1024-entry candidate lists per query row; larger k: 2048-entry lists).
+ * dtype MMB200_F8E4M3: queries and passages [., dim] e4m3, dim % 128 == 0, 128 <= dim <= 1024 (outside:
+ *          MMB200_ERR_INVALID); scores in the scaled domain (see MMB200_F8E4M3).
  * ------------------------------------------------------------------------------------------ */
 MMB200_API int64_t mmb200_flat_ip_workspace_bytes(int64_t nq, int64_t n_pass, int32_t k);
 /* The work decomposition mmb200_flat_ip_topk uses on a device with `sm_count` SMs (pure host arithmetic, no device
@@ -394,7 +405,9 @@ MMB200_API int mmb200_ivf_search(const void* queries, const void* rows, const in
  * entry in [0, n_rows); ids [n_rows] are indexed by row, not by list position.  Every other argument, the result and
  * the envelope are those of mmb200_ivf_search, including the workspace (mmb200_ivf_workspace_bytes).  This lets one
  * passage-ordered copy of the rows (ColBERT's token store) serve an inverted-file scan and per-passage scoring: the
- * scan gathers each tile's rows with 16-byte cp.async copies instead of one TMA box. */
+ * scan gathers each tile's rows with 16-byte cp.async copies instead of one TMA box.
+ * dtype MMB200_F8E4M3 (queries and rows e4m3, dim % 128 == 0, 128 <= dim <= 1024) is accepted here and by
+ * mmb200_ivf_workspace_bytes, not by mmb200_ivf_search; scores in the scaled domain (see MMB200_F8E4M3). */
 MMB200_API int mmb200_ivf_search_gather(const void* queries, const void* rows, const int64_t* ids,
                                         const int64_t* row_index, const int64_t* list_offsets, const int64_t* probes,
                                         float* out_scores, int64_t* out_ids, void* workspace, int64_t workspace_bytes,

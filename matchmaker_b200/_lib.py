@@ -16,7 +16,7 @@ LIB_PATH = os.environ.get("MMB200_LIB") or os.path.join(_HERE, "csrc", "libmatch
 
 OK = 0
 ERR_INVALID, ERR_CUDA, ERR_UNSUPPORTED = -1, -2, -3
-F16, BF16, F32, F32_SPLIT16 = 0, 1, 2, 3
+F16, BF16, F32, F32_SPLIT16, F8E4M3 = 0, 1, 2, 3, 4
 MASK_NONE, MASK_U8, MASK_I32, MASK_I64, MASK_F32 = 0, 1, 2, 3, 4
 IMPL_AUTO, IMPL_SIMT, IMPL_TCGEN05, IMPL_TCGEN05_DOCM, IMPL_TCGEN05_RAGGED = 0, 1, 2, 3, 4
 

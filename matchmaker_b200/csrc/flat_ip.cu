@@ -26,6 +26,7 @@
 // (arithmetic intensity ~ nq flops per passage byte).
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+#include <cuda_fp8.h>
 
 #include <algorithm>
 #include <cmath>
@@ -230,6 +231,10 @@ template <>
 __device__ __forceinline__ void wgmma_n128<__nv_bfloat16>(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) {
   wgmma_m64n128k16_bf16(d, a, b, acc);
 }
+template <>
+__device__ __forceinline__ void wgmma_n128<__nv_fp8_e4m3>(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) {
+  wgmma_m64n128k32_e4m3(d, a, b, acc);
+}
 
 // IVF = true: the probed-list scan of mmb200_ivf_search.  A work item is (list, chunk of <= BM probing queries) from
 // V.items; the query tile is the chunk's rows of the pre-gathered queries (TMA cannot gather rows), the passage tiles
@@ -264,6 +269,7 @@ __device__ __forceinline__ void flat_ip_tc_body(const CUtensorMap& tmap_q, const
   constexpr int kCap = 32 * EPL;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int kblocks = P.kblocks;
+  constexpr int kKbElems = 128 / (int)sizeof(T);   // elements of a k-block: one 128-byte swizzled row
   const int n_qgroups = (P.n_qblocks + CL - 1) / CL;   // CL consecutive query blocks per cluster work item
   const int n_items = IVF ? *V.n_items : n_qgroups * P.n_ranges;
   const int rank = CL > 1 ? (int)cluster_ctarank() : 0;
@@ -311,7 +317,7 @@ __device__ __forceinline__ void flat_ip_tc_body(const CUtensorMap& tmap_q, const
             uint8_t* st = smem + (size_t)stage * kStageBytes;
             if (warp == 8 && elect_one_sync()) {
               mbar_arrive_expect_tx(&S->full[stage], (uint32_t)kABytes);
-              tma_load_2d(&tmap_q, st, &S->full[stage], kb * 64, it.y, kEvictLast);
+              tma_load_2d(&tmap_q, st, &S->full[stage], kb * kKbElems, it.y, kEvictLast);
             }
             uint8_t* dst = st + kABytes + p * 128;
             const uint16_t* tab = rtab + ((kb * 64) << RB);
@@ -364,12 +370,12 @@ __device__ __forceinline__ void flat_ip_tc_body(const CUtensorMap& tmap_q, const
           if (elect_one_sync()) {
             mbar_arrive_expect_tx(&S->full[stage], (uint32_t)(GATHER ? kABytes : kStageBytes));
             const int kbp = kb < P.kb_wrap ? kb : kb - P.kb_wrap;   // fp32-split storage: [q_hi|q_lo|q_hi] x [p_hi|p_hi|p_lo]
-            tma_load_2d(&tmap_q, st, &S->full[stage], kb * 64, qrow0, kEvictLast);
+            tma_load_2d(&tmap_q, st, &S->full[stage], kb * kKbElems, qrow0, kEvictLast);
             if constexpr (!GATHER) {
               if (CL == 1)
-                tma_load_2d(tmap_p, st + kABytes, &S->full[stage], kbp * 64, prow0 + t * BN, kEvictFirst);
+                tma_load_2d(tmap_p, st + kABytes, &S->full[stage], kbp * kKbElems, prow0 + t * BN, kEvictFirst);
               else  // this CTA's slice of the passage tile, written into every CTA of the cluster
-                tma_load_2d_multicast(tmap_p, st + kABytes + rank * (kBBytes / CL), &S->full[stage], kbp * 64,
+                tma_load_2d_multicast(tmap_p, st + kABytes + rank * (kBBytes / CL), &S->full[stage], kbp * kKbElems,
                                       t * BN + rank * (BN / CL), kAllCtas, kEvictFirst);
             }
           }
@@ -635,6 +641,22 @@ flat_ip_tc_residual_kernel(const __grid_constant__ CUtensorMap tmap_q, FipParams
   flat_ip_tc_body<__half, 1, EPL, true, true, RB>(tmap_q, nullptr, P, V, G, R);
 }
 
+// E4M3 queries and rows (MMB200_F8E4M3): the same bodies, with 128-element k-blocks and wgmma m64n128k32.  Kernels of
+// their own name, not instantiations of the two above: those names stand for the HGMMA (16-bit) kernels, while these
+// emit QGMMA.
+template <int CL, int EPL>
+__global__ void __launch_bounds__(kThreads, 1)
+flat_ip_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_p, FipParams P,
+                      IvfParams V) {
+  flat_ip_tc_body<__nv_fp8_e4m3, CL, EPL, false, false>(tmap_q, &tmap_p, P, V, GatherParams{});
+}
+
+template <int EPL>
+__global__ void __launch_bounds__(kThreads, 1)
+flat_ip_tc_gather_fp8_kernel(const __grid_constant__ CUtensorMap tmap_q, FipParams P, IvfParams V, GatherParams G) {
+  flat_ip_tc_body<__nv_fp8_e4m3, 1, EPL, true, true>(tmap_q, nullptr, P, V, G);
+}
+
 
 // ---------------------------------------------------------------------------------------------
 // merge: per query, sort L candidates by (score desc, id asc), emit the first k.
@@ -890,7 +912,7 @@ struct IvfLayout {
 };
 
 // slot = per-(query, probe) candidates: a list of len rows yields at most min(k, len) of them
-IvfLayout ivf_layout(int64_t nq, int nprobe, int64_t nlist, int64_t max_list_len, int qcols, int k, int sm_count) {
+IvfLayout ivf_layout(int64_t nq, int nprobe, int64_t nlist, int64_t max_list_len, int qbytes, int k, int sm_count) {
   IvfLayout L{};
   L.grid = sm_count;
   L.n_pairs = nq * nprobe;
@@ -902,7 +924,7 @@ IvfLayout ivf_layout(int64_t nq, int nprobe, int64_t nlist, int64_t max_list_len
   L.lists = take((size_t)L.grid * BM * 32 * epl_for_k(k) * sizeof(uint2));
   L.cand_s = take((size_t)L.n_pairs * L.kslot * sizeof(float));
   L.cand_i = take((size_t)L.n_pairs * L.kslot * sizeof(int64_t));
-  L.gathered = take((size_t)L.n_pairs * qcols * 2);
+  L.gathered = take((size_t)L.n_pairs * qbytes);
   L.pair = take((size_t)L.n_pairs * sizeof(int32_t));
   L.cnt = take((size_t)nlist * sizeof(int));
   L.fill = take((size_t)nlist * sizeof(int));
@@ -945,9 +967,11 @@ extern "C" int mmb200_flat_ip_topk(const void* queries, const void* passages, co
   using namespace mmb;
   MMB_REQUIRE(nq >= 0 && n_pass > 0, "need at least one passage");
   MMB_REQUIRE(k >= 1 && k <= kMaxK, "fused top-k supports 1 <= k <= 1024");
-  MMB_REQUIRE(dtype == MMB200_F16 || dtype == MMB200_BF16 || dtype == MMB200_F32_SPLIT16,
-              "passage storage must be fp16, bf16 or the fp16 hi/lo split of fp32 (MMB200_F32_SPLIT16)");
+  MMB_REQUIRE(dtype == MMB200_F16 || dtype == MMB200_BF16 || dtype == MMB200_F32_SPLIT16 || dtype == MMB200_F8E4M3,
+              "passage storage must be fp16, bf16, e4m3 or the fp16 hi/lo split of fp32 (MMB200_F32_SPLIT16)");
   MMB_REQUIRE(dim % 64 == 0 && dim >= 64, "vector dim must be a multiple of 64");
+  const bool fp8 = dtype == MMB200_F8E4M3;
+  MMB_REQUIRE(!fp8 || (dim % 128 == 0 && dim >= 128 && dim <= 1024), "e4m3 vectors need dim % 128 == 0, 128 <= dim <= 1024");
   MMB_REQUIRE(n_pass < (1ll << 32) - 512, "at most 2^32 passages per shard");
   if (nq == 0) return MMB200_OK;   // an empty batch: nothing to read or write (its tensors may be null), no device needed
   MMB_REQUIRE(queries && passages && out_scores && out_ids && workspace, "null pointer");
@@ -959,13 +983,16 @@ extern "C" int mmb200_flat_ip_topk(const void* queries, const void* passages, co
   const Plan pl = make_plan(nq, n_pass, k, dev.sm_count);
   MMB_REQUIRE((size_t)workspace_bytes_given >= total_workspace_bytes(nq, n_pass, k, dev.sm_count),
               "workspace too small (see mmb200_flat_ip_workspace_bytes)");
-  const CUtensorMapDataType tdt = dtype == MMB200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  const CUtensorMapDataType tdt = fp8                  ? CU_TENSOR_MAP_DATA_TYPE_UINT8
+                                  : dtype == MMB200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                                         : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   const uint64_t q_cols = split ? 3ull * dim : (uint64_t)dim, p_cols = split ? 2ull * dim : (uint64_t)dim;
+  const uint32_t esize = fp8 ? 1u : 2u, kbe = 128u / esize;   // bytes per element, elements per 128-byte k-block
   CUtensorMap tq;
   {
     const uint64_t dims[2] = {q_cols, (uint64_t)nq};
-    const uint64_t strides[1] = {q_cols * 2};
-    const uint32_t box[2] = {64, BM};
+    const uint64_t strides[1] = {q_cols * esize};
+    const uint32_t box[2] = {kbe, BM};
     if (int rc = encode_tensor_map(&tq, tdt, 2, queries, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B,
                                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B))
       return rc;
@@ -987,13 +1014,13 @@ extern "C" int mmb200_flat_ip_topk(const void* queries, const void* passages, co
     P.cand_ids = reinterpret_cast<int64_t*>(w);
     P.ids = pass_ids; P.id_base = pass_id_base; P.nq = nq; P.n_pass = n_rows; P.dim = dim; P.k = k; P.kpad = pp.kpad;
     P.n_qblocks = pp.n_qblocks; P.n_ranges = pp.n_ranges; P.tiles_per_range = pp.tiles_per_range; P.n_tiles = pp.n_tiles;
-    P.kblocks = (int32_t)(q_cols / 64);
+    P.kblocks = (int32_t)(q_cols / kbe);
     P.kb_wrap = split ? dim / 64 : P.kblocks;
     CUtensorMap tp;
     {
       const uint64_t dims[2] = {p_cols, (uint64_t)n_rows};
       const uint64_t strides[1] = {row_pitch};
-      const uint32_t box[2] = {64, (uint32_t)(BN / pp.cl)};   // each CTA of a cluster fetches (and multicasts) its slice
+      const uint32_t box[2] = {kbe, (uint32_t)(BN / pp.cl)};   // each CTA of a cluster fetches (and multicasts) its slice
       if (int rc = encode_tensor_map(&tp, tdt, 2, passages, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B,
                                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B))
         return rc;
@@ -1024,14 +1051,21 @@ extern "C" int mmb200_flat_ip_topk(const void* queries, const void* passages, co
              : pp.cl == 2 ? launch(flat_ip_tc_kernel<T, 2, E>)
                           : launch(flat_ip_tc_kernel<T, 4, E>);
     };
+    auto fp8_by_cluster = [&](auto epl) -> int {
+      constexpr int E = decltype(epl)::value;
+      return pp.cl == 1   ? launch(flat_ip_tc_fp8_kernel<1, E>)
+             : pp.cl == 2 ? launch(flat_ip_tc_fp8_kernel<2, E>)
+                          : launch(flat_ip_tc_fp8_kernel<4, E>);
+    };
     using E32 = std::integral_constant<int, 32>;
     using E64 = std::integral_constant<int, 64>;
+    if (fp8) return epl_for_k(k) == 32 ? fp8_by_cluster(E32{}) : fp8_by_cluster(E64{});
     if (dtype == MMB200_BF16) return epl_for_k(k) == 32 ? by_cluster(__nv_bfloat16{}, E32{}) : by_cluster(__nv_bfloat16{}, E64{});
     return epl_for_k(k) == 32 ? by_cluster(__half{}, E32{}) : by_cluster(__half{}, E64{});
   };
 
   FipParams P{};
-  if (int rc = run_pass(pl, n_pass, p_cols * 2, ids, id_base, &P)) return rc;
+  if (int rc = run_pass(pl, n_pass, p_cols * esize, ids, id_base, &P)) return rc;
   return launch_merge(P.cand_scores, P.cand_ids, nq, pl.n_ranges * pl.kpad, k, out_scores, out_ids, dev, stream);
 }
 
@@ -1069,11 +1103,12 @@ extern "C" int64_t mmb200_ivf_workspace_bytes(int64_t nq, int32_t nprobe, int64_
   if (nq <= 0 || nprobe <= 0 || nprobe > kIvfMaxProbe || nlist <= 0 || k <= 0 || k > kMaxK || dim <= 0 || dim % 64 ||
       nq * nprobe >= (1ll << 31) - BM)
     return 0;
-  if (dtype != MMB200_F16 && dtype != MMB200_BF16 && dtype != MMB200_F32_SPLIT16) return 0;
+  if (dtype != MMB200_F16 && dtype != MMB200_BF16 && dtype != MMB200_F32_SPLIT16 && dtype != MMB200_F8E4M3) return 0;
+  if (dtype == MMB200_F8E4M3 && (dim % 128 || dim < 128 || dim > 1024)) return 0;
   DeviceInfo dev;
   if (current_device_info(&dev)) return -1;
-  const int qcols = dtype == MMB200_F32_SPLIT16 ? 3 * dim : dim;
-  return (int64_t)ivf_layout(nq, nprobe, nlist, max_list_len, qcols, k, dev.sm_count).total;
+  const int qbytes = dtype == MMB200_F32_SPLIT16 ? 6 * dim : dtype == MMB200_F8E4M3 ? dim : 2 * dim;
+  return (int64_t)ivf_layout(nq, nprobe, nlist, max_list_len, qbytes, k, dev.sm_count).total;
 }
 
 namespace mmb {
@@ -1089,9 +1124,13 @@ int ivf_search_impl(const void* queries, const void* rows, const int64_t* ids, c
   MMB_REQUIRE(nq > 0 && nlist > 0 && n_rows > 0, "need at least one query, one list and one row");
   MMB_REQUIRE(k >= 1 && k <= kMaxK, "fused top-k supports 1 <= k <= 1024");
   MMB_REQUIRE(nprobe >= 1 && nprobe <= kIvfMaxProbe, "1 <= nprobe <= 1024");
-  MMB_REQUIRE(dtype == MMB200_F16 || dtype == MMB200_BF16 || dtype == MMB200_F32_SPLIT16,
-              "list storage must be fp16, bf16 or the fp16 hi/lo split of fp32 (MMB200_F32_SPLIT16)");
+  MMB_REQUIRE(dtype == MMB200_F16 || dtype == MMB200_BF16 || dtype == MMB200_F32_SPLIT16 ||
+                  (dtype == MMB200_F8E4M3 && row_index && !R),
+              "list storage must be fp16, bf16 or the fp16 hi/lo split of fp32 (MMB200_F32_SPLIT16); e4m3 rows are "
+              "scanned in gather mode only");
   MMB_REQUIRE(dim % 64 == 0 && dim >= 64, "vector dim must be a multiple of 64");
+  const bool fp8 = dtype == MMB200_F8E4M3;
+  MMB_REQUIRE(!fp8 || (dim % 128 == 0 && dim >= 128 && dim <= 1024), "e4m3 vectors need dim % 128 == 0, 128 <= dim <= 1024");
   MMB_REQUIRE(n_rows < (1ll << 31) - BN, "at most 2^31 - 128 rows per shard");
   MMB_REQUIRE(max_list_len >= 0 && max_list_len <= n_rows, "max_list_len must bound the list lengths");
   MMB_REQUIRE(nq * nprobe < (1ll << 31) - BM, "nq * nprobe must stay below 2^31 (search the queries in batches)");
@@ -1101,7 +1140,8 @@ int ivf_search_impl(const void* queries, const void* rows, const int64_t* ids, c
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const bool split = dtype == MMB200_F32_SPLIT16;
   const int qcols = split ? 3 * dim : dim, pcols = split ? 2 * dim : dim;
-  const IvfLayout L = ivf_layout(nq, nprobe, nlist, max_list_len, qcols, k, dev.sm_count);
+  const int esize = fp8 ? 1 : 2, kbe = 128 / esize;   // bytes per element, elements per 128-byte k-block
+  const IvfLayout L = ivf_layout(nq, nprobe, nlist, max_list_len, qcols * esize, k, dev.sm_count);
   MMB_REQUIRE((size_t)workspace_bytes_given >= L.total, "workspace too small (see mmb200_ivf_workspace_bytes)");
   uint8_t* w = static_cast<uint8_t*>(workspace);
   int* cnt = reinterpret_cast<int*>(w + L.cnt);
@@ -1119,7 +1159,7 @@ int ivf_search_impl(const void* queries, const void* rows, const int64_t* ids, c
   ivf_count_kernel<<<g, 256, 0, stream>>>(probes, L.n_pairs, nlist, cnt);
   ivf_scan_kernel<<<1, 1024, 0, stream>>>(cnt, nlist, row_base, item_base, n_items);
   ivf_gather_kernel<<<std::max(1, std::min(dev.sm_count * 8, (int)((L.n_pairs + 7) / 8))), 256, 0, stream>>>(
-      probes, L.n_pairs, nlist, nprobe, row_base, fill, static_cast<const uint4*>(queries), qcols * 2 / 16, gathered,
+      probes, L.n_pairs, nlist, nprobe, row_base, fill, static_cast<const uint4*>(queries), qcols * esize / 16, gathered,
       pair_of_row, reinterpret_cast<float*>(w + L.cand_s), reinterpret_cast<int64_t*>(w + L.cand_i), L.kslot);
   ivf_items_kernel<<<std::max(1, std::min(dev.sm_count * 4, (int)((nlist + 255) / 256))), 256, 0, stream>>>(
       cnt, nlist, row_base, item_base, items);
@@ -1127,13 +1167,15 @@ int ivf_search_impl(const void* queries, const void* rows, const int64_t* ids, c
   fill_u32<<<64, 256, 0, stream>>>(tau_glob, nq, kKeyNegInf);
   MMB_CHECK_CUDA(cudaGetLastError());
 
-  const CUtensorMapDataType tdt = dtype == MMB200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  const CUtensorMapDataType tdt = fp8                  ? CU_TENSOR_MAP_DATA_TYPE_UINT8
+                                  : dtype == MMB200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                                         : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   const bool gather = row_index != nullptr;
   CUtensorMap tq, tp;
   {
     const uint64_t dims[2] = {(uint64_t)qcols, (uint64_t)L.n_pairs};
-    const uint64_t strides[1] = {(uint64_t)qcols * 2};
-    const uint32_t box[2] = {64, BM};
+    const uint64_t strides[1] = {(uint64_t)qcols * esize};
+    const uint32_t box[2] = {(uint32_t)kbe, BM};
     if (int rc = encode_tensor_map(&tq, tdt, 2, gathered, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B,
                                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B))
       return rc;
@@ -1148,7 +1190,7 @@ int ivf_search_impl(const void* queries, const void* rows, const int64_t* ids, c
   }
   FipParams P{};
   P.ids = ids; P.id_base = 0; P.nq = nq; P.n_pass = n_rows; P.dim = dim; P.k = k; P.kpad = L.kslot;
-  P.kblocks = qcols / 64;
+  P.kblocks = qcols / kbe;
   P.kb_wrap = split ? dim / 64 : P.kblocks;
   P.n_qblocks = 0; P.n_ranges = 1; P.tiles_per_range = 0; P.n_tiles = 0;
   P.tau_glob = tau_glob;
@@ -1165,7 +1207,7 @@ int ivf_search_impl(const void* queries, const void* rows, const int64_t* ids, c
     MMB_CHECK_CUDA(cudaGetLastError());
     return MMB200_OK;
   };
-  const GatherParams G{static_cast<const uint8_t*>(rows), row_index, (int64_t)pcols * 2};
+  const GatherParams G{static_cast<const uint8_t*>(rows), row_index, (int64_t)pcols * esize};
   auto launch_gather = [&](auto kernel) -> int {
     MMB_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kernel<<<L.grid, kThreads, smem, stream>>>(tq, P, V, G);
@@ -1186,7 +1228,9 @@ int ivf_search_impl(const void* queries, const void* rows, const int64_t* ids, c
     else
       rc = e32 ? launch_residual(flat_ip_tc_residual_kernel<32, 2>) : launch_residual(flat_ip_tc_residual_kernel<64, 2>);
   } else if (gather) {
-    if (dtype == MMB200_BF16)
+    if (fp8)
+      rc = e32 ? launch_gather(flat_ip_tc_gather_fp8_kernel<32>) : launch_gather(flat_ip_tc_gather_fp8_kernel<64>);
+    else if (dtype == MMB200_BF16)
       rc = e32 ? launch_gather(flat_ip_tc_gather_kernel<__nv_bfloat16, 32>) : launch_gather(flat_ip_tc_gather_kernel<__nv_bfloat16, 64>);
     else
       rc = e32 ? launch_gather(flat_ip_tc_gather_kernel<__half, 32>) : launch_gather(flat_ip_tc_gather_kernel<__half, 64>);

@@ -34,8 +34,10 @@
 // -1000 fill (there is no mask).
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
+#include <cuda_fp8.h>
 
 #include <algorithm>
+#include <type_traits>
 #include <vector>
 
 #include "device_util.cuh"
@@ -183,6 +185,10 @@ template <>
 __device__ __forceinline__ void wgmma_n32<__nv_bfloat16>(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc) {
   wgmma_m64n32k16_bf16(d, a, b, acc);
 }
+template <>
+__device__ __forceinline__ void wgmma_n32<__nv_fp8_e4m3>(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc) {
+  wgmma_m64n32k32_e4m3(d, a, b, acc);
+}
 
 // NC = npad / 32 accumulator chunks of 16 registers per thread.
 //
@@ -279,19 +285,29 @@ __device__ __forceinline__ void maxsim_tc_body(const CUtensorMap& tmap_q, const 
     }
   } else if (warp == 0) {
     // ------------------------------- TMA producer -------------------------------
-    if (lane == 0) {
+    // The e4m3 kernel walks the loop with the whole warp and issues from one elected lane, so its TMA operands stay
+    // uniform (no ELECT / R2UR waterfall loop around the loads, ptx.cuh); the 16-bit kernels keep their lane-0 loop.
+    constexpr bool kWarpIssue = std::is_same<T, __nv_fp8_e4m3>::value;
+    if (kWarpIssue || lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       int64_t prev_q = -1;
       uint32_t qcount = 0;
+      auto issuer = [&]() -> bool {
+        if constexpr (kWarpIssue) return elect_one_sync();
+        else return true;
+      };
       for (int64_t p = p_begin; p < p_end; ++p) {
         const int64_t qi = pair_query(P, p), di = pair_doc(P, p);
         if (qi != prev_q) {
           const uint32_t slot = L.qslots == 2 ? (qcount & 1u) : 0u, use = L.qslots == 2 ? (qcount >> 1) : qcount;
           mbar_wait(&S->qempty[slot], (use & 1u) ^ 1u);
-          mbar_arrive_expect_tx(&S->qfull[slot], (uint32_t)L.qslot_bytes);
-          tma_load_4d(&tmap_q, q_base + (size_t)slot * L.qslot_bytes, &S->qfull[slot], 0, 0, 0, (int)qi,
-                      kEvictLast);
+          if (issuer()) {
+            mbar_arrive_expect_tx(&S->qfull[slot], (uint32_t)L.qslot_bytes);
+            tma_load_4d(&tmap_q, q_base + (size_t)slot * L.qslot_bytes, &S->qfull[slot], 0, 0, 0, (int)qi,
+                        kEvictLast);
+          }
+          if constexpr (kWarpIssue) __syncwarp();
           ++qcount;
           prev_q = qi;
         }
@@ -303,13 +319,16 @@ __device__ __forceinline__ void maxsim_tc_body(const CUtensorMap& tmap_q, const 
         for (int t = 0; t < L.tiles; ++t) {
           for (int ks = 0; ks < ksteps; ++ks) {
             mbar_wait(&S->empty[stage], phase ^ 1u);
-            if (t * kTileRows < nrows) {
-              mbar_arrive_expect_tx(&S->full[stage], (uint32_t)kStageBytes);
-              tma_load_4d(tmap_d, stage_base + (size_t)stage * kStageBytes, &S->full[stage], 0, (int)row0 + t * kTileRows,
-                          ks * KBS, dcoord, kEvictFirst);
-            } else {
-              mbar_arrive(&S->full[stage]);
+            if (issuer()) {
+              if (t * kTileRows < nrows) {
+                mbar_arrive_expect_tx(&S->full[stage], (uint32_t)kStageBytes);
+                tma_load_4d(tmap_d, stage_base + (size_t)stage * kStageBytes, &S->full[stage], 0,
+                            (int)row0 + t * kTileRows, ks * KBS, dcoord, kEvictFirst);
+              } else {
+                mbar_arrive(&S->full[stage]);
+              }
             }
+            if constexpr (kWarpIssue) __syncwarp();
             if (++stage == L.stages) { stage = 0; phase ^= 1u; }
           }
         }
@@ -369,7 +388,7 @@ __device__ __forceinline__ void maxsim_tc_body(const CUtensorMap& tmap_q, const 
             const uint32_t a_kb = aaddr + kb * kKBlockBytes;
             const uint32_t b_kb = qaddr + (uint32_t)((ks * KBS + kb) * L.npad * 128);
 #pragma unroll
-            for (int k = 0; k < 4; ++k) {  // 64 / wgmma K (16)
+            for (int k = 0; k < 4; ++k) {  // 128 bytes / 32 bytes per wgmma K step (k16 of 16-bit, k32 of e4m3)
               const uint64_t adesc = make_wgmma_sw128_desc(a_kb + k * 32);
 #pragma unroll
               for (int h = 0; h < NC; ++h)
@@ -452,6 +471,24 @@ maxsim_tc_residual_kernel(const __grid_constant__ CUtensorMap tmap_q, MaxsimPara
   maxsim_tc_body<__half, KBS, NC, RB>(tmap_q, nullptr, P, L, R, list_ids);
 }
 
+// Store-mode max-sim over an E4M3 store with E4M3 queries (mmb200_maxsim_store_fwd, MMB200_F8E4M3): the same body with
+// 128-element k-blocks and wgmma m64n32k32.  A name of its own: maxsim_tc_kernel stands for the HGMMA (16-bit) kernel.
+template <int KBS, int NC>
+__global__ void __launch_bounds__(kTcThreads, 1)
+maxsim_tc_fp8_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_d,
+                     MaxsimParams P, TcLaunch L) {
+  maxsim_tc_body<__nv_fp8_e4m3, KBS, NC>(tmap_q, &tmap_d, P, L);
+}
+
+template <typename T, int KBS, int NC>
+struct TcKernel {
+  static constexpr auto fn = maxsim_tc_kernel<T, KBS, NC>;
+};
+template <int KBS, int NC>
+struct TcKernel<__nv_fp8_e4m3, KBS, NC> {
+  static constexpr auto fn = maxsim_tc_fp8_kernel<KBS, NC>;
+};
+
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
@@ -470,9 +507,9 @@ static int launch_tc_nc(int nc, int grid, size_t smem_bytes, cudaStream_t stream
                         const MaxsimParams& P, const TcLaunch& L) {
 #define MMB_TC_CASE(N)                                                                                                  \
   case N:                                                                                                               \
-    MMB_CHECK_CUDA(cudaFuncSetAttribute(maxsim_tc_kernel<T, KBS, N>, cudaFuncAttributeMaxDynamicSharedMemorySize,       \
+    MMB_CHECK_CUDA(cudaFuncSetAttribute(TcKernel<T, KBS, N>::fn, cudaFuncAttributeMaxDynamicSharedMemorySize,          \
                                         (int)smem_bytes));                                                              \
-    maxsim_tc_kernel<T, KBS, N><<<grid, kTcThreads, smem_bytes, stream>>>(tq, td, P, L);                                \
+    TcKernel<T, KBS, N>::fn<<<grid, kTcThreads, smem_bytes, stream>>>(tq, td, P, L);                                    \
     break;
   switch (nc) {
     MMB_TC_CASE(1)
@@ -488,11 +525,11 @@ static int launch_tc_nc(int nc, int grid, size_t smem_bytes, cudaStream_t stream
   return MMB200_OK;
 }
 
-// Tile plan of the documents-on-M kernel; `extra` bytes of shared memory follow TcShared.
-static int plan_tc(const MaxsimParams& P, const DeviceInfo& dev, int extra, TcLaunch* out, size_t* smem_out) {
+// Tile plan of the documents-on-M kernel over elements of `esize` bytes; `extra` bytes of shared memory follow TcShared.
+static int plan_tc(const MaxsimParams& P, const DeviceInfo& dev, int extra, int esize, TcLaunch* out, size_t* smem_out) {
   TcLaunch L;
   L.npad = ((P.Lq + 31) / 32) * 32;
-  L.kblocks = P.dim / 64;
+  L.kblocks = P.dim * esize / 128;
   L.kbs = (L.kblocks % 2 == 0) ? 2 : 1;
   L.tiles = (P.Ld + kTileRows - 1) / kTileRows;
   L.qslot_bytes = L.kblocks * L.npad * 128;
@@ -514,11 +551,13 @@ static int plan_tc(const MaxsimParams& P, const DeviceInfo& dev, int extra, TcLa
   return MMB200_OK;
 }
 
-// TMA map of the query tiles of the documents-on-M kernel: [NPAD rows][64 halfs] per k-block, all k-blocks of a query.
-static int encode_tc_query_map(CUtensorMap* tq, const MaxsimParams& P, const TcLaunch& L, CUtensorMapDataType tdt) {
-  const uint64_t dims[4] = {64, (uint64_t)P.Lq, (uint64_t)L.kblocks, (uint64_t)P.n_q};
-  const uint64_t strides[3] = {(uint64_t)P.dim * 2, 128, (uint64_t)P.Lq * P.dim * 2};
-  const uint32_t box[4] = {64, (uint32_t)L.npad, (uint32_t)L.kblocks, 1};
+// TMA map of the query tiles of the documents-on-M kernel: [NPAD rows][128 bytes] per k-block, all k-blocks of a query.
+static int encode_tc_query_map(CUtensorMap* tq, const MaxsimParams& P, const TcLaunch& L, CUtensorMapDataType tdt,
+                               int esize) {
+  const uint32_t kbe = 128 / esize;
+  const uint64_t dims[4] = {kbe, (uint64_t)P.Lq, (uint64_t)L.kblocks, (uint64_t)P.n_q};
+  const uint64_t strides[3] = {(uint64_t)P.dim * esize, 128, (uint64_t)P.Lq * P.dim * esize};
+  const uint32_t box[4] = {kbe, (uint32_t)L.npad, (uint32_t)L.kblocks, 1};
   return encode_tensor_map(tq, tdt, 4, P.q, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B,
                            CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
 }
@@ -526,23 +565,30 @@ static int encode_tc_query_map(CUtensorMap* tq, const MaxsimParams& P, const TcL
 static int launch_tc(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cudaStream_t stream) {
   TcLaunch L;
   size_t smem_bytes;
-  if (int rc = plan_tc(P, dev, 0, &L, &smem_bytes)) return rc;
-  const CUtensorMapDataType tdt = dtype == MMB200_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  const int esize = dtype == MMB200_F8E4M3 ? 1 : 2;
+  const uint32_t kbe = 128 / esize;
+  if (int rc = plan_tc(P, dev, 0, esize, &L, &smem_bytes)) return rc;
+  const CUtensorMapDataType tdt = dtype == MMB200_F16       ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
+                                  : dtype == MMB200_F8E4M3 ? CU_TENSOR_MAP_DATA_TYPE_UINT8
+                                                           : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   CUtensorMap tq, td;
-  if (int rc = encode_tc_query_map(&tq, P, L, tdt)) return rc;
+  if (int rc = encode_tc_query_map(&tq, P, L, tdt, esize)) return rc;
   {
     // store mode: the [n_rows, dim] store is one "document"; a passage's tile starts at its first row
     const uint64_t d_rows = P.doc_offsets ? (uint64_t)P.n_rows : (uint64_t)P.Ld;
     const uint64_t d_count = P.doc_offsets ? 1 : (uint64_t)P.n_d;
-    const uint64_t dims[4] = {64, d_rows, (uint64_t)L.kblocks, d_count};
-    const uint64_t strides[3] = {(uint64_t)P.dim * 2, 128, d_rows * P.dim * 2};
-    const uint32_t box[4] = {64, (uint32_t)kTileRows, (uint32_t)L.kbs, 1};
+    const uint64_t dims[4] = {kbe, d_rows, (uint64_t)L.kblocks, d_count};
+    const uint64_t strides[3] = {(uint64_t)P.dim * esize, 128, d_rows * P.dim * esize};
+    const uint32_t box[4] = {kbe, (uint32_t)kTileRows, (uint32_t)L.kbs, 1};
     if (int rc = encode_tensor_map(&td, tdt, 4, P.d, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B,
                                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B))
       return rc;
   }
   const int grid = (int)std::min<int64_t>(dev.sm_count, P.n_pairs);
   const int nc = L.npad / 32;
+  if (dtype == MMB200_F8E4M3)
+    return L.kbs == 2 ? launch_tc_nc<__nv_fp8_e4m3, 2>(nc, grid, smem_bytes, stream, tq, td, P, L)
+                      : launch_tc_nc<__nv_fp8_e4m3, 1>(nc, grid, smem_bytes, stream, tq, td, P, L);
   if (dtype == MMB200_F16)
     return L.kbs == 2 ? launch_tc_nc<__half, 2>(nc, grid, smem_bytes, stream, tq, td, P, L)
                       : launch_tc_nc<__half, 1>(nc, grid, smem_bytes, stream, tq, td, P, L);
@@ -595,6 +641,25 @@ int maxsim_fwd_device(const MaxsimParams& P, int dtype, int impl, cudaStream_t s
   return launch_tc(P, dtype, dev, stream);
 }
 
+// Store mode over an e4m3 store: only the documents-on-M kernel reads e4m3, so there is no kernel choice to make and
+// no SIMT kernel to fall back to.
+static int maxsim_store_fp8(const MaxsimParams& P, int impl, cudaStream_t stream) {
+  if (impl != MMB200_IMPL_AUTO && impl != MMB200_IMPL_TCGEN05_DOCM) {
+    set_error("e4m3 max-sim runs on the documents-on-M tensor-core kernel only (impl auto or tcgen05_docm)");
+    return MMB200_ERR_UNSUPPORTED;
+  }
+  MMB_REQUIRE(P.n_pairs >= 0 && P.n_q >= 0, "bad counts");
+  if (P.n_pairs == 0) return MMB200_OK;
+  MMB_REQUIRE(P.q && P.d && P.out, "null pointer: q, store, out must be non-null");
+  MMB_REQUIRE(P.n_q >= 1, "need at least one query");
+  MMB_REQUIRE(P.Lq >= 1 && P.Lq <= 128, "e4m3 max-sim needs 1 <= Lq <= 128");
+  MMB_REQUIRE(P.dim % 128 == 0 && P.dim >= 128 && P.dim <= 1024, "e4m3 max-sim needs dim % 128 == 0, 128 <= dim <= 1024");
+  MMB_REQUIRE(((reinterpret_cast<uintptr_t>(P.q) | reinterpret_cast<uintptr_t>(P.d)) & 15) == 0, "16-byte alignment");
+  DeviceInfo dev;
+  if (int rc = require_sm90(&dev)) return rc;
+  return launch_tc(P, MMB200_F8E4M3, dev, stream);
+}
+
 }  // namespace mmb
 
 extern "C" int mmb200_maxsim_fwd(const void* q, const void* d, const void* q_mask, const void* d_mask,
@@ -620,6 +685,7 @@ extern "C" int mmb200_maxsim_store_fwd(const void* q, const void* store, const i
   P.q = q; P.d = store; P.pair_q = pair_q; P.pair_d = pair_d; P.out = out; P.n_q = n_q; P.n_d = n_docs;
   P.n_pairs = n_pairs; P.Lq = Lq; P.Ld = max_doc_len; P.dim = dim;
   P.doc_offsets = doc_offsets; P.n_rows = n_rows;
+  if (dtype == MMB200_F8E4M3) return mmb::maxsim_store_fp8(P, impl, static_cast<cudaStream_t>(stream));
   return mmb::maxsim_fwd_device(P, dtype, impl, static_cast<cudaStream_t>(stream));
 }
 
@@ -673,9 +739,9 @@ extern "C" int mmb200_maxsim_store_residual_fwd(const void* q, const uint8_t* co
   P.Lq = Lq; P.Ld = max_doc_len; P.dim = dim; P.doc_offsets = doc_offsets; P.n_rows = n_rows;
   TcLaunch L;
   size_t smem_bytes;
-  if (int rc = plan_tc(P, dev, (dim << bits) * (int)sizeof(__half), &L, &smem_bytes)) return rc;
+  if (int rc = plan_tc(P, dev, (dim << bits) * (int)sizeof(__half), 2, &L, &smem_bytes)) return rc;
   CUtensorMap tq;
-  if (int rc = encode_tc_query_map(&tq, P, L, CU_TENSOR_MAP_DATA_TYPE_FLOAT16)) return rc;
+  if (int rc = encode_tc_query_map(&tq, P, L, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2)) return rc;
   const ResidualCodes R{codes, static_cast<const __half*>(base), static_cast<const __half*>(weight), bits};
   const int grid = (int)std::min<int64_t>(dev.sm_count, n_pairs);
   const int nc = L.npad / 32;

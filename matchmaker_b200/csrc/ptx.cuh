@@ -193,22 +193,26 @@ __device__ __forceinline__ void wgmma_fence_regs(float (&d)[N]) {
   MMB_REGS32 ", %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "                    \
              "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
 
-// 16-bit inputs, both operands from shared-memory descriptors (K-major)
-#define MMB_WGMMA_SS(N, TY, NR, REGS, PI, AI, BI, ...)                                                               \
-  __device__ __forceinline__ void wgmma_m64n##N##k16_##TY(float (&d)[NR], uint64_t adesc, uint64_t bdesc,              \
-                                                          uint32_t accumulate) {                                     \
+// Both operands from shared-memory descriptors (K-major).  16-bit inputs take K = 16 and the two transpose flags
+// (TNSP ", 0, 0"); e4m3 inputs take K = 32 and no transpose flags (8-bit wgmma reads K-major operands only), so a k32
+// e4m3 step advances the same 32 bytes along a 128-byte swizzled row as a k16 step of 16-bit data.
+#define MMB_WGMMA_SS(N, K, TY, TNSP, NR, REGS, PI, AI, BI, ...)                                                      \
+  __device__ __forceinline__ void wgmma_m64n##N##k##K##_##TY(float (&d)[NR], uint64_t adesc, uint64_t bdesc,           \
+                                                             uint32_t accumulate) {                                  \
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, " PI ", 0;\n\t"                                                 \
-                 "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32." #TY "." #TY " {" REGS "}, " AI ", " BI              \
-                 ", p, 1, 1, 0, 0;\n\t}"                                                                               \
+                 "wgmma.mma_async.sync.aligned.m64n" #N "k" #K ".f32." #TY "." #TY " {" REGS "}, " AI ", " BI          \
+                 ", p, 1, 1" TNSP ";\n\t}"                                                                             \
                  : __VA_ARGS__                                                                                       \
                  : "l"(adesc), "l"(bdesc), "r"(accumulate));                                                        \
   }
-MMB_WGMMA_SS(32, f16, 16, MMB_REGS16, "%18", "%16", "%17", MMB_ACC16(0))
-MMB_WGMMA_SS(32, bf16, 16, MMB_REGS16, "%18", "%16", "%17", MMB_ACC16(0))
-MMB_WGMMA_SS(64, f16, 32, MMB_REGS32, "%34", "%32", "%33", MMB_ACC16(0), MMB_ACC16(16))
-MMB_WGMMA_SS(64, bf16, 32, MMB_REGS32, "%34", "%32", "%33", MMB_ACC16(0), MMB_ACC16(16))
-MMB_WGMMA_SS(128, f16, 64, MMB_REGS64, "%66", "%64", "%65", MMB_ACC16(0), MMB_ACC16(16), MMB_ACC16(32), MMB_ACC16(48))
-MMB_WGMMA_SS(128, bf16, 64, MMB_REGS64, "%66", "%64", "%65", MMB_ACC16(0), MMB_ACC16(16), MMB_ACC16(32), MMB_ACC16(48))
+MMB_WGMMA_SS(32, 16, f16, ", 0, 0", 16, MMB_REGS16, "%18", "%16", "%17", MMB_ACC16(0))
+MMB_WGMMA_SS(32, 16, bf16, ", 0, 0", 16, MMB_REGS16, "%18", "%16", "%17", MMB_ACC16(0))
+MMB_WGMMA_SS(64, 16, f16, ", 0, 0", 32, MMB_REGS32, "%34", "%32", "%33", MMB_ACC16(0), MMB_ACC16(16))
+MMB_WGMMA_SS(64, 16, bf16, ", 0, 0", 32, MMB_REGS32, "%34", "%32", "%33", MMB_ACC16(0), MMB_ACC16(16))
+MMB_WGMMA_SS(128, 16, f16, ", 0, 0", 64, MMB_REGS64, "%66", "%64", "%65", MMB_ACC16(0), MMB_ACC16(16), MMB_ACC16(32), MMB_ACC16(48))
+MMB_WGMMA_SS(128, 16, bf16, ", 0, 0", 64, MMB_REGS64, "%66", "%64", "%65", MMB_ACC16(0), MMB_ACC16(16), MMB_ACC16(32), MMB_ACC16(48))
+MMB_WGMMA_SS(32, 32, e4m3, "", 16, MMB_REGS16, "%18", "%16", "%17", MMB_ACC16(0))
+MMB_WGMMA_SS(128, 32, e4m3, "", 64, MMB_REGS64, "%66", "%64", "%65", MMB_ACC16(0), MMB_ACC16(16), MMB_ACC16(32), MMB_ACC16(48))
 
 // tf32 with the A operand in registers (K = 8): thread (warp w, lane l) supplies
 //   a[0] = A[16w + l/4][l%4], a[1] = A[16w + l/4 + 8][l%4], a[2] = A[16w + l/4][l%4 + 4], a[3] = A[16w + l/4 + 8][l%4 + 4]

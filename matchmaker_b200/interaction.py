@@ -452,6 +452,65 @@ def flat_ip_split_f32(x: torch.Tensor, role: str, scale_log2: Optional[int] = No
     return torch.cat(parts, dim=1).contiguous(), scale_log2
 
 
+FP8_MAX = 448.0   # largest finite torch.float8_e4m3fn value
+
+
+def fp8_scale_log2(amax: torch.Tensor) -> torch.Tensor:
+    """The E4M3 scale rule, elementwise: the largest integer s with amax * 2^s <= 448 (int32), 0 where amax is 0.
+    Exact: with amax = m * 2^e (0.5 <= m < 1), s = 9 - e when m <= 0.875 and 8 - e otherwise.  Runs on the tensor's
+    device without a host synchronisation (the per-query scales of a search); a non-finite amax gives a meaningless
+    s, so callers that must refuse one check it (:func:`fp8_store_scale`)."""
+    m, e = torch.frexp(amax.float())
+    s = torch.where(m <= 0.875, 9 - e, 8 - e)
+    return torch.where(amax > 0, s, torch.zeros_like(s)).to(torch.int32)
+
+
+def fp8_store_scale(amax: float) -> int:
+    """The E4M3 scale rule for one host value (a store's largest |x|); raises on a non-finite or negative amax."""
+    import math
+    if not math.isfinite(amax) or amax < 0:
+        raise _lib.MatchmakerB200Error(f"fp8 store scale: the largest |x| of the rows is {amax}, not a finite value")
+    return int(fp8_scale_log2(torch.tensor([amax], dtype=torch.float32))[0])
+
+
+def _pow2_f32(e: torch.Tensor) -> torch.Tensor:
+    """2^e as fp32 for integer e in [-126, 127], built from the exponent bits (exact)."""
+    return ((e.to(torch.int32) + 127) << 23).view(torch.float32)
+
+
+def fp8_quantize(x: torch.Tensor, scale_log2) -> torch.Tensor:
+    """e4m3_rn(x * 2^s) as torch.float8_e4m3fn: torch's cast of the fp32 value x * 2^s.  scale_log2 is an int or an
+    integer tensor over the leading dimensions of x (one scale per query of a [N, Lq, dim] batch).  The product is
+    taken as two power-of-two factors, so it is exact for every s the scale rule gives.  Elementwise format
+    conversion, not scoring arithmetic."""
+    s = torch.as_tensor(scale_log2, dtype=torch.int32, device=x.device)
+    while s.dim() < x.dim():
+        s = s.unsqueeze(-1)
+    h = torch.div(s, 2, rounding_mode="floor")
+    y = x.to(torch.float32, copy=True)
+    y.mul_(_pow2_f32(h)).mul_(_pow2_f32(s - h))
+    return y.to(torch.float8_e4m3fn)
+
+
+def fp8_unscale(scores: torch.Tensor, scale_log2: torch.Tensor) -> torch.Tensor:
+    """scores * 2^-scale_log2 (an integer tensor over the leading dimensions of scores), exact, in fp32; void scores
+    (-inf, -3.4028235e38) are left as they are."""
+    e = scale_log2.to(torch.float64)
+    while e.dim() < scores.dim():
+        e = e.unsqueeze(-1)
+    out = (scores.double() * torch.exp2(-e)).float()
+    return torch.where(scores > -3.0e38, out, scores)
+
+
+def _fp8_pair(a: torch.Tensor, b: torch.Tensor, what: str) -> bool:
+    """True when both operands are e4m3; raises when only one is."""
+    fa, fb = a.dtype == torch.float8_e4m3fn, b.dtype == torch.float8_e4m3fn
+    if fa != fb:
+        raise _lib.MatchmakerB200Error(f"{what}: e4m3 needs both operands in torch.float8_e4m3fn, got {a.dtype}, "
+                                       f"{b.dtype}")
+    return fa
+
+
 def flat_ip_topk(queries: torch.Tensor, passages: torch.Tensor, k: int, ids: Optional[torch.Tensor] = None,
                  id_base: int = 0, split_scale: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor]:
     """Exact inner-product top-k of every query against a resident passage shard (faiss IndexFlatIP
@@ -459,9 +518,13 @@ def flat_ip_topk(queries: torch.Tensor, passages: torch.Tensor, k: int, ids: Opt
     (scores [nq,k] f32 descending, ids [nq,k] int64); ties by id ascending.  1 <= k <= 1024.
 
     fp32 storage (``token_dtype: float32``): pass ``passages`` = flat_ip_split_f32(p, "passages")[0] ([n, 2*dim] fp16)
-    together with its scale as ``split_scale``; queries (fp32 [nq, dim]) are split here, scores are returned unscaled."""
+    together with its scale as ``split_scale``; queries (fp32 [nq, dim]) are split here, scores are returned unscaled.
+
+    E4M3 (both operands torch.float8_e4m3fn, dim % 128 == 0, 128 <= dim <= 1024): the scores are the sums of products
+    of the stored values, i.e. in the scaled domain of :func:`fp8_quantize`; the caller unscales."""
     dev = _require_cuda(queries, passages, ids)
-    if passages.dtype not in (torch.float16, torch.bfloat16):
+    fp8 = _fp8_pair(queries, passages, "flat_ip_topk")
+    if not fp8 and passages.dtype not in (torch.float16, torch.bfloat16):
         raise _lib.MatchmakerB200Error("flat_ip_topk: passage storage must be fp16 / bf16, or the fp16 split of fp32 "
                                        "(flat_ip_split_f32)")
     n = passages.shape[0]
@@ -480,7 +543,7 @@ def flat_ip_topk(queries: torch.Tensor, passages: torch.Tensor, k: int, ids: Opt
             raise _lib.MatchmakerB200Error(f"flat_ip_topk: queries have dim {queries.shape[1]}, passages {passages.shape[1]}")
         queries = queries.to(passages.dtype).contiguous()
         dim = queries.shape[1]
-        dcode = _DTYPES[passages.dtype]
+        dcode = _lib.F8E4M3 if fp8 else _DTYPES[passages.dtype]
     passages = passages.contiguous()
     nq = queries.shape[0]
     if ids is not None:
@@ -572,9 +635,14 @@ def ivf_search(queries: torch.Tensor, rows: torch.Tensor, ids: torch.Tensor, lis
 
     row_index (int64 [list_offsets[-1]], optional): the rows are NOT sorted by list; list position p is row
     ``row_index[p]`` of ``rows``, and ``ids`` is indexed by row (mmb200_ivf_search_gather).  The result equals the call
-    without row_index over ``rows[row_index]`` with ids ``ids[row_index]``, without that copy of the rows."""
+    without row_index over ``rows[row_index]`` with ids ``ids[row_index]``, without that copy of the rows.
+
+    E4M3 (queries and rows torch.float8_e4m3fn, with row_index only): scores in the scaled domain, as flat_ip_topk."""
     dev = _require_cuda(queries, rows, ids, list_offsets, probes, row_index)
-    if rows.dtype not in (torch.float16, torch.bfloat16):
+    fp8 = _fp8_pair(queries, rows, "ivf_search")
+    if fp8 and row_index is None:
+        raise _lib.MatchmakerB200Error("ivf_search: e4m3 rows are scanned in place through row_index only")
+    if not fp8 and rows.dtype not in (torch.float16, torch.bfloat16):
         raise _lib.MatchmakerB200Error("ivf_search: rows must be fp16 / bf16, or the fp16 split of fp32 (flat_ip_split_f32)")
     if probes.dim() != 2 or probes.shape[0] != queries.shape[0]:
         raise _lib.MatchmakerB200Error(f"ivf_search: probes must be [nq, nprobe], got {tuple(probes.shape)}")
@@ -595,7 +663,7 @@ def ivf_search(queries: torch.Tensor, rows: torch.Tensor, ids: torch.Tensor, lis
             raise _lib.MatchmakerB200Error(f"ivf_search: queries have dim {queries.shape[1]}, rows {rows.shape[1]}")
         queries = queries.to(rows.dtype).contiguous()
         dim = queries.shape[1]
-        dcode = _DTYPES[rows.dtype]
+        dcode = _lib.F8E4M3 if fp8 else _DTYPES[rows.dtype]
     if ids.numel() != rows.shape[0] or list_offsets.dim() != 1 or nlist < 1:
         raise _lib.MatchmakerB200Error(f"ivf_search: {ids.numel()} ids for {rows.shape[0]} rows, list_offsets "
                                        f"{tuple(list_offsets.shape)} (need [nlist + 1], nlist >= 1)")
@@ -616,7 +684,8 @@ def ivf_search(queries: torch.Tensor, rows: torch.Tensor, ids: torch.Tensor, lis
             return lib.mmb200_ivf_workspace_bytes(b, nprobe, nlist, max_list_len, dim, k, dcode)
         if wsb(1) <= 0:
             raise _lib.MatchmakerB200Error(f"ivf_search: unsupported sizes nprobe={nprobe} nlist={nlist} dim={dim} k={k} "
-                                           f"(1 <= k <= {FLAT_IP_MAX_K}, 1 <= nprobe <= {IVF_MAX_PROBE}, dim % 64 == 0)")
+                                           f"(1 <= k <= {FLAT_IP_MAX_K}, 1 <= nprobe <= {IVF_MAX_PROBE}, dim % 64 == 0; "
+                                           "e4m3: dim % 128 == 0, 128 <= dim <= 1024)")
         b = ivf_query_batch(nq, wsb, IVF_WORKSPACE_CAP)
         ws = torch.empty(wsb(b), dtype=torch.uint8, device=dev)
         for b0 in range(0, nq, b):
@@ -968,9 +1037,13 @@ def maxsim_store(q: torch.Tensor, store: torch.Tensor, doc_offsets: torch.Tensor
     store [n_rows, dim]; passage d is rows ``doc_offsets[d] : doc_offsets[d+1]`` (int64 [n_docs+1], non-decreasing,
     at most ``max_doc_len`` rows read).  Pair p scores query ``pair_q[p]`` of q [n_q, Lq, dim] against passage
     ``pair_d[p]``; ``pair_d[p] < 0`` and passages without rows score -inf.  Same kernels and bit-identical scores as
-    :func:`maxsim` on the passages padded to ``max_doc_len`` with a mask."""
+    :func:`maxsim` on the passages padded to ``max_doc_len`` with a mask.
+
+    E4M3 (q and store torch.float8_e4m3fn, 1 <= Lq <= 128, dim % 128 == 0, 128 <= dim <= 1024; impl "auto" or
+    "tcgen05_docm"): the documents-on-M tensor-core kernel, scores in the scaled domain of :func:`fp8_quantize`."""
     dev = _require_cuda(q, store, doc_offsets, pair_q, pair_d)
-    if q.dtype != store.dtype or q.dtype not in _DTYPES:
+    fp8 = _fp8_pair(q, store, "maxsim_store")
+    if not fp8 and (q.dtype != store.dtype or q.dtype not in _DTYPES):
         raise _lib.MatchmakerB200Error(f"q/store must share a dtype in fp16/bf16/fp32, got {q.dtype}, {store.dtype}")
     if q.dim() != 3 or store.dim() != 2 or q.shape[-1] != store.shape[-1]:
         raise _lib.MatchmakerB200Error(f"expected q [n_q,Lq,dim], store [n_rows,dim]; got {tuple(q.shape)}, "
@@ -987,7 +1060,7 @@ def maxsim_store(q: torch.Tensor, store: torch.Tensor, doc_offsets: torch.Tensor
     with torch.cuda.device(dev):
         rc = lib.mmb200_maxsim_store_fwd(_ptr(q), _ptr(store), _ptr(doc_offsets), _ptr(pair_q), _ptr(pair_d), _ptr(out),
                                          n_q, store.shape[0], doc_offsets.numel() - 1, pair_q.numel(), Lq, int(max_doc_len),
-                                         dim, _DTYPES[q.dtype], _IMPLS[impl], _stream(dev))
+                                         dim, _lib.F8E4M3 if fp8 else _DTYPES[q.dtype], _IMPLS[impl], _stream(dev))
     _lib.check(rc, "mmb200_maxsim_store_fwd")
     return out
 
