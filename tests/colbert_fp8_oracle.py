@@ -5,7 +5,8 @@ Test infrastructure: plain Python and torch on the CPU, no library call.
 - scale rule: the largest integer s with A * 2^s <= 448, found by stepping from a float estimate and checked with
   exact ldexp; 0 when A == 0; a non-finite A raises;
 - stored value: torch's CPU cast to float8_e4m3fn of the fp32 value x * 2^s (taken exactly in fp64 first);
-- scores: fp64 products and sums of the stored values (the scaled domain), unscaled by 2^-(s_q + s_d)."""
+- scores: fp64 products and sums of the stored values (the scaled domain), unscaled by 2^-(s_q + s_d).  Subnormal
+  stored values (m * 2^-9) count as they are: the FP8 tensor cores keep them (tests/test_maxsim_envelope_gpu.py)."""
 from __future__ import annotations
 
 import math

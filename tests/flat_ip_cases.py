@@ -13,14 +13,18 @@ Routing (``csrc/flat_ip.cu``):
 - kernels (:1020-1030, :1184-1197): ``flat_ip_topk`` runs ``flat_ip_tc_kernel<T, CL, EPL, false>`` with T = __half
   for fp16 and the fp32 split, __nv_bfloat16 for bf16; ``ivf_search`` runs ``flat_ip_tc_kernel<T, 1, EPL, true>``,
   with ``row_index`` ``flat_ip_tc_gather_kernel<T, EPL>``; ``ivf_search_residual`` runs
-  ``flat_ip_tc_residual_kernel<EPL, bits>``.
+  ``flat_ip_tc_residual_kernel<EPL, bits>``.  E4M3 (dtype "e4m3", both operands float8_e4m3fn, flat_ip.cu:1054-1062,
+  :1231-1232): ``flat_ip_topk`` runs ``flat_ip_tc_fp8_kernel<CL, EPL>`` under the same plan; ``ivf_search`` only with
+  ``row_index``, on ``flat_ip_tc_gather_fp8_kernel<EPL>`` (without it the call is refused).
 - merge (:792, :795-849): ``topk_merge_kernel`` sorts at most 8192 candidates at once; more (flat mode: ``n_ranges *
   kpad``, IVF: ``nprobe * kslot``) are cut to their k best in groups and merged again.
 
 Inputs are small integers (fp16), integers of magnitude <= 4 (bf16), integer queries against passages a + b * 2^-10
 (the fp32 split: q_lo = 0, hi and lo exact), and residual codes over integer base and weight tables.  ``make_case``
 asserts that sum_i |q_i p_i| < 2^24 grains for every (query, row) pair, so every fp32 sum is exact in any order: then
-(score desc, signed id asc) is a total order and ids and scores are bit-exact, including the (-FLT_MAX, -1) tail."""
+(score desc, signed id asc) is a total order and ids and scores are bit-exact, including the (-FLT_MAX, -1) tail.  The
+e4m3 rows hold integers e4m3 holds exactly with sum_i |q_i p_i| < 2^11, the bound under which the FP8 MMA's own
+accumulation is exact (test_maxsim_envelope_gpu.py::test_fp8_mma_accumulates_exactly)."""
 from __future__ import annotations
 
 import functools
@@ -34,7 +38,9 @@ import colbert_residual_oracle as RO
 import ivf_oracle
 
 FLAT, IVF_GATHER, RESIDUAL = "flat_ip_tc_kernel", "flat_ip_tc_gather_kernel", "flat_ip_tc_residual_kernel"
-KERNELS = (FLAT, IVF_GATHER, RESIDUAL)
+FLAT_FP8, GATHER_FP8 = "flat_ip_tc_fp8_kernel", "flat_ip_tc_gather_fp8_kernel"
+KERNELS = (FLAT, IVF_GATHER, RESIDUAL, FLAT_FP8, GATHER_FP8)
+E4M3_EXACT_GRAINS = 2 ** 11   # the e4m3 rows' bound (maxsim_cases.E4M3_EXACT_GRAINS)
 TNAME = {"f16": "__half", "split": "__half", "bf16": "__nv_bfloat16"}
 BM = BN = 128
 MAX_RANGES = 32
@@ -91,7 +97,7 @@ def plan(nq: int, n: int, k: int, sm_count: int, cluster: Optional[int] = None, 
 @dataclass(frozen=True)
 class Row:
     mode: str              # "flat" (flat_ip_topk), "ivf" (ivf_search with and without row_index), "residual"
-    dtype: str             # "f16", "bf16", "split" (fp32 storage as fp16 hi / lo); residual rows are "f16"
+    dtype: str             # "f16", "bf16", "split" (fp32 storage as fp16 hi / lo), "e4m3"; residual rows are "f16"
     nq: int
     n: int                 # flat: passages; ivf / residual: rows in the lists (the store has padding rows besides)
     dim: int
@@ -140,10 +146,17 @@ def dispatched(row: Row) -> frozenset:
     """The instantiations the envelope test runs for a row."""
     e = epl_for_k(row.k)
     if row.mode == "flat":
-        return frozenset({inst(FLAT, TNAME[row.dtype], row.plan()["cl"], e, False)})
+        return frozenset({flat_inst(row.dtype, row.plan()["cl"], e)})
+    if row.dtype == "e4m3":
+        return frozenset({inst(GATHER_FP8, e)})   # e4m3 IVF runs through row_index only
     if row.mode == "ivf":
         return frozenset({inst(FLAT, TNAME[row.dtype], 1, e, True), inst(IVF_GATHER, TNAME[row.dtype], e)})
     return frozenset({inst(RESIDUAL, e, row.bits)})
+
+
+def flat_inst(dtype: str, cl: int, epl: int) -> str:
+    """The flat_ip_topk kernel of a dtype at a cluster size and list width."""
+    return inst(FLAT_FP8, cl, epl) if dtype == "e4m3" else inst(FLAT, TNAME[dtype], cl, epl, False)
 
 
 def _big_lists():
@@ -203,6 +216,28 @@ MATRIX = (
         lists=(300, 5, 400, 0, 128), nprobe=3, bits=1),
     Row("residual", "f16", 9, 3631, 64, 1024, 34, "2-bit codes at k = 1024, every score < 0",
         regime="neg", ids="extreme", lists=(700, 800, 1500, 10, 600, 20, 1), nprobe=2, bits=2),
+    # ---- e4m3 flat_ip_topk: flat_ip_tc_fp8_kernel<CL, EPL>
+    Row("flat", "e4m3", 1, 127, 128, 33, 41, "e4m3 <1,32>: one query against 127 rows, every score < 0 (the zero fill "
+        "of the tile's row 127 would win)", regime="neg"),
+    Row("flat", "e4m3", 5, 640, 384, 1, 42, "e4m3 <1,32>: k = 1 over tied rows, implicit ids from a negative base",
+        regime="tie", ids="implicit", id_base=-3000, run=40),
+    Row("flat", "e4m3", 128, 4097, 384, 1024, 43, "e4m3 <1,64>: 32 ranges asked of 33 tiles (17 run), merged in three "
+        "groups; INT64 edge ids", ranges=32, ids="extreme"),
+    Row("flat", "e4m3", 256, 3000, 128, 256, 44, "e4m3 <2,32>: a run of 1500 equal rows (over the 1024-entry list) "
+        "straddles k = 256", regime="tie", ids="extreme", run=1500),
+    Row("flat", "e4m3", 129, 256, 1024, 257, 45, "e4m3 <2,64> at dim 1024: k = 257 > n = 256"),
+    Row("flat", "e4m3", 300, 2000, 1024, 32, 46, "e4m3 <4,32> forced at dim 1024, one range", cl=4, ranges=1),
+    Row("flat", "e4m3", 600, 5000, 128, 1000, 47, "e4m3 <4,64> forced: a run of 2600 equal rows (over the 2048-entry "
+        "list) straddles k = 1000", cl=4, regime="tie", ids="extreme", run=2600),
+    # ---- e4m3 ivf_search with row_index: flat_ip_tc_gather_fp8_kernel<EPL>
+    Row("ivf", "e4m3", 200, 1239, 128, 31, 51, "e4m3 gather: empty, one-row, 128-row and multi-tile lists; probes of -1 "
+        "and >= nlist; INT64 edge ids", ids="extreme", lists=(0, 1, 128, 300, 5, 77, 256, 0, 129, 40, 303), nprobe=4),
+    Row("ivf", "e4m3", 130, 814, 128, 256, 52, "e4m3 gather, nprobe = 1, every score < 0: the next list and the padding "
+        "rows outrank every candidate", regime="neg", lists=(60, 70, 1, 90, 128, 20, 0, 30, 200, 215), nprobe=1),
+    Row("ivf", "e4m3", 70, 2792, 256, 257, 53, "e4m3 gather <64>: a run of 2600 equal rows, 2100 in one list, straddles "
+        "k = 257", regime="tie", ids="extreme", run=2600, lists=(2100, 300, 203, 128, 1, 0, 60), nprobe=5),
+    Row("ivf", "e4m3", 3, sum(BIG_LISTS), 128, 1000, 54, "e4m3 gather, nprobe = 1024 of 1100 short lists, k = 1000",
+        lists=BIG_LISTS, nprobe=1024),
 )
 
 METAMORPHIC_ROW = MATRIX[6]   # run under CL 1 / 2 / 4 x ranges 1 / auto / 32
@@ -215,6 +250,8 @@ K_EDGES = (1, 31, 32, 33, 256, 257, 1000, 1024)
 
 
 def features(row: Row, sm_count: int = SM_COUNT_H100) -> frozenset:
+    if row.dtype == "e4m3":
+        return _e4m3_features(row, sm_count)
     f = set()
     if row.k in K_EDGES:
         f.add(f"k {row.k}")
@@ -273,7 +310,56 @@ def features(row: Row, sm_count: int = SM_COUNT_H100) -> frozenset:
     return frozenset(f)
 
 
-REQUIRED_FEATURES = frozenset(
+E4M3_K_EDGES = (1, 32, 33, 256, 257, 1024)
+
+
+def _e4m3_features(row: Row, sm_count: int = SM_COUNT_H100) -> frozenset:
+    """The features of an e4m3 row, named apart from the 16-bit rows' (none is shared with them)."""
+    f = {f"e4m3 {row.regime} {row.mode}"}
+    if row.regime == "tie" and row.run > 32 * epl_for_k(row.k):
+        f.add(f"e4m3 tie run over the list capacity, EPL {epl_for_k(row.k)}, {row.mode}")
+    if row.ids == "extreme":
+        f.add(f"e4m3 INT64 edge ids, {row.mode}")
+    if row.mode == "flat":
+        if row.k in E4M3_K_EDGES:
+            f.add(f"e4m3 k {row.k}")
+        if row.k > row.n:
+            f.add("e4m3 k > n")
+        f.update({1: {"e4m3 n 128m + 1"}, 0: {"e4m3 n 128m"}, BN - 1: {"e4m3 n 128m - 1"}}.get(row.n % BN, set()))
+        if row.dim in (128, 384, 1024):
+            f.add(f"e4m3 dim {row.dim}")
+        if row.cl is not None or row.ranges is not None:
+            f.add("e4m3 forced plan")
+        if row.merge_candidates(sm_count) > MERGE_SEG:
+            f.add("e4m3 multi-pass merge")
+    else:
+        L = row.lists
+        f.update({"e4m3 empty list"} if 0 in L else set())
+        f.update({"e4m3 one-row list"} if 1 in L else set())
+        if any(v and v % BN == 0 for v in L):
+            f.add("e4m3 list of 128m rows")
+        if any(v > 2 * BN for v in L):
+            f.add("e4m3 multi-tile list")
+        if row.nprobe in (1, 1024):
+            f.add(f"e4m3 nprobe {row.nprobe}")
+        if row.nprobe > 1 and row.regime != "neg":
+            f.add("e4m3 probes of -1 and >= nlist")
+        if row.nq > BM and row.regime == "rand":
+            f.add("e4m3 a list probed by more than 128 queries")
+    return frozenset(f)
+
+
+E4M3_REQUIRED_FEATURES = frozenset(
+    {f"e4m3 k {k}" for k in E4M3_K_EDGES} | {f"e4m3 dim {d}" for d in (128, 384, 1024)}
+    | {"e4m3 k > n", "e4m3 n 128m - 1", "e4m3 n 128m", "e4m3 n 128m + 1", "e4m3 forced plan", "e4m3 multi-pass merge"}
+    | {f"e4m3 {r} {m}" for r in ("rand", "neg", "tie") for m in ("flat", "ivf")}
+    | {f"e4m3 tie run over the list capacity, EPL {e}, flat" for e in (32, 64)}
+    | {"e4m3 tie run over the list capacity, EPL 64, ivf", "e4m3 INT64 edge ids, flat", "e4m3 INT64 edge ids, ivf"}
+    | {"e4m3 empty list", "e4m3 one-row list", "e4m3 list of 128m rows", "e4m3 multi-tile list", "e4m3 nprobe 1",
+       "e4m3 nprobe 1024", "e4m3 probes of -1 and >= nlist", "e4m3 a list probed by more than 128 queries"})
+
+
+REQUIRED_FEATURES = E4M3_REQUIRED_FEATURES | frozenset(
     {f"k {k}" for k in K_EDGES}
     | {"k = n", "k > n", "n 1", "n < 128", "n 128m - 1", "n 128m", "n 128m + 1"}
     | {f"nq {n}" for n in (1, 127, 128, 129)} | {f"dim {d}" for d in (64, 128, 768, 1024)}
@@ -348,6 +434,12 @@ def _assert_exact(row: Row, q: torch.Tensor, p: torch.Tensor):
         grain = 2.0 ** (sq + sp - 10)
         mass = qs[:, :d].abs() @ (ps[:, :d].abs() + ps[:, d:].abs()).T / grain
         assert torch.equal(p * 1024, (p * 1024).round())
+    elif row.dtype == "e4m3":
+        E4 = torch.float8_e4m3fn
+        assert torch.equal(q.float().to(E4).double(), q) and torch.equal(p.float().to(E4).double(), p)
+        assert torch.equal(p, p.round()) and torch.equal(q, q.round())
+        assert float((q.abs() @ p.abs().T).max()) < E4M3_EXACT_GRAINS
+        return
     else:
         mass = q.abs() @ p.abs().T
         lim = 4 if row.dtype == "bf16" else 8
@@ -357,7 +449,17 @@ def _assert_exact(row: Row, q: torch.Tensor, p: torch.Tensor):
 
 def _flat_rows(row: Row, g, n: int, dim: int):
     """(q, p, run positions) for the regime: "rand" values in [-3, 3]; "neg" queries in [-3, -1] against rows in
-    [1, 3]; "tie" positive queries, `run` rows of all 3 at shuffled positions and 3 rows above them (one entry 4)."""
+    [1, 3]; "tie" positive queries, `run` rows of all 3 at shuffled positions and 3 rows above them (one entry 4).
+    e4m3 (sums below 2^11): "rand" queries in [-1, 1] against rows in [-2, 2]; "neg" queries in {-1, 0} against rows in
+    [1, 2]; "tie" queries of all 1 against rows in [-1, 1], the run all 1 and the rows above it with one entry 2."""
+    if row.dtype == "e4m3":
+        if row.regime == "neg":
+            q = -(torch.rand(row.nq, dim, generator=g) < 0.5).double()
+            q[:, 0] = -1.0
+            return q, _randint(g, 1, 2, (n, dim))
+        if row.regime == "tie":
+            return torch.ones(row.nq, dim, dtype=torch.float64), _randint(g, -1, 1, (n, dim))
+        return _randint(g, -1, 1, (row.nq, dim)), _randint(g, -2, 2, (n, dim))
     if row.regime == "neg":
         q, p = _randint(g, -3, -1, (row.nq, dim)), _randint(g, 1, 3, (n, dim))
     elif row.regime == "tie":
@@ -371,13 +473,14 @@ def _flat_rows(row: Row, g, n: int, dim: int):
 
 def _place_run(row: Row, g, p: torch.Tensor, pos: torch.Tensor):
     """Rows `pos` become the tie run (all 3; the split adds a common fraction); up to 3 more rows score above it."""
-    v = torch.full((p.shape[1],), 3.0, dtype=torch.float64)
+    top = 1.0 if row.dtype == "e4m3" else 3.0
+    v = torch.full((p.shape[1],), top, dtype=torch.float64)
     if row.dtype == "split":
         v += 17 / 1024
     p[pos[: row.run]] = v
     for j, r in enumerate(pos[row.run: row.run + 3].tolist()):
         p[r] = v
-        p[r, j] = 4.0
+        p[r, j] = top + 1.0
     return pos[: row.run]
 
 
@@ -437,6 +540,8 @@ def _make_ivf_case(row: Row, g) -> Case:
     _assert_exact(row, q, p)
     ids = _ids(row, g, n, run_pos)
     store, store_ids, row_index = _gather_store(row, g, p, ids)
+    if row.dtype == "e4m3":
+        _assert_exact(row, q, store)   # the padding rows too: the gather kernel reads them if it reads wrong
     return Case(q, p, ids, offsets, probes, store, store_ids, row_index)
 
 

@@ -100,8 +100,10 @@ def test_rows_claim_what_the_routing_gives_them():
     expect = ({C.inst(C.FLAT, t, cl, e, False) for t in ("__half", "__nv_bfloat16") for cl in (1, 2, 4) for e in (32, 64)}
               | {C.inst(C.FLAT, t, 1, e, True) for t in ("__half", "__nv_bfloat16") for e in (32, 64)}
               | {C.inst(C.IVF_GATHER, t, e) for t in ("__half", "__nv_bfloat16") for e in (32, 64)}
-              | {C.inst(C.RESIDUAL, e, b) for e in (32, 64) for b in (1, 2)})
-    assert len(expect) == 24
+              | {C.inst(C.RESIDUAL, e, b) for e in (32, 64) for b in (1, 2)}
+              | {C.inst(C.FLAT_FP8, cl, e) for cl in (1, 2, 4) for e in (32, 64)}
+              | {C.inst(C.GATHER_FP8, e) for e in (32, 64)})
+    assert len(expect) == 32
     assert every == expect
 
 
@@ -172,7 +174,7 @@ def instantiations():
 
 
 def test_every_compiled_instantiation_is_claimed_by_a_row(instantiations):
-    assert len(instantiations) == len(set(instantiations)) == 24, sorted(instantiations)
+    assert len(instantiations) == len(set(instantiations)) == 32, sorted(instantiations)
     claimed = set().union(*(C.dispatched(r) for r in C.MATRIX))
     assert set(instantiations) == claimed, (sorted(set(instantiations) - claimed), sorted(claimed - set(instantiations)))
 

@@ -21,7 +21,18 @@ DEV = "cuda"
 FLAT_ROWS = [r for r in C.MATRIX if r.mode == "flat"]
 IVF_ROWS = [r for r in C.MATRIX if r.mode == "ivf"]
 RESIDUAL_ROWS = [r for r in C.MATRIX if r.mode == "residual"]
-TORCH = {"f16": torch.float16, "bf16": torch.bfloat16}
+TORCH = {"f16": torch.float16, "bf16": torch.bfloat16, "e4m3": torch.float8_e4m3fn}
+
+
+def _dev(x: torch.Tensor, dtype: str) -> torch.Tensor:
+    return x.float().to(TORCH[dtype]).to(DEV)
+
+
+def _take(x: torch.Tensor, idx: torch.Tensor) -> torch.Tensor:
+    """x[idx] by rows, through the bytes for e4m3."""
+    if x.dtype == torch.float8_e4m3fn:
+        return x.view(torch.uint8)[idx].view(torch.float8_e4m3fn)
+    return x[idx]
 
 
 def _env(monkeypatch, cl=None, ranges=None):
@@ -48,7 +59,7 @@ def _flat_inputs(row: C.Row):
     if row.dtype == "split":
         ps, scale = interaction.flat_ip_split_f32(c.p.float().to(DEV), "passages")
         return c.q.float().to(DEV), ps, scale
-    return c.q.to(TORCH[row.dtype]).to(DEV), c.p.to(TORCH[row.dtype]).to(DEV), None
+    return _dev(c.q, row.dtype), _dev(c.p, row.dtype), None
 
 
 def _flat(row: C.Row, q, p, scale, ids=None):
@@ -70,7 +81,7 @@ def test_flat_rows_bit_exact(row, monkeypatch):
     assert torch.equal(again[0], got[0]) and torch.equal(again[1], got[1]), "two runs differ"
     perm = torch.randperm(row.n, generator=torch.Generator().manual_seed(row.seed)).to(DEV)
     pid = C.row_ids(row, c).to(DEV)[perm]
-    _exact(interaction.flat_ip_topk(q, p[perm], row.k, ids=pid, split_scale=scale), ref, f"{row} permuted")
+    _exact(interaction.flat_ip_topk(q, _take(p, perm), row.k, ids=pid, split_scale=scale), ref, f"{row} permuted")
 
 
 def test_one_row_under_every_cluster_size_and_range_count(monkeypatch):
@@ -98,28 +109,49 @@ def test_plan_on_the_device(monkeypatch):
         out = (ctypes.c_int32 * 8)()
         assert lib.mmb200_flat_ip_plan(row.nq, row.n, row.k, sm, out) == _lib.OK, _lib.last_error()
         (claimed,) = C.dispatched(row)
-        assert claimed == C.inst(C.FLAT, C.TNAME[row.dtype], out[5], C.epl_for_k(row.k), False), str(row)
+        assert claimed == C.flat_inst(row.dtype, out[5], C.epl_for_k(row.k)), str(row)
         assert out[2] == row.plan(sm)["n_ranges"], str(row)
 
 
 def _ivf_args(row: C.Row, c: C.Case):
-    dt = TORCH[row.dtype]
-    return (c.q.to(dt).to(DEV), c.offsets.to(DEV), c.probes.to(DEV))
+    return (_dev(c.q, row.dtype), c.offsets.to(DEV), c.probes.to(DEV))
 
 
 @pytest.mark.parametrize("row", IVF_ROWS, ids=str)
-def test_ivf_rows_bit_exact(row):
+def test_ivf_rows_bit_exact(row, monkeypatch):
     """ivf_search over the rows in list order, and with row_index over the shuffled store with padding rows: both equal
-    the oracle over the union of each query's probed lists, and each other."""
+    the oracle over the union of each query's probed lists, and each other.  e4m3: the plain scan is refused; the
+    gather gives the same bits with its queries cut into batches by a lowered workspace cap, and at full probe it gives
+    the bits of the e4m3 flat scan."""
     c = C.make_case(row)
-    dt = TORCH[row.dtype]
     q, offsets, probes = _ivf_args(row, c)
     ref = C.expected(row)
-    plain = interaction.ivf_search(q, c.p.to(dt).to(DEV), c.ids.to(DEV), offsets, probes, row.k, row.max_list_len)
-    _exact(plain, ref, f"{row} plain")
-    gather = interaction.ivf_search(q, c.store.to(dt).to(DEV), c.store_ids.to(DEV), offsets, probes, row.k,
-                                    row.max_list_len, row_index=c.row_index.to(DEV))
+    rows = _dev(c.p, row.dtype)
+    args = (c.store_ids.to(DEV), offsets, probes, row.k, row.max_list_len)
+    gather = interaction.ivf_search(q, _dev(c.store, row.dtype), *args, row_index=c.row_index.to(DEV))
     _exact(gather, ref, f"{row} gather")
+    if row.dtype == "e4m3":
+        with pytest.raises(_lib.MatchmakerB200Error):
+            interaction.ivf_search(q, rows, c.ids.to(DEV), offsets, probes, row.k, row.max_list_len)
+        lib = _lib.load()
+        nprobe, nlist = probes.shape[1], len(row.lists)
+        def wsb(b):
+            return lib.mmb200_ivf_workspace_bytes(b, nprobe, nlist, row.max_list_len, row.dim, row.k, _lib.F8E4M3)
+        monkeypatch.setattr(interaction, "IVF_WORKSPACE_CAP", wsb(max(1, row.nq // 3)))
+        assert interaction.ivf_query_batch(row.nq, wsb, interaction.IVF_WORKSPACE_CAP) < row.nq
+        batched = interaction.ivf_search(q, _dev(c.store, row.dtype), *args, row_index=c.row_index.to(DEV))
+        assert torch.equal(batched[0], gather[0]) and torch.equal(batched[1], gather[1]), "batched queries differ"
+        monkeypatch.undo()
+        if nlist > interaction.IVF_MAX_PROBE:
+            return
+        full = torch.arange(nlist).repeat(row.nq, 1).to(DEV)
+        s_g, i_g = interaction.ivf_search(q, _dev(c.store, row.dtype), c.store_ids.to(DEV), offsets, full, row.k,
+                                          row.max_list_len, row_index=c.row_index.to(DEV))
+        s_f, i_f = interaction.flat_ip_topk(q, rows, row.k, ids=c.ids.to(DEV))
+        assert torch.equal(s_g, s_f) and torch.equal(i_g, i_f), "full probe differs from the flat scan"
+        return
+    plain = interaction.ivf_search(q, rows, c.ids.to(DEV), offsets, probes, row.k, row.max_list_len)
+    _exact(plain, ref, f"{row} plain")
     assert torch.equal(gather[0], plain[0]) and torch.equal(gather[1], plain[1])
 
 

@@ -76,8 +76,10 @@ def test_rows_claim_what_the_routing_gives_them():
     T = [C.TNAME[t] for t in (C.H, C.BF)]
     expect = ({C.inst(C.TC, t, k, n) for t in T for k in (1, 2) for n in (1, 2, 3, 4)}
               | {C.inst(C.QM, t, a, s) for t in T for a, s in ((False, False), (True, False), (False, True))}
-              | {C.inst(k, C.TNAME[t]) for k in (C.SIMT, C.BWD_D, C.BWD_Q) for t in (C.H, C.BF, C.F32)})
-    assert len(expect) == 31
+              | {C.inst(k, C.TNAME[t]) for k in (C.SIMT, C.BWD_D, C.BWD_Q) for t in (C.H, C.BF, C.F32)}
+              | {C.inst(C.TC_FP8, k, n) for k in (1, 2) for n in (1, 2, 3, 4)}
+              | {C.inst(C.TC_RES, k, n, b) for k in (1, 2) for n in (1, 2, 3, 4) for b in (1, 2)})
+    assert len(expect) == 55
     assert every == expect
 
 
@@ -108,8 +110,82 @@ def test_launch_configurations_and_envelope_edges():
     assert C.last_lq(C.F32, 768, False) == 74   # f32 runs on the SIMT kernel only
 
 
+def test_e4m3_and_residual_envelopes():
+    """plan_tc over e4m3 (1-byte elements) and over residual codes (16-bit tiles beside the weight table) on an H100."""
+    e4 = {dim: C.last_lq_e4m3(dim) for dim in range(128, 1025, 128)}
+    assert set(e4.values()) == {128}
+    one_slot = {dim: min([lq for lq in range(1, 129) if C.plan_tc(lq, dim, C.SMEM_OPTIN_H100, 1)["qslots"] == 1]
+                         or [0]) for dim in e4}
+    assert one_slot == {128: 0, 256: 0, 384: 0, 512: 0, 640: 0, 768: 97, 896: 97, 1024: 65}
+    assert C.plan_tc(128, 1024, C.SMEM_OPTIN_H100, 1) == {"kbs": 2, "nc": 4, "qslots": 1, "stages": 2}
+    for bits in (1, 2):
+        res = {dim: C.last_lq_residual(dim, bits) for dim in range(64, 1025, 64)}
+        assert {d for d, lq in res.items() if lq == 96} == ({640, 768, 832, 960} if bits == 1 else {640, 768, 832})
+        assert {d for d, lq in res.items() if lq == 64} == ({896, 1024} if bits == 1 else {896, 960, 1024})
+        assert res[704] == 128 and all(lq == 128 for d, lq in res.items() if d < 640)
+        for lq in range(1, 65):
+            assert C.plan_tc(lq, 1024, C.SMEM_OPTIN_H100, 2, C.residual_extra(1024, bits))["stages"] == 2
+    assert C.route_e4m3(30, 768, "simt") is None and C.route_e4m3(30, 768, "tcgen05") is None
+    assert C.route_e4m3(30, 768, "auto") == C.route_e4m3(30, 768, "tcgen05_docm") == "maxsim_tc_fp8_kernel<2,1>"
+    assert C.route_e4m3(30, 704, "auto") is None and C.route_e4m3(129, 128, "auto") is None
+
+
+CODED_ROWS = [(r, b) for r in C.MATRIX if r.coded for b in ((0,) if r.dtype == C.E4 else C.RESIDUAL_BITS)]
+
+
+@pytest.mark.parametrize("row,bits", CODED_ROWS, ids=lambda v: str(v) if isinstance(v, C.Row) else f"b{v}")
+def test_store_cases_hold_their_preconditions(row, bits):
+    """e4m3 and residual store rows: exact inputs, the layout the row claims, and inputs that would change the result if
+    a kernel read past a window (neg rows), flushed subnormals (the subnormal passage) or read a poisoned row."""
+    c = C.make_store_case(row, bits)
+    score = C.store_oracle(c, row.Ld)
+    assert not torch.isnan(score).any(), "a window holds a poisoned row"
+    lens = c.offsets[1:] - c.offsets[:-1]
+    void = (c.pair_d < 0) | (lens[c.pair_d.clamp(min=0)] == 0)
+    assert torch.equal(torch.isinf(score), void) and bool((score[void] < 0).all())
+    assert int(c.offsets[-1]) == c.store.shape[0]
+    if row.dtype == C.E4:
+        C.assert_exact_e4m3(c, row.Ld)
+    else:
+        assert torch.equal(c.q, c.q.round()) and float(c.q.abs().max()) <= 3
+        live = ~torch.isnan(c.store)
+        assert torch.equal(c.store[live], c.store[live].round()) and float(c.store[live].abs().max()) <= 5
+        assert torch.isnan(c.base[-1]).all() and not torch.isnan(c.base[:-1]).any()
+    if row.pairs > 1:
+        assert tuple(lens[: len(C.LAYOUT)].tolist()) == C.LAYOUT and (lens > row.Ld).any()
+        assert (c.pair_d == -1).any()
+        last = c.store.shape[0] - 1
+        assert any(c.window(d, row.Ld)[1] - 1 == last for d in c.pair_d.tolist()), "no window ends at the last row"
+        assert (c.pair_q[1:] != c.pair_q[:-1]).all(), "the query must change every pair"
+        returns = [p for p in range(2, c.pair_q.numel()) if int(c.pair_q[p]) in c.pair_q[max(0, p - 3):p - 1].tolist()]
+        assert returns, "no pair comes back to an earlier query"
+        hot = c.pair_q[c.pair_d == C.LAYOUT.index(257)]
+        assert hot.numel() > row.n_q and torch.unique(hot).numel() >= min(row.n_q, 2)
+        referenced = set(c.pair_d.tolist())
+        assert all(d in referenced for d in range(row.n_d) if d != c.poison_doc)
+    if row.regime == "neg":
+        live = ~void
+        assert (C.store_oracle(c, row.Ld, extra=1)[live] != score[live]).all(), "reading one more row changes nothing"
+        for p in live.nonzero().flatten().tolist():
+            a, b = c.window(int(c.pair_d[p]), row.Ld)
+            assert (c.q[c.pair_q[p]] @ c.store[a:b].T < 0).all()
+    else:
+        assert torch.isnan(c.store).any(), "no poison"
+        if row.pairs > 1:
+            a, b = int(c.offsets[c.poison_doc]), int(c.offsets[c.poison_doc + 1])
+            assert b > a and torch.isnan(c.store[a:b]).all() and c.poison_doc not in c.pair_d.tolist()
+    if c.subnormal_doc >= 0:
+        a, b = int(c.offsets[c.subnormal_doc]), int(c.offsets[c.subnormal_doc + 1])
+        sub = c.store[a:b]
+        assert ((sub.abs() < C.E4M3_MIN_NORMAL) & (sub != 0)).any(1).all() and (sub.abs() < C.E4M3_MIN_NORMAL).all()
+        sel = c.pair_d == c.subnormal_doc
+        assert sel.any() and (C.store_oracle(c, row.Ld, flush=True)[sel] != score[sel]).all(), "flushing changes nothing"
+
+
 def test_cases_hold_their_preconditions():
     for row in C.MATRIX:
+        if row.coded:
+            continue
         c = C.make_case(row)
         for t in (c.q, c.d, c.gout):
             assert torch.equal(t, t.round()) and t.abs().max() <= 8
@@ -157,7 +233,27 @@ def test_every_compiled_instantiation_is_claimed_by_a_row(instantiations):
     claimed = set().union(*(row.claims for row in C.MATRIX))
     missing = sorted(instantiations - claimed)
     assert not missing, f"compiled but claimed by no row of maxsim_cases.MATRIX: {missing}"
-    assert len(instantiations) == 31
+    assert len(instantiations) == 55
+
+
+def test_every_maxsim_and_flat_ip_kernel_belongs_to_a_matrix():
+    """Every kernel named maxsim_*_kernel or flat_ip_tc*_kernel in the library's SASS is named by the KERNELS of an
+    instantiation matrix (maxsim_cases, flat_ip_cases, and the in-batch backward's own list): a new kernel family fails
+    here until it has rows."""
+    import flat_ip_cases
+    import test_maxsim_inbatch_bwd_cpu
+    try:
+        out = subprocess.run([CUOBJDUMP, "-sass", _lib.LIB_PATH], capture_output=True, text=True, timeout=300)
+        if out.returncode != 0:
+            pytest.skip("cuobjdump failed: " + out.stderr[-200:])
+        names = re.findall(r"Function : (\S+)", out.stdout)
+        dem = subprocess.run([DEMANGLE], input="\n".join(names), capture_output=True, text=True, timeout=60)
+    except (FileNotFoundError, subprocess.TimeoutExpired) as e:
+        pytest.skip(f"cuobjdump / c++filt unavailable: {e}")
+    found = set(re.findall(r"\b(maxsim_\w*_kernel|flat_ip_tc\w*_kernel)<", dem.stdout))
+    owned = set(C.KERNELS) | set(flat_ip_cases.KERNELS) | set(test_maxsim_inbatch_bwd_cpu.KERNELS)
+    assert found, "no max-sim or flat-IP kernel in the library"
+    assert not found - owned, f"kernels no instantiation matrix names: {sorted(found - owned)}"
 
 
 def test_empty_batch_is_accepted_at_the_abi():

@@ -6,7 +6,10 @@ The inputs are small integers, so every kernel's fp32 arithmetic is exact: score
 bit-exactly to the fp64 oracle (colbert.py:68-75 with an explicit argmax).  NaN / +-inf in masked query tokens, masked
 document rows, rows past a passage's max_doc_len and the memory after the document tensor must change nothing.  The
 end-to-end autograd test runs real values at the reference configuration against fp64 autograd of the reference
-expression; its worst error / scale per gradient is recorded as a test property (``--junitxml``)."""
+expression; its worst error / scale per gradient is recorded as a test property (``--junitxml``).  The e4m3 and
+residual store rows are held bit-exactly to the fp64 store oracle, to the 16-bit kernel on the same values, and under a
+permutation of their pairs; the premise of the exact e4m3 rows (the FP8 MMA sums below 2^11 grains exactly, subnormals
+kept) has its own test."""
 import ctypes
 import functools
 
@@ -67,8 +70,63 @@ def _exact(got, ref, what):
                            f"{got[bad][0].item()} vs {ref[bad][0].item()}")
 
 
+@functools.lru_cache(maxsize=2)
+def _coded(row: C.Row, bits: int):
+    """An e4m3 or residual store row on the device, with its oracle scores."""
+    c = C.make_store_case(row, bits)
+    P = {"c": c, "score": C.store_oracle(c, row.Ld), "offsets": c.offsets.to(DEV),
+         "pair_q": c.pair_q.to(torch.int32).to(DEV), "pair_d": c.pair_d.to(torch.int32).to(DEV)}
+    if row.dtype == C.E4:
+        store8 = c.store.float().to(C.E4)
+        nan = torch.isnan(c.store)
+        assert bool(((store8.view(torch.uint8)[nan] & 0x7F) == 0x7F).all())   # the e4m3 NaN, in rows no pair reads
+        P["q"], P["store"] = c.q.float().to(C.E4).to(DEV), store8.to(DEV)
+    else:
+        P["q"] = c.q.half().to(DEV)
+        P["codes"], P["list_ids"] = c.codes.to(DEV), c.list_ids.to(DEV)
+        P["base"], P["weight"] = c.base.to(DEV), c.weight.to(DEV)
+        P["store"] = c.store.half().to(DEV)   # the decoded rows (NaN where the poison list stands)
+    return P
+
+
+def _call_coded(row: C.Row, P, key, pair_q=None, pair_d=None):
+    pq = P["pair_q"] if pair_q is None else pair_q
+    pd = P["pair_d"] if pair_d is None else pair_d
+    if key[0] == "score":
+        return interaction.maxsim_store(P["q"], P["store"], P["offsets"], pq, pd, row.Ld, impl=key[1])
+    return interaction.maxsim_store_residual(P["q"], P["codes"], P["list_ids"], P["base"], P["weight"], key[1],
+                                             P["offsets"], pq, pd, row.Ld)
+
+
+def _coded_rows_bit_exact(row: C.Row):
+    """Every path of an e4m3 / residual store row against the fp64 store oracle; two runs; a permutation of the pairs;
+    the 16-bit documents-on-M kernel on the same values (e4m3) or on the decoded rows (residual) where it takes the
+    shape."""
+    runs = C.runs(row, _smem())
+    fp16_docm = C.route(C.H, row.Lq, row.Ld, row.dim, "tcgen05_docm", store=True, smem=_smem())
+    for key, name in runs.items():
+        P = _coded(row, 0 if key[0] == "score" else key[1])
+        if name is None:
+            with pytest.raises(_lib.MatchmakerB200Error):
+                _call_coded(row, P, key)
+            continue
+        got = _call_coded(row, P, key)
+        _exact(got, P["score"], f"{row} {key} ({name})")
+        assert torch.equal(_call_coded(row, P, key), got), f"{row} {key}: two runs differ"
+        perm = torch.randperm(row.n_pairs, generator=torch.Generator().manual_seed(row.seed)).to(DEV)
+        permuted = _call_coded(row, P, key, P["pair_q"][perm], P["pair_d"][perm])
+        assert torch.equal(permuted, got[perm]), f"{row} {key}: permuted pairs"
+        if fp16_docm is not None and key != ("score", "tcgen05_docm"):
+            q16 = P["q"].half() if row.dtype == C.E4 else P["q"]
+            h = interaction.maxsim_store(q16, P["store"].half(), P["offsets"], P["pair_q"], P["pair_d"], row.Ld,
+                                         impl="tcgen05_docm")
+            assert torch.equal(h, got), f"{row} {key}: the fp16 kernel {fp16_docm} on the same values differs"
+
+
 @pytest.mark.parametrize("row", C.MATRIX, ids=str)
 def test_scores_bit_exact_on_every_path(row):
+    if row.coded:
+        return _coded_rows_bit_exact(row)
     runs = C.runs(row, _smem())
     for impl in C.IMPLS:
         if runs[("score", impl)] is None:
@@ -80,7 +138,7 @@ def test_scores_bit_exact_on_every_path(row):
             _exact(got, _prepared(row)["score"], f"{row} {impl} ({runs[('score', impl)]}) poisoned={poisoned}")
 
 
-@pytest.mark.parametrize("row", [r for r in C.MATRIX if r.mode != "store"], ids=str)
+@pytest.mark.parametrize("row", [r for r in C.MATRIX if r.mode in ("pairs", "inbatch")], ids=str)
 def test_argmax_bit_exact_on_both_producers(row):
     runs = C.runs(row, _smem())
     P = _prepared(row)
@@ -217,3 +275,91 @@ def test_envelope_edge_per_dim(dim, train):
         assert out.item() == 12345.0 and (am is None or (am == -7).all()), "a kernel ran"
         with pytest.raises(_lib.MatchmakerB200Error):
             interaction.maxsim(cq, cd, cqm, cdm, return_argmax=train)
+
+
+def _one_row_passages(q: torch.Tensor, rows: torch.Tensor):
+    """maxsim_store over e4m3 passages of one row each with a one-token query: the dot product of every row."""
+    n = rows.shape[0]
+    off = torch.arange(n + 1, dtype=torch.int64, device=DEV)
+    pd = torch.arange(n, dtype=torch.int32, device=DEV)
+    return interaction.maxsim_store(q.view(1, 1, -1).to(C.E4).to(DEV), rows.to(C.E4).to(DEV), off,
+                                    torch.zeros(n, dtype=torch.int32, device=DEV), pd, 1)
+
+
+def test_fp8_mma_accumulates_exactly():
+    """The premise of the exact e4m3 rows, at dim 1024 (32 k32 steps): sums of products below 2^11 grains come out
+    exact in both e4m3 kernels (max-sim and the flat top-k), whatever the order: partial sums at the bound before the
+    last k32 step with a +-1 product in it, a large early sum cancelled back to a small total, and the grain at 2^-9
+    (e4m3 subnormals).  Fails if the FP8 MMA drops low bits of its accumulator or flushes subnormal inputs."""
+    dim = 1024
+    q = torch.zeros(dim, dtype=torch.float64)
+    rows = []
+    # 2046 in the first 992 dimensions (511 products of 4, one of 2), then +-1 in the last k32 step
+    qa = q.clone()
+    qa[:512] = 2.0
+    qa[1000] = 1.0
+    for last in (1.0, -1.0):
+        r = torch.zeros(dim, dtype=torch.float64)
+        r[:511], r[511] = 2.0, 1.0
+        r[1000] = last
+        rows.append(r)
+    # +1024 in the first 16 steps, -1020 in the next 8, +1 in the last: 5 out of a mass of 2045
+    qb = q.clone()
+    qb[:512], qb[512:767], qb[1000] = 2.0, 4.0, 1.0
+    r = torch.zeros(dim, dtype=torch.float64)
+    r[:512], r[512:767], r[1000] = 1.0, -1.0, 1.0
+    rows.append(r)
+    # the grain at 2^-9: one subnormal product, and 2047 of them
+    sub1 = torch.zeros(dim, dtype=torch.float64)
+    sub1[1023] = 2.0 ** -9
+    sub2 = torch.zeros(dim, dtype=torch.float64)
+    sub2[:1023] = 2.0 ** -9
+    sub2[1023] = 2.0 ** -8
+    cases = [(qa, rows[0]), (qa, rows[1]), (qb, rows[2]), (torch.ones(dim, dtype=torch.float64), sub1),
+             (torch.ones(dim, dtype=torch.float64), sub2)]
+    for i, (qq, r) in enumerate(cases):
+        assert torch.equal(qq.to(C.E4).double(), qq) and torch.equal(r.to(C.E4).double(), r)
+        grain = 2.0 ** -9 if (r != r.round()).any() else 1.0
+        mass = float((qq * r).abs().sum()) / grain
+        assert mass < C.E4M3_EXACT_GRAINS, (i, mass)
+        want = float((qq * r).sum())
+        got = _one_row_passages(qq, r.view(1, -1)).item()
+        assert got == want, f"case {i}: max-sim {got} vs {want} (mass {mass} grains)"
+        s, _ = interaction.flat_ip_topk(qq.view(1, -1).to(C.E4).to(DEV), r.view(1, -1).to(C.E4).to(DEV), 1)
+        assert s.item() == want, f"case {i}: flat top-k {s.item()} vs {want}"
+
+
+@pytest.mark.parametrize("dim", list(range(64, 1025, 64)))
+def test_e4m3_and_residual_envelope_edge_per_dim(dim):
+    """The last Lq each coded store kernel runs at this dim matches the oracle, and the next one is refused."""
+    g = torch.Generator().manual_seed(dim)
+    off = torch.tensor([0, 5, 9], dtype=torch.int64)
+    pq, pd = torch.tensor([0, 0, 0], dtype=torch.int32), torch.tensor([1, -1, 0], dtype=torch.int32)
+    kinds = [("residual", b, C.last_lq_residual(dim, b, _smem())) for b in C.RESIDUAL_BITS]
+    if dim % 128 == 0:
+        kinds.append(("e4m3", 0, C.last_lq_e4m3(dim, _smem())))
+    for kind, bits, last in kinds:
+        for Lq in (last, last + 1):
+            q = torch.randint(-1, 2, (1, Lq, dim), generator=g).double()
+            if kind == "e4m3":
+                store = torch.randint(-2, 3, (9, dim), generator=g).double()
+                c = C.StoreCase(q, store, off, pq.long(), pd.long())
+                call = functools.partial(interaction.maxsim_store, q.float().to(C.E4).to(DEV),
+                                         store.float().to(C.E4).to(DEV))
+            else:
+                base = torch.randint(-1, 2, (2, dim), generator=g).half()
+                weight = torch.randint(-2, 3, (dim, 1 << bits), generator=g).half()
+                raw = torch.randint(0, 1 << bits, (9, dim), generator=g)
+                lid = torch.tensor([0, 1, 0, 1, 0, 1, 1, 0, 0], dtype=torch.int32)
+                import colbert_residual_oracle as RO
+                packed = torch.from_numpy(RO.pack(raw.numpy().astype("uint8"), bits))
+                dec = RO.decode(packed.numpy(), lid.numpy(), base.numpy(), weight.numpy(), bits)
+                c = C.StoreCase(q, torch.from_numpy(dec.astype("float64")), off, pq.long(), pd.long())
+                call = functools.partial(interaction.maxsim_store_residual, q.half().to(DEV), packed.to(DEV),
+                                         lid.to(DEV), base.to(DEV), weight.to(DEV), bits)
+            args = (off.to(DEV), pq.to(DEV), pd.to(DEV), 7)
+            if Lq == last:
+                _exact(call(*args), C.store_oracle(c, 7), f"{kind} b{bits} dim {dim} Lq {Lq}")
+            else:
+                with pytest.raises(_lib.MatchmakerB200Error):
+                    call(*args)
