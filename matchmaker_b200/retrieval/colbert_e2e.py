@@ -20,11 +20,8 @@ The store is what the reference's encode loop writes (``token_reps_N.npy`` + ``d
 Multi-GPU: one process per GPU, each rank owns a contiguous range of whole passages (``sharding.passage_shard_bounds``)
 and the per-rank top lists are merged with ``sharding.all_gather_merge``.
 
-``colbert_store_dtype: "float8_e4m3"`` keeps the store as E4M3 values (DESIGN 3.4i): row x is held as
-e4m3(x * 2^s_d), with s_d the scale rule (``interaction.fp8_scale_log2``) over the largest |x| of the whole store (a
-MAX all-reduce over the ranks, so the stored values do not depend on the world size).  A search quantizes each query
-with its own scale s_q, runs both stages on the FP8 tensor cores and multiplies the scores by 2^-(s_q + s_d).  Needs
-token_dim % 128 == 0 and 128 <= token_dim <= 1024; not combined with ``colbert_residual_bits``.
+The token store's format (dense rows, E4M3 or residual codes) is ``colbert_store``'s: the indexer holds one store
+and runs both stages through it.
 """
 from __future__ import annotations
 
@@ -34,23 +31,12 @@ import numpy
 import torch
 
 from .. import _lib, interaction, sharding
-from .base_index import BaseNNIndexer
+from . import colbert_store
+from .base_index import GPUIndexer
+from .colbert_store import fp8_store_scale  # noqa: F401  (public name of this module)
 
 CANDIDATE_CAP = 4096          # candidate passages per query and rank (the topk_unique limit)
 _VOID_SCORE = -3.4028234663852886e38
-STORE_DTYPES = ("float8_e4m3",)   # values of colbert_store_dtype
-FP8_CHUNK_ROWS = 1 << 20          # rows per chunk of an fp8 index(): peak device memory is the store plus one chunk
-
-
-def fp8_store_scale(local_amax: torch.Tensor, group=None) -> int:
-    """The store scale s_d from this rank's largest |x| (a one-element fp32 tensor on the rank's device): the MAX
-    all-reduce over the ranks of ``group`` when torch.distributed is initialized, then the scale rule.  Raises on a
-    non-finite maximum."""
-    import torch.distributed as dist
-    amax = local_amax.reshape(1).to(torch.float32).clone()
-    if dist.is_available() and dist.is_initialized():
-        dist.all_reduce(amax, op=dist.ReduceOp.MAX, group=group)
-    return interaction.fp8_store_scale(float(amax.item()))
 
 
 def doc_offsets_from_id_mapping(id_mapping: List[numpy.ndarray]) -> numpy.ndarray:
@@ -67,43 +53,31 @@ def doc_offsets_from_id_mapping(id_mapping: List[numpy.ndarray]) -> numpy.ndarra
     return numpy.searchsorted(rows, numpy.arange(n_docs + 1, dtype=numpy.int64), side="left").astype(numpy.int64)
 
 
-class ColBERTEndToEndIndexer(BaseNNIndexer):
+def token_store_attribute(name: str, doc: str) -> property:
+    """An attribute of the indexer's token store (``tokens``), read and set under the indexer's name."""
+    return property(lambda self: getattr(self.tokens, name), lambda self, v: setattr(self.tokens, name, v), doc=doc)
+
+
+class ColBERTEndToEndIndexer(GPUIndexer):
+    residual = False   # the store keeps residual codes (ColBERTResidualIndexer)
+    store = token_store_attribute("rows", "[rows of this rank, ...] the stored rows as the kernels read them")
+    store_scale = token_store_attribute("scale", "s_d of an E4M3 store, else None")
+    chunk_rows = token_store_attribute("slab_rows", "rows per slab of a streamed build")
+
     def __init__(self, config, device: Optional[torch.device] = None, process_group=None):
-        super().__init__(config)
-        if not self.use_gpu:
-            raise _lib.MatchmakerB200Error("ColBERTEndToEndIndexer runs on the GPU only (faiss_use_gpu must be True); "
-                                           "there is no CPU fallback")
-        self.store_dtype = torch.float16 if self.use_fp16 else torch.float32   # of the rows (and queries) as given
-        sd = config.get("colbert_store_dtype")
-        if sd is not None:
-            if sd not in STORE_DTYPES:
-                raise _lib.MatchmakerB200Error(f"colbert_store_dtype must be one of {STORE_DTYPES}, got {sd!r}")
-            if self.token_dim % 128 or not 128 <= self.token_dim <= 1024:
-                raise _lib.MatchmakerB200Error(f"the float8_e4m3 token store needs token_dim % 128 == 0 and 128 <= "
-                                               f"token_dim <= 1024, got {self.token_dim}")
-            if config.get("colbert_residual_bits") is not None:
-                raise _lib.MatchmakerB200Error("colbert_store_dtype and colbert_residual_bits are two different token "
-                                               "store formats: configure one of them")
-        self.fp8 = sd == "float8_e4m3"
-        self.store_scale: Optional[int] = None          # s_d of an fp8 store
-        self.saved_store_scale: Optional[int] = None    # s_d recorded by load(): a re-index must reproduce it
-        self.chunk_rows = FP8_CHUNK_ROWS
-        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        self.group = process_group
-        self.store: Optional[torch.Tensor] = None       # [rows of this rank, dim] in store_dtype
-        self.flat: Optional[torch.Tensor] = None        # what flat_ip_topk reads (the fp16 hi / lo split for fp32)
-        self.split_scale = None
+        super().__init__(config, device, process_group)
+        self.tokens = colbert_store.select(config, self.token_dim, self.store_dtype, self.device, process_group,
+                                           self.residual)
         self.row_ids: Optional[torch.Tensor] = None     # [rows] int64 passage id (seq_ids position) of every row
         self.offsets: Optional[torch.Tensor] = None     # [passages of this rank + 1] int64, local row offsets
         self.max_doc_len = 1
         self.d_lo = self.d_hi = 0
         self.n_docs = 0
 
-    def _world(self):
-        import torch.distributed as dist
-        if dist.is_available() and dist.is_initialized():
-            return dist.get_rank(self.group), dist.get_world_size(self.group)
-        return 0, 1
+    @property
+    def fp8(self) -> bool:
+        """The store holds E4M3 rows (``colbert_store_dtype: "float8_e4m3"``)."""
+        return isinstance(self.tokens, colbert_store.E4M3TokenStore)
 
     def index(self, id_mapping: List[numpy.ndarray], storage: List[numpy.ndarray]):
         """id_mapping, storage: the first two results of ``token_storage.load_token_storage`` (per-block row -> passage
@@ -119,23 +93,12 @@ class ColBERTEndToEndIndexer(BaseNNIndexer):
         rank, world = self._world()
         self.n_docs = len(off) - 1
         d_lo, d_hi, r_lo, r_hi = sharding.passage_shard_bounds(off, rank, world) if self.n_docs else (0, 0, 0, 0)
-        self.d_lo, self.d_hi = d_lo, d_hi
-        if self.fp8:   # every rank takes part in the all-reduce of the store scale, with or without rows
-            def load(a, b):
-                with torch.cuda.device(self.device):
-                    return blocks_to_device(storage, r_lo + a, r_lo + b, self.device)
-            self._index_fp8(load, r_hi - r_lo)
-            if r_hi > r_lo:
-                self._set_passages(off[d_lo:d_hi + 1] - r_lo, d_lo)
-            else:
-                self.offsets, self.row_ids = None, None
-        elif r_hi > r_lo:
+
+        def load(a, b):
             with torch.cuda.device(self.device):
-                rows = blocks_to_device(storage, r_lo, r_hi, self.device)
-            self.index_device(rows, off[d_lo:d_hi + 1] - r_lo, d_lo)
-        else:
-            self.store = torch.empty((0, self.token_dim), dtype=self.store_dtype, device=self.device)
-            self.flat, self.offsets, self.row_ids = self.store, None, None
+                return blocks_to_device(storage, r_lo + a, r_lo + b, self.device)
+        # every rank builds, with or without rows: the E4M3 store scale is an all-reduce
+        self._build(load, r_hi - r_lo, off[d_lo:d_hi + 1] - r_lo, d_lo)
 
     def index_device(self, rows: torch.Tensor, doc_offsets: numpy.ndarray, first_doc: int = 0):
         """Index this rank's passages from a device tensor: rows [n_rows, token_dim]; passage first_doc + d is rows
@@ -144,14 +107,12 @@ class ColBERTEndToEndIndexer(BaseNNIndexer):
         if rows.dim() != 2 or rows.shape[1] != self.token_dim or off[0] != 0 or off[-1] != rows.shape[0] or \
                 (numpy.diff(off) < 0).any():
             raise _lib.MatchmakerB200Error("index_device: rows [n_rows, token_dim] and non-decreasing offsets from 0")
-        if self.fp8:
-            self._index_fp8(lambda a, b: rows[a:b].to(self.device), rows.shape[0])
-        else:
-            self.store = rows.to(self.device, self.store_dtype)
-            if self.store_dtype == torch.float16:
-                self.flat, self.split_scale = self.store, None
-            else:
-                self.flat, self.split_scale = interaction.flat_ip_split_f32(self.store, "passages")
+        self._build(lambda a, b: rows[a:b].to(self.device), rows.shape[0], off, first_doc)
+
+    def _build(self, load, n: int, off: numpy.ndarray, first_doc: int):
+        """The store of this rank's n rows (``load(a, b)``: rows [a, b) on the device), and its passages: passage
+        first_doc + d is rows [off[d], off[d+1])."""
+        self.tokens.build(load, n)
         self._set_passages(off, first_doc)
 
     def _set_passages(self, off: numpy.ndarray, first_doc: int):
@@ -161,43 +122,11 @@ class ColBERTEndToEndIndexer(BaseNNIndexer):
         self.row_ids = torch.repeat_interleave(torch.arange(first_doc, first_doc + len(off) - 1, device=self.device), lens)
         self.d_lo, self.d_hi = first_doc, first_doc + len(off) - 1
 
-    def _index_fp8(self, load, n: int):
-        """The fp8 store of this rank's n rows, streamed: ``load(a, b)`` returns rows [a, b) on the device.  Pass 1 takes
-        the largest |x|, the all-reduce makes it the store's, pass 2 quantizes each chunk into the preallocated store
-        (``_fp8_chunk`` sees every chunk first).  Peak device memory: the store plus one chunk and its fp32 copy."""
-        amax = torch.zeros((), dtype=torch.float32, device=self.device)
-        for a in range(0, n, self.chunk_rows):
-            lo, hi = torch.aminmax(load(a, min(n, a + self.chunk_rows)))
-            amax = torch.maximum(amax, torch.maximum(hi, -lo).float())
-        s = fp8_store_scale(amax, self.group)
-        if self.saved_store_scale is not None and s != self.saved_store_scale:
-            raise _lib.MatchmakerB200Error(f"the loaded index was built for an fp8 store with scale 2^{self.saved_store_scale}"
-                                           f", these rows give 2^{s}: re-index without load()")
-        self.store = torch.empty((n, self.token_dim), dtype=torch.float8_e4m3fn, device=self.device)
-        for a in range(0, n, self.chunk_rows):
-            b = min(n, a + self.chunk_rows)
-            rows = load(a, b)
-            self._fp8_chunk(rows, a, b, n)
-            self.store[a:b] = interaction.fp8_quantize(rows, s)
-            del rows
-        self.flat, self.split_scale, self.store_scale = self.store, None, s
-
-    def _fp8_chunk(self, rows: torch.Tensor, a: int, b: int, n: int):
-        """Rows [a, b) of n, as given, before they are quantized (a subclass's hook)."""
-
-    def _score_queries(self, q: torch.Tensor):
-        """(what the kernels read, per-query scale or None): an fp8 store scores e4m3 queries, each scaled by its own
-        largest |x| (on the device, no host synchronisation)."""
-        if not self.fp8:
-            return q, None
-        sq = interaction.fp8_scale_log2(q.abs().amax(dim=(1, 2)))
-        return interaction.fp8_quantize(q, sq), sq
-
     def search(self, query_vec: numpy.ndarray, top_n: int, token_top_k: Optional[int] = None):
         """query_vec [Nq, Lq, dim] (the query_encode output of ColBERT.forward_representation: padded tokens are
         all-zero rows).  Returns (scores [Nq, top_n] f32, ids [Nq, top_n] i64): ids are positions in ``seq_ids``,
         missing results (-3.4028235e38, -1)."""
-        if self.store is None:
+        if self.tokens.rows is None:
             raise _lib.MatchmakerB200Error("search() before index()")
         q = torch.from_numpy(numpy.ascontiguousarray(query_vec))
         if q.dim() == 2:
@@ -207,7 +136,7 @@ class ColBERTEndToEndIndexer(BaseNNIndexer):
 
     def search_device(self, q: torch.Tensor, top_n: int, token_top_k: Optional[int] = None):
         """search() with device tensors in and out.  token_top_k (k') defaults to min(top_n, 1024)."""
-        if self.store is None:
+        if self.tokens.rows is None:
             raise _lib.MatchmakerB200Error("search() before index()")
         if q.dim() != 3 or q.shape[-1] != self.token_dim:
             raise _lib.MatchmakerB200Error(f"expected queries [Nq, Lq, {self.token_dim}], got {tuple(q.shape)}")
@@ -219,7 +148,7 @@ class ColBERTEndToEndIndexer(BaseNNIndexer):
         rank, world = self._world()
         nq, lq, dim = q.shape
         q = q.to(self.device, self.store_dtype).contiguous()
-        if self.store.shape[0] == 0:
+        if self.tokens.rows.shape[0] == 0:
             s = torch.full((nq, top_n), _VOID_SCORE, device=self.device)
             i = torch.full((nq, top_n), -1, dtype=torch.int64, device=self.device)
         else:
@@ -231,28 +160,30 @@ class ColBERTEndToEndIndexer(BaseNNIndexer):
     def candidates_device(self, q: torch.Tensor, kp: int, qs: Optional[torch.Tensor] = None):
         """Stage 1 on this rank: (best single-token score, passage id) [Nq, C] of every candidate passage, best first;
         void entries are (-3.4028235e38, -1).  q [Nq, Lq, dim] in the store dtype on the device; qs what the scan
-        reads (``_score_queries(q)[0]``, computed here when not given).  With an fp8 store the scores are in the
+        reads (``tokens.queries(q)[0]``, computed here when not given).  With an E4M3 store the scores are in the
         scaled domain of each query."""
         nq, lq, dim = q.shape
         toks = q.reshape(nq * lq, dim)
-        stoks = (self._score_queries(q)[0] if qs is None else qs).reshape(nq * lq, dim)
-        # token hits -> passage ids; all-zero query rows are padding and their hits are voided
-        hs, hi = interaction.flat_ip_topk(stoks, self.flat, kp, ids=self.row_ids, split_scale=self.split_scale)
-        pad = (toks == 0).all(dim=1, keepdim=True)
-        hs = hs.masked_fill(pad, float("-inf"))
+        stoks = (self.tokens.queries(q)[0] if qs is None else qs).reshape(nq * lq, dim)
+        hs, hi = self._scan(toks, stoks, kp)
         c = min(lq * kp, CANDIDATE_CAP)
         return interaction.topk_unique(hs.view(nq, lq * kp), hi.view(nq, lq * kp), c)
 
+    def _scan(self, toks, stoks, kp: int):
+        """The kp best (score, passage id) of every query token (toks as given, stoks as the store reads them):
+        token hits -> passage ids; all-zero query rows are padding and their hits are voided."""
+        hs, hi = self.tokens.scan(stoks, kp, self.row_ids)
+        pad = (toks == 0).all(dim=1, keepdim=True)
+        return hs.masked_fill(pad, float("-inf")), hi
+
     def _search_local(self, q: torch.Tensor, top_n: int, kp: int):
         nq = q.shape[0]
-        qs, sq = self._score_queries(q)
+        qs, sq = self.tokens.queries(q)
         _, cand = self.candidates_device(q, kp, qs)
         c = cand.shape[1]
         # stage 2: exact max-sim of every candidate; void candidates (id -1) are skipped and score -inf
         pair_d = torch.where(cand >= 0, cand - self.d_lo, torch.full_like(cand, -1))
         pair_q = torch.arange(nq, device=self.device, dtype=torch.int32).repeat_interleave(c)
-        scores = interaction.maxsim_store(qs, self.store, self.offsets, pair_q, pair_d, self.max_doc_len).view(nq, c)
+        scores = self.tokens.maxsim(qs, self.offsets, pair_q, pair_d, self.max_doc_len).view(nq, c)
         s, i = interaction.topk_merge(scores, cand, top_n)
-        if sq is not None:   # a positive per-query factor: the ranking above is the unscaled one
-            s = interaction.fp8_unscale(s, sq + self.store_scale)
-        return s, i
+        return self.tokens.unscale(s, sq), i

@@ -17,29 +17,16 @@ import numpy
 import torch
 
 from .. import _lib, interaction, sharding
-from .base_index import BaseNNIndexer
+from .base_index import GPUIndexer
 
 
-class FlatIPIndexer(BaseNNIndexer):
+class FlatIPIndexer(GPUIndexer):
     def __init__(self, config, device: Optional[torch.device] = None, process_group=None):
-        super().__init__(config)
-        if not self.use_gpu:
-            raise _lib.MatchmakerB200Error("FlatIPIndexer runs on the GPU only (faiss_use_gpu must be True); "
-                                           "there is no CPU fallback")
-        # token_dtype float16 -> fp16 storage (faiss useFloat16, faiss_indices.py:65); anything else -> fp32 storage
-        self.store_dtype = torch.float16 if self.use_fp16 else torch.float32
-        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        self.group = process_group
+        super().__init__(config, device, process_group)
         self.passages: Optional[torch.Tensor] = None   # [n_local, dim] fp16 on self.device
         self.ids: Optional[torch.Tensor] = None        # [n_local] int64
         self.n_total = 0
         self.split_scale = None
-
-    def _world(self):
-        import torch.distributed as dist
-        if dist.is_available() and dist.is_initialized():
-            return dist.get_rank(self.group), dist.get_world_size(self.group)
-        return 0, 1
 
     def index(self, ids: List[numpy.ndarray], data_chunks: List[numpy.ndarray]):
         """ids: list of int64 arrays; data_chunks: list of [n_i, token_dim] arrays (the fp16 memmaps of
@@ -114,10 +101,6 @@ class FlatIPIndexer(BaseNNIndexer):
         s, i = interaction.topk_unique(s, i, top_n)
         return s.cpu().numpy(), i.cpu().numpy()
 
-    def _shard_path(self, path: str) -> str:
-        rank, world = self._world()
-        return path if world == 1 else f"{path}.rank{rank}of{world}"
-
     def save(self, path: str):
         """dense_retrieval.py calls indexer.save(run_folder/faiss.index) after index().  One file per rank
         (`<path>.rank<r>of<w>` when the job has more than one rank -- every rank owns a different slab, so they must
@@ -128,18 +111,8 @@ class FlatIPIndexer(BaseNNIndexer):
                     "token_dtype": str(self.store_dtype)}, self._shard_path(path))
 
     def load(self, path: str, config_overwrites=None):
-        rank, world = self._world()
-        blob = torch.load(self._shard_path(path))
-        saved_world, saved_rank = blob.get("world", 1), blob.get("rank", 0)
-        lo, hi = sharding.shard_bounds(blob["n_total"], rank, world)
-        if saved_world != world or saved_rank != rank or (blob.get("lo", lo), blob.get("hi", hi)) != (lo, hi):
-            raise _lib.MatchmakerB200Error(
-                f"index file {self._shard_path(path)} holds rows [{blob.get('lo')},{blob.get('hi')}) of rank {saved_rank} of "
-                f"{saved_world}; this job is rank {rank} of {world} and needs rows [{lo},{hi}) -- re-index or load with the "
-                "same world size")
-        if blob.get("token_dtype", "torch.float16") != str(self.store_dtype):
-            raise _lib.MatchmakerB200Error(f"index file was written with token_dtype {blob.get('token_dtype')}, this indexer "
-                                           f"is configured for {self.store_dtype}")
+        blob = self._load_shard(self._shard_path(path))
+        lo, hi = sharding.shard_bounds(blob["n_total"], *self._world())
         self.passages, self.split_scale = blob["passages"].to(self.device), blob.get("split_scale")
         self.ids = blob["ids"].to(self.device)
         self.n_total, self.lo, self.hi = blob["n_total"], lo, hi

@@ -25,7 +25,7 @@ import numpy
 import torch
 
 from .. import _lib, interaction, sharding
-from .base_index import BaseNNIndexer
+from .base_index import GPUIndexer
 
 GRAPH_SEED = 1234
 KNN_WORKSPACE_CAP = 2 << 30   # device scratch of one k-NN batch of flat_ip_topk
@@ -134,31 +134,23 @@ def reverse_merge(pruned: torch.Tensor) -> torch.Tensor:
     return out
 
 
-class GraphIndexer(BaseNNIndexer):
+class GraphIndexer(GPUIndexer):
     """faiss_index_type "hnsw" on the GPU.  ``faiss_use_gpu`` is read and ignored (see the module docstring)."""
+    gpu_only = False
 
     def __init__(self, config, device: Optional[torch.device] = None, process_group=None):
-        super().__init__(config)
+        super().__init__(config, device, process_group)
         self.M = int(config["faiss_hnsw_graph_neighbors"])
         self.ef_construction = int(config["faiss_hnsw_efConstruction"])
         self.ef_search = int(config["faiss_hnsw_efSearch"])
         self.R, self.K = graph_degrees(self.M, self.ef_construction)
         search_list_size(self.ef_search, 1)
-        self.store_dtype = torch.float16 if self.use_fp16 else torch.float32
-        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        self.group = process_group
         self.rows: Optional[torch.Tensor] = None         # [n_local, dim] fp16 / fp32
         self.ids: Optional[torch.Tensor] = None          # [n_local] int64
         self.graph: Optional[torch.Tensor] = None        # [n_local, R] int32 row positions, -1 padded
         self.entry_pos: Optional[torch.Tensor] = None    # [E] int64 row positions
         self.entry_store, self.entry_scale = None, None  # the entry rows as flat_ip_topk reads them
         self.n_total = 0
-
-    def _world(self):
-        import torch.distributed as dist
-        if dist.is_available() and dist.is_initialized():
-            return dist.get_rank(self.group), dist.get_world_size(self.group)
-        return 0, 1
 
     def prepare(self, data_chunks: List[numpy.ndarray], subsample=-1):
         """Nothing to train (the reference's prepare only trains faiss's fp16 scalar quantizer)."""
@@ -242,10 +234,6 @@ class GraphIndexer(BaseNNIndexer):
         return s.cpu().numpy(), i.cpu().numpy()
 
     # ------------------------------------------------------------------ persistence
-    def _shard_path(self, path: str) -> str:
-        rank, world = self._world()
-        return path if world == 1 else f"{path}.rank{rank}of{world}"
-
     def save(self, path: str):
         """One file per rank (`<path>.rank<r>of<w>` with more than one rank), holding its row range, the world size it
         was cut for, the graph and the entry sample."""
@@ -258,18 +246,8 @@ class GraphIndexer(BaseNNIndexer):
 
     def load(self, path: str, config_overwrites=None):
         """efSearch comes from config_overwrites["faiss_hnsw_efSearch"] when given, else from the file."""
-        rank, world = self._world()
-        blob = torch.load(self._shard_path(path))
-        saved_world, saved_rank = blob["world"], blob["rank"]
-        lo, hi = sharding.shard_bounds(blob["n_total"], rank, world)
-        if saved_world != world or saved_rank != rank or (blob["lo"], blob["hi"]) != (lo, hi):
-            raise _lib.MatchmakerB200Error(
-                f"index file {self._shard_path(path)} holds rows [{blob['lo']},{blob['hi']}) of rank {saved_rank} of "
-                f"{saved_world}; this job is rank {rank} of {world} and needs rows [{lo},{hi}) -- re-index or load with the "
-                "same world size")
-        if blob["token_dtype"] != str(self.store_dtype):
-            raise _lib.MatchmakerB200Error(f"index file was written with token_dtype {blob['token_dtype']}, this indexer "
-                                           f"is configured for {self.store_dtype}")
+        blob = self._load_shard(self._shard_path(path))
+        lo, hi = sharding.shard_bounds(blob["n_total"], *self._world())
         self.M, self.ef_construction, self.ef_search = int(blob["M"]), int(blob["ef_construction"]), int(blob["ef_search"])
         if config_overwrites and "faiss_hnsw_efSearch" in config_overwrites:
             self.ef_search = int(config_overwrites["faiss_hnsw_efSearch"])

@@ -23,7 +23,7 @@ import numpy
 import torch
 
 from .. import _lib, interaction, sharding
-from .base_index import BaseNNIndexer
+from .base_index import GPUIndexer
 
 KMEANS_ITERATIONS = 10
 KMEANS_MAX_POINTS_PER_LIST = 256     # training uses at most this many points per list (a seeded subsample)
@@ -32,19 +32,13 @@ _SPLIT_EPS = 1.0 / 1024.0            # relative perturbation when an empty list 
 _NO_RESULT = -3.4028234663852886e38
 
 
-class IVFIndexer(BaseNNIndexer):
+class IVFIndexer(GPUIndexer):
     def __init__(self, config, device: Optional[torch.device] = None, process_group=None):
-        super().__init__(config)
-        if not self.use_gpu:
-            raise _lib.MatchmakerB200Error("IVFIndexer runs on the GPU only (faiss_use_gpu must be True); "
-                                           "there is no CPU fallback")
+        super().__init__(config, device, process_group)
         self.nlist = int(config["faiss_ivf_list_count"])
         self.nprobe = int(config["faiss_ivf_search_probe_count"])
         if self.nlist < 1 or self.nprobe < 1:
             raise _lib.MatchmakerB200Error("faiss_ivf_list_count and faiss_ivf_search_probe_count must be >= 1")
-        self.store_dtype = torch.float16 if self.use_fp16 else torch.float32
-        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        self.group = process_group
         self.centroids: Optional[torch.Tensor] = None    # [nlist, dim] f32, unit rows
         self.rows: Optional[torch.Tensor] = None         # [n_local, dim] fp16 or [n_local, 2*dim] split, sorted by list
         self.split_scale = None
@@ -54,12 +48,6 @@ class IVFIndexer(BaseNNIndexer):
         self.n_total = 0
         self.train_objective: List[float] = []           # sum of the assigned inner products, per iteration
         self.train_splits: List[int] = []                # empty lists re-seeded after each iteration
-
-    def _world(self):
-        import torch.distributed as dist
-        if dist.is_available() and dist.is_initialized():
-            return dist.get_rank(self.group), dist.get_world_size(self.group)
-        return 0, 1
 
     # ------------------------------------------------------------------ training
     def prepare(self, data_chunks: List[numpy.ndarray], subsample=-1):
@@ -252,10 +240,6 @@ class IVFIndexer(BaseNNIndexer):
         return s.cpu().numpy(), i.cpu().numpy()
 
     # ------------------------------------------------------------------ persistence
-    def _shard_path(self, path: str) -> str:
-        rank, world = self._world()
-        return path if world == 1 else f"{path}.rank{rank}of{world}"
-
     def save(self, path: str):
         """One file per rank (`<path>.rank<r>of<w>` with more than one rank), holding its row range, the world size it
         was cut for and the centroids."""
@@ -268,18 +252,8 @@ class IVFIndexer(BaseNNIndexer):
 
     def load(self, path: str, config_overwrites=None):
         """nprobe comes from config_overwrites["faiss_ivf_search_probe_count"] when given, else from the file."""
-        rank, world = self._world()
-        blob = torch.load(self._shard_path(path))
-        saved_world, saved_rank = blob["world"], blob["rank"]
-        lo, hi = sharding.shard_bounds(blob["n_total"], rank, world)
-        if saved_world != world or saved_rank != rank or (blob["lo"], blob["hi"]) != (lo, hi):
-            raise _lib.MatchmakerB200Error(
-                f"index file {self._shard_path(path)} holds rows [{blob['lo']},{blob['hi']}) of rank {saved_rank} of "
-                f"{saved_world}; this job is rank {rank} of {world} and needs rows [{lo},{hi}) -- re-index or load with the "
-                "same world size")
-        if blob["token_dtype"] != str(self.store_dtype):
-            raise _lib.MatchmakerB200Error(f"index file was written with token_dtype {blob['token_dtype']}, this indexer "
-                                           f"is configured for {self.store_dtype}")
+        blob = self._load_shard(self._shard_path(path))
+        lo, hi = sharding.shard_bounds(blob["n_total"], *self._world())
         self.nlist = int(blob["nlist"])
         self.nprobe = int(blob["nprobe"])
         if config_overwrites and "faiss_ivf_search_probe_count" in config_overwrites:

@@ -29,7 +29,7 @@ import numpy
 import torch
 
 from .. import _lib, interaction, sharding
-from .base_index import BaseNNIndexer
+from .base_index import GPUIndexer
 from .ivf_index import IVFIndexer
 
 AH_THRESHOLD = 0.2            # ScaNN's anisotropic_quantization_threshold
@@ -218,18 +218,16 @@ def encode(r: torch.Tensor, xhat: torch.Tensor, codebook: torch.Tensor, eta: flo
     return coordinate_descent(r, xhat, codebook, nearest_codes(r, codebook), eta, sweeps)
 
 
-class ScaNNIndexer(BaseNNIndexer):
+class ScaNNIndexer(GPUIndexer):
     """faiss_index_type "scann" on the GPU.  ``faiss_use_gpu`` is read and ignored (see the module docstring)."""
+    gpu_only = False
 
     def __init__(self, config, device: Optional[torch.device] = None, process_group=None):
-        super().__init__(config)
+        super().__init__(config, device, process_group)
         self.top_n = build_top_n(config)
         shortlist_size(self.top_n, 1)
         if int(self.token_dim) % 64:
             raise _lib.MatchmakerB200Error(f"token_dim = {self.token_dim}: the AH index needs a multiple of 64")
-        self.store_dtype = torch.float16 if self.use_fp16 else torch.float32
-        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        self.group = process_group
         self.eta = anisotropic_eta(int(self.token_dim))
         self.nlist = self.nprobe = 0
         self.ivf: Optional[IVFIndexer] = None            # leaves: centroids, layout
@@ -243,12 +241,6 @@ class ScaNNIndexer(BaseNNIndexer):
         self.n_total = 0
         self.train_loss: List[float] = []
         self.build_seconds = {}
-
-    def _world(self):
-        import torch.distributed as dist
-        if dist.is_available() and dist.is_initialized():
-            return dist.get_rank(self.group), dist.get_world_size(self.group)
-        return 0, 1
 
     def _leaves(self, nlist: int, nprobe: int):
         self.nlist, self.nprobe = nlist, nprobe
@@ -428,20 +420,8 @@ class ScaNNIndexer(BaseNNIndexer):
                     "top_n": self.top_n, "train_loss": self.train_loss}, self._shard_file(path))
 
     def load(self, path: str):
-        rank, world = self._world()
-        f = self._shard_file(path)
-        if not os.path.isfile(f):
-            raise _lib.MatchmakerB200Error(f"{f} not found: the index in {path} was not saved by {world} rank(s) -- "
-                                           "re-index or load with the same world size")
-        blob = torch.load(f)
-        lo, hi = sharding.shard_bounds(blob["n_total"], rank, world)
-        if blob["world"] != world or blob["rank"] != rank or (blob["lo"], blob["hi"]) != (lo, hi):
-            raise _lib.MatchmakerB200Error(
-                f"index file {f} holds rows [{blob['lo']},{blob['hi']}) of rank {blob['rank']} of {blob['world']}; this "
-                f"job is rank {rank} of {world} and needs rows [{lo},{hi}) -- re-index or load with the same world size")
-        if blob["token_dtype"] != str(self.store_dtype):
-            raise _lib.MatchmakerB200Error(f"index file was written with token_dtype {blob['token_dtype']}, this indexer "
-                                           f"is configured for {self.store_dtype}")
+        blob = self._load_shard(self._shard_file(path))
+        lo, hi = sharding.shard_bounds(blob["n_total"], *self._world())
         self._leaves(int(blob["nlist"]), int(blob["nprobe"]))
         self.ivf.set_centroids(blob["centroids"])
         self.codebook = blob["codebook"].to(self.device)

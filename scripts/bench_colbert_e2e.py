@@ -94,8 +94,8 @@ def main():
         toks = q.reshape(nq * lq, args.dim)
         c = min(lq * kp, 4096)
         st = {}
-        st["stage1"] = timed(lambda: interaction.flat_ip_topk(toks, idx.flat, kp, ids=idx.row_ids), args.reps, args.warmup)
-        hs, hi = interaction.flat_ip_topk(toks, idx.flat, kp, ids=idx.row_ids)
+        st["stage1"] = timed(lambda: interaction.flat_ip_topk(toks, idx.tokens.flat, kp, ids=idx.row_ids), args.reps, args.warmup)
+        hs, hi = interaction.flat_ip_topk(toks, idx.tokens.flat, kp, ids=idx.row_ids)
         st["unique"] = timed(lambda: interaction.topk_unique(hs.view(nq, lq * kp), hi.view(nq, lq * kp), c),
                              args.reps, args.warmup)
         _, cand = interaction.topk_unique(hs.view(nq, lq * kp), hi.view(nq, lq * kp), c)
@@ -124,7 +124,7 @@ def main():
     kp = args.token_top_k[0]
     c = min(lq * kp, 4096)
     toks = q.reshape(nq * lq, args.dim)
-    hs, hi = interaction.flat_ip_topk(toks, idx.flat, kp, ids=idx.row_ids)
+    hs, hi = interaction.flat_ip_topk(toks, idx.tokens.flat, kp, ids=idx.row_ids)
     _, cand = interaction.topk_unique(hs.view(nq, lq * kp), hi.view(nq, lq * kp), c)
     keep = (cand >= 0).reshape(-1)
     pair_d = cand.reshape(-1)[keep]

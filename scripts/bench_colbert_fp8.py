@@ -66,7 +66,7 @@ def run_point(args, dim, passages, nprobe, dev, g):
     t = {f"{k}_{s}": [] for k in idx for s in ("stage1", "stage2", "e2e")}
     cands, stage2 = {}, {}
     for k, x in idx.items():
-        qs = x._score_queries(q)[0]
+        qs = x.tokens.queries(q)[0]
         cands[k] = x.candidates_device(q, kp, qs)[1]
         pair_d = cands[k]
         pair_q = torch.arange(nq, device=dev, dtype=torch.int32).repeat_interleave(c)

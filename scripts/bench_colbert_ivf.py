@@ -75,18 +75,14 @@ def main():
     torch.cuda.synchronize()
     t1 = time.perf_counter()
     # index_device(exact.store) shares the exact indexer's rows: both indexers read the same HBM copy
-    ColBERTEndToEndIndexer.index_device(ivf, exact.store, off_np)
-    assign = ivf.assign(ivf.store)
+    ivf.index_device(exact.store, off_np)
     torch.cuda.synchronize()
     t2 = time.perf_counter()
-    ivf._set_layout(*ivf.ivf._layout(assign))
-    torch.cuda.synchronize()
-    t3 = time.perf_counter()
-    del assign, store
+    del store
     lens = (ivf.list_offsets[1:] - ivf.list_offsets[:-1]).float()
     res = {"card": torch.cuda.get_device_name(dev), "power_limit_w": power_limit_w(), "passages": args.passages,
            "rows": n_rows, "dim": dim, "queries": args.queries, "lq": args.lq, "top_n": args.top_n, "nlist": args.nlist,
-           "build_s": {"kmeans": t1 - t0, "assign": t2 - t1, "layout": t3 - t2},
+           "build_s": {"kmeans": t1 - t0, "assign_layout": t2 - t1},
            "list_len": {"mean": float(lens.mean()), "max": int(lens.max()), "empty": int((lens == 0).sum())},
            "runs": {}}
     nq, lq = args.queries, args.lq
@@ -99,14 +95,14 @@ def main():
             probes = ivf.ivf.coarse(toks)
 
             def gather():
-                return interaction.ivf_search(toks, ivf.flat, ivf.row_ids, ivf.list_offsets, probes, kp,
+                return interaction.ivf_search(toks, ivf.tokens.flat, ivf.row_ids, ivf.list_offsets, probes, kp,
                                               ivf.max_list_len, row_index=ivf.row_index)
             st = {"stage1_exact": [], "stage1_ivf": []}
             for _ in range(args.warmup):
-                interaction.flat_ip_topk(toks, exact.flat, kp, ids=exact.row_ids)
+                interaction.flat_ip_topk(toks, exact.tokens.flat, kp, ids=exact.row_ids)
                 ivf.candidates_device(q, kp)
             for _ in range(args.reps):   # alternated in one run
-                st["stage1_exact"] += timed(lambda: interaction.flat_ip_topk(toks, exact.flat, kp, ids=exact.row_ids), 1, 0)
+                st["stage1_exact"] += timed(lambda: interaction.flat_ip_topk(toks, exact.tokens.flat, kp, ids=exact.row_ids), 1, 0)
                 st["stage1_ivf"] += timed(lambda: (ivf.ivf.coarse(toks), gather()), 1, 0)
             st["coarse"] = timed(lambda: ivf.ivf.coarse(toks), args.reps, args.warmup)
             st["gather_scan"] = timed(gather, args.reps, args.warmup)
@@ -128,7 +124,7 @@ def main():
                         "stage1_speedup": statistics.median(st["stage1_exact"]) / statistics.median(st["stage1_ivf"]),
                         "queries_per_s": nq / statistics.median(st["end_to_end"])})
             if kp == args.token_top_k[0]:   # A/B: gather against a materialised list-ordered copy of the same rows
-                rows_c, ids_c = ivf.flat[ivf.row_index].contiguous(), ivf.row_ids[ivf.row_index].contiguous()
+                rows_c, ids_c = ivf.tokens.flat[ivf.row_index].contiguous(), ivf.row_ids[ivf.row_index].contiguous()
 
                 def copy():
                     return interaction.ivf_search(toks, rows_c, ids_c, ivf.list_offsets, probes, kp, ivf.max_list_len)

@@ -57,8 +57,7 @@ def run_point(args, dim, passages, nprobes, dev, g):
     ivf.prepare(blocks)
     torch.cuda.synchronize()
     t1 = time.perf_counter()
-    ColBERTEndToEndIndexer.index_device(ivf, exact.store, off_np)   # shares the exact indexer's rows
-    ivf._set_layout(*ivf.ivf._layout(ivf.assign(ivf.store)))
+    ivf.index_device(exact.store, off_np)   # shares the exact indexer's rows
     torch.cuda.synchronize()
     t2 = time.perf_counter()
     point = {"dim": dim, "passages": passages, "rows": n_rows,

@@ -131,3 +131,35 @@ def test_index_before_prepare_raises():
     idx = ColBERTIVFIndexer(_cfg(), device=CPU)
     with pytest.raises(_lib.MatchmakerB200Error, match="centroids"):
         idx.index([np.zeros(3, dtype=np.int64)], [np.zeros((3, 64), dtype=np.float16)])
+
+
+def _blobs_equal(a, b):
+    assert a.keys() == b.keys()
+    for k in a:
+        assert torch.equal(a[k], b[k]) if isinstance(a[k], torch.Tensor) else a[k] == b[k], k
+
+
+def test_e4m3_layout_file_loads_and_saves_in_its_format(tmp_path):
+    """An IVF token layout of an E4M3 store as the format was first written: it loads into an E4M3 indexer only, a
+    re-index must reproduce its store scale, and a save of the same layout writes the same keys and values."""
+    dim, nlist, n_rows = 128, 8, 40
+    blob = {"centroids": torch.nn.functional.normalize(torch.randn(nlist, dim), dim=1),
+            "row_index": torch.arange(n_rows), "list_offsets": torch.tensor([0] + [n_rows] * nlist), "nlist": nlist,
+            "nprobe": 3, "token_dtype": "torch.float16", "store_dtype": "float8_e4m3", "store_scale": 5,
+            "fingerprint": {"n_rows": n_rows, "d_lo": 0, "d_hi": 5, "world": 1}, "rank": 0}
+    path = str(tmp_path / "fp8.ivf")
+    torch.save(blob, path)
+    fp8 = dict(_cfg(dim=dim), colbert_store_dtype="float8_e4m3")
+    with pytest.raises(_lib.MatchmakerB200Error, match="colbert_store_dtype"):
+        ColBERTIVFIndexer(_cfg(dim=dim), device=CPU).load(path)
+    with pytest.raises(_lib.MatchmakerB200Error, match="colbert_store_dtype"):
+        ColBERTIVFIndexer(fp8, device=CPU).load(_saved(tmp_path, dim=dim))     # an fp16 layout
+    idx = ColBERTIVFIndexer(fp8, device=CPU)
+    idx.load(path)
+    assert idx.nprobe == 3 and idx.tokens.loaded_scale == 5
+    # what index() leaves behind on the same store: its rows, passages and scale, and the loaded layout
+    idx.store = torch.zeros(n_rows, dim, dtype=torch.float8_e4m3fn)
+    idx.store_scale, idx.d_lo, idx.d_hi = 5, 0, 5
+    idx._set_layout(*idx._saved_layout[1:])
+    idx.save(str(tmp_path / "again.ivf"))
+    _blobs_equal(torch.load(str(tmp_path / "again.ivf")), blob)

@@ -146,3 +146,47 @@ def test_list_means_are_sequential_fp64_sums_of_whole_lists(chunk, monkeypatch):
         ref[l] = (s / max(1, len(rows))).astype(np.float16)
     assert np.array_equal(got.view(np.int16), ref.view(np.int16))
     assert not got[nlist - 1].any()
+
+
+def _residual_file(dim=64, bits=2, nlist=4, world=1, rank=0):
+    """A residual index file as the format was first written: three passages of 2, 0 and 3 rows from passage 7 on."""
+    torch = pytest.importorskip("torch")
+    g = torch.Generator().manual_seed(bits)
+    n = 5
+    return {"centroids": torch.nn.functional.normalize(torch.randn(nlist, dim, generator=g), dim=1),
+            "base": torch.randn(nlist, dim, generator=g).half(), "weight": torch.randn(dim, 1 << bits, generator=g).half(),
+            "cutoff": torch.randn(dim, (1 << bits) - 1, generator=g), "bits": bits, "dim": dim,
+            "codes": torch.randint(0, 256, (n, dim * bits // 8), generator=g, dtype=torch.uint8),
+            "list_ids": torch.tensor([0, 2, 2, 3, 0], dtype=torch.int32), "row_index": torch.tensor([0, 4, 1, 2, 3]),
+            "list_offsets": torch.tensor([0, 2, 2, 4, 5]), "offsets": torch.tensor([0, 2, 2, 5]), "d_lo": 7,
+            "n_docs": 12, "nlist": nlist, "nprobe": 2, "rank": rank, "world": world}
+
+
+def test_residual_file_loads_and_saves_in_its_format(tmp_path):
+    torch = pytest.importorskip("torch")
+    from matchmaker_b200.retrieval import ColBERTResidualIndexer
+    cfg = {"token_dim": 64, "faiss_use_gpu": True, "token_dtype": "float16", "faiss_ivf_list_count": 4,
+           "faiss_ivf_search_probe_count": 1, "colbert_residual_bits": 2}
+    blob = _residual_file()
+    path = str(tmp_path / "res.pt")
+    torch.save(blob, path)
+    idx = ColBERTResidualIndexer(cfg, device=torch.device("cpu"))
+    idx.load(path)
+    for name, got in (("codes", idx.store), ("list_ids", idx.list_ids), ("base", idx.base), ("weight", idx.weight),
+                      ("cutoff", idx.cutoff), ("row_index", idx.row_index), ("list_offsets", idx.list_offsets),
+                      ("offsets", idx.offsets)):
+        assert torch.equal(got, blob[name]), name
+    assert torch.equal(idx.row_ids, torch.tensor([7, 7, 9, 9, 9]))
+    assert (idx.d_lo, idx.d_hi, idx.n_docs, idx.max_doc_len, idx.max_list_len, idx.nprobe) == (7, 10, 12, 3, 2, 2)
+    idx.save(str(tmp_path / "again.pt"))
+    again = torch.load(str(tmp_path / "again.pt"))
+    assert again.keys() == blob.keys()
+    for k in blob:
+        assert torch.equal(again[k], blob[k]) if isinstance(blob[k], torch.Tensor) else again[k] == blob[k], k
+    for bad in (_residual_file(bits=1), _residual_file(dim=128)):
+        torch.save(bad, path)
+        with pytest.raises(_lib.MatchmakerB200Error, match="codes"):
+            ColBERTResidualIndexer(cfg, device=torch.device("cpu")).load(path)
+    torch.save(_residual_file(world=2), path)
+    with pytest.raises(_lib.MatchmakerB200Error, match="world size"):
+        ColBERTResidualIndexer(cfg, device=torch.device("cpu")).load(path)
