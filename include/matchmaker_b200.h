@@ -459,6 +459,40 @@ MMB200_API int mmb200_maxsim_store_residual_fwd(const void* q, const uint8_t* co
                                                 int32_t dim, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * PLAID centroid interaction (Santhanam et al., "PLAID", CIKM 2022) over a ColBERT IVF token index: candidate passages
+ * are scored from their rows' list (centroid) ids alone, with a query x centroid score table.
+ *
+ * mmb200_plaid_centroid_scores: queries [nq, Lq, dim] fp16 (all-zero rows are padding), centroids [nlist, dim] fp16.
+ *          scores [nq, nlist, LQP] fp16, LQP = 32 * ceil(Lq / 32): scores[q][c][i] = fp16_rn(fp32 sum over d of
+ *          q[i][d] * centroid[c][d]) (wgmma), 0 for i >= Lq.  keep [nq, ceil(nlist / 32)] uint32: bit c % 32 of word
+ *          c / 32 is set when the max over the query's live tokens (a nonzero element) of float(scores[q][c][i]) is
+ *          >= threshold; a query without live tokens keeps nothing.  threshold may be -inf, not NaN.
+ * mmb200_plaid_candidates: probes [nq, n_probes] int64 list ids (outside [0, nlist): nothing); the passages of list l
+ *          are plist_pids[plist_offsets[l] .. plist_offsets[l+1]) (int32 local ids in [0, n_docs)).  out_ids [nq, cap]
+ *          int64: the union of the query's probed lists' passages as first_doc + pid, ascending, then -1.  A union
+ *          larger than cap is truncated to its cap smallest ids.  bitmap: scratch of nq * max(1, ceil(n_docs / 32))
+ *          uint32, cleared here.
+ * mmb200_plaid_interaction: the scores and keep mask above, list_ids [n_rows] int32 (the list of every row),
+ *          doc_offsets [n_docs + 1] int64 (passage d is rows [doc_offsets[d], doc_offsets[d+1])), cand_ids
+ *          [nq, n_cand] int64 global ids (void: outside [first_doc, first_doc + n_docs), -1 included).  out [nq, n_cand]
+ *          f32: sum over i < Lq of the max over the passage's rows r whose list is kept (prune != 0; every row when
+ *          prune == 0) of float(scores[q][list_ids[r]][i]), summed in a fixed order; -inf when no row qualifies or the
+ *          candidate is void.  keep may be NULL when prune == 0.
+ * Envelope: 1 <= Lq <= 128, 1 <= nlist <= 2^18, dim % 64 == 0, 64 <= dim <= 1024, nq <= 65535 (scores, interaction),
+ * 16-byte aligned queries, centroids and scores.  Outside it: MMB200_ERR_INVALID.  No host synchronisation.
+ * ------------------------------------------------------------------------------------------ */
+MMB200_API int mmb200_plaid_centroid_scores(const void* queries, const void* centroids, void* scores, uint32_t* keep,
+                                            int64_t nq, int32_t Lq, int64_t nlist, int32_t dim, float threshold,
+                                            void* stream);
+MMB200_API int mmb200_plaid_candidates(const int64_t* probes, const int64_t* plist_offsets, const int32_t* plist_pids,
+                                       uint32_t* bitmap, int64_t* out_ids, int64_t nq, int32_t n_probes, int64_t nlist,
+                                       int64_t n_docs, int64_t cap, int64_t first_doc, void* stream);
+MMB200_API int mmb200_plaid_interaction(const void* scores, const uint32_t* keep, const int32_t* list_ids,
+                                        const int64_t* doc_offsets, const int64_t* cand_ids, float* out, int64_t nq,
+                                        int32_t Lq, int64_t nlist, int64_t n_docs, int64_t n_cand, int64_t first_doc,
+                                        int32_t prune, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Graph index: detour pruning of an exact k-NN graph, and a beam search over the graph
  *
  * Replaces: FaissHNSWIndexer   matchmaker/retrieval/faiss_indices.py:76-104 (faiss IndexHNSWFlat, CPU only), with one

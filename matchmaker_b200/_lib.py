@@ -55,6 +55,9 @@ SIGNATURES = {
                                                                                 _i32, _vp]),
     "mmb200_maxsim_store_residual_fwd": (_c.c_int, [_vp] * 5 + [_i32] + [_vp] * 4 + [_i64, _i64, _i64, _i64, _i32, _i32,
                                                                                         _i32, _vp]),
+    "mmb200_plaid_centroid_scores": (_c.c_int, [_vp] * 4 + [_i64, _i32, _i64, _i32, _f32, _vp]),
+    "mmb200_plaid_candidates": (_c.c_int, [_vp] * 5 + [_i64, _i32, _i64, _i64, _i64, _i64, _vp]),
+    "mmb200_plaid_interaction": (_c.c_int, [_vp] * 6 + [_i64, _i32, _i64, _i64, _i64, _i64, _i32, _vp]),
     "mmb200_ah_workspace_bytes": (_i64, [_i64, _i32, _i64, _i64, _i32, _i32]),
     "mmb200_ah_search": (_c.c_int, [_vp] * 8 + [_i64, _i64, _i32, _i64, _i64, _i64, _i32, _i32, _vp]),
     "mmb200_ah_reorder": (_c.c_int, [_vp] * 6 + [_i64, _i64, _i32, _i32, _i32, _i32, _vp]),

@@ -878,6 +878,119 @@ def maxsim_store_residual(q: torch.Tensor, codes: torch.Tensor, list_ids: torch.
     return out
 
 
+PLAID_MAX_LQ = 128
+PLAID_MAX_NLIST = 1 << 18
+PLAID_MAX_QUERIES = 65535   # queries per launch (grid y)
+
+
+def plaid_lqp(lq: int) -> int:
+    """Width of a query's centroid score row: Lq rounded up to a multiple of 32."""
+    return 32 * ((lq + 31) // 32)
+
+
+def _plaid_envelope(lq: int, nlist: int, what: str, dim: Optional[int] = None):
+    if not 1 <= lq <= PLAID_MAX_LQ:
+        raise _lib.MatchmakerB200Error(f"{what}: PLAID needs 1 <= Lq <= {PLAID_MAX_LQ}, got {lq}")
+    if not 1 <= nlist <= PLAID_MAX_NLIST:
+        raise _lib.MatchmakerB200Error(f"{what}: PLAID needs 1 <= nlist <= 2^18, got {nlist}")
+    if dim is not None and (dim % 64 or not 64 <= dim <= 1024):
+        raise _lib.MatchmakerB200Error(f"{what}: PLAID needs dim % 64 == 0 and 64 <= dim <= 1024, got {dim}")
+
+
+def plaid_centroid_scores(q: torch.Tensor, centroids: torch.Tensor, threshold: float) -> Tuple[torch.Tensor, torch.Tensor]:
+    """PLAID's query x centroid table of queries q [nq, Lq, dim] and centroids [nlist, dim] (both cast to fp16):
+    (scores [nq, nlist, LQP] fp16, scores[q][c][i] = fp16_rn(fp32 sum_d q[i][d] * centroid[c][d]), 0 for i >= Lq;
+    keep [nq, ceil(nlist / 32)] int32 bitmask, bit c set when the max over the query's live tokens (rows with a nonzero
+    fp16 element) of scores[q][c] is >= threshold).  threshold -inf keeps every centroid of a query with a live token.
+    1 <= Lq <= 128, 1 <= nlist <= 2^18, dim % 64 == 0, 64 <= dim <= 1024."""
+    dev = _require_cuda(q, centroids)
+    if q.dim() != 3 or centroids.dim() != 2 or centroids.shape[1] != q.shape[2]:
+        raise _lib.MatchmakerB200Error(f"plaid_centroid_scores: q [nq, Lq, dim] and centroids [nlist, dim], got "
+                                       f"{tuple(q.shape)} and {tuple(centroids.shape)}")
+    nq, lq, dim = q.shape
+    nlist = centroids.shape[0]
+    _plaid_envelope(lq, nlist, "plaid_centroid_scores", dim)
+    if threshold != threshold:
+        raise _lib.MatchmakerB200Error("plaid_centroid_scores: the centroid score threshold is NaN")
+    q, centroids = q.to(torch.float16).contiguous(), centroids.to(torch.float16).contiguous()
+    scores = torch.empty((nq, nlist, plaid_lqp(lq)), dtype=torch.float16, device=dev)
+    keep = torch.empty((nq, (nlist + 31) // 32), dtype=torch.int32, device=dev)
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        for b0 in range(0, nq, PLAID_MAX_QUERIES):
+            b1 = min(nq, b0 + PLAID_MAX_QUERIES)
+            rc = lib.mmb200_plaid_centroid_scores(_ptr(q[b0:b1]), _ptr(centroids), _ptr(scores[b0:b1]), _ptr(keep[b0:b1]),
+                                                  b1 - b0, lq, nlist, dim, float(threshold), _stream(dev))
+            _lib.check(rc, "mmb200_plaid_centroid_scores")
+    return scores, keep
+
+
+def plaid_candidates(probes: torch.Tensor, plist_offsets: torch.Tensor, plist_pids: torch.Tensor, n_docs: int, cap: int,
+                     first_doc: int = 0) -> torch.Tensor:
+    """The candidate passages of every query: probes [nq, n_probes] int64 list ids (entries outside [0, nlist) probe
+    nothing); list l holds local passages plist_pids[plist_offsets[l]:plist_offsets[l+1]] (int32 in [0, n_docs)).
+    Returns [nq, cap] int64: the union of the probed lists' passages as first_doc + pid, ascending, then -1.  A union
+    larger than cap keeps its cap smallest ids: cap = min(n_docs, n_probes * longest list) never truncates."""
+    dev = _require_cuda(probes, plist_offsets, plist_pids)
+    if probes.dim() != 2 or plist_offsets.dim() != 1 or plist_offsets.numel() < 2 or plist_pids.dim() != 1:
+        raise _lib.MatchmakerB200Error("plaid_candidates: probes [nq, n_probes], plist_offsets [nlist + 1], plist_pids [n]")
+    if not 1 <= cap <= max(n_docs, 1):
+        raise _lib.MatchmakerB200Error(f"plaid_candidates: cap must be in [1, max(n_docs, 1)], got {cap}")
+    nq, n_probes = probes.shape
+    probes, plist_offsets = probes.to(torch.int64).contiguous(), plist_offsets.to(torch.int64).contiguous()
+    plist_pids = plist_pids.to(torch.int32).contiguous()
+    out = torch.empty((nq, cap), dtype=torch.int64, device=dev)
+    if nq == 0 or n_probes == 0:
+        return out.fill_(-1)
+    bitmap = torch.empty(nq * max(1, (n_docs + 31) // 32), dtype=torch.int32, device=dev)
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        rc = lib.mmb200_plaid_candidates(_ptr(probes), _ptr(plist_offsets), _ptr(plist_pids), _ptr(bitmap), _ptr(out), nq,
+                                         n_probes, plist_offsets.numel() - 1, n_docs, cap, first_doc, _stream(dev))
+    _lib.check(rc, "mmb200_plaid_candidates")
+    return out
+
+
+def plaid_interaction(scores: torch.Tensor, keep: Optional[torch.Tensor], list_ids: torch.Tensor,
+                      doc_offsets: torch.Tensor, cand: torch.Tensor, lq: int, first_doc: int = 0) -> torch.Tensor:
+    """Centroid interaction [nq, C] f32 of candidates cand [nq, C] (global ids; ids outside [first_doc, first_doc +
+    n_docs) are void): the sum over query tokens i < lq of the max over the passage's rows r of
+    float(scores[q][list_ids[r]][i]), over the rows whose list is kept in ``keep`` (pruned; None: every row); -inf
+    when no row qualifies or the candidate is void.  scores, keep: :func:`plaid_centroid_scores`; list_ids [n_rows]
+    int32; doc_offsets [n_docs + 1] int64.  Bit-reproducible (fixed-order sums)."""
+    dev = _require_cuda(scores, keep, list_ids, doc_offsets, cand)
+    if scores.dim() != 3 or scores.dtype != torch.float16 or cand.dim() != 2 or cand.shape[0] != scores.shape[0]:
+        raise _lib.MatchmakerB200Error(f"plaid_interaction: scores [nq, nlist, LQP] fp16 and cand [nq, C], got "
+                                       f"{tuple(scores.shape)} {scores.dtype} and {tuple(cand.shape)}")
+    nq, nlist, lqp = scores.shape
+    _plaid_envelope(lq, nlist, "plaid_interaction")
+    if lqp != plaid_lqp(lq):
+        raise _lib.MatchmakerB200Error(f"plaid_interaction: score rows of {lqp} for Lq {lq} (need {plaid_lqp(lq)})")
+    if keep is not None and tuple(keep.shape) != (nq, (nlist + 31) // 32):
+        raise _lib.MatchmakerB200Error(f"plaid_interaction: keep must be [{nq}, {(nlist + 31) // 32}], got "
+                                       f"{tuple(keep.shape)}")
+    n_docs = doc_offsets.numel() - 1
+    if list_ids.dim() != 1 or doc_offsets.dim() != 1 or n_docs < 0:
+        raise _lib.MatchmakerB200Error("plaid_interaction: list_ids [n_rows], doc_offsets [n_docs + 1]")
+    scores, cand = scores.contiguous(), cand.to(torch.int64).contiguous()
+    list_ids, doc_offsets = list_ids.to(torch.int32).contiguous(), doc_offsets.to(torch.int64).contiguous()
+    keep = None if keep is None else keep.contiguous()
+    n_cand = cand.shape[1]
+    out = torch.empty((nq, n_cand), dtype=torch.float32, device=dev)
+    if nq == 0 or n_cand == 0:
+        return out
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        for b0 in range(0, nq, PLAID_MAX_QUERIES):
+            b1 = min(nq, b0 + PLAID_MAX_QUERIES)
+            rc = lib.mmb200_plaid_interaction(_ptr(scores[b0:b1]), None if keep is None else _ptr(keep[b0:b1]),
+                                              _ptr(list_ids), _ptr(doc_offsets), _ptr(cand[b0:b1]), _ptr(out[b0:b1]),
+                                              b1 - b0, lq, nlist, n_docs, n_cand, first_doc, int(keep is not None),
+                                              _stream(dev))
+            _lib.check(rc, "mmb200_plaid_interaction")
+    return out
+
+
 AH_MAX_KR = 1024
 # Device scratch one ah_search call may take; it grows with nq * nprobe (one candidate slot per (query, probe)), so
 # larger query sets are searched in batches that fit.

@@ -60,12 +60,17 @@ def token_store_attribute(name: str, doc: str) -> property:
 
 class ColBERTEndToEndIndexer(GPUIndexer):
     residual = False   # the store keeps residual codes (ColBERTResidualIndexer)
+    plaid_capable = False   # accepts the PLAID search keys (an IVF token index: ColBERTIVFIndexer)
     store = token_store_attribute("rows", "[rows of this rank, ...] the stored rows as the kernels read them")
     store_scale = token_store_attribute("scale", "s_d of an E4M3 store, else None")
     chunk_rows = token_store_attribute("slab_rows", "rows per slab of a streamed build")
 
     def __init__(self, config, device: Optional[torch.device] = None, process_group=None):
         super().__init__(config, device, process_group)
+        if not self.plaid_capable and any(config.get(k) is not None for k in
+                                          ("colbert_plaid_ndocs", "colbert_plaid_centroid_score_threshold")):
+            raise _lib.MatchmakerB200Error("PLAID search (colbert_plaid_*) needs the centroids of an IVF token index: "
+                                           "ColBERTIVFIndexer or ColBERTResidualIndexer")
         self.tokens = colbert_store.select(config, self.token_dim, self.store_dtype, self.device, process_group,
                                            self.residual)
         self.row_ids: Optional[torch.Tensor] = None     # [rows] int64 passage id (seq_ids position) of every row

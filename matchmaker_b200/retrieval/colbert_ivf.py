@@ -25,6 +25,7 @@ import numpy
 import torch
 
 from .. import _lib, interaction
+from . import colbert_plaid
 from .colbert_e2e import ColBERTEndToEndIndexer
 from .ivf_index import IVFIndexer
 
@@ -32,9 +33,15 @@ ASSIGN_BATCH = 1 << 20      # rows per assignment call: bounds the flat_ip_topk 
 
 
 class ColBERTIVFIndexer(ColBERTEndToEndIndexer):
+    plaid_capable = True
+
     def __init__(self, config, device: Optional[torch.device] = None, process_group=None):
         super().__init__(config, device, process_group)
         self.ivf = IVFIndexer(config, device=self.device, process_group=process_group)   # quantizer + k-means
+        keys = colbert_plaid.config_keys(config)
+        if keys is not None:
+            colbert_plaid.check_envelope(self.ivf.nlist, self.token_dim)
+        self.plaid = None if keys is None else colbert_plaid.PLAIDSearch(*keys)   # PLAID search, when configured
         self.row_index: Optional[torch.Tensor] = None      # [rows] int64 store row of every list position
         self.list_offsets: Optional[torch.Tensor] = None   # [nlist + 1] int64
         self.max_list_len = 0
@@ -87,6 +94,27 @@ class ColBERTIVFIndexer(ColBERTEndToEndIndexer):
             raise _lib.MatchmakerB200Error("IVF token layout does not cover the store's rows")
         self.row_index, self.list_offsets = row_index.contiguous(), list_offsets.contiguous()
         self.max_list_len = int((list_offsets[1:] - list_offsets[:-1]).max().item()) if self.nlist else 0
+        if self.plaid is not None:
+            self.plaid.set_layout(self)
+
+    # ------------------------------------------------------------------ search
+    def search_device(self, q: torch.Tensor, top_n: int, token_top_k: Optional[int] = None):
+        """search() with device tensors in and out.  With PLAID search, top_n <= colbert_plaid_ndocs // 4 and
+        token_top_k must not be given."""
+        if self.plaid is not None:
+            if token_top_k is not None:
+                raise _lib.MatchmakerB200Error("token_top_k has no meaning in a PLAID search (colbert_plaid_ndocs)")
+            if top_n > self.plaid.ndocs // 4:
+                raise _lib.MatchmakerB200Error(f"PLAID search needs top_n <= colbert_plaid_ndocs // 4 = "
+                                               f"{self.plaid.ndocs // 4}, got {top_n}")
+            if q.dim() == 3 and q.shape[1] > interaction.PLAID_MAX_LQ:
+                raise _lib.MatchmakerB200Error(f"PLAID search needs Lq <= {interaction.PLAID_MAX_LQ}, got {q.shape[1]}")
+        return super().search_device(q, top_n, token_top_k)
+
+    def _search_local(self, q: torch.Tensor, top_n: int, kp: int):
+        if self.plaid is None:
+            return super()._search_local(q, top_n, kp)
+        return self.plaid.search(self, q, top_n)
 
     # ------------------------------------------------------------------ stage 1
     def _scan(self, toks, stoks, kp: int):
