@@ -237,10 +237,15 @@ MMB200_API int mmb200_kernel_pool_bwd_ex(const float* q, const float* d, const v
  *   mmb200_kernel_pool_bwd_saved = mmb200_kernel_pool_bwd_ex (doc_gate / grad_gate as there, or NULL) computed from `saved` with both contractions
  *   (G q^ and G^T d^) as tf32 wgmma on the raw fp32 embeddings; gradients agree with the fp32 expression to a few
  *   1e-4 relative (tf32 operands; the reference trains under fp16 autocast).  grad_q / grad_d must be 16-byte aligned.
- *   Envelope: mmb200_kernel_pool_train_tc_supported(Lq, Ld, D, K) != 0  (Lq <= 32, K <= 32, D % 4 == 0, D <= 320);
- *   outside it both calls return MMB200_ERR_UNSUPPORTED and the caller uses _fwd_ex / _bwd_ex. */
+ *   Envelope: mmb200_kernel_pool_train_tc_supported(Lq, Ld, D, K) != 0  (Lq <= 32, K <= 32; D % 4 == 0 and D <= 320, or
+ *   D % 64 == 0 and 512 < D <= 1024: the BERT-base / -large widths); outside it both calls return MMB200_ERR_UNSUPPORTED
+ *   and the caller uses _fwd_ex / _bwd_ex (which stops at D <= 512).
+ *   `workspace` of mmb200_kernel_pool_bwd_saved: mmb200_kernel_pool_bwd_saved_workspace_floats(B, Lq, Ld, D, K) floats,
+ *   16-byte aligned.  That is 2 * B * K (as for _bwd_ex) up to D = 320; at 512 < D <= 1024 it also holds the backward's
+ *   per-pair G matrices, B * (65 * Ldp + 32) floats more with Ldp = Ld rounded up to 64. */
 MMB200_API int32_t mmb200_kernel_pool_train_tc_supported(int32_t Lq, int32_t Ld, int32_t D, int32_t K);
 MMB200_API int64_t mmb200_kernel_pool_saved_floats(int64_t B, int32_t Ld);
+MMB200_API int64_t mmb200_kernel_pool_bwd_saved_workspace_floats(int64_t B, int32_t Lq, int32_t Ld, int32_t D, int32_t K);
 MMB200_API int mmb200_kernel_pool_fwd_train(const float* q, const float* d, const void* q_mask, const void* d_mask,
                                             const float* doc_gate, const float* mu, const float* sigma, const float* alpha,
                                             const float* weight, float* score, float* per_kernel, float* per_kernel_query, float* saved,

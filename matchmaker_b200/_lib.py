@@ -71,6 +71,7 @@ SIGNATURES = {
     "mmb200_kernel_pool_bwd_ex": (_c.c_int, [_vp] * 17 + [_i64, _i32, _i32, _i32, _i32, _f32, _f32, _i32, _vp]),
     "mmb200_kernel_pool_train_tc_supported": (_i32, [_i32, _i32, _i32, _i32]),
     "mmb200_kernel_pool_saved_floats": (_i64, [_i64, _i32]),
+    "mmb200_kernel_pool_bwd_saved_workspace_floats": (_i64, [_i64, _i32, _i32, _i32, _i32]),
     "mmb200_kernel_pool_fwd_train": (_c.c_int, [_vp] * 13 + [_i64, _i32, _i32, _i32, _i32, _f32, _f32, _f32, _i32, _vp]),
     "mmb200_kernel_pool_bwd_saved": (_c.c_int, [_vp] * 18 + [_i64, _i32, _i32, _i32, _i32, _f32, _f32, _i32, _vp]),
     "mmb200_storage_load": (_c.c_int, [_c.POINTER(_c.c_char_p), _c.POINTER(_i64), _c.POINTER(_i64), _i32, _vp, _i64, _vp]),

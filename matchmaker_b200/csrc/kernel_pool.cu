@@ -488,10 +488,15 @@ static int launch_bwd(const KpParams& P, const DeviceInfo& dev, cudaStream_t str
   return MMB200_OK;
 }
 
-// the envelope of the tensor-core training pair (forward that saves its cosines + backward that consumes them)
+// the envelope of the tensor-core training pair (forward that saves its cosines + backward that consumes them): D <= 320
+// on kernel_pool_bwd_wg.cu, 512 < D <= 1024 in whole 64-feature blocks (BERT widths) on kernel_pool_wide.cu
 static bool kp_train_tc_shape_ok(int Lq, int Ld, int D, int K) {
-  return Lq >= 1 && Lq <= 32 && Ld >= 1 && K >= 1 && K <= 32 && D >= 4 && D % 4 == 0 && D <= 320;
+  return (Lq >= 1 && Lq <= 32 && Ld >= 1 && K >= 1 && K <= 32 && D >= 4 && D % 4 == 0 && D <= 320) ||
+         kp_wide_shape_ok(Lq, Ld, D, K);
 }
+
+// first float of the wide backward's part of the workspace, after ws_weight / ws_alpha (16-byte aligned)
+static int64_t kp_wide_ws_off(int64_t B, int K) { return (2 * B * K + 3) / 4 * 4; }
 
 static int kp_fwd_impl(const float* q, const float* d, const void* q_mask, const void* d_mask, const float* doc_gate,
                        const float* mu, const float* sigma, const float* alpha, const float* weight, float* score,
@@ -531,7 +536,7 @@ static int kp_bwd_impl(const float* q, const float* d, const void* q_mask, const
                        const float* per_kernel_query, const float* saved, const float* grad_score, float* grad_q,
                        float* grad_d, float* grad_gate, float* grad_alpha, float* grad_weight, float* workspace,
                        int64_t B, int32_t Lq, int32_t Ld, int32_t D, int32_t K, float log_scale, float clamp_min,
-                       int32_t mask_dtype, void* stream_) {
+                       int32_t mask_dtype, bool from_saved, void* stream_) {
   MMB_REQUIRE(clamp_min > 0.f, "clamp_min must be positive");
   KpParams P{};
   P.saved = const_cast<float*>(saved);
@@ -547,7 +552,8 @@ static int kp_bwd_impl(const float* q, const float* d, const void* q_mask, const
   P.S = per_kernel_query; P.grad_score = grad_score; P.grad_q = grad_q; P.grad_d = grad_d;
   if (int rc = kp_validate(P)) return rc;
   MMB_REQUIRE(B == 0 || (per_kernel_query && grad_score && grad_q && grad_d && workspace), "null pointer");
-  MMB_REQUIRE(D <= 512, "kernel_pool backward supports embedding dim <= 512");
+  const bool wide = from_saved && kp_wide_shape_ok(Lq, Ld, D, K);   // BERT widths, from the saved state (null when B = 0)
+  MMB_REQUIRE(D <= 512 || wide, "kernel_pool backward supports embedding dim <= 512");
   P.ws_weight = workspace;
   P.ws_alpha = workspace + B * K;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
@@ -559,6 +565,12 @@ static int kp_bwd_impl(const float* q, const float* d, const void* q_mask, const
   DeviceInfo dev;
   if (int rc = require_sm90(&dev)) return rc;
   int rc;
+  if (wide) {
+    if ((rc = kernel_pool_bwd_wide(P, workspace + kp_wide_ws_off(B, K), dev, stream))) return rc;
+    kp_reduce_batch<<<K, 256, 0, stream>>>(P.ws_weight, P.ws_alpha, grad_weight, grad_alpha, B, K);
+    MMB_CHECK_CUDA(cudaGetLastError());
+    return MMB200_OK;
+  }
   if (saved) {
     bool handled = false;
     rc = kernel_pool_bwd_tc(P, dev, stream, &handled);
@@ -613,6 +625,11 @@ extern "C" int32_t mmb200_kernel_pool_train_tc_supported(int32_t Lq, int32_t Ld,
 
 extern "C" int64_t mmb200_kernel_pool_saved_floats(int64_t B, int32_t Ld) { return mmb::kp_saved_floats(B, Ld); }
 
+extern "C" int64_t mmb200_kernel_pool_bwd_saved_workspace_floats(int64_t B, int32_t Lq, int32_t Ld, int32_t D, int32_t K) {
+  if (!mmb::kp_wide_shape_ok(Lq, Ld, D, K)) return 2 * B * K;
+  return mmb::kp_wide_ws_off(B, K) + mmb::kp_wide_ws_floats(B, Ld);
+}
+
 extern "C" int mmb200_kernel_pool_fwd_train(const float* q, const float* d, const void* q_mask, const void* d_mask,
                                             const float* doc_gate, const float* mu, const float* sigma, const float* alpha,
                                             const float* weight,
@@ -622,7 +639,7 @@ extern "C" int mmb200_kernel_pool_fwd_train(const float* q, const float* d, cons
   using namespace mmb;
   MMB_REQUIRE((saved != nullptr && per_kernel_query != nullptr) || B == 0, "saved and per_kernel_query must be non-null");
   if (!kp_train_tc_shape_ok(Lq, Ld, D, K)) {
-    set_error("kernel_pool_fwd_train: shape outside the tensor-core training envelope (Lq <= 32, K <= 32, D % 4 == 0, D <= 320)");
+    set_error("kernel_pool_fwd_train: shape outside the tensor-core training envelope (Lq <= 32, K <= 32; D % 4 == 0 and D <= 320, or D % 64 == 0 and 512 < D <= 1024)");
     return MMB200_ERR_UNSUPPORTED;
   }
   return kp_fwd_impl(q, d, q_mask, d_mask, doc_gate, mu, sigma, alpha, weight, score, per_kernel, per_kernel_query, nullptr,
@@ -639,12 +656,12 @@ extern "C" int mmb200_kernel_pool_bwd_saved(const float* q, const float* d, cons
   using namespace mmb;
   MMB_REQUIRE(saved != nullptr || B == 0, "saved must be non-null");
   if (!kp_train_tc_shape_ok(Lq, Ld, D, K)) {
-    set_error("kernel_pool_bwd_saved: shape outside the tensor-core training envelope (Lq <= 32, K <= 32, D % 4 == 0, D <= 320)");
+    set_error("kernel_pool_bwd_saved: shape outside the tensor-core training envelope (Lq <= 32, K <= 32; D % 4 == 0 and D <= 320, or D % 64 == 0 and 512 < D <= 1024)");
     return MMB200_ERR_UNSUPPORTED;
   }
   return kp_bwd_impl(q, d, q_mask, d_mask, doc_gate, mu, sigma, alpha, weight, per_kernel_query, saved, grad_score, grad_q,
                      grad_d, grad_gate, grad_alpha, grad_weight, workspace, B, Lq, Ld, D, K, log_scale, clamp_min, mask_dtype,
-                     stream_);
+                     true, stream_);
 }
 
 extern "C" int mmb200_kernel_pool_bwd(const float* q, const float* d, const void* q_mask, const void* d_mask,
@@ -667,5 +684,5 @@ extern "C" int mmb200_kernel_pool_bwd_ex(const float* q, const float* d, const v
                                          void* stream_) {
   return mmb::kp_bwd_impl(q, d, q_mask, d_mask, doc_gate, mu, sigma, alpha, weight, per_kernel_query, nullptr, grad_score,
                           grad_q, grad_d, grad_gate, grad_alpha, grad_weight, workspace, B, Lq, Ld, D, K, log_scale, clamp_min,
-                          mask_dtype, stream_);
+                          mask_dtype, false, stream_);
 }

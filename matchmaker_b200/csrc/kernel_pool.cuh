@@ -59,4 +59,20 @@ int kernel_pool_fwd_ts(const KpParams& P, const DeviceInfo& dev, cudaStream_t st
 // tensor-core backward from the state saved by the forward (kernel_pool_bwd_wg.cu); same convention
 int kernel_pool_bwd_tc(const KpParams& P, const DeviceInfo& dev, cudaStream_t stream, bool* handled);
 
+// The wide backward's part of the workspace (kernel_pool_wide.cu), Ldp = Ld rounded up to 64 document rows, per pair:
+// G1 [Ldp][32] and G2^T [32][Ldp] as tf32 bit patterns, the document terms prd [Ldp], the query terms prq [32].
+struct KpWideWs {
+  uint32_t* g1;
+  uint32_t* g2t;
+  float* prd;
+  float* prq;
+  int32_t Ldp;
+};
+// its envelope: 512 < D <= 1024, D % 64 == 0, Lq <= 32, K <= 32
+bool kp_wide_shape_ok(int Lq, int Ld, int D, int K);
+// floats of the wide part of the workspace, B * (65 Ldp + 32)
+int64_t kp_wide_ws_floats(int64_t B, int Ld);
+// saved-state backward at 512 < D <= 1024: the G pass then the gradient GEMMs; ws = the wide part of the workspace
+int kernel_pool_bwd_wide(const KpParams& P, float* ws, const DeviceInfo& dev, cudaStream_t stream);
+
 }  // namespace mmb

@@ -302,11 +302,13 @@ def kernel_pool_bwd(q, d, q_mask, d_mask, mu, sigma, weight, alpha, per_kernel_q
     gd = torch.empty_like(d)
     ga = torch.empty(K, dtype=torch.float32, device=dev)
     gw = torch.empty(K, dtype=torch.float32, device=dev)
-    ws = torch.empty(2 * B * K, dtype=torch.float32, device=dev)
     gate = None if doc_gate is None else _f32c(doc_gate).reshape(B, Ld)
     gg = None if doc_gate is None else torch.empty((B, Ld), dtype=torch.float32, device=dev)
     lib = _lib.load()
     if saved is not None:
+        # at BERT widths (512 < D <= 1024) the workspace also carries the backward's per-pair G matrices
+        ws = torch.empty(int(lib.mmb200_kernel_pool_bwd_saved_workspace_floats(B, Lq, Ld, D, K)), dtype=torch.float32,
+                         device=dev)
         with torch.cuda.device(dev):
             rc = lib.mmb200_kernel_pool_bwd_saved(_ptr(q), _ptr(d), _ptr(q_mask), _ptr(d_mask), _ptr(gate), _ptr(mu), _ptr(sigma),
                                                   _ptr(alpha_c), _ptr(weight), _ptr(per_kernel_query.contiguous()),
@@ -317,6 +319,7 @@ def kernel_pool_bwd(q, d, q_mask, d_mask, mu, sigma, weight, alpha, per_kernel_q
         if doc_gate is not None:
             return gq, gd, (ga if alpha is not None else None), gw, gg
         return gq, gd, (ga if alpha is not None else None), gw
+    ws = torch.empty(2 * B * K, dtype=torch.float32, device=dev)
     with torch.cuda.device(dev):
         rc = lib.mmb200_kernel_pool_bwd_ex(_ptr(q), _ptr(d), _ptr(q_mask), _ptr(d_mask), _ptr(gate), _ptr(mu), _ptr(sigma),
                                            _ptr(alpha_c), _ptr(weight), _ptr(per_kernel_query.contiguous()),
