@@ -5,6 +5,7 @@ PyTorch is plumbing here: it owns device memory and the current stream; the arit
 """
 from __future__ import annotations
 
+import ctypes
 from typing import Optional, Tuple
 
 import torch
@@ -40,8 +41,35 @@ def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
     return None if t is None else t.data_ptr()
 
 
-def _stream(dev: torch.device) -> int:
-    return torch.cuda.current_stream(dev).cuda_stream
+def _launch(dev: torch.device, name: str, *args) -> None:
+    """Call library entry ``name`` on ``dev``'s current stream (appended as its last argument); a tensor or None in a
+    pointer slot passes its data pointer or null.  ``args`` keeps every tensor alive until the call returns: a
+    temporary built in the argument list whose block went back to the caching allocator could otherwise be handed to
+    the next temporary of the same list, whose copy kernel would overwrite it before the launch reads it."""
+    fn = getattr(_lib.load(), name)
+    with torch.cuda.device(dev):
+        rc = fn(*[_ptr(a) if t is ctypes.c_void_p else a for t, a in zip(fn.argtypes, args)],
+                torch.cuda.current_stream(dev).cuda_stream)
+    _lib.check(rc, name)
+
+
+def _query_slices(nq: int, b: int):
+    """[b0, b1) slices of at most b of nq queries, in order."""
+    for b0 in range(0, nq, b):
+        yield b0, min(nq, b0 + b)
+
+
+def _scan_batches(dev: torch.device, nq: int, workspace_bytes, cap: int, envelope_error: str, scan) -> None:
+    """Run ``scan(b0, b1, ws)`` over query slices whose scratch ``workspace_bytes(b1 - b0)`` fits ``cap``, in one
+    workspace ``ws`` (uint8) sized for the largest slice.  A size of 0 for one query raises ``envelope_error``.  The
+    sizes are asked under ``dev``'s context: they depend on its SM count."""
+    with torch.cuda.device(dev):
+        if workspace_bytes(1) <= 0:
+            raise _lib.MatchmakerB200Error(envelope_error)
+        b = ivf_query_batch(nq, workspace_bytes, cap)
+        ws = torch.empty(workspace_bytes(b), dtype=torch.uint8, device=dev)
+        for b0, b1 in _query_slices(nq, b):
+            scan(b0, b1, ws)
 
 
 def _prep_mask(m: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
@@ -63,6 +91,22 @@ def _common_mask_dtype(a: Optional[torch.Tensor], b: Optional[torch.Tensor]):
     return a, b, code
 
 
+def _check_qd(q: torch.Tensor, d: torch.Tensor) -> None:
+    if q.dtype != d.dtype or q.dtype not in _DTYPES:
+        raise _lib.MatchmakerB200Error(f"q/d must share a dtype in fp16/bf16/fp32, got {q.dtype}, {d.dtype}")
+    if q.dim() != 3 or d.dim() != 3 or q.shape[-1] != d.shape[-1]:
+        raise _lib.MatchmakerB200Error(f"expected q [n_q,Lq,dim], d [n_d,Ld,dim]; got {tuple(q.shape)}, {tuple(d.shape)}")
+
+
+def _pairs(pair_q: torch.Tensor, pair_d: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The (query, document) index of every pair as flat int32, of one length."""
+    pair_q = pair_q.to(torch.int32).contiguous().view(-1)
+    pair_d = pair_d.to(torch.int32).contiguous().view(-1)
+    if pair_q.numel() != pair_d.numel():
+        raise _lib.MatchmakerB200Error("pair_q / pair_d length mismatch")
+    return pair_q, pair_d
+
+
 def maxsim(q: torch.Tensor, d: torch.Tensor, q_mask: Optional[torch.Tensor] = None,
            d_mask: Optional[torch.Tensor] = None, docs_per_query: int = 1,
            pair_q: Optional[torch.Tensor] = None, pair_d: Optional[torch.Tensor] = None,
@@ -74,10 +118,7 @@ def maxsim(q: torch.Tensor, d: torch.Tensor, q_mask: Optional[torch.Tensor] = No
     ``pair_d[p]`` (default ``p``).  Semantics: matchmaker/models/colbert.py:68-75 / :100-112.
     """
     dev = _require_cuda(q, d, q_mask, d_mask, pair_q, pair_d, pair_dmask)
-    if q.dtype != d.dtype or q.dtype not in _DTYPES:
-        raise _lib.MatchmakerB200Error(f"q/d must share a dtype in fp16/bf16/fp32, got {q.dtype}, {d.dtype}")
-    if q.dim() != 3 or d.dim() != 3 or q.shape[-1] != d.shape[-1]:
-        raise _lib.MatchmakerB200Error(f"expected q [n_q,Lq,dim], d [n_d,Ld,dim]; got {tuple(q.shape)}, {tuple(d.shape)}")
+    _check_qd(q, d)
     q = q.contiguous()
     d = d.contiguous()
     q_mask, d_mask, mcode = _common_mask_dtype(_prep_mask(q_mask), _prep_mask(d_mask))
@@ -90,11 +131,8 @@ def maxsim(q: torch.Tensor, d: torch.Tensor, q_mask: Optional[torch.Tensor] = No
     if pair_q is not None or pair_d is not None:
         if pair_q is None or pair_d is None:
             raise _lib.MatchmakerB200Error("pair_q and pair_d must be given together")
-        pair_q = pair_q.to(torch.int32).contiguous()
-        pair_d = pair_d.to(torch.int32).contiguous()
+        pair_q, pair_d = _pairs(pair_q, pair_d)
         n_pairs = pair_q.numel()
-        if pair_d.numel() != n_pairs:
-            raise _lib.MatchmakerB200Error("pair_q / pair_d length mismatch")
         if pair_dmask is not None:
             pair_dmask = pair_dmask.to(torch.int32).contiguous()
             if pair_dmask.numel() != n_pairs:
@@ -105,12 +143,8 @@ def maxsim(q: torch.Tensor, d: torch.Tensor, q_mask: Optional[torch.Tensor] = No
             raise _lib.MatchmakerB200Error("n_q * docs_per_query < n_d")
     out = torch.empty(n_pairs, dtype=torch.float32, device=dev)
     argmax = torch.empty((n_pairs, Lq), dtype=torch.int32, device=dev) if return_argmax else None
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        rc = lib.mmb200_maxsim_fwd(_ptr(q), _ptr(d), _ptr(q_mask), _ptr(d_mask), _ptr(pair_q), _ptr(pair_d),
-                                   _ptr(pair_dmask), _ptr(out), _ptr(argmax), n_q, n_d, n_pairs, docs_per_query, Lq, Ld, dim,
-                                   _DTYPES[q.dtype], mcode, _IMPLS[impl], _stream(dev))
-    _lib.check(rc, "mmb200_maxsim_fwd")
+    _launch(dev, "mmb200_maxsim_fwd", q, d, q_mask, d_mask, pair_q, pair_d, pair_dmask, out, argmax, n_q, n_d, n_pairs,
+            docs_per_query, Lq, Ld, dim, _DTYPES[q.dtype], mcode, _IMPLS[impl])
     return (out, argmax) if return_argmax else out
 
 
@@ -145,10 +179,7 @@ def maxsim_allpairs_bwd(q: torch.Tensor, d: torch.Tensor, grad_out: torch.Tensor
     grad_out [n_q, n_d] and the forward's argmax [n_q * n_d, Lq] (either mask indexing: the gradient
     follows the argmax)."""
     dev = _require_cuda(q, d, grad_out, argmax)
-    if q.dtype != d.dtype or q.dtype not in _DTYPES:
-        raise _lib.MatchmakerB200Error(f"q/d must share a dtype in fp16/bf16/fp32, got {q.dtype}, {d.dtype}")
-    if q.dim() != 3 or d.dim() != 3 or q.shape[-1] != d.shape[-1]:
-        raise _lib.MatchmakerB200Error(f"expected q [n_q,Lq,dim], d [n_d,Ld,dim]; got {tuple(q.shape)}, {tuple(d.shape)}")
+    _check_qd(q, d)
     q = q.contiguous()
     d = d.contiguous()
     n_q, Lq, dim = q.shape
@@ -161,11 +192,8 @@ def maxsim_allpairs_bwd(q: torch.Tensor, d: torch.Tensor, grad_out: torch.Tensor
     grad_out = grad_out.to(torch.float32).contiguous()
     gq = torch.empty((n_q, Lq, dim), dtype=torch.float32, device=dev)
     gd = torch.empty((n_d, Ld, dim), dtype=torch.float32, device=dev)
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        rc = lib.mmb200_maxsim_allpairs_bwd(_ptr(q), _ptr(d), _ptr(grad_out), _ptr(argmax.contiguous()), _ptr(gq),
-                                            _ptr(gd), n_q, n_d, Lq, Ld, dim, _DTYPES[q.dtype], _stream(dev))
-    _lib.check(rc, "mmb200_maxsim_allpairs_bwd")
+    _launch(dev, "mmb200_maxsim_allpairs_bwd", q, d, grad_out, argmax.contiguous(), gq, gd, n_q, n_d, Lq, Ld, dim,
+            _DTYPES[q.dtype])
     return gq, gd
 
 
@@ -180,11 +208,8 @@ def maxsim_bwd(q: torch.Tensor, d: torch.Tensor, grad_out: torch.Tensor, argmax:
     grad_out = grad_out.to(torch.float32).contiguous()
     gq = torch.empty((n_q, Lq, dim), dtype=torch.float32, device=dev)
     gd = torch.empty((n_d, Ld, dim), dtype=torch.float32, device=dev)
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        rc = lib.mmb200_maxsim_bwd(_ptr(q), _ptr(d), _ptr(grad_out), _ptr(argmax.contiguous()), _ptr(gq), _ptr(gd),
-                                   n_q, n_d, n_d, docs_per_query, Lq, Ld, dim, _DTYPES[q.dtype], _stream(dev))
-    _lib.check(rc, "mmb200_maxsim_bwd")
+    _launch(dev, "mmb200_maxsim_bwd", q, d, grad_out, argmax.contiguous(), gq, gd, n_q, n_d, n_d, docs_per_query, Lq,
+            Ld, dim, _DTYPES[q.dtype])
     return gq, gd
 
 
@@ -220,6 +245,16 @@ def _f32c(t: torch.Tensor) -> torch.Tensor:
     return t.detach().to(torch.float32).contiguous()
 
 
+def _kernel_pool_operands(q_mask, d_mask, mu, sigma, weight, alpha, doc_gate, B: int, Ld: int):
+    """The operands every kernel-pooling entry takes after q and d, in its argument order (q_mask, d_mask, gate, mu,
+    sigma, alpha, weight): masks of one element type, the rest fp32 (gate [B, Ld]); with the mask code and K."""
+    q_mask, d_mask, mcode = _common_mask_dtype(_prep_mask(q_mask), _prep_mask(d_mask))
+    mu, sigma, weight = _f32c(mu).view(-1), _f32c(sigma).view(-1), _f32c(weight).view(-1)
+    alpha = None if alpha is None else _f32c(alpha).view(-1)
+    gate = None if doc_gate is None else _f32c(doc_gate).reshape(B, Ld)
+    return (q_mask, d_mask, gate, mu, sigma, alpha, weight), mcode, mu.numel()
+
+
 def kernel_pool(q: torch.Tensor, d: torch.Tensor, q_mask: torch.Tensor, d_mask: torch.Tensor,
                 mu: torch.Tensor, sigma: torch.Tensor, weight: torch.Tensor, alpha: Optional[torch.Tensor] = None,
                 log_scale: float = 1.0, want_per_kernel: bool = False, want_per_kernel_query: bool = False,
@@ -245,37 +280,22 @@ def kernel_pool(q: torch.Tensor, d: torch.Tensor, q_mask: torch.Tensor, d_mask: 
     _, Ld, _ = d.shape
     if d.shape[0] != B or d.shape[2] != D:
         raise _lib.MatchmakerB200Error(f"shape mismatch: q {tuple(q.shape)} d {tuple(d.shape)}")
-    q_mask, d_mask, mcode = _common_mask_dtype(_prep_mask(q_mask), _prep_mask(d_mask))
-    mu, sigma, weight = _f32c(mu).view(-1), _f32c(sigma).view(-1), _f32c(weight).view(-1)
-    alpha = None if alpha is None else _f32c(alpha).view(-1)
-    K = mu.numel()
+    ops, mcode, K = _kernel_pool_operands(q_mask, d_mask, mu, sigma, weight, alpha, doc_gate, B, Ld)
     score = torch.empty(B, dtype=torch.float32, device=dev)
     pk = torch.empty((B, K), dtype=torch.float32, device=dev) if want_per_kernel else None
     pkq = torch.empty((B, Lq, K), dtype=torch.float32, device=dev) if want_per_kernel_query else None
     cos = torch.empty((B, Lq, Ld), dtype=torch.float32, device=dev) if want_cosine else None
-    gate = None
-    if doc_gate is not None:
-        gate = _f32c(doc_gate).reshape(B, Ld)
-    lib = _lib.load()
     if save_for_backward:
         if want_cosine or not kernel_pool_train_supported(Lq, Ld, D, K):
             raise _lib.MatchmakerB200Error("kernel_pool(save_for_backward=True): outside the tensor-core training envelope")
         if pkq is None:
             pkq = torch.empty((B, Lq, K), dtype=torch.float32, device=dev)
-        saved = torch.empty(int(lib.mmb200_kernel_pool_saved_floats(B, Ld)), dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            rc = lib.mmb200_kernel_pool_fwd_train(_ptr(q), _ptr(d), _ptr(q_mask), _ptr(d_mask), _ptr(gate), _ptr(mu), _ptr(sigma),
-                                                  _ptr(alpha), _ptr(weight), _ptr(score), _ptr(pk), _ptr(pkq), _ptr(saved),
-                                                  B, Lq, Ld, D, K, float(log_scale), float(clamp_min), float(bias), mcode,
-                                                  _stream(dev))
-        _lib.check(rc, "mmb200_kernel_pool_fwd_train")
+        saved = torch.empty(int(_lib.load().mmb200_kernel_pool_saved_floats(B, Ld)), dtype=torch.float32, device=dev)
+        _launch(dev, "mmb200_kernel_pool_fwd_train", q, d, *ops, score, pk, pkq, saved, B, Lq, Ld, D, K,
+                float(log_scale), float(clamp_min), float(bias), mcode)
         return {"score": score, "per_kernel": pk, "per_kernel_query": pkq, "cosine": None, "saved": saved}
-    with torch.cuda.device(dev):
-        rc = lib.mmb200_kernel_pool_fwd_ex(_ptr(q), _ptr(d), _ptr(q_mask), _ptr(d_mask), _ptr(gate), _ptr(mu), _ptr(sigma),
-                                           _ptr(alpha), _ptr(weight), _ptr(score), _ptr(pk), _ptr(pkq), _ptr(cos),
-                                           B, Lq, Ld, D, K, float(log_scale), float(clamp_min), float(bias), mcode,
-                                           _IMPLS[impl], _stream(dev))
-    _lib.check(rc, "mmb200_kernel_pool_fwd_ex")
+    _launch(dev, "mmb200_kernel_pool_fwd_ex", q, d, *ops, score, pk, pkq, cos, B, Lq, Ld, D, K, float(log_scale),
+            float(clamp_min), float(bias), mcode, _IMPLS[impl])
     return {"score": score, "per_kernel": pk, "per_kernel_query": pkq, "cosine": cos}
 
 
@@ -294,42 +314,24 @@ def kernel_pool_bwd(q, d, q_mask, d_mask, mu, sigma, weight, alpha, per_kernel_q
     q, d = q.float().contiguous(), d.float().contiguous()
     B, Lq, D = q.shape
     Ld = d.shape[1]
-    q_mask, d_mask, mcode = _common_mask_dtype(_prep_mask(q_mask), _prep_mask(d_mask))
-    mu, sigma, weight = _f32c(mu).view(-1), _f32c(sigma).view(-1), _f32c(weight).view(-1)
-    alpha_c = None if alpha is None else _f32c(alpha).view(-1)
-    K = mu.numel()
+    ops, mcode, K = _kernel_pool_operands(q_mask, d_mask, mu, sigma, weight, alpha, doc_gate, B, Ld)
     gq = torch.empty_like(q)
     gd = torch.empty_like(d)
     ga = torch.empty(K, dtype=torch.float32, device=dev)
     gw = torch.empty(K, dtype=torch.float32, device=dev)
-    gate = None if doc_gate is None else _f32c(doc_gate).reshape(B, Ld)
     gg = None if doc_gate is None else torch.empty((B, Ld), dtype=torch.float32, device=dev)
-    lib = _lib.load()
     if saved is not None:
         # at BERT widths (512 < D <= 1024) the workspace also carries the backward's per-pair G matrices
-        ws = torch.empty(int(lib.mmb200_kernel_pool_bwd_saved_workspace_floats(B, Lq, Ld, D, K)), dtype=torch.float32,
-                         device=dev)
-        with torch.cuda.device(dev):
-            rc = lib.mmb200_kernel_pool_bwd_saved(_ptr(q), _ptr(d), _ptr(q_mask), _ptr(d_mask), _ptr(gate), _ptr(mu), _ptr(sigma),
-                                                  _ptr(alpha_c), _ptr(weight), _ptr(per_kernel_query.contiguous()),
-                                                  _ptr(saved), _ptr(_f32c(grad_score)), _ptr(gq), _ptr(gd), _ptr(gg), _ptr(ga),
-                                                  _ptr(gw), _ptr(ws), B, Lq, Ld, D, K, float(log_scale), float(clamp_min),
-                                                  mcode, _stream(dev))
-        _lib.check(rc, "mmb200_kernel_pool_bwd_saved")
-        if doc_gate is not None:
-            return gq, gd, (ga if alpha is not None else None), gw, gg
-        return gq, gd, (ga if alpha is not None else None), gw
-    ws = torch.empty(2 * B * K, dtype=torch.float32, device=dev)
-    with torch.cuda.device(dev):
-        rc = lib.mmb200_kernel_pool_bwd_ex(_ptr(q), _ptr(d), _ptr(q_mask), _ptr(d_mask), _ptr(gate), _ptr(mu), _ptr(sigma),
-                                           _ptr(alpha_c), _ptr(weight), _ptr(per_kernel_query.contiguous()),
-                                           _ptr(_f32c(grad_score)), _ptr(gq), _ptr(gd), _ptr(gg), _ptr(ga), _ptr(gw),
-                                           _ptr(ws), B, Lq, Ld, D, K, float(log_scale), float(clamp_min), mcode,
-                                           _stream(dev))
-    _lib.check(rc, "mmb200_kernel_pool_bwd_ex")
-    if doc_gate is not None:
-        return gq, gd, (ga if alpha is not None else None), gw, gg
-    return gq, gd, (ga if alpha is not None else None), gw
+        ws = torch.empty(int(_lib.load().mmb200_kernel_pool_bwd_saved_workspace_floats(B, Lq, Ld, D, K)),
+                         dtype=torch.float32, device=dev)
+        _launch(dev, "mmb200_kernel_pool_bwd_saved", q, d, *ops, per_kernel_query.contiguous(), saved,
+                _f32c(grad_score), gq, gd, gg, ga, gw, ws, B, Lq, Ld, D, K, float(log_scale), float(clamp_min), mcode)
+    else:
+        ws = torch.empty(2 * B * K, dtype=torch.float32, device=dev)
+        _launch(dev, "mmb200_kernel_pool_bwd_ex", q, d, *ops, per_kernel_query.contiguous(), _f32c(grad_score), gq, gd,
+                gg, ga, gw, ws, B, Lq, Ld, D, K, float(log_scale), float(clamp_min), mcode)
+    grads = (gq, gd, ga if alpha is not None else None, gw)
+    return grads if doc_gate is None else grads + (gg,)
 
 
 def dot_pairs(qv: torch.Tensor, dv: torch.Tensor) -> torch.Tensor:
@@ -340,11 +342,7 @@ def dot_pairs(qv: torch.Tensor, dv: torch.Tensor) -> torch.Tensor:
                                        f"{qv.dtype} / {tuple(dv.shape)} {dv.dtype}")
     qv, dv = qv.contiguous(), dv.contiguous()
     out = torch.empty(qv.shape[0], dtype=torch.float32, device=dev)
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        rc = lib.mmb200_dot_pairs(_ptr(qv), _ptr(dv), _ptr(out), qv.shape[0], qv.shape[1], _DTYPES[qv.dtype],
-                                  _stream(dev))
-    _lib.check(rc, "mmb200_dot_pairs")
+    _launch(dev, "mmb200_dot_pairs", qv, dv, out, qv.shape[0], qv.shape[1], _DTYPES[qv.dtype])
     return out
 
 
@@ -379,6 +377,30 @@ def tkl_kernel_set_covers(mu: torch.Tensor, sigma: torch.Tensor) -> bool:
     return ok
 
 
+def _tkl_slot_map(packed_indices: torch.Tensor) -> torch.Tensor:
+    """Packed index of every chunk slot (-1 = dropped by the packing), one kernel launch (mmb200_tkl_slot_map)."""
+    pk = packed_indices.reshape(-1)
+    if pk.dtype not in (torch.bool, torch.uint8):
+        pk = pk != 0
+    pk = pk.contiguous()
+    out = torch.empty(pk.numel(), dtype=torch.int32, device=pk.device)
+    _launch(pk.device, "mmb200_tkl_slot_map", pk, out, pk.numel())
+    return out
+
+
+def _tkl_operands(q_mask, chunk_mask, packed_indices, mu, sigma, dense_weight, sat_red_weight, sat_params,
+                  saturation: str):
+    """The operands both TKL entries share: masks of one element type and their code, the slot map, the kernel and
+    saturation parameters as flat fp32, and the saturation code."""
+    slot = _tkl_slot_map(packed_indices)
+    q_mask, chunk_mask, mcode = _common_mask_dtype(_prep_mask(q_mask), _prep_mask(chunk_mask))
+    mu, sigma, dense_weight = _f32c(mu).view(-1), _f32c(sigma).view(-1), _f32c(dense_weight).view(-1)
+    sat_params = _f32c(sat_params).view(-1)
+    red = None if sat_red_weight is None else _f32c(sat_red_weight).view(-1)
+    sat_code = {"embedding": 0, "log": 1}[saturation]
+    return q_mask, chunk_mask, mcode, slot, mu, sigma, dense_weight, red, sat_params, sat_code
+
+
 def tkl_window_scores(q_ctx: torch.Tensor, q_mask: torch.Tensor, doc_chunks: torch.Tensor, chunk_mask: torch.Tensor,
                       packed_indices: torch.Tensor, chunk_pieces: int, mu: torch.Tensor, sigma: torch.Tensor,
                       dense_weight: torch.Tensor, saturation: str, sat_params: torch.Tensor,
@@ -394,12 +416,8 @@ def tkl_window_scores(q_ctx: torch.Tensor, q_mask: torch.Tensor, doc_chunks: tor
     C = int(chunk_pieces)
     if packed_indices.numel() != B * C or doc_chunks.shape[1] != TKL_CHUNK:
         raise _lib.MatchmakerB200Error("tkl_window_scores: inconsistent chunk packing")
-    slot_to_packed = _tkl_slot_map(packed_indices)
-    q_mask, chunk_mask, mcode = _common_mask_dtype(_prep_mask(q_mask), _prep_mask(chunk_mask))
-    mu, sigma, dense_weight = _f32c(mu).view(-1), _f32c(sigma).view(-1), _f32c(dense_weight).view(-1)
-    sat_params = _f32c(sat_params).view(-1)
-    sat_code = {"embedding": 0, "log": 1}[saturation]
-    red = None if sat_red_weight is None else _f32c(sat_red_weight).view(-1)
+    q_mask, chunk_mask, mcode, slot, mu, sigma, dense_weight, red, sat_params, sat_code = _tkl_operands(
+        q_mask, chunk_mask, packed_indices, mu, sigma, dense_weight, sat_red_weight, sat_params, saturation)
     K = mu.numel()
     W = (C * TKL_CHUNK - TKL_WINDOW) // 2 + 1
     out = torch.empty((B, W), dtype=torch.float32, device=dev)
@@ -407,13 +425,8 @@ def tkl_window_scores(q_ctx: torch.Tensor, q_mask: torch.Tensor, doc_chunks: tor
         # decide on the host (cached per parameter version) so that only ONE of the two kernels is enqueued; the library's
         # own device-side check stays in force (a forced tensor-core call on a kernel set without cover writes zeros)
         impl = "tcgen05" if (Lq * K <= 512 and K <= 16 and tkl_kernel_set_covers(mu, sigma)) else "simt"
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        rc = lib.mmb200_tkl_window_scores(_ptr(q_ctx), _ptr(q_mask), _ptr(doc_chunks), _ptr(chunk_mask),
-                                          _ptr(slot_to_packed), _ptr(mu), _ptr(sigma), _ptr(dense_weight), _ptr(red),
-                                          _ptr(sat_params), _ptr(out), B, doc_chunks.shape[0], Lq, D, C, K, sat_code, mcode,
-                                          _IMPLS[impl], _stream(dev))
-    _lib.check(rc, "mmb200_tkl_window_scores")
+    _launch(dev, "mmb200_tkl_window_scores", q_ctx, q_mask, doc_chunks, chunk_mask, slot, mu, sigma, dense_weight, red,
+            sat_params, out, B, doc_chunks.shape[0], Lq, D, C, K, sat_code, mcode, _IMPLS[impl])
     return out
 
 
@@ -427,11 +440,7 @@ def tkl_top_hills(window_score: torch.Tensor, chunk_scoring: torch.Tensor):
     top_idx = torch.empty((B, 3), dtype=torch.int64, device=dev)
     top15 = torch.empty((B, 15), dtype=torch.float32, device=dev)
     score = torch.empty(B, dtype=torch.float32, device=dev)
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        rc = lib.mmb200_tkl_top_hills(_ptr(ws), _ptr(orig), _ptr(_f32c(chunk_scoring).view(-1)), _ptr(top_idx), _ptr(top15),
-                                      _ptr(score), B, W, _stream(dev))
-    _lib.check(rc, "mmb200_tkl_top_hills")
+    _launch(dev, "mmb200_tkl_top_hills", ws, orig, _f32c(chunk_scoring).view(-1), top_idx, top15, score, B, W)
     return score, orig, top_idx, top15
 
 
@@ -514,6 +523,32 @@ def _fp8_pair(a: torch.Tensor, b: torch.Tensor, what: str) -> bool:
     return fa
 
 
+def _search_queries(queries: torch.Tensor, store: torch.Tensor, fp8: bool, split_scale: Optional[int], what: str,
+                    rows_name: str):
+    """Queries [nq, dim] in the operand format of a search over ``store``: split like it when ``split_scale`` is given
+    (:func:`flat_ip_split_f32`), else cast to its dtype.  Returns (queries, dim, dtype code, unscale), unscale the
+    exponent of the power of two that takes the search's scores back to the unscaled domain (None: no scaling)."""
+    if split_scale is None:
+        if queries.shape[1] != store.shape[1]:
+            raise _lib.MatchmakerB200Error(f"{what}: queries have dim {queries.shape[1]}, {rows_name} {store.shape[1]}")
+        queries = queries.to(store.dtype).contiguous()
+        return queries, queries.shape[1], _lib.F8E4M3 if fp8 else _DTYPES[store.dtype], None
+    if store.dtype != torch.float16 or store.shape[1] % 2:
+        raise _lib.MatchmakerB200Error(f"{what}: split storage is [n, 2*dim] fp16")
+    dim = store.shape[1] // 2
+    if queries.shape[1] != dim:
+        raise _lib.MatchmakerB200Error(f"{what}: queries have dim {queries.shape[1]}, split {rows_name} {dim}")
+    queries, sq = flat_ip_split_f32(queries, "queries")
+    return queries, dim, _lib.F32_SPLIT16, -(sq + split_scale)
+
+
+def _unscale(scores: torch.Tensor, unscale: Optional[int]) -> torch.Tensor:
+    if unscale is None:
+        return scores
+    # back to the unscaled domain: a power of two, exact; faiss's "no result" filler (-FLT_MAX) stays what it is
+    return torch.where(scores > -3.0e38, torch.ldexp(scores, torch.tensor(unscale, device=scores.device)), scores)
+
+
 def flat_ip_topk(queries: torch.Tensor, passages: torch.Tensor, k: int, ids: Optional[torch.Tensor] = None,
                  id_base: int = 0, split_scale: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor]:
     """Exact inner-product top-k of every query against a resident passage shard (faiss IndexFlatIP
@@ -531,22 +566,7 @@ def flat_ip_topk(queries: torch.Tensor, passages: torch.Tensor, k: int, ids: Opt
         raise _lib.MatchmakerB200Error("flat_ip_topk: passage storage must be fp16 / bf16, or the fp16 split of fp32 "
                                        "(flat_ip_split_f32)")
     n = passages.shape[0]
-    unscale = None
-    if split_scale is not None:
-        if passages.dtype != torch.float16 or passages.shape[1] % 2:
-            raise _lib.MatchmakerB200Error("flat_ip_topk: split storage is [n, 2*dim] fp16")
-        dim = passages.shape[1] // 2
-        if queries.shape[1] != dim:
-            raise _lib.MatchmakerB200Error(f"flat_ip_topk: queries have dim {queries.shape[1]}, split passages {dim}")
-        queries, sq = flat_ip_split_f32(queries, "queries")
-        unscale = -(sq + split_scale)
-        dcode = _lib.F32_SPLIT16
-    else:
-        if queries.shape[1] != passages.shape[1]:
-            raise _lib.MatchmakerB200Error(f"flat_ip_topk: queries have dim {queries.shape[1]}, passages {passages.shape[1]}")
-        queries = queries.to(passages.dtype).contiguous()
-        dim = queries.shape[1]
-        dcode = _lib.F8E4M3 if fp8 else _DTYPES[passages.dtype]
+    queries, dim, dcode, unscale = _search_queries(queries, passages, fp8, split_scale, "flat_ip_topk", "passages")
     passages = passages.contiguous()
     nq = queries.shape[0]
     if ids is not None:
@@ -554,22 +574,16 @@ def flat_ip_topk(queries: torch.Tensor, passages: torch.Tensor, k: int, ids: Opt
     if nq == 0 and 1 <= k <= FLAT_IP_MAX_K:   # as ivf_search: an empty batch has an empty result
         return (torch.empty((0, k), dtype=torch.float32, device=dev),
                 torch.empty((0, k), dtype=torch.int64, device=dev))
-    lib = _lib.load()
     with torch.cuda.device(dev):
-        wsb = lib.mmb200_flat_ip_workspace_bytes(nq, n, k)
-        if wsb <= 0:
-            raise _lib.MatchmakerB200Error(f"flat_ip_topk: unsupported sizes nq={nq} n={n} k={k} (1 <= k <= {FLAT_IP_MAX_K}): "
-                                           + _lib.last_error())
-        ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
-        out_s = torch.empty((nq, k), dtype=torch.float32, device=dev)
-        out_i = torch.empty((nq, k), dtype=torch.int64, device=dev)
-        rc = lib.mmb200_flat_ip_topk(_ptr(queries), _ptr(passages), _ptr(ids), _ptr(out_s), _ptr(out_i), _ptr(ws), wsb,
-                                     nq, n, dim, k, dcode, id_base, _stream(dev))
-    _lib.check(rc, "mmb200_flat_ip_topk")
-    if unscale is not None:
-        # back to the unscaled domain: a power of two, exact; faiss's "no result" filler (-FLT_MAX) stays what it is
-        out_s = torch.where(out_s > -3.0e38, torch.ldexp(out_s, torch.tensor(unscale, device=dev)), out_s)
-    return out_s, out_i
+        wsb = _lib.load().mmb200_flat_ip_workspace_bytes(nq, n, k)
+    if wsb <= 0:
+        raise _lib.MatchmakerB200Error(f"flat_ip_topk: unsupported sizes nq={nq} n={n} k={k} (1 <= k <= {FLAT_IP_MAX_K}): "
+                                       + _lib.last_error())
+    ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+    out_s = torch.empty((nq, k), dtype=torch.float32, device=dev)
+    out_i = torch.empty((nq, k), dtype=torch.int64, device=dev)
+    _launch(dev, "mmb200_flat_ip_topk", queries, passages, ids, out_s, out_i, ws, wsb, nq, n, dim, k, dcode, id_base)
+    return _unscale(out_s, unscale), out_i
 
 
 def topk_merge(cand_scores: torch.Tensor, cand_ids: torch.Tensor, k: int) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -580,10 +594,7 @@ def topk_merge(cand_scores: torch.Tensor, cand_ids: torch.Tensor, k: int) -> Tup
     nq, L = cand_scores.shape
     out_s = torch.empty((nq, k), dtype=torch.float32, device=dev)
     out_i = torch.empty((nq, k), dtype=torch.int64, device=dev)
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        rc = lib.mmb200_topk_merge(_ptr(cand_scores), _ptr(cand_ids), _ptr(out_s), _ptr(out_i), nq, L, k, _stream(dev))
-    _lib.check(rc, "mmb200_topk_merge")
+    _launch(dev, "mmb200_topk_merge", cand_scores, cand_ids, out_s, out_i, nq, L, k)
     return out_s, out_i
 
 
@@ -602,10 +613,7 @@ def topk_unique(cand_scores: torch.Tensor, cand_ids: torch.Tensor, k: int) -> Tu
         raise _lib.MatchmakerB200Error(f"topk_unique: scores {tuple(cand_scores.shape)} vs ids {tuple(cand_ids.shape)}")
     out_s = torch.empty((nq, k), dtype=torch.float32, device=dev)
     out_i = torch.empty((nq, k), dtype=torch.int64, device=dev)
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        rc = lib.mmb200_topk_unique(_ptr(cand_scores), _ptr(cand_ids), _ptr(out_s), _ptr(out_i), nq, L, k, _stream(dev))
-    _lib.check(rc, "mmb200_topk_unique")
+    _launch(dev, "mmb200_topk_unique", cand_scores, cand_ids, out_s, out_i, nq, L, k)
     return out_s, out_i
 
 
@@ -651,22 +659,7 @@ def ivf_search(queries: torch.Tensor, rows: torch.Tensor, ids: torch.Tensor, lis
         raise _lib.MatchmakerB200Error(f"ivf_search: probes must be [nq, nprobe], got {tuple(probes.shape)}")
     nq, nprobe = probes.shape
     nlist = list_offsets.numel() - 1
-    unscale = None
-    if split_scale is not None:
-        if rows.dtype != torch.float16 or rows.shape[1] % 2:
-            raise _lib.MatchmakerB200Error("ivf_search: split storage is [n, 2*dim] fp16")
-        dim = rows.shape[1] // 2
-        if queries.shape[1] != dim:
-            raise _lib.MatchmakerB200Error(f"ivf_search: queries have dim {queries.shape[1]}, split rows {dim}")
-        queries, sq = flat_ip_split_f32(queries, "queries")
-        unscale = -(sq + split_scale)
-        dcode = _lib.F32_SPLIT16
-    else:
-        if queries.shape[1] != rows.shape[1]:
-            raise _lib.MatchmakerB200Error(f"ivf_search: queries have dim {queries.shape[1]}, rows {rows.shape[1]}")
-        queries = queries.to(rows.dtype).contiguous()
-        dim = queries.shape[1]
-        dcode = _lib.F8E4M3 if fp8 else _DTYPES[rows.dtype]
+    queries, dim, dcode, unscale = _search_queries(queries, rows, fp8, split_scale, "ivf_search", "rows")
     if ids.numel() != rows.shape[0] or list_offsets.dim() != 1 or nlist < 1:
         raise _lib.MatchmakerB200Error(f"ivf_search: {ids.numel()} ids for {rows.shape[0]} rows, list_offsets "
                                        f"{tuple(list_offsets.shape)} (need [nlist + 1], nlist >= 1)")
@@ -681,30 +674,23 @@ def ivf_search(queries: torch.Tensor, rows: torch.Tensor, ids: torch.Tensor, lis
     out_i = torch.empty((nq, k), dtype=torch.int64, device=dev)
     if nq == 0:
         return out_s, out_i
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        def wsb(b):
-            return lib.mmb200_ivf_workspace_bytes(b, nprobe, nlist, max_list_len, dim, k, dcode)
-        if wsb(1) <= 0:
-            raise _lib.MatchmakerB200Error(f"ivf_search: unsupported sizes nprobe={nprobe} nlist={nlist} dim={dim} k={k} "
-                                           f"(1 <= k <= {FLAT_IP_MAX_K}, 1 <= nprobe <= {IVF_MAX_PROBE}, dim % 64 == 0; "
-                                           "e4m3: dim % 128 == 0, 128 <= dim <= 1024)")
-        b = ivf_query_batch(nq, wsb, IVF_WORKSPACE_CAP)
-        ws = torch.empty(wsb(b), dtype=torch.uint8, device=dev)
-        for b0 in range(0, nq, b):
-            b1 = min(nq, b0 + b)
-            tail = (_ptr(probes[b0:b1]), _ptr(out_s[b0:b1]), _ptr(out_i[b0:b1]), _ptr(ws), ws.numel(), b1 - b0, nprobe,
-                    nlist, rows.shape[0], max_list_len, dim, k, dcode, _stream(dev))
-            if row_index is None:
-                rc = lib.mmb200_ivf_search(_ptr(queries[b0:b1]), _ptr(rows), _ptr(ids), _ptr(list_offsets), *tail)
-                _lib.check(rc, "mmb200_ivf_search")
-            else:
-                rc = lib.mmb200_ivf_search_gather(_ptr(queries[b0:b1]), _ptr(rows), _ptr(ids), _ptr(row_index),
-                                                  _ptr(list_offsets), *tail)
-                _lib.check(rc, "mmb200_ivf_search_gather")
-    if unscale is not None:
-        out_s = torch.where(out_s > -3.0e38, torch.ldexp(out_s, torch.tensor(unscale, device=dev)), out_s)
-    return out_s, out_i
+
+    def workspace_bytes(b):
+        return _lib.load().mmb200_ivf_workspace_bytes(b, nprobe, nlist, max_list_len, dim, k, dcode)
+
+    def scan(b0, b1, ws):
+        tail = (probes[b0:b1], out_s[b0:b1], out_i[b0:b1], ws, ws.numel(), b1 - b0, nprobe, nlist, rows.shape[0],
+                max_list_len, dim, k, dcode)
+        if row_index is None:
+            _launch(dev, "mmb200_ivf_search", queries[b0:b1], rows, ids, list_offsets, *tail)
+        else:
+            _launch(dev, "mmb200_ivf_search_gather", queries[b0:b1], rows, ids, row_index, list_offsets, *tail)
+
+    _scan_batches(dev, nq, workspace_bytes, IVF_WORKSPACE_CAP,
+                  f"ivf_search: unsupported sizes nprobe={nprobe} nlist={nlist} dim={dim} k={k} "
+                  f"(1 <= k <= {FLAT_IP_MAX_K}, 1 <= nprobe <= {IVF_MAX_PROBE}, dim % 64 == 0; "
+                  "e4m3: dim % 128 == 0, 128 <= dim <= 1024)", scan)
+    return _unscale(out_s, unscale), out_i
 
 
 def ivf_list_means(x: torch.Tensor, perm: torch.Tensor, offsets: torch.Tensor) -> torch.Tensor:
@@ -716,11 +702,7 @@ def ivf_list_means(x: torch.Tensor, perm: torch.Tensor, offsets: torch.Tensor) -
     x, perm, offsets = x.contiguous(), perm.to(torch.int64).contiguous(), offsets.to(torch.int64).contiguous()
     nlist = offsets.numel() - 1
     out = torch.empty((nlist, x.shape[1]), dtype=torch.float32, device=dev)
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        rc = lib.mmb200_ivf_list_means(_ptr(x), _ptr(perm), _ptr(offsets), _ptr(out), nlist, x.shape[1], _DTYPES[x.dtype],
-                                       _stream(dev))
-    _lib.check(rc, "mmb200_ivf_list_means")
+    _launch(dev, "mmb200_ivf_list_means", x, perm, offsets, out, nlist, x.shape[1], _DTYPES[x.dtype])
     return out
 
 
@@ -772,11 +754,7 @@ def residual_encode(rows: torch.Tensor, list_ids: torch.Tensor, base: torch.Tens
     list_ids = _residual_list_ids(list_ids, n, base.shape[0], "residual_encode")
     rows, cutoff = rows.contiguous(), cutoff.contiguous()
     out = torch.empty((n, dim * bits // 8), dtype=torch.uint8, device=dev)
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        rc = lib.mmb200_residual_encode(_ptr(rows), _ptr(list_ids), _ptr(base), _ptr(cutoff), _ptr(out), n, dim, bits,
-                                        _stream(dev))
-    _lib.check(rc, "mmb200_residual_encode")
+    _launch(dev, "mmb200_residual_encode", rows, list_ids, base, cutoff, out, n, dim, bits)
     return out
 
 
@@ -791,11 +769,7 @@ def residual_decode(codes: torch.Tensor, list_ids: torch.Tensor, base: torch.Ten
     n = codes.shape[0]
     list_ids = _residual_list_ids(list_ids, n, base.shape[0], "residual_decode")
     out = torch.empty((n, dim), dtype=torch.float16, device=dev)
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        rc = lib.mmb200_residual_decode(_ptr(codes), _ptr(list_ids), _ptr(base), _ptr(weight), _ptr(out), n, dim, bits,
-                                        _stream(dev))
-    _lib.check(rc, "mmb200_residual_decode")
+    _launch(dev, "mmb200_residual_decode", codes, list_ids, base, weight, out, n, dim, bits)
     return out
 
 
@@ -829,22 +803,18 @@ def ivf_search_residual(queries: torch.Tensor, codes: torch.Tensor, base: torch.
     out_i = torch.empty((nq, k), dtype=torch.int64, device=dev)
     if nq == 0:
         return out_s, out_i
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        def wsb(b):
-            return lib.mmb200_ivf_workspace_bytes(b, nprobe, nlist, max_list_len, dim, k, _lib.F16)
-        if wsb(1) <= 0:
-            raise _lib.MatchmakerB200Error(f"ivf_search_residual: unsupported sizes nprobe={nprobe} nlist={nlist} k={k} "
-                                           f"(1 <= k <= {FLAT_IP_MAX_K}, 1 <= nprobe <= {IVF_MAX_PROBE})")
-        b = ivf_query_batch(nq, wsb, IVF_WORKSPACE_CAP)
-        ws = torch.empty(wsb(b), dtype=torch.uint8, device=dev)
-        for b0 in range(0, nq, b):
-            b1 = min(nq, b0 + b)
-            rc = lib.mmb200_ivf_search_residual(_ptr(queries[b0:b1]), _ptr(codes), _ptr(base), _ptr(weight), bits,
-                                                _ptr(ids), _ptr(row_index), _ptr(list_offsets), _ptr(probes[b0:b1]),
-                                                _ptr(out_s[b0:b1]), _ptr(out_i[b0:b1]), _ptr(ws), ws.numel(), b1 - b0,
-                                                nprobe, nlist, codes.shape[0], max_list_len, dim, k, _stream(dev))
-            _lib.check(rc, "mmb200_ivf_search_residual")
+
+    def workspace_bytes(b):
+        return _lib.load().mmb200_ivf_workspace_bytes(b, nprobe, nlist, max_list_len, dim, k, _lib.F16)
+
+    def scan(b0, b1, ws):
+        _launch(dev, "mmb200_ivf_search_residual", queries[b0:b1], codes, base, weight, bits, ids, row_index, list_offsets,
+                probes[b0:b1], out_s[b0:b1], out_i[b0:b1], ws, ws.numel(), b1 - b0, nprobe, nlist, codes.shape[0],
+                max_list_len, dim, k)
+
+    _scan_batches(dev, nq, workspace_bytes, IVF_WORKSPACE_CAP,
+                  f"ivf_search_residual: unsupported sizes nprobe={nprobe} nlist={nlist} k={k} "
+                  f"(1 <= k <= {FLAT_IP_MAX_K}, 1 <= nprobe <= {IVF_MAX_PROBE})", scan)
     return out_s, out_i
 
 
@@ -865,19 +835,11 @@ def maxsim_store_residual(q: torch.Tensor, codes: torch.Tensor, list_ids: torch.
     q = q.to(torch.float16).contiguous()
     list_ids = list_ids.to(torch.int32).contiguous()
     doc_offsets = doc_offsets.to(torch.int64).contiguous()
-    pair_q = pair_q.to(torch.int32).contiguous().view(-1)
-    pair_d = pair_d.to(torch.int32).contiguous().view(-1)
-    if pair_q.numel() != pair_d.numel():
-        raise _lib.MatchmakerB200Error("pair_q / pair_d length mismatch")
+    pair_q, pair_d = _pairs(pair_q, pair_d)
     n_q, Lq, _ = q.shape
     out = torch.empty(pair_q.numel(), dtype=torch.float32, device=dev)
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        rc = lib.mmb200_maxsim_store_residual_fwd(_ptr(q), _ptr(codes), _ptr(list_ids), _ptr(base), _ptr(weight), bits,
-                                                  _ptr(doc_offsets), _ptr(pair_q), _ptr(pair_d), _ptr(out), n_q,
-                                                  codes.shape[0], doc_offsets.numel() - 1, pair_q.numel(), Lq,
-                                                  int(max_doc_len), dim, _stream(dev))
-    _lib.check(rc, "mmb200_maxsim_store_residual_fwd")
+    _launch(dev, "mmb200_maxsim_store_residual_fwd", q, codes, list_ids, base, weight, bits, doc_offsets, pair_q, pair_d,
+            out, n_q, codes.shape[0], doc_offsets.numel() - 1, pair_q.numel(), Lq, int(max_doc_len), dim)
     return out
 
 
@@ -918,13 +880,9 @@ def plaid_centroid_scores(q: torch.Tensor, centroids: torch.Tensor, threshold: f
     q, centroids = q.to(torch.float16).contiguous(), centroids.to(torch.float16).contiguous()
     scores = torch.empty((nq, nlist, plaid_lqp(lq)), dtype=torch.float16, device=dev)
     keep = torch.empty((nq, (nlist + 31) // 32), dtype=torch.int32, device=dev)
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        for b0 in range(0, nq, PLAID_MAX_QUERIES):
-            b1 = min(nq, b0 + PLAID_MAX_QUERIES)
-            rc = lib.mmb200_plaid_centroid_scores(_ptr(q[b0:b1]), _ptr(centroids), _ptr(scores[b0:b1]), _ptr(keep[b0:b1]),
-                                                  b1 - b0, lq, nlist, dim, float(threshold), _stream(dev))
-            _lib.check(rc, "mmb200_plaid_centroid_scores")
+    for b0, b1 in _query_slices(nq, PLAID_MAX_QUERIES):
+        _launch(dev, "mmb200_plaid_centroid_scores", q[b0:b1], centroids, scores[b0:b1], keep[b0:b1], b1 - b0, lq, nlist,
+                dim, float(threshold))
     return scores, keep
 
 
@@ -946,11 +904,8 @@ def plaid_candidates(probes: torch.Tensor, plist_offsets: torch.Tensor, plist_pi
     if nq == 0 or n_probes == 0:
         return out.fill_(-1)
     bitmap = torch.empty(nq * max(1, (n_docs + 31) // 32), dtype=torch.int32, device=dev)
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        rc = lib.mmb200_plaid_candidates(_ptr(probes), _ptr(plist_offsets), _ptr(plist_pids), _ptr(bitmap), _ptr(out), nq,
-                                         n_probes, plist_offsets.numel() - 1, n_docs, cap, first_doc, _stream(dev))
-    _lib.check(rc, "mmb200_plaid_candidates")
+    _launch(dev, "mmb200_plaid_candidates", probes, plist_offsets, plist_pids, bitmap, out, nq, n_probes,
+            plist_offsets.numel() - 1, n_docs, cap, first_doc)
     return out
 
 
@@ -982,15 +937,9 @@ def plaid_interaction(scores: torch.Tensor, keep: Optional[torch.Tensor], list_i
     out = torch.empty((nq, n_cand), dtype=torch.float32, device=dev)
     if nq == 0 or n_cand == 0:
         return out
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        for b0 in range(0, nq, PLAID_MAX_QUERIES):
-            b1 = min(nq, b0 + PLAID_MAX_QUERIES)
-            rc = lib.mmb200_plaid_interaction(_ptr(scores[b0:b1]), None if keep is None else _ptr(keep[b0:b1]),
-                                              _ptr(list_ids), _ptr(doc_offsets), _ptr(cand[b0:b1]), _ptr(out[b0:b1]),
-                                              b1 - b0, lq, nlist, n_docs, n_cand, first_doc, int(keep is not None),
-                                              _stream(dev))
-            _lib.check(rc, "mmb200_plaid_interaction")
+    for b0, b1 in _query_slices(nq, PLAID_MAX_QUERIES):
+        _launch(dev, "mmb200_plaid_interaction", scores[b0:b1], None if keep is None else keep[b0:b1], list_ids,
+                doc_offsets, cand[b0:b1], out[b0:b1], b1 - b0, lq, nlist, n_docs, n_cand, first_doc, int(keep is not None))
     return out
 
 
@@ -1027,21 +976,17 @@ def ah_search(luts: torch.Tensor, codes: torch.Tensor, list_offsets: torch.Tenso
     out_p = torch.empty((nq, kr), dtype=torch.int64, device=dev)
     if nq == 0:
         return out_s, out_p
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        def wsb(b):
-            return lib.mmb200_ah_workspace_bytes(b, nprobe, nlist, max_list_len, dim, kr)
-        if wsb(1) <= 0:
-            raise _lib.MatchmakerB200Error(f"ah_search: unsupported sizes nprobe={nprobe} nlist={nlist} dim={dim} kr={kr} "
-                                           f"(1 <= kr <= {AH_MAX_KR}, 1 <= nprobe <= {IVF_MAX_PROBE}, dim % 64 == 0)")
-        b = ivf_query_batch(nq, wsb, AH_WORKSPACE_CAP)
-        ws = torch.empty(wsb(b), dtype=torch.uint8, device=dev)
-        for b0 in range(0, nq, b):
-            b1 = min(nq, b0 + b)
-            rc = lib.mmb200_ah_search(_ptr(luts[b0:b1]), _ptr(codes), _ptr(list_offsets), _ptr(probes[b0:b1]),
-                                      _ptr(bias[b0:b1]), _ptr(out_s[b0:b1]), _ptr(out_p[b0:b1]), _ptr(ws), ws.numel(),
-                                      b1 - b0, nprobe, nlist, n, max_list_len, dim, kr, _stream(dev))
-            _lib.check(rc, "mmb200_ah_search")
+
+    def workspace_bytes(b):
+        return _lib.load().mmb200_ah_workspace_bytes(b, nprobe, nlist, max_list_len, dim, kr)
+
+    def scan(b0, b1, ws):
+        _launch(dev, "mmb200_ah_search", luts[b0:b1], codes, list_offsets, probes[b0:b1], bias[b0:b1], out_s[b0:b1],
+                out_p[b0:b1], ws, ws.numel(), b1 - b0, nprobe, nlist, n, max_list_len, dim, kr)
+
+    _scan_batches(dev, nq, workspace_bytes, AH_WORKSPACE_CAP,
+                  f"ah_search: unsupported sizes nprobe={nprobe} nlist={nlist} dim={dim} kr={kr} "
+                  f"(1 <= kr <= {AH_MAX_KR}, 1 <= nprobe <= {IVF_MAX_PROBE}, dim % 64 == 0)", scan)
     return out_s, out_p
 
 
@@ -1069,11 +1014,8 @@ def ah_reorder(queries: torch.Tensor, rows: torch.Tensor, ids: Optional[torch.Te
     out_i = torch.empty((nq, top_n), dtype=torch.int64, device=dev)
     if nq == 0:
         return out_s, out_i
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        rc = lib.mmb200_ah_reorder(_ptr(queries), _ptr(rows), _ptr(ids), _ptr(shortlist), _ptr(out_s), _ptr(out_i), nq, n,
-                                   dim, kr, int(top_n), _DTYPES[rows.dtype], _stream(dev))
-    _lib.check(rc, "mmb200_ah_reorder")
+    _launch(dev, "mmb200_ah_reorder", queries, rows, ids, shortlist, out_s, out_i, nq, n, dim, kr, int(top_n),
+            _DTYPES[rows.dtype])
     return out_s, out_i
 
 
@@ -1100,10 +1042,7 @@ def graph_prune(knn: torch.Tensor, R: int) -> torch.Tensor:
                                        f"got K={K} R={R}")
     knn = knn.to(torch.int32).contiguous()
     out = torch.empty((n, R), dtype=torch.int32, device=dev)
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        rc = lib.mmb200_graph_prune(_ptr(knn), _ptr(out), n, K, int(R), _stream(dev))
-    _lib.check(rc, "mmb200_graph_prune")
+    _launch(dev, "mmb200_graph_prune", knn, out, n, K, int(R))
     return out
 
 
@@ -1137,12 +1076,8 @@ def graph_search(queries: torch.Tensor, rows: torch.Tensor, ids: torch.Tensor, g
     out_i = torch.empty((nq, k), dtype=torch.int64, device=dev)
     if nq == 0:
         return out_s, out_i
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        rc = lib.mmb200_graph_search(_ptr(queries), _ptr(rows), _ptr(ids), _ptr(graph), _ptr(entries), _ptr(out_s),
-                                     _ptr(out_i), nq, n, dim, graph.shape[1], entries.shape[1], int(L), int(k),
-                                     _DTYPES[rows.dtype], _stream(dev))
-    _lib.check(rc, "mmb200_graph_search")
+    _launch(dev, "mmb200_graph_search", queries, rows, ids, graph, entries, out_s, out_i, nq, n, dim, graph.shape[1],
+            entries.shape[1], int(L), int(k), _DTYPES[rows.dtype])
     return out_s, out_i
 
 
@@ -1166,32 +1101,12 @@ def maxsim_store(q: torch.Tensor, store: torch.Tensor, doc_offsets: torch.Tensor
                                        f"{tuple(store.shape)}")
     q, store = q.contiguous(), store.contiguous()
     doc_offsets = doc_offsets.to(torch.int64).contiguous()
-    pair_q = pair_q.to(torch.int32).contiguous().view(-1)
-    pair_d = pair_d.to(torch.int32).contiguous().view(-1)
-    if pair_q.numel() != pair_d.numel():
-        raise _lib.MatchmakerB200Error("pair_q / pair_d length mismatch")
+    pair_q, pair_d = _pairs(pair_q, pair_d)
     n_q, Lq, dim = q.shape
     out = torch.empty(pair_q.numel(), dtype=torch.float32, device=dev)
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        rc = lib.mmb200_maxsim_store_fwd(_ptr(q), _ptr(store), _ptr(doc_offsets), _ptr(pair_q), _ptr(pair_d), _ptr(out),
-                                         n_q, store.shape[0], doc_offsets.numel() - 1, pair_q.numel(), Lq, int(max_doc_len),
-                                         dim, _lib.F8E4M3 if fp8 else _DTYPES[q.dtype], _IMPLS[impl], _stream(dev))
-    _lib.check(rc, "mmb200_maxsim_store_fwd")
-    return out
-
-
-def _tkl_slot_map(packed_indices: torch.Tensor) -> torch.Tensor:
-    """Packed index of every chunk slot (-1 = dropped by the packing), one kernel launch (mmb200_tkl_slot_map)."""
-    pk = packed_indices.reshape(-1)
-    if pk.dtype not in (torch.bool, torch.uint8):
-        pk = pk != 0
-    pk = pk.contiguous()
-    out = torch.empty(pk.numel(), dtype=torch.int32, device=pk.device)
-    lib = _lib.load()
-    with torch.cuda.device(pk.device):
-        rc = lib.mmb200_tkl_slot_map(_ptr(pk), _ptr(out), pk.numel(), _stream(pk.device))
-    _lib.check(rc, "mmb200_tkl_slot_map")
+    _launch(dev, "mmb200_maxsim_store_fwd", q, store, doc_offsets, pair_q, pair_d, out, n_q, store.shape[0],
+            doc_offsets.numel() - 1, pair_q.numel(), Lq, int(max_doc_len), dim,
+            _lib.F8E4M3 if fp8 else _DTYPES[q.dtype], _IMPLS[impl])
     return out
 
 
@@ -1208,27 +1123,18 @@ def tkl_bwd(q_ctx, q_mask, doc_chunks, chunk_mask, packed_indices, chunk_pieces,
     doc_chunks = doc_chunks.float().contiguous()
     B, Lq, D = q_ctx.shape
     C = int(chunk_pieces)
-    slot = _tkl_slot_map(packed_indices)
-    q_mask, chunk_mask, mcode = _common_mask_dtype(_prep_mask(q_mask), _prep_mask(chunk_mask))
-    mu, sigma, dense_weight = _f32c(mu).view(-1), _f32c(sigma).view(-1), _f32c(dense_weight).view(-1)
-    sat_params = _f32c(sat_params).view(-1)
-    red = None if sat_red_weight is None else _f32c(sat_red_weight).view(-1)
+    q_mask, chunk_mask, mcode, slot, mu, sigma, dense_weight, red, sat_params, sat_code = _tkl_operands(
+        q_mask, chunk_mask, packed_indices, mu, sigma, dense_weight, sat_red_weight, sat_params, saturation)
     K = mu.numel()
-    sat_code = {"embedding": 0, "log": 1}[saturation]
     n_sat = 13 if sat_code == 0 else K
     stride = K + 15 + n_sat + (D if sat_code == 0 else 0)
     gq = torch.empty_like(q_ctx)
     gc = torch.empty_like(doc_chunks)
     gp = torch.empty(stride, dtype=torch.float32, device=dev)
     ws = torch.empty(max(1, B) * stride, dtype=torch.float32, device=dev)
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        rc = lib.mmb200_tkl_bwd(_ptr(q_ctx), _ptr(q_mask), _ptr(doc_chunks), _ptr(chunk_mask), _ptr(slot), _ptr(mu),
-                                _ptr(sigma), _ptr(dense_weight), _ptr(red), _ptr(sat_params),
-                                _ptr(_f32c(chunk_scoring).view(-1)), _ptr(top_idx.contiguous()),
-                                _ptr(orig_score.contiguous()), _ptr(_f32c(grad_score)), _ptr(gq), _ptr(gc), _ptr(gp),
-                                _ptr(ws), B, doc_chunks.shape[0], Lq, D, C, K, sat_code, mcode, _stream(dev))
-    _lib.check(rc, "mmb200_tkl_bwd")
+    _launch(dev, "mmb200_tkl_bwd", q_ctx, q_mask, doc_chunks, chunk_mask, slot, mu, sigma, dense_weight, red, sat_params,
+            _f32c(chunk_scoring).view(-1), top_idx.contiguous(), orig_score.contiguous(), _f32c(grad_score), gq, gc, gp,
+            ws, B, doc_chunks.shape[0], Lq, D, C, K, sat_code, mcode)
     g_dense, g_cs, g_sat = gp[:K], gp[K:K + 15], gp[K + 15:K + 15 + n_sat]
     g_red = gp[K + 15 + n_sat:] if sat_code == 0 else None
     return gq, gc, g_dense, g_cs, g_sat, g_red
