@@ -221,6 +221,26 @@ MMB200_API int mmb200_kernel_pool_fwd_ex(const float* q, const float* d, const v
                                          float* cosine, int64_t B, int32_t Lq, int32_t Ld, int32_t D, int32_t K,
                                          float log_scale, float clamp_min, float score_bias, int32_t mask_dtype,
                                          int32_t impl, void* stream);
+/* Store mode of mmb200_kernel_pool_fwd_ex (inference only): documents are read from a store of live rows that was
+ * encoded once (TK / TK-Sparse document contextualisation does not depend on the query):
+ *
+ *   score[p] = mmb200_kernel_pool_fwd_ex of query pair_q[p] against the rows doc_offsets[d] .. doc_offsets[d+1] - 1
+ *              of `store` (at most max_doc_len of them), d = pair_d[p], every row unmasked
+ *
+ * store [n_rows, D] f32; doc_offsets [n_docs + 1] int64, non-decreasing, doc_offsets[n_docs] <= n_rows; q [n_q, Lq, D]
+ * f32, q_mask [n_q, Lq] (mask_dtype) or NULL; pair_q / pair_d [n_pairs] int32, pairs of one query adjacent for L2 reuse
+ * of its rows (any order is correct).  gate [n_rows] f32 in store order or NULL: the doc_gate of the row (TK-Sparse).
+ * pair_d[p] < 0 and a passage without rows score -inf and fetch nothing.  impl as mmb200_kernel_pool_fwd_ex: AUTO
+ * picks the kernel it would pick for the padded [n_docs, max_doc_len, D] layout, and scores are bit-identical to that
+ * layout with the passages' rows unmasked and the rest masked.  The tensor-core kernel addresses the store with the
+ * passage's first row as the TMA row coordinate: n_rows < 2^31 - 1024. */
+MMB200_API int mmb200_kernel_pool_store_fwd(const float* q, const void* q_mask, const float* store,
+                                            const int64_t* doc_offsets, const float* gate, const int32_t* pair_q,
+                                            const int32_t* pair_d, const float* mu, const float* sigma,
+                                            const float* alpha, const float* weight, float* score, int64_t n_q,
+                                            int64_t n_rows, int64_t n_pairs, int32_t Lq, int32_t max_doc_len,
+                                            int32_t D, int32_t K, float log_scale, float clamp_min, float score_bias,
+                                            int32_t mask_dtype, int32_t impl, void* stream);
 MMB200_API int mmb200_kernel_pool_bwd_ex(const float* q, const float* d, const void* q_mask, const void* d_mask,
                                          const float* doc_gate, const float* mu, const float* sigma, const float* alpha,
                                          const float* weight, const float* per_kernel_query, const float* grad_score,

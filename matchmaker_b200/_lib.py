@@ -68,6 +68,8 @@ SIGNATURES = {
     "mmb200_dot_pairs": (_c.c_int, [_vp, _vp, _vp, _i64, _i32, _i32, _vp]),
     "mmb200_kernel_pool_bwd": (_c.c_int, [_vp] * 15 + [_i64, _i32, _i32, _i32, _i32, _f32, _i32, _vp]),
     "mmb200_kernel_pool_fwd_ex": (_c.c_int, [_vp] * 13 + [_i64, _i32, _i32, _i32, _i32, _f32, _f32, _f32, _i32, _i32, _vp]),
+    "mmb200_kernel_pool_store_fwd": (_c.c_int, [_vp] * 12 + [_i64, _i64, _i64, _i32, _i32, _i32, _i32, _f32, _f32, _f32,
+                                                            _i32, _i32, _vp]),
     "mmb200_kernel_pool_bwd_ex": (_c.c_int, [_vp] * 17 + [_i64, _i32, _i32, _i32, _i32, _f32, _f32, _i32, _vp]),
     "mmb200_kernel_pool_train_tc_supported": (_i32, [_i32, _i32, _i32, _i32]),
     "mmb200_kernel_pool_saved_floats": (_i64, [_i64, _i32]),

@@ -106,8 +106,10 @@ __device__ __forceinline__ void kp_cos_tile(const float* __restrict__ qs, const 
 // ---------------------------------------------------------------------------------------------
 // forward
 // ---------------------------------------------------------------------------------------------
-template <int KB, int JR>
-__global__ void __launch_bounds__(kKpThreads) kernel_pool_fwd_simt(KpParams P) {
+// The body of both forward entry points below; STORE: store mode (KpParams::doc_offsets), pair b reads query pair_q[b]
+// and its passage's rows from the store
+template <int KB, int JR, bool STORE>
+__device__ __forceinline__ void kp_fwd_simt_body(const KpParams& P) {
   constexpr int TJ = 32 * JR;
   extern __shared__ __align__(16) float sm[];
   const int D = P.D, dp = padded_row_stride(D), Lq = P.Lq, Ld = P.Ld, K = P.K;
@@ -133,23 +135,29 @@ __global__ void __launch_bounds__(kKpThreads) kernel_pool_fwd_simt(KpParams P) {
     w_s[t] = ok ? P.weight[t] : 0.f;
   }
   for (int64_t b = blockIdx.x; b < P.B; b += gridDim.x) {
-    const float* qb = P.q + b * (int64_t)Lq * D;
-    const float* db = P.d + b * (int64_t)Ld * D;
+    int64_t qz = b, drow0 = b * (int64_t)Ld;   // query of the pair, first document row (and gate entry)
+    int len = Ld;                              // document rows of the pair
+    if constexpr (STORE) {
+      qz = P.pair_q[b];
+      len = kp_store_rows(P, b, &drow0);
+    }
+    const float* qb = P.q + qz * (int64_t)Lq * D;
+    const float* db = P.d + drow0 * D;
     __syncthreads();
     if (t < 32) pk_s[t] = 0.f;
     for (int i0 = 0; i0 < Lq; i0 += kKpQ) {
       __syncthreads();
       kp_load_rows(qb, i0, Lq, D, dp, kKpQ, qs, nullptr, nullptr);
-      if (t < 32) qm_s[t] = (i0 + t < Lq && mask_at(P.q_mask, P.q_mask ? P.mask_dtype : 0, b * (int64_t)Lq + i0 + t)) ? 1.f : 0.f;
+      if (t < 32) qm_s[t] = (i0 + t < Lq && mask_at(P.q_mask, P.q_mask ? P.mask_dtype : 0, qz * Lq + i0 + t)) ? 1.f : 0.f;
       float acc[KB];
 #pragma unroll
       for (int k = 0; k < KB; ++k) acc[k] = 0.f;
-      for (int j0 = 0; j0 < Ld; j0 += TJ) {
+      for (int j0 = 0; j0 < len; j0 += TJ) {
         __syncthreads();  // previous tile fully consumed
-        kp_load_rows(db, j0, Ld, D, dp, TJ, ds, nullptr, nullptr);
+        kp_load_rows(db, j0, len, D, dp, TJ, ds, nullptr, nullptr);
         if (t < TJ) {   // dm_s = mask x gate: the weight of document term j in every activation sum
-          const bool live = j0 + t < Ld && mask_at(P.d_mask, P.d_mask ? P.mask_dtype : 0, b * (int64_t)Ld + j0 + t);
-          dm_s[t] = live ? (P.gate ? fmaxf(P.gate[b * (int64_t)Ld + j0 + t], 0.f) : 1.f) : 0.f;
+          const bool live = j0 + t < len && mask_at(P.d_mask, P.d_mask ? P.mask_dtype : 0, drow0 + j0 + t);
+          dm_s[t] = live ? (P.gate ? fmaxf(P.gate[drow0 + j0 + t], 0.f) : 1.f) : 0.f;
         }
         __syncthreads();
         kp_cos_tile<JR>(qs, ds, D, dp, cs, TJ + 1);
@@ -209,9 +217,20 @@ __global__ void __launch_bounds__(kKpThreads) kernel_pool_fwd_simt(KpParams P) {
     if (t == 0) {
       float s = 0.f;
       for (int k = 0; k < K; ++k) s = fmaf(pk_s[k], w_s[k], s);
-      P.score[b] = s + P.bias;
+      P.score[b] = STORE && len == 0 ? -INFINITY : s + P.bias;   // store mode: a pair without rows scores -inf
     }
   }
+}
+
+template <int KB, int JR>
+__global__ void __launch_bounds__(kKpThreads) kernel_pool_fwd_simt(KpParams P) {
+  kp_fwd_simt_body<KB, JR, false>(P);
+}
+
+// store mode (mmb200_kernel_pool_store_fwd); one CTA per SM: at the padded kernel's register choice (128) KB = 24 spills
+template <int KB, int JR>
+__global__ void __launch_bounds__(kKpThreads, 1) kernel_pool_fwd_simt_store(KpParams P) {
+  kp_fwd_simt_body<KB, JR, true>(P);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -458,7 +477,7 @@ static int kp_validate(const KpParams& P) {
   return MMB200_OK;
 }
 
-template <int KB, int JR>
+template <int KB, int JR, bool STORE = false>
 static int launch_fwd(const KpParams& P, const DeviceInfo& dev, cudaStream_t stream) {
   const int dp = padded_row_stride(P.D), TJ = 32 * JR;
   const size_t need = ((size_t)(kKpQ + TJ) * dp + kKpQ * (TJ + 1) + 32 * 6 + TJ + (size_t)9 * KB * 32) * sizeof(float);
@@ -466,9 +485,14 @@ static int launch_fwd(const KpParams& P, const DeviceInfo& dev, cudaStream_t str
     set_error("kernel_pool forward: embedding dim too large for the shared-memory tiles");
     return MMB200_ERR_UNSUPPORTED;
   }
-  MMB_CHECK_CUDA(cudaFuncSetAttribute(kernel_pool_fwd_simt<KB, JR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)need));
   const int grid = (int)std::min<int64_t>(P.B, (int64_t)dev.sm_count * 4);
-  kernel_pool_fwd_simt<KB, JR><<<grid, kKpThreads, need, stream>>>(P);
+  if constexpr (STORE) {
+    MMB_CHECK_CUDA(cudaFuncSetAttribute(kernel_pool_fwd_simt_store<KB, JR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)need));
+    kernel_pool_fwd_simt_store<KB, JR><<<grid, kKpThreads, need, stream>>>(P);
+  } else {
+    MMB_CHECK_CUDA(cudaFuncSetAttribute(kernel_pool_fwd_simt<KB, JR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)need));
+    kernel_pool_fwd_simt<KB, JR><<<grid, kKpThreads, need, stream>>>(P);
+  }
   MMB_CHECK_CUDA(cudaGetLastError());
   return MMB200_OK;
 }
@@ -529,6 +553,32 @@ static int kp_fwd_impl(const float* q, const float* d, const void* q_mask, const
   if (K <= 12) return wide ? launch_fwd<12, 2>(P, dev, stream) : launch_fwd<12, 1>(P, dev, stream);
   if (K <= 24) return wide ? launch_fwd<24, 2>(P, dev, stream) : launch_fwd<24, 1>(P, dev, stream);
   return wide ? launch_fwd<32, 2>(P, dev, stream) : launch_fwd<32, 1>(P, dev, stream);
+}
+
+// store mode: the routing of kp_fwd_impl (tensor-core kernel when it takes the shape, else the FFMA kernel with the tile
+// width the padded [n_docs, max_doc_len, D] layout would get), so scores are bit-identical to that layout
+static int kp_store_fwd_impl(KpParams& P, int32_t impl, cudaStream_t stream) {
+  MMB_REQUIRE(P.clamp_min > 0.f, "clamp_min must be positive");
+  if (int rc = kp_validate(P)) return rc;
+  MMB_REQUIRE(P.B == 0 || (P.doc_offsets && P.pair_q && P.pair_d && P.score), "null pointer");
+  MMB_REQUIRE(P.n_q >= 1 && P.n_rows >= 1, "the store needs at least one row and one query");
+  MMB_REQUIRE(P.n_rows < (1ll << 31) - 1024, "at most 2^31 - 1024 store rows per device (TMA row coordinates are int32)");
+  if (P.B == 0) return MMB200_OK;
+  DeviceInfo dev;
+  if (int rc = require_sm90(&dev)) return rc;
+  if (impl != MMB200_IMPL_SIMT) {
+    bool handled = false;
+    int rc = kernel_pool_fwd_ts(P, dev, stream, &handled);
+    if (handled) return rc;
+    if (impl == MMB200_IMPL_TCGEN05) {
+      if (rc == MMB200_OK) { set_error("kernel_pool_store: shape not supported by the tensor-core kernel"); rc = MMB200_ERR_UNSUPPORTED; }
+      return rc;
+    }
+  }
+  const bool wide = P.Ld > 48;
+  if (P.K <= 12) return wide ? launch_fwd<12, 2, true>(P, dev, stream) : launch_fwd<12, 1, true>(P, dev, stream);
+  if (P.K <= 24) return wide ? launch_fwd<24, 2, true>(P, dev, stream) : launch_fwd<24, 1, true>(P, dev, stream);
+  return wide ? launch_fwd<32, 2, true>(P, dev, stream) : launch_fwd<32, 1, true>(P, dev, stream);
 }
 
 static int kp_bwd_impl(const float* q, const float* d, const void* q_mask, const void* d_mask, const float* doc_gate,
@@ -617,6 +667,21 @@ extern "C" int mmb200_kernel_pool_fwd_ex(const float* q, const float* d, const v
                                          int32_t impl, void* stream_) {
   return mmb::kp_fwd_impl(q, d, q_mask, d_mask, doc_gate, mu, sigma, alpha, weight, score, per_kernel, per_kernel_query,
                           cosine, nullptr, B, Lq, Ld, D, K, log_scale, clamp_min, score_bias, mask_dtype, impl, stream_);
+}
+
+extern "C" int mmb200_kernel_pool_store_fwd(const float* q, const void* q_mask, const float* store,
+                                            const int64_t* doc_offsets, const float* gate, const int32_t* pair_q,
+                                            const int32_t* pair_d, const float* mu, const float* sigma,
+                                            const float* alpha, const float* weight, float* score, int64_t n_q,
+                                            int64_t n_rows, int64_t n_pairs, int32_t Lq, int32_t max_doc_len,
+                                            int32_t D, int32_t K, float log_scale, float clamp_min, float score_bias,
+                                            int32_t mask_dtype, int32_t impl, void* stream) {
+  mmb::KpParams P{};
+  P.q = q; P.d = store; P.q_mask = q_mask; P.gate = gate; P.mu = mu; P.sigma = sigma; P.alpha = alpha; P.weight = weight;
+  P.B = n_pairs; P.Lq = Lq; P.Ld = max_doc_len; P.D = D; P.K = K; P.mask_dtype = mask_dtype; P.log_scale = log_scale;
+  P.clamp_min = clamp_min; P.bias = score_bias; P.score = score;
+  P.doc_offsets = doc_offsets; P.pair_q = pair_q; P.pair_d = pair_d; P.n_q = n_q; P.n_rows = n_rows;
+  return mmb::kp_store_fwd_impl(P, impl, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int32_t mmb200_kernel_pool_train_tc_supported(int32_t Lq, int32_t Ld, int32_t D, int32_t K) {

@@ -45,7 +45,23 @@ struct KpParams {
   // rows of the block; the rows sit at q_row0 .. of Lq_total in q, q_mask and per_kernel_query.  0 / Lq otherwise.
   int32_t q_row0, Lq_total;
   float tf32_comp;   // backward: factor undoing the mean truncation of the raw fp32 operands to tf32 (1 + 2^-11), or 1
+  // store mode (mmb200_kernel_pool_store_fwd, forward only): d is the store [n_rows, D] of live rows, B the number of
+  // pairs; pair p scores query pair_q[p] of q [n_q, Lq_total, D] against passage pair_d[p], its rows
+  // doc_offsets[pair_d[p]] .. (at most Ld of them).  The gate, if any, is [n_rows] in store order.  Null otherwise.
+  const int64_t* doc_offsets;
+  const int32_t* pair_q;
+  const int32_t* pair_d;
+  int64_t n_q, n_rows;
 };
+
+// store mode: the passage of pair p -- its first store row and its row count (0 for pair_d < 0 or an empty passage)
+__device__ __forceinline__ int kp_store_rows(const KpParams& P, int64_t p, int64_t* row0) {
+  const int64_t di = P.pair_d[p];
+  if (di < 0) { *row0 = 0; return 0; }
+  const int64_t a = P.doc_offsets[di], b = P.doc_offsets[di + 1];
+  *row0 = a;
+  return (int)max((int64_t)0, min(b - a, (int64_t)P.Ld));
+}
 
 __host__ __device__ inline int64_t kp_saved_floats(int64_t B, int Ld) { return B * ((int64_t)33 * Ld + 32); }
 __host__ __device__ inline int64_t kp_saved_cos_off(int64_t p, int Ld) { return p * (int64_t)Ld * 32; }

@@ -67,10 +67,13 @@ struct KpShared {
   int live[2][8];                // per cosine tile: last unmasked document row + 1 of each MMA warp's 16 rows
 };
 
-template <int KB, bool SAVE>
-__global__ void __launch_bounds__(kThreads, 1)
-kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_d,
-                      const __grid_constant__ CUtensorMap tmap_d_last, KpParams P, int n_raw, int last_box_rows) {
+// The body of both entry points below: the padded layout, or (STORE) the store mode, where pair p reads query
+// pair_q[p] and its passage's rows from the store (KpParams::doc_offsets) with the passage's first row as the tile's
+// TMA row coordinate
+template <int KB, bool SAVE, bool STORE>
+__device__ __forceinline__ void kernel_pool_ts_body(const CUtensorMap& tmap_q, const CUtensorMap& tmap_d,
+                                                    const CUtensorMap& tmap_d_last, const KpParams& P, int n_raw,
+                                                    int last_box_rows) {
   extern __shared__ uint8_t smem_raw[];
   // 1024-B alignment for SWIZZLE_128B tiles, derived by pointer arithmetic on the __shared__ array so the
   // compiler keeps the shared address space (LDS/STS instead of generic LD/ST)
@@ -82,7 +85,13 @@ kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
   KpShared* S = reinterpret_cast<KpShared*>(spart + 8 * 32 * 32);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int tiles = (P.Ld + 127) / 128;
+  const int tiles_padded = (P.Ld + 127) / 128;
+  // store mode: the passage of pair p is rows row0 .. row0 + len of the store; its tiles start at row0
+  auto pair_rows = [&](int64_t p, int64_t* row0) -> int {
+    if constexpr (STORE) return kp_store_rows(P, p, row0);
+    *row0 = 0;
+    return P.Ld;
+  };
   const int nch = (P.D + 31) / 32;
   int64_t p_begin, p_end;
   cta_share(P.B, &p_begin, &p_end);
@@ -115,21 +124,36 @@ kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     int stage = 0;
     uint32_t phase = 0;
     const uint32_t last_bytes = (uint32_t)(last_box_rows * 128 + kQxBytes);
-    for (int64_t p = p_begin; p < p_end; ++p)
+    for (int64_t p = p_begin; p < p_end; ++p) {
+      int64_t row0;
+      const int len = pair_rows(p, &row0);
+      const int tiles = STORE ? (len + 127) / 128 : tiles_padded;
+      const int qz = STORE ? P.pair_q[p] : (int)p;
       for (int t = 0; t < tiles; ++t) {
         const bool last = t == tiles - 1;
+        // store mode: the tile's rows rounded up to 8, fetched as 32-row boxes (tmap_d) then 8-row boxes (tmap_d_last)
+        const int rows8 = STORE ? (min(128, len - t * 128) + 7) & ~7 : 0;
         for (int ck = 0; ck < nch; ++ck) {
           mbar_wait(&S->raw_empty[stage], phase ^ 1u);
           uint8_t* st = raws + (size_t)stage * kRawBytes;
           if (elect_one_sync()) {
-            mbar_arrive_expect_tx(&S->raw_full[stage], last ? last_bytes : (uint32_t)kRawBytes);
-            tma_load_3d(last ? &tmap_d_last : &tmap_d, st, &S->raw_full[stage], ck * 32, t * 128, (int)p, kEvictFirst);
-            tma_load_3d(&tmap_q, st + kDxBytes, &S->raw_full[stage], ck * 32, P.q_row0, (int)p, kEvictLast);
+            if constexpr (STORE) {
+              mbar_arrive_expect_tx(&S->raw_full[stage], (uint32_t)(rows8 * 128 + kQxBytes));
+              const int y = (int)row0 + t * 128;
+              int r = 0;
+              for (; r + 32 <= rows8; r += 32) tma_load_3d(&tmap_d, st + r * 128, &S->raw_full[stage], ck * 32, y + r, 0, kEvictFirst);
+              for (; r < rows8; r += 8) tma_load_3d(&tmap_d_last, st + r * 128, &S->raw_full[stage], ck * 32, y + r, 0, kEvictFirst);
+            } else {
+              mbar_arrive_expect_tx(&S->raw_full[stage], last ? last_bytes : (uint32_t)kRawBytes);
+              tma_load_3d(last ? &tmap_d_last : &tmap_d, st, &S->raw_full[stage], ck * 32, t * 128, (int)p, kEvictFirst);
+            }
+            tma_load_3d(&tmap_q, st + kDxBytes, &S->raw_full[stage], ck * 32, P.q_row0, qz, kEvictLast);
           }
           __syncwarp();
           if (++stage == n_raw) { stage = 0; phase ^= 1u; }
         }
       }
+    }
   } else if (warp == 1) {
     setmaxnreg_dec<kRegsLight>();
   } else if (warp < 4) {
@@ -140,7 +164,9 @@ kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     const int sw = row & 7;
     int rs_ = 0, os_ = 0, nr = 0;
     uint32_t rphase = 0, ophase = 0;
-    for (int64_t p = p_begin; p < p_end; ++p)
+    for (int64_t p = p_begin; p < p_end; ++p) {
+      int64_t row0;
+      const int tiles = STORE ? (pair_rows(p, &row0) + 127) / 128 : tiles_padded;
       for (int t = 0; t < tiles; ++t) {
         float4 ss4 = make_float4(0.f, 0.f, 0.f, 0.f);
         for (int ck = 0; ck < nch; ++ck) {
@@ -185,6 +211,7 @@ kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
         }
         if (++nr == kNormRing) nr = 0;
       }
+    }
   } else if (warp < kFirstEpiWarp) {
     // ------------------------------- document operand + wgmma + cosine tile (phase A) ------------------------------
     setmaxnreg_dec<kRegsMma>();
@@ -197,11 +224,16 @@ kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     int rs_ = 0, os_ = 0, nr = 0;
     uint32_t rphase = 0, ophase = 0;
     int64_t tile_seq = 0;
-    for (int64_t p = p_begin; p < p_end; ++p)
+    for (int64_t p = p_begin; p < p_end; ++p) {
+      int64_t row0;
+      const int len = pair_rows(p, &row0);
+      const int tiles = STORE ? (len + 127) / 128 : tiles_padded;
+      // first gate entry of the pair: the passage's first store row, or row p of the padded [B, Ld] gate
+      const int64_t gate0 = STORE ? row0 : p * (int64_t)P.Ld;
       for (int t = 0; t < tiles; ++t, ++tile_seq) {
         const int g0 = t * 128 + r0, g1 = t * 128 + r1;
-        const uint64_t draw0 = g0 < P.Ld ? (dmt != MMB200_MASK_NONE ? mask_raw(P.d_mask, dmt, p * (int64_t)P.Ld + g0) : 1) : 0;
-        const uint64_t draw1 = g1 < P.Ld ? (dmt != MMB200_MASK_NONE ? mask_raw(P.d_mask, dmt, p * (int64_t)P.Ld + g1) : 1) : 0;
+        const uint64_t draw0 = g0 < len ? (dmt != MMB200_MASK_NONE ? mask_raw(P.d_mask, dmt, p * (int64_t)P.Ld + g0) : 1) : 0;
+        const uint64_t draw1 = g1 < len ? (dmt != MMB200_MASK_NONE ? mask_raw(P.d_mask, dmt, p * (int64_t)P.Ld + g1) : 1) : 0;
         float acc[32];   // columns 0..31: D . Qhi, 32..63: D . Qlo (rows r0 / r1)
 #pragma unroll
         for (int j = 0; j < 32; ++j) acc[j] = 0.f;
@@ -245,7 +277,7 @@ kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
         ss0 += __shfl_xor_sync(0xffffffffu, ss0, 1); ss0 += __shfl_xor_sync(0xffffffffu, ss0, 2);
         ss1 += __shfl_xor_sync(0xffffffffu, ss1, 1); ss1 += __shfl_xor_sync(0xffffffffu, ss1, 2);
         const float rsd0 = 1.0f / (sqrtf(ss0) + kTinyNorm), rsd1 = 1.0f / (sqrtf(ss1) + kTinyNorm);
-        const bool valid0 = g0 < P.Ld && mask_test(draw0, dmt), valid1 = g1 < P.Ld && mask_test(draw1, dmt);
+        const bool valid0 = g0 < len && mask_test(draw0, dmt), valid1 = g1 < len && mask_test(draw1, dmt);
         const int buf = (int)(tile_seq & 1);
         float* cbuf = cs + buf * (128 * 32);
         mbar_wait(&S->cs_empty[buf], (uint32_t)((tile_seq >> 1) & 1) ^ 1u);
@@ -278,13 +310,14 @@ kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
         if (lane == 0) S->live[buf][ew] = live;
         if (tq == 0) {
           // gate g_j * exp(-x^2) = 2^(-u^2 + log2 g_j): one exponent term per document row, no extra multiply
-          S->lg[buf][r0] = (P.gate && g0 < P.Ld) ? __log2f(fmaxf(P.gate[p * (int64_t)P.Ld + g0], 0.f)) : 0.f;
-          S->lg[buf][r1] = (P.gate && g1 < P.Ld) ? __log2f(fmaxf(P.gate[p * (int64_t)P.Ld + g1], 0.f)) : 0.f;
+          S->lg[buf][r0] = (P.gate && g0 < len) ? __log2f(fmaxf(P.gate[gate0 + g0], 0.f)) : 0.f;
+          S->lg[buf][r1] = (P.gate && g1 < len) ? __log2f(fmaxf(P.gate[gate0 + g1], 0.f)) : 0.f;
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(&S->cs_full[buf]);
         if (++nr == kNormRing) nr = 0;
       }
+    }
   } else {
     // ------------------------------- epilogue (phase B) ------------------------------------
     setmaxnreg_inc<kRegsEpilogue>();
@@ -303,8 +336,12 @@ kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
       float acc[KB];
 #pragma unroll
       for (int k = 0; k < KB; ++k) acc[k] = 0.f;
+      int64_t row0;
+      const int len = pair_rows(p, &row0);
+      const int tiles = STORE ? (len + 127) / 128 : tiles_padded;
+      const int64_t qz = STORE ? P.pair_q[p] : p;
       uint64_t qraw = 0;
-      if (lane < P.Lq) qraw = qmt != MMB200_MASK_NONE ? mask_raw(P.q_mask, qmt, p * (int64_t)P.Lq_total + P.q_row0 + lane) : 1;
+      if (lane < P.Lq) qraw = qmt != MMB200_MASK_NONE ? mask_raw(P.q_mask, qmt, qz * P.Lq_total + P.q_row0 + lane) : 1;
       // Short queries: phase B has lane = query row, so a 6-token query would leave 26 lanes of every MUFU instruction
       // idle.  With q_hi = 1 + last unmasked query row, the warp's lanes are dealt as 32 / qp sub-streams of qp query rows
       // (qp = 4, 8, 16 or 32 >= q_hi); sub-stream s takes the document rows r + 16 s, and the sub-streams are added at
@@ -387,10 +424,26 @@ kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
         float sc = v * S->w[lane];
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) sc += __shfl_xor_sync(0xffffffffu, sc, o);
-        if (lane == 0) P.score[p] = sc + P.bias;
+        // store mode: a pair without rows (pair_d < 0 or an empty passage) scores -inf
+        if (lane == 0) P.score[p] = STORE && len == 0 ? -INFINITY : sc + P.bias;
       }
     }
   }
+}
+
+template <int KB, bool SAVE>
+__global__ void __launch_bounds__(kThreads, 1)
+kernel_pool_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_d,
+                      const __grid_constant__ CUtensorMap tmap_d_last, KpParams P, int n_raw, int last_box_rows) {
+  kernel_pool_ts_body<KB, SAVE, false>(tmap_q, tmap_d, tmap_d_last, P, n_raw, last_box_rows);
+}
+
+// store mode (mmb200_kernel_pool_store_fwd): tmap_d / tmap_d_last are 32- / 8-row boxes over the whole store
+template <int KB>
+__global__ void __launch_bounds__(kThreads, 1)
+kernel_pool_ts_store_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_d,
+                            const __grid_constant__ CUtensorMap tmap_d_last, KpParams P, int n_raw) {
+  kernel_pool_ts_body<KB, false, true>(tmap_q, tmap_d, tmap_d_last, P, n_raw, 0);
 }
 
 template <int KB>
@@ -408,6 +461,9 @@ int launch(const KpParams& P, const DeviceInfo& dev, cudaStream_t stream, const 
   if (P.saved) {
     MMB_CHECK_CUDA(cudaFuncSetAttribute(kernel_pool_ts_kernel<KB, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kernel_pool_ts_kernel<KB, true><<<grid, kThreads, smem, stream>>>(tq, td, td_last, P, n_raw, last_box_rows);
+  } else if (P.doc_offsets) {
+    MMB_CHECK_CUDA(cudaFuncSetAttribute(kernel_pool_ts_store_kernel<KB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel_pool_ts_store_kernel<KB><<<grid, kThreads, smem, stream>>>(tq, td, td_last, P, n_raw);
   } else {
     MMB_CHECK_CUDA(cudaFuncSetAttribute(kernel_pool_ts_kernel<KB, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kernel_pool_ts_kernel<KB, false><<<grid, kThreads, smem, stream>>>(tq, td, td_last, P, n_raw, last_box_rows);
@@ -435,7 +491,7 @@ __global__ void kp_combine_query_blocks(const float* __restrict__ score_blk, con
 static int kernel_pool_fwd_ts_block(const KpParams& P, const DeviceInfo& dev, cudaStream_t stream) {
   CUtensorMap tq, td, td_last;
   {
-    const uint64_t dims[3] = {(uint64_t)P.D, (uint64_t)P.Lq_total, (uint64_t)P.B};
+    const uint64_t dims[3] = {(uint64_t)P.D, (uint64_t)P.Lq_total, (uint64_t)(P.doc_offsets ? P.n_q : P.B)};
     const uint64_t strides[2] = {(uint64_t)P.D * 4, (uint64_t)P.Lq_total * P.D * 4};
     const uint32_t box[3] = {32, 32, 1};
     if (int rc = encode_tensor_map(&tq, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, P.q, dims, strides, box,
@@ -444,7 +500,19 @@ static int kernel_pool_fwd_ts_block(const KpParams& P, const DeviceInfo& dev, cu
   }
   const int last_rows = P.Ld - ((P.Ld + 127) / 128 - 1) * 128;       // rows of the last document tile, 1..128
   const int last_box_rows = std::min(128, (last_rows + 7) & ~7);
-  {
+  if (P.doc_offsets) {
+    // store mode: one map over the whole store, row coordinate = the passage's first row + the tile's; each tile is
+    // fetched as 32-row boxes (td) and then 8-row boxes (td_last), so at most 7 rows past a passage are read
+    const uint64_t dims[3] = {(uint64_t)P.D, (uint64_t)P.n_rows, 1};
+    const uint64_t strides[2] = {(uint64_t)P.D * 4, (uint64_t)P.n_rows * P.D * 4};
+    const uint32_t box[3] = {32, 32, 1}, box8[3] = {32, 8, 1};
+    if (int rc = encode_tensor_map(&td, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, P.d, dims, strides, box,
+                                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))
+      return rc;
+    if (int rc = encode_tensor_map(&td_last, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, P.d, dims, strides, box8,
+                                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B))
+      return rc;
+  } else {
     const uint64_t dims[3] = {(uint64_t)P.D, (uint64_t)P.Ld, (uint64_t)P.B};
     const uint64_t strides[2] = {(uint64_t)P.D * 4, (uint64_t)P.Ld * P.D * 4};
     const uint32_t box[3] = {32, 128, 1};

@@ -299,6 +299,59 @@ def kernel_pool(q: torch.Tensor, d: torch.Tensor, q_mask: torch.Tensor, d_mask: 
     return {"score": score, "per_kernel": pk, "per_kernel_query": pkq, "cosine": cos}
 
 
+KERNEL_POOL_MAX_K = 32
+KERNEL_POOL_STORE_MAX_ROWS = (1 << 31) - 1024   # the tensor-core kernel's TMA row coordinates are int32
+
+
+def kernel_pool_store(q: torch.Tensor, q_mask: Optional[torch.Tensor], store: torch.Tensor, doc_offsets: torch.Tensor,
+                      pair_q: torch.Tensor, pair_d: torch.Tensor, mu: torch.Tensor, sigma: torch.Tensor,
+                      weight: torch.Tensor, alpha: Optional[torch.Tensor] = None, log_scale: float = 1.0,
+                      max_doc_len: Optional[int] = None, impl: str = "auto", gate: Optional[torch.Tensor] = None,
+                      clamp_min: float = 1e-10, bias: float = 0.0) -> torch.Tensor:
+    """:func:`kernel_pool` against a store of document rows that was encoded once, fp32 scores [n_pairs] (inference).
+
+    store [n_rows, D] fp32 holds only live rows; passage d is rows ``doc_offsets[d] : doc_offsets[d+1]`` (int64
+    [n_docs+1], non-decreasing, at most ``max_doc_len`` rows read; None = the longest passage, which costs a host
+    synchronisation).  Pair p scores query ``pair_q[p]`` of q [n_q, Lq, D] (q_mask [n_q, Lq] or None) against passage
+    ``pair_d[p]``; keep the pairs of one query adjacent.  ``pair_d[p] < 0`` and passages without rows score -inf.
+    ``gate`` [n_rows] in store order is TK-Sparse's per-row gate (``doc_gate`` of :func:`kernel_pool`).
+
+    Same kernels and bit-identical scores as :func:`kernel_pool` on the passages gathered into [n_pairs, max_doc_len, D]
+    with their rows unmasked and the padding masked (same ``impl``)."""
+    if q.dim() != 3 or store.dim() != 2 or q.shape[-1] != store.shape[-1]:
+        raise _lib.MatchmakerB200Error(f"kernel_pool_store: expected q [n_q, Lq, D], store [n_rows, D]; got "
+                                       f"{tuple(q.shape)}, {tuple(store.shape)}")
+    n_q, Lq, D = q.shape
+    n_rows = store.shape[0]
+    if D % 4 != 0:
+        raise _lib.MatchmakerB200Error(f"kernel_pool_store: D must be a multiple of 4, got {D}")
+    if not 1 <= mu.numel() <= KERNEL_POOL_MAX_K or sigma.numel() != mu.numel() or weight.numel() != mu.numel():
+        raise _lib.MatchmakerB200Error(f"kernel_pool_store: 1 <= K <= {KERNEL_POOL_MAX_K} kernels with one sigma and "
+                                       f"weight each; got mu {mu.numel()}, sigma {sigma.numel()}, weight {weight.numel()}")
+    if n_q < 1 or Lq < 1 or not 1 <= n_rows < KERNEL_POOL_STORE_MAX_ROWS:
+        raise _lib.MatchmakerB200Error(f"kernel_pool_store: need n_q, Lq >= 1 and 1 <= n_rows < "
+                                       f"{KERNEL_POOL_STORE_MAX_ROWS}; got q {tuple(q.shape)}, {n_rows} rows")
+    if doc_offsets.dim() != 1 or doc_offsets.numel() < 2:
+        raise _lib.MatchmakerB200Error("kernel_pool_store: doc_offsets must be [n_docs + 1] with n_docs >= 1")
+    if q_mask is not None and tuple(q_mask.shape) != (n_q, Lq):
+        raise _lib.MatchmakerB200Error("kernel_pool_store: q_mask shape mismatch")
+    if gate is not None and gate.numel() != n_rows:
+        raise _lib.MatchmakerB200Error("kernel_pool_store: gate must hold one value per store row")
+    dev = _require_cuda(q, q_mask, store, doc_offsets, pair_q, pair_d, mu, sigma, weight, alpha, gate)
+    q, store = _f32c(q), _f32c(store)
+    doc_offsets = doc_offsets.to(torch.int64).contiguous()
+    pair_q, pair_d = _pairs(pair_q, pair_d)
+    if max_doc_len is None:
+        max_doc_len = max(1, int((doc_offsets[1:] - doc_offsets[:-1]).max()))
+    (q_mask, _, gate, mu, sigma, alpha, weight), mcode, K = _kernel_pool_operands(
+        q_mask, None, mu, sigma, weight, alpha, gate, 1, n_rows)
+    score = torch.empty(pair_q.numel(), dtype=torch.float32, device=dev)
+    _launch(dev, "mmb200_kernel_pool_store_fwd", q, q_mask, store, doc_offsets, gate, pair_q, pair_d, mu, sigma, alpha,
+            weight, score, n_q, n_rows, pair_q.numel(), Lq, int(max_doc_len), D, K, float(log_scale),
+            float(clamp_min), float(bias), mcode, _IMPLS[impl])
+    return score
+
+
 def kernel_pool_train_supported(Lq: int, Ld: int, D: int, K: int) -> bool:
     """True when the tensor-core training pair (forward that saves its cosines + tensor-core backward) covers the shape."""
     return bool(_lib.load().mmb200_kernel_pool_train_tc_supported(int(Lq), int(Ld), int(D), int(K)))

@@ -3,7 +3,7 @@ Mirrors matchmaker/models/published/ecai20_tk.py."""
 from __future__ import annotations
 
 import math
-from typing import List
+from typing import List, Optional
 
 import torch
 import torch.nn as nn
@@ -88,6 +88,26 @@ class ECAI20_TK(nn.Module):
         -> linear, one kernel launch forward, one backward."""
         return autograd.kernel_pool(query_ctx, document_ctx, query_mask, document_mask, self.mu, self.sigma,
                                     self.kernel_bin_weights.weight, self.kernel_alpha_scaler, 1.0)
+
+    @torch.no_grad()
+    def encode_documents(self, document_embeddings: torch.Tensor, document_mask: torch.Tensor):
+        """The document side of ``forward`` (ecai20_tk.py:93-103), which does not depend on the query, for a store that
+        is encoded once: (rows [n_live, D] fp32, the contextualised embeddings of the unmasked terms in passage order,
+        lengths [B] int64).  ``score_store`` over them gives ``forward``'s scores."""
+        ctx = self.forward_representation(document_embeddings, document_mask,
+                                          self.positional_features_d[:, :document_embeddings.shape[1], :])
+        live = document_mask.bool()
+        return ctx[live].float().contiguous(), live.sum(dim=1)
+
+    def score_store(self, query_ctx: torch.Tensor, query_mask: torch.Tensor, store: torch.Tensor,
+                    doc_offsets: torch.Tensor, pair_q: torch.Tensor, pair_d: torch.Tensor,
+                    max_doc_len: Optional[int] = None) -> torch.Tensor:
+        """The counterpart of ``score_contextualized`` over rows from ``encode_documents`` (inference): pair p scores
+        query ``pair_q[p]`` of query_ctx [n_q, Lq, D] against passage ``pair_d[p]``, rows ``doc_offsets[d] :
+        doc_offsets[d+1]`` of store (see ``interaction.kernel_pool_store``)."""
+        return interaction.kernel_pool_store(query_ctx, query_mask, store, doc_offsets, pair_q, pair_d, self.mu,
+                                             self.sigma, self.kernel_bin_weights.weight, self.kernel_alpha_scaler, 1.0,
+                                             max_doc_len=max_doc_len)
 
     def forward_representation(self, sequence_embeddings: torch.Tensor, sequence_mask: torch.Tensor,
                                positional_features=None) -> torch.Tensor:

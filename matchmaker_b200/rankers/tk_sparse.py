@@ -3,12 +3,12 @@ Mirrors matchmaker/models/published/cikm20_tk_sparse.py; the interaction stage (
 kernels with the gate applied inside the activation sum (one more exponent term per document row, no extra pass)."""
 from __future__ import annotations
 
-from typing import List
+from typing import List, Optional
 
 import torch
 import torch.nn as nn
 
-from .. import autograd
+from .. import autograd, interaction
 from .tk import sinusoid_position_features
 
 
@@ -77,6 +77,35 @@ class CIKM20_TK_Sparse(nn.Module):
             return score, {"score": score, "per_kernel": per_kernel, "query_mean_vector": query_mean_vector,
                            "document_stop_words": document_stop_words}, document_stop_words
         return score, document_stop_words
+
+    @torch.no_grad()
+    def encode_documents(self, document_embeddings: torch.Tensor, document_mask: torch.Tensor):
+        """The document side of ``forward`` (cikm20_tk_sparse.py:104-135), which does not depend on the query, for a
+        store that is encoded once: (rows [n_live, D] fp32, lengths [B] int64, gate [n_live] fp32).  A term whose gate is
+        exactly 0 adds exactly 0 to every kernel sum of every query, so only terms with a nonzero gate are kept: rows
+        are the mixed embeddings of those terms in passage order and gate their gate values.  A passage whose terms are all
+        gated to 0 keeps its first term (gate 0): it scores what ``forward`` gives it, not the -inf of a passage without
+        rows.  ``score_store`` over them gives ``forward``'s scores."""
+        document_ctx, document_context_only = self.forward_representation(
+            document_embeddings, document_mask, self.positional_features_d[:, :document_embeddings.shape[1], :])
+        stop_in = self.mixer_stop * document_embeddings + (1 - self.mixer_stop) * document_context_only
+        gate = torch.nn.functional.relu(self.stop_word_reducer2(torch.tanh(self.stop_word_reducer(stop_in))).squeeze(-1)) \
+            * document_mask
+        mask = document_mask.bool()
+        live = mask & (gate != 0)
+        all_gated = ~live.any(dim=1) & mask.any(dim=1)
+        live[all_gated, mask[all_gated].float().argmax(dim=1)] = True
+        return document_ctx[live].float().contiguous(), live.sum(dim=1), gate[live].float().contiguous()
+
+    def score_store(self, query_ctx: torch.Tensor, query_mask: torch.Tensor, store: torch.Tensor,
+                    doc_offsets: torch.Tensor, pair_q: torch.Tensor, pair_d: torch.Tensor, gate: torch.Tensor,
+                    max_doc_len: Optional[int] = None) -> torch.Tensor:
+        """The interaction stage of ``forward`` over rows and gates from ``encode_documents`` (inference): pair p scores
+        query ``pair_q[p]`` of query_ctx [n_q, Lq, D] against passage ``pair_d[p]``, rows ``doc_offsets[d] :
+        doc_offsets[d+1]`` of store with their gate (see ``interaction.kernel_pool_store``)."""
+        return interaction.kernel_pool_store(query_ctx, query_mask, store, doc_offsets, pair_q, pair_d, self.mu,
+                                             self.sigma, self.kernel_bin_weights.weight, self.kernel_alpha_scaler, 1.0,
+                                             max_doc_len=max_doc_len, gate=gate)
 
     def forward_representation(self, sequence_embeddings: torch.Tensor, sequence_mask: torch.Tensor, positional_features=None):
         """Returns (mixed embeddings, context-only embeddings) as cikm20_tk_sparse.py:154-169."""
