@@ -85,15 +85,18 @@ def local_pairs(candidates: torch.Tensor, d_lo: int, d_hi: int) -> Tuple[torch.T
 
 
 def merge(scores: torch.Tensor, ids: torch.Tensor, k: int, group=None) -> Tuple[torch.Tensor, torch.Tensor]:
-    """The top k of every row of this rank's scores [Nq, C] under (score desc, id asc), merged across ranks."""
+    """The top k of every row of this rank's scores [Nq, C] under (score desc, id asc), merged across ranks; missing
+    entries are (-inf, -1)."""
     if scores.is_cuda:
         s, i = interaction.topk_merge(scores, ids, k)
     else:   # the gloo tests of the merge run on the CPU
         s, i = sharding.rank_topk(scores, ids, k)
     import torch.distributed as dist
     if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1:
-        return sharding.all_gather_merge(s, i, k, group)
-    return s, i
+        s, i = sharding.all_gather_merge(s, i, k, group)
+    # topk_merge fills missing results as faiss does, (-FLT_MAX, -1); a re-ranked candidate list reports them with the
+    # score of a candidate that is not there, -inf
+    return s.masked_fill(i < 0, float("-inf")), i
 
 
 class TKDocumentStore(GPUIndexer):
