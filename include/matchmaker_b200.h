@@ -319,6 +319,26 @@ MMB200_API int mmb200_tkl_window_scores(const float* q, const void* q_mask, cons
                                         int32_t C, int32_t K, int32_t saturation, int32_t mask_dtype, int32_t impl,
                                         void* stream);
 
+/* Store mode of mmb200_tkl_window_scores (inference only): the chunks come from a store of passages that were chunked,
+ * packed and contextualised once (TKL contextualises every packed chunk alone, so a chunk does not depend on the query
+ * or on the rest of the batch):
+ *
+ *   window_score[p] = mmb200_tkl_window_scores of query pair_q[p] against the chunk slots doc_slots[pair_d[p], 0..C-1]
+ *
+ * q [n_q, Lq, D] f32, q_mask [n_q, Lq] (mask_dtype) or NULL; chunks [n_chunks, 40, D] f32, chunk_mask [n_chunks, 40]
+ * (mask_dtype) or NULL; doc_slots [n_docs, C] int32: the store index of passage d's chunk in slot c, -1 where the
+ * packing dropped the slot or the passage is shorter; pair_q / pair_d [n_pairs] int32, pair_d[p] < 0 = no slots (its
+ * windows are all 0); window_score [n_pairs, W] out, W = (C*40 - 30)/2 + 1.  Everything else as
+ * mmb200_tkl_window_scores, including the routing of impl; the windows are bit-identical to that entry's on the same
+ * chunks gathered into the padded layout with q[pair_q] (same impl).  mmb200_tkl_top_hills selects on the result. */
+MMB200_API int mmb200_tkl_store_window_scores(const float* q, const void* q_mask, const float* chunks,
+                                              const void* chunk_mask, const int32_t* doc_slots, const int32_t* pair_q,
+                                              const int32_t* pair_d, const float* mu, const float* sigma,
+                                              const float* dense_w, const float* sat_red_w, const float* sat_params,
+                                              float* window_score, int64_t n_q, int64_t n_chunks, int64_t n_docs,
+                                              int64_t n_pairs, int32_t Lq, int32_t D, int32_t C, int32_t K,
+                                              int32_t saturation, int32_t mask_dtype, int32_t impl, void* stream);
+
 /* window_score [B,W] in; orig_score [B,W] out (may be the same buffer): the reference's "orig_score" (exact zeros ->
  * -9900 sentinel during selection, written back as 0).  chunk_scoring [15]; top_idx [B,3] int64;
  * top15 [B,15] ("top_k_non_overlapping"); score [B]. */

@@ -37,6 +37,7 @@ SIGNATURES = {
                                           _i64]),
     "mmb200_kernel_pool_fwd": (_c.c_int, [_vp] * 12 + [_i64, _i32, _i32, _i32, _i32, _f32, _i32, _i32, _vp]),
     "mmb200_tkl_window_scores": (_c.c_int, [_vp] * 11 + [_i64, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "mmb200_tkl_store_window_scores": (_c.c_int, [_vp] * 13 + [_i64] * 4 + [_i32] * 7 + [_vp]),
     "mmb200_tkl_bwd": (_c.c_int, [_vp] * 18 + [_i64, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
     "mmb200_tkl_top_hills": (_c.c_int, [_vp] * 6 + [_i64, _i32, _vp]),
     "mmb200_tkl_slot_map": (_c.c_int, [_vp, _vp, _i64, _vp]),

@@ -105,9 +105,10 @@ __device__ __forceinline__ void cos_40x40(const float* __restrict__ qs, const fl
     for (int s = 0; s < 2; ++s) cs[(ti + 10 * r) * 41 + tj + 20 * s] = acc[r][s];
 }
 
-// PROF (MMB200_TKL_PROF=1): debugging aid, thread 0 of CTA 0 accumulates the cycles of each phase of the chunk loop
-template <int KB, bool PROF = false>
-__global__ void __launch_bounds__(kThreads) tkl_window_kernel(TklParams P, long long* prof = nullptr) {
+// PROF (MMB200_TKL_PROF=1): debugging aid, thread 0 of CTA 0 accumulates the cycles of each phase of the chunk loop.
+// STORE: document b is pair b (TklPairs): query row pair_q[b], chunk slots from row pair_d[b] of the passages' slot table.
+template <int KB, bool PROF, bool STORE>
+__global__ void __launch_bounds__(kThreads) tkl_window_kernel(TklParams P, long long* prof, TklPairs X) {
   long long pc[5] = {0, 0, 0, 0, 0};
   long long t_mark = PROF ? clock64() : 0;
   auto lap = [&](int slot) {
@@ -154,12 +155,15 @@ __global__ void __launch_bounds__(kThreads) tkl_window_kernel(TklParams P, long 
     const int c_first = seg * P.chunks_per_seg;
     const int c_last = min(P.C, c_first + P.chunks_per_seg);
     if (c_first >= c_last) continue;
+    const int64_t qb = tkl_q_row<STORE>(X, b);
     __syncthreads();
-    load_rows_norm(P.q + b * (int64_t)Lq * D, Lq, kMaxLq, D, dp, qs, P.saturation == 0 ? P.sat_red_w : nullptr, red);
-    if (t < kMaxLq) qm_s[t] = (t < Lq && mask_at(P.q_mask, P.q_mask ? P.mask_dtype : 0, b * (int64_t)Lq + t)) ? 1.f : 0.f;
+    load_rows_norm(P.q + qb * (int64_t)Lq * D, Lq, kMaxLq, D, dp, qs, P.saturation == 0 ? P.sat_red_w : nullptr, red);
+    if (t < kMaxLq) qm_s[t] = (t < Lq && mask_at(P.q_mask, P.q_mask ? P.mask_dtype : 0, qb * (int64_t)Lq + t)) ? 1.f : 0.f;
     // one halo chunk in front supplies the 14 pairs that windows ending in this segment reach back to
     for (int c = max(0, c_first - 1); c < c_last; ++c) {
-      const int pk_idx = P.slot_to_packed[b * P.C + c];
+      // store mode reads the pair's passage again per chunk (an L1 hit) rather than holding it across the loop
+      const int64_t sb = tkl_slot_row<STORE>(X, b);
+      const int pk_idx = (STORE && sb < 0) ? -1 : P.slot_to_packed[sb * P.C + c];
       __syncthreads();
       lap(4);
       if (pk_idx >= 0) {
@@ -372,6 +376,88 @@ __global__ void __launch_bounds__(1024) tkl_slot_map_kernel(const uint8_t* __res
   for (int64_t i = lo; i < hi; ++i) slot_to_packed[i] = packed[i] ? run++ : -1;
 }
 
+// The routing both window-score entries share: the tensor-core kernel where its envelope and the device-side cover test
+// allow, the FFMA kernel otherwise.  X.pair_q != nullptr selects the store-mode instantiations.
+template <bool STORE>
+int tkl_window_scores_run(TklParams& P, const TklPairs& X, const DeviceInfo& dev, int impl, cudaStream_t stream) {
+  const int64_t B = P.B;
+  const int C = P.C, K = P.K, D = P.D;
+  // split long documents over several CTAs when there are fewer documents than SMs
+  int segs = 1;
+  if (B < dev.sm_count) segs = std::min<int>(C, std::max<int>(1, (int)((2 * dev.sm_count + B - 1) / B)));
+  P.chunks_per_seg = (C + segs - 1) / segs;
+  P.segs = (C + P.chunks_per_seg - 1) / P.chunks_per_seg;
+  const int KB = K <= 12 ? 12 : 16;
+  const int dp = padded_row_stride(D);
+  const size_t need = ((size_t)2 * kMaxLq * dp + kMaxLq * 41 + (size_t)kMaxLq * (kRing * KB + 1) + kMaxLq * kZStride + 3 * kMaxLq +
+                       4 * KB + 16 + 20 * KB + (size_t)20 * kMaxLq * KB) * sizeof(float);
+  const bool ffma_fits = need <= (size_t)dev.max_smem_optin;
+  // Tensor-core kernel first (tkl_ts.cu).  Its plan kernel decides ON THE DEVICE whether the kernel set lets it run
+  // ("cover", see there); the FFMA kernel below is enqueued as well and returns at once when the plan says the
+  // tensor-core kernel took the call -- no host synchronisation either way.
+  int32_t* plan = nullptr;
+  if (impl != MMB200_IMPL_SIMT) {
+    if (!ffma_fits) P.segs = 0;   // tells the tensor-core kernel that nothing can take over
+    bool handled = false;
+    if (int rc = tkl_window_ts_launch(P, X, dev, stream, &handled, &plan)) return rc;
+    if (impl == MMB200_IMPL_TCGEN05 && !handled) {
+      set_error("tkl_window_scores: shape outside the tensor-core kernel's envelope (Lq <= 40, K <= 16, Lq * K <= 512)");
+      return MMB200_ERR_UNSUPPORTED;
+    }
+    if (handled && (impl == MMB200_IMPL_TCGEN05 || !ffma_fits)) {
+      MMB_CHECK_CUDA(cudaFreeAsync(plan, stream));
+      return MMB200_OK;
+    }
+  }
+  if (!ffma_fits) {
+    set_error("TKL kernel: embedding dim / kernel count too large for the shared-memory plan (D=300 fits with K <= 12)");
+    return MMB200_ERR_UNSUPPORTED;
+  }
+  const int grid = (int)std::min<int64_t>(B * P.segs, (int64_t)dev.sm_count * 2);
+#ifdef MMB200_ENABLE_PROF
+  if (!STORE && KB == 12 && getenv("MMB200_TKL_PROF")) {
+    long long* prof = nullptr;
+    long long h[5] = {0};
+    MMB_CHECK_CUDA(cudaMalloc(&prof, sizeof(h)));
+    MMB_CHECK_CUDA(cudaMemset(prof, 0, sizeof(h)));
+    MMB_CHECK_CUDA(cudaFuncSetAttribute(tkl_window_kernel<12, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)need));
+    tkl_window_kernel<12, true, false><<<grid, kThreads, need, stream>>>(P, prof, X);
+    MMB_CHECK_CUDA(cudaStreamSynchronize(stream));
+    MMB_CHECK_CUDA(cudaMemcpy(h, prof, sizeof(h), cudaMemcpyDeviceToHost));
+    MMB_CHECK_CUDA(cudaFree(prof));
+    fprintf(stderr, "tkl_prof cycles (CTA 0): load+norm %lld | cosine %lld | activations %lld | windows %lld | other %lld\n", h[0], h[1],
+            h[2], h[3], h[4]);
+    return MMB200_OK;
+  }
+#endif
+  if (KB == 12) {
+    MMB_CHECK_CUDA(cudaFuncSetAttribute(tkl_window_kernel<12, false, STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)need));
+    tkl_window_kernel<12, false, STORE><<<grid, kThreads, need, stream>>>(P, nullptr, X);
+  } else {
+    MMB_CHECK_CUDA(cudaFuncSetAttribute(tkl_window_kernel<16, false, STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)need));
+    tkl_window_kernel<16, false, STORE><<<grid, kThreads, need, stream>>>(P, nullptr, X);
+  }
+  MMB_CHECK_CUDA(cudaGetLastError());
+  if (plan) MMB_CHECK_CUDA(cudaFreeAsync(plan, stream));
+  return MMB200_OK;
+}
+
+// Argument checks both window-score entries share.
+int tkl_window_scores_check(const float* q, const float* chunks, const int32_t* slots, const float* mu, const float* sigma,
+                            const float* dense_w, const float* sat_red_w, const float* sat_params, float* window_score,
+                            const void* q_mask, const void* chunk_mask, int32_t Lq, int32_t D, int32_t C, int32_t K,
+                            int32_t saturation, int32_t mask_dtype, int32_t impl) {
+  MMB_REQUIRE(q && chunks && slots && mu && sigma && dense_w && sat_params && window_score, "null pointer");
+  MMB_REQUIRE(impl == MMB200_IMPL_AUTO || impl == MMB200_IMPL_SIMT || impl == MMB200_IMPL_TCGEN05, "impl: auto, simt or tcgen05");
+  MMB_REQUIRE(Lq >= 1 && Lq <= kMaxLq, "TKL kernel supports 1 <= Lq <= 40");
+  MMB_REQUIRE(D > 0 && D % 4 == 0, "embedding dim must be a multiple of 4");
+  MMB_REQUIRE(C >= 1 && K >= 1 && K <= 16, "need C >= 1 and K <= 16");
+  MMB_REQUIRE(saturation == 0 || saturation == 1, "saturation: 0 = embedding, 1 = log");
+  MMB_REQUIRE(saturation == 1 || sat_red_w != nullptr, "embedding saturation needs sat_emb_reduce1 weights");
+  if (q_mask || chunk_mask) MMB_REQUIRE(mask_dtype_size(mask_dtype) != 0, "unknown mask dtype");
+  return MMB200_OK;
+}
+
 }  // namespace
 
 }  // namespace mmb
@@ -393,14 +479,10 @@ extern "C" int mmb200_tkl_window_scores(const float* q, const void* q_mask, cons
                                         int32_t C, int32_t K, int32_t saturation, int32_t mask_dtype, int32_t impl,
                                         void* stream_) {
   using namespace mmb;
-  MMB_REQUIRE(q && chunks && slot_to_packed && mu && sigma && dense_w && sat_params && window_score, "null pointer");
-  MMB_REQUIRE(impl == MMB200_IMPL_AUTO || impl == MMB200_IMPL_SIMT || impl == MMB200_IMPL_TCGEN05, "impl: auto, simt or tcgen05");
-  MMB_REQUIRE(B >= 0 && Lq >= 1 && Lq <= kMaxLq, "TKL kernel supports 1 <= Lq <= 40");
-  MMB_REQUIRE(D > 0 && D % 4 == 0, "embedding dim must be a multiple of 4");
-  MMB_REQUIRE(C >= 1 && K >= 1 && K <= 16, "need C >= 1 and K <= 16");
-  MMB_REQUIRE(saturation == 0 || saturation == 1, "saturation: 0 = embedding, 1 = log");
-  MMB_REQUIRE(saturation == 1 || sat_red_w != nullptr, "embedding saturation needs sat_emb_reduce1 weights");
-  if (q_mask || chunk_mask) MMB_REQUIRE(mask_dtype_size(mask_dtype) != 0, "unknown mask dtype");
+  if (int rc = tkl_window_scores_check(q, chunks, slot_to_packed, mu, sigma, dense_w, sat_red_w, sat_params, window_score,
+                                       q_mask, chunk_mask, Lq, D, C, K, saturation, mask_dtype, impl))
+    return rc;
+  MMB_REQUIRE(B >= 0, "B >= 0");
   if (B == 0) return MMB200_OK;
   DeviceInfo dev;
   if (int rc = require_sm90(&dev)) return rc;
@@ -411,65 +493,36 @@ extern "C" int mmb200_tkl_window_scores(const float* q, const void* q_mask, cons
   P.mask_dtype = mask_dtype;
   P.saturation = saturation;
   P.W = (C * kChunk - kWindow) / 2 + 1;
-  // split long documents over several CTAs when there are fewer documents than SMs
-  int segs = 1;
-  if (B < dev.sm_count) segs = std::min<int>(C, std::max<int>(1, (int)((2 * dev.sm_count + B - 1) / B)));
-  P.chunks_per_seg = (C + segs - 1) / segs;
-  P.segs = (C + P.chunks_per_seg - 1) / P.chunks_per_seg;
-  const int KB = K <= 12 ? 12 : 16;
-  const int dp = padded_row_stride(D);
-  const size_t need = ((size_t)2 * kMaxLq * dp + kMaxLq * 41 + (size_t)kMaxLq * (kRing * KB + 1) + kMaxLq * kZStride + 3 * kMaxLq +
-                       4 * KB + 16 + 20 * KB + (size_t)20 * kMaxLq * KB) * sizeof(float);
-  const bool ffma_fits = need <= (size_t)dev.max_smem_optin;
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  // Tensor-core kernel first (tkl_ts.cu).  Its plan kernel decides ON THE DEVICE whether the kernel set lets it run
-  // ("cover", see there); the FFMA kernel below is enqueued as well and returns at once when the plan says the
-  // tensor-core kernel took the call -- no host synchronisation either way.
-  int32_t* plan = nullptr;
-  if (impl != MMB200_IMPL_SIMT) {
-    if (!ffma_fits) P.segs = 0;   // tells the tensor-core kernel that nothing can take over
-    bool handled = false;
-    if (int rc = tkl_window_ts_launch(P, dev, stream, &handled, &plan)) return rc;
-    if (impl == MMB200_IMPL_TCGEN05 && !handled) {
-      set_error("tkl_window_scores: shape outside the tensor-core kernel's envelope (Lq <= 40, K <= 16, Lq * K <= 512)");
-      return MMB200_ERR_UNSUPPORTED;
-    }
-    if (handled && (impl == MMB200_IMPL_TCGEN05 || !ffma_fits)) {
-      MMB_CHECK_CUDA(cudaFreeAsync(plan, stream));
-      return MMB200_OK;
-    }
-  }
-  if (!ffma_fits) {
-    set_error("TKL kernel: embedding dim / kernel count too large for the shared-memory plan (D=300 fits with K <= 12)");
-    return MMB200_ERR_UNSUPPORTED;
-  }
-  const int grid = (int)std::min<int64_t>(B * P.segs, (int64_t)dev.sm_count * 2);
-#ifdef MMB200_ENABLE_PROF
-  if (KB == 12 && getenv("MMB200_TKL_PROF")) {
-    long long* prof = nullptr;
-    long long h[5] = {0};
-    MMB_CHECK_CUDA(cudaMalloc(&prof, sizeof(h)));
-    MMB_CHECK_CUDA(cudaMemset(prof, 0, sizeof(h)));
-    MMB_CHECK_CUDA(cudaFuncSetAttribute(tkl_window_kernel<12, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)need));
-    tkl_window_kernel<12, true><<<grid, kThreads, need, stream>>>(P, prof);
-    MMB_CHECK_CUDA(cudaStreamSynchronize(stream));
-    MMB_CHECK_CUDA(cudaMemcpy(h, prof, sizeof(h), cudaMemcpyDeviceToHost));
-    MMB_CHECK_CUDA(cudaFree(prof));
-    fprintf(stderr, "tkl_prof cycles (CTA 0): load+norm %lld | cosine %lld | activations %lld | windows %lld | other %lld\n", h[0], h[1],
-            h[2], h[3], h[4]);
-    return MMB200_OK;
-  }
-#endif
-  if (KB == 12) {
-    MMB_CHECK_CUDA(cudaFuncSetAttribute(tkl_window_kernel<12, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)need));
-    tkl_window_kernel<12, false><<<grid, kThreads, need, stream>>>(P, nullptr);
-  } else {
-    MMB_CHECK_CUDA(cudaFuncSetAttribute(tkl_window_kernel<16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)need));
-    tkl_window_kernel<16, false><<<grid, kThreads, need, stream>>>(P, nullptr);
-  }
-  MMB_CHECK_CUDA(cudaGetLastError());
-  if (plan) MMB_CHECK_CUDA(cudaFreeAsync(plan, stream));
-  return MMB200_OK;
+  return tkl_window_scores_run<false>(P, TklPairs{nullptr, nullptr, B}, dev, impl, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int mmb200_tkl_store_window_scores(const float* q, const void* q_mask, const float* chunks,
+                                              const void* chunk_mask, const int32_t* doc_slots, const int32_t* pair_q,
+                                              const int32_t* pair_d, const float* mu, const float* sigma,
+                                              const float* dense_w, const float* sat_red_w, const float* sat_params,
+                                              float* window_score, int64_t n_q, int64_t n_chunks, int64_t n_docs,
+                                              int64_t n_pairs, int32_t Lq, int32_t D, int32_t C, int32_t K,
+                                              int32_t saturation, int32_t mask_dtype, int32_t impl, void* stream_) {
+  using namespace mmb;
+  MMB_REQUIRE(n_pairs >= 0, "n_pairs >= 0");
+  if (n_pairs == 0) return MMB200_OK;   // nothing to write: the empty outputs may be null
+  if (int rc = tkl_window_scores_check(q, chunks, doc_slots, mu, sigma, dense_w, sat_red_w, sat_params, window_score,
+                                       q_mask, chunk_mask, Lq, D, C, K, saturation, mask_dtype, impl))
+    return rc;
+  MMB_REQUIRE(pair_q && pair_d, "null pointer");
+  MMB_REQUIRE(n_q >= 1 && n_q < (1ll << 31) && n_docs >= 1, "need 1 <= n_q < 2^31 and n_docs >= 1");
+  // chunk indices are int32 TMA coordinates
+  MMB_REQUIRE(n_chunks >= 1 && n_chunks < (1ll << 31), "need 1 <= n_chunks < 2^31");
+  DeviceInfo dev;
+  if (int rc = require_sm90(&dev)) return rc;
+  TklParams P{};
+  P.q = q; P.q_mask = q_mask; P.chunks = chunks; P.chunk_mask = chunk_mask; P.slot_to_packed = doc_slots;
+  P.mu = mu; P.sigma = sigma; P.dense_w = dense_w; P.sat_red_w = sat_red_w; P.sat_params = sat_params;
+  P.window_score = window_score; P.B = n_pairs; P.n_chunks = n_chunks; P.Lq = Lq; P.D = D; P.C = C; P.K = K;
+  P.mask_dtype = mask_dtype;
+  P.saturation = saturation;
+  P.W = (C * kChunk - kWindow) / 2 + 1;
+  return tkl_window_scores_run<true>(P, TklPairs{pair_q, pair_d, n_q}, dev, impl, static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int mmb200_tkl_top_hills(const float* window_score, float* orig_score, const float* chunk_scoring,

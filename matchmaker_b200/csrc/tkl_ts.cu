@@ -140,10 +140,12 @@ __device__ __forceinline__ void block_exclusive_scan_inplace(int32_t* v, int64_t
   __syncthreads();
 }
 
-__global__ void __launch_bounds__(1024) tkl_plan_kernel(const int32_t* __restrict__ slot_to_packed, const void* __restrict__ q_mask,
-                                                        int mask_dtype, int64_t B, int C, int Lq, const float* __restrict__ mu,
-                                                        const float* __restrict__ sigma, int K, int grid, int force_cover,
-                                                        int32_t* __restrict__ plan) {
+// STORE: document b is pair b, its slots are row pair_d[b] of slot_to_packed and its query mask row pair_q[b].
+template <bool STORE>
+__device__ __forceinline__ void tkl_plan_body(const int32_t* __restrict__ slot_to_packed, const void* __restrict__ q_mask,
+                                              int mask_dtype, int64_t B, int C, int Lq, const float* __restrict__ mu,
+                                              const float* __restrict__ sigma, int K, int grid, int force_cover,
+                                              int32_t* __restrict__ plan, const TklPairs& X) {
   __shared__ int sums[1024];
   __shared__ int carry;
   __shared__ int total_tiles, total_cost;
@@ -173,10 +175,13 @@ __global__ void __launch_bounds__(1024) tkl_plan_kernel(const int32_t* __restric
     for (int a = 0; a < 4; ++a) {
       const int64_t b = b0 + a;
       const bool ok = small && b < B;
-      pk0[a] = ok && lane < C && slot_to_packed[b * C + lane] >= 0;
-      pk1[a] = ok && lane + 32 < C && slot_to_packed[b * C + lane + 32] >= 0;
-      lv0[a] = ok && lane < Lq && mask_at(q_mask, qmt, b * Lq + lane);
-      lv1[a] = ok && lane + 32 < Lq && mask_at(q_mask, qmt, b * Lq + lane + 32);
+      const int64_t sb = STORE ? (ok ? tkl_slot_row<true>(X, b) : -1) : b;
+      const int64_t qb = STORE ? (ok ? tkl_q_row<true>(X, b) : 0) : b;
+      const bool live = ok && (!STORE || sb >= 0);
+      pk0[a] = live && lane < C && slot_to_packed[sb * C + lane] >= 0;
+      pk1[a] = live && lane + 32 < C && slot_to_packed[sb * C + lane + 32] >= 0;
+      lv0[a] = ok && lane < Lq && mask_at(q_mask, qmt, qb * Lq + lane);
+      lv1[a] = ok && lane + 32 < Lq && mask_at(q_mask, qmt, qb * Lq + lane + 32);
     }
 #pragma unroll
     for (int a = 0; a < 4; ++a) {
@@ -189,14 +194,15 @@ __global__ void __launch_bounds__(1024) tkl_plan_kernel(const int32_t* __restric
         const unsigned q0 = __ballot_sync(0xffffffffu, lv0[a]), q1 = __ballot_sync(0xffffffffu, lv1[a]);
         q_hi = q1 ? 64 - __clz(q1) : (q0 ? 32 - __clz(q0) : 0);
       } else {
+        const int64_t sb = tkl_slot_row<STORE>(X, b), qb = tkl_q_row<STORE>(X, b);
         for (int c0 = 0; c0 < C; c0 += 32) {
           const int c = c0 + lane;
-          const unsigned m = __ballot_sync(0xffffffffu, c < C && slot_to_packed[b * C + c] >= 0);
+          const unsigned m = __ballot_sync(0xffffffffu, (!STORE || sb >= 0) && c < C && slot_to_packed[sb * C + c] >= 0);
           if (m) c_last = c0 + 31 - __clz(m);
         }
         for (int i0 = 0; i0 < Lq; i0 += 32) {
           const int i = i0 + lane;
-          const unsigned m = __ballot_sync(0xffffffffu, i < Lq && mask_at(q_mask, qmt, b * Lq + i));
+          const unsigned m = __ballot_sync(0xffffffffu, i < Lq && mask_at(q_mask, qmt, qb * Lq + i));
           if (m) q_hi = i0 + 32 - __clz(m);
         }
       }
@@ -251,6 +257,21 @@ __global__ void __launch_bounds__(1024) tkl_plan_kernel(const int32_t* __restric
   }
 }
 
+__global__ void __launch_bounds__(1024) tkl_plan_kernel(const int32_t* __restrict__ slot_to_packed, const void* __restrict__ q_mask,
+                                                        int mask_dtype, int64_t B, int C, int Lq, const float* __restrict__ mu,
+                                                        const float* __restrict__ sigma, int K, int grid, int force_cover,
+                                                        int32_t* __restrict__ plan) {
+  tkl_plan_body<false>(slot_to_packed, q_mask, mask_dtype, B, C, Lq, mu, sigma, K, grid, force_cover, plan, TklPairs{});
+}
+
+// One CTA per SM at most (minBlocks 1): 64 registers, where the default bound spills the pair loads of the store mode.
+__global__ void __launch_bounds__(1024, 1) tkl_plan_store_kernel(const int32_t* __restrict__ doc_slots, const void* __restrict__ q_mask,
+                                                                 int mask_dtype, int64_t B, int C, int Lq, const float* __restrict__ mu,
+                                                                 const float* __restrict__ sigma, int K, int grid, int force_cover,
+                                                                 int32_t* __restrict__ plan, TklPairs X) {
+  tkl_plan_body<true>(doc_slots, q_mask, mask_dtype, B, C, Lq, mu, sigma, K, grid, force_cover, plan, X);
+}
+
 // The tiles a CTA walks, identically in every role: [g_begin, g_end) of the global tile sequence, preceded by a halo
 // tile when the share starts inside a document.
 struct TileWalk {
@@ -292,10 +313,12 @@ struct TileWalk {
   }
 };
 
-template <int SAT>
+// STORE: document b of the tile walk is pair b (TklPairs): its query box, query mask and saturation table come from query
+// row pair_q[b], its chunk slots from row pair_d[b] of the passages' slot table.
+template <int SAT, bool STORE>
 __global__ void __launch_bounds__(kThreads, 1)
 tkl_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_c, TklParams P,
-              int n_raw, int fallback_available) {
+              int n_raw, int fallback_available, TklPairs X) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* qring = smem;                                                    // [kOps][Qhi;Qlo]
@@ -339,12 +362,14 @@ tkl_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant_
       for (; tw.valid(); tw.next()) {
         int pk[kTileSlots];
         int n_present = 0;
+        const int64_t sb = tkl_slot_row<STORE>(X, tw.b);
 #pragma unroll
         for (int s = 0; s < kTileSlots; ++s) {
           const int c = tw.t * kTileSlots + s;
-          pk[s] = (c < P.C && !(tw.halo && s < kTileSlots - 1)) ? P.slot_to_packed[(int64_t)tw.b * P.C + c] : -1;
+          pk[s] = ((!STORE || sb >= 0) && c < P.C && !(tw.halo && s < kTileSlots - 1)) ? P.slot_to_packed[sb * P.C + c] : -1;
           n_present += pk[s] >= 0 ? 1 : 0;
         }
+        const int qbox = (int)tkl_q_row<STORE>(X, tw.b);
         const uint32_t bytes = (uint32_t)(n_present * kSlotBytes + kQxBytes);
         for (int ck = 0; ck < nch; ++ck) {
           mbar_wait(&S->raw_empty[stage], phase ^ 1u);
@@ -353,7 +378,7 @@ tkl_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant_
 #pragma unroll
           for (int s = 0; s < kTileSlots; ++s)
             if (pk[s] >= 0) tma_load_3d(&tmap_c, st + s * kSlotBytes, &S->raw_full[stage], ck * 32, 0, pk[s], kEvictFirst);
-          tma_load_3d(&tmap_q, st + kDxBytes, &S->raw_full[stage], ck * 32, 0, (int)tw.b, kEvictLast);
+          tma_load_3d(&tmap_q, st + kDxBytes, &S->raw_full[stage], ck * 32, 0, qbox, kEvictLast);
           if (++stage == n_raw) { stage = 0; phase ^= 1u; }
         }
       }
@@ -430,13 +455,14 @@ tkl_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant_
       int64_t tile_seq = 0;
       for (; tw.valid(); tw.next(), ++tile_seq) {
         const int t = tw.t;
+        const int64_t sb = tkl_slot_row<STORE>(X, tw.b);
         uint64_t draw[4];
         bool present[4];
 #pragma unroll
         for (int e = 0; e < 4; ++e) {   // the position's packed chunk, then its mask word: in flight during the MMAs
           const int row = rb + 8 * (e & 1) + 64 * (e >> 1);
           const int c = t * kTileSlots + row / kChunk;
-          const int pk = (row < kTileRows && c < P.C) ? P.slot_to_packed[(int64_t)tw.b * P.C + c] : -1;
+          const int pk = ((!STORE || sb >= 0) && row < kTileRows && c < P.C) ? P.slot_to_packed[sb * P.C + c] : -1;
           present[e] = pk >= 0;
           draw[e] = pk < 0 ? 0 : dmt != MMB200_MASK_NONE ? mask_raw(P.chunk_mask, dmt, (int64_t)pk * kChunk + (row % kChunk)) : 1;
         }
@@ -552,8 +578,9 @@ tkl_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant_
         if (b != cur_doc) {
           // ---- new document: query mask, sat_emb_reduce1(q_i), saturation table indexed by (query row, token count)
           cur_doc = b;
+          const int64_t qb = tkl_q_row<STORE>(X, b);
           named_bar_sync(1, kEpiThreads);   // nobody still reads the previous document's table / qm
-          if (et < kMaxLq) S->qm[et] = (et < P.Lq && mask_at(P.q_mask, qmt, (int64_t)b * P.Lq + et)) ? 1.f : 0.f;
+          if (et < kMaxLq) S->qm[et] = (et < P.Lq && mask_at(P.q_mask, qmt, qb * P.Lq + et)) ? 1.f : 0.f;
           if (SAT == 0) {
             // the warp's rows ew, ew + 16, ew + 32 side by side: their loads are independent and in flight together (one
             // global-memory latency per document switch instead of one per row and 128-byte step)
@@ -566,7 +593,7 @@ tkl_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant_
 #pragma unroll
               for (int a = 0; a < 3; ++a) {
                 const int i = ew + kEpiWarps * a;
-                v[a] = i < P.Lq ? __ldg(reinterpret_cast<const float4*>(P.q + ((int64_t)b * P.Lq + i) * P.D) + c4)
+                v[a] = i < P.Lq ? __ldg(reinterpret_cast<const float4*>(P.q + (qb * P.Lq + i) * P.D) + c4)
                                 : make_float4(0.f, 0.f, 0.f, 0.f);
               }
 #pragma unroll
@@ -730,9 +757,11 @@ tkl_ts_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant_
 
 }  // namespace
 
-int tkl_window_ts_launch(TklParams& P, const DeviceInfo& dev, cudaStream_t stream, bool* handled, int32_t** plan_out) {
+int tkl_window_ts_launch(TklParams& P, const TklPairs& X, const DeviceInfo& dev, cudaStream_t stream, bool* handled,
+                         int32_t** plan_out) {
   *handled = false;
   *plan_out = nullptr;
+  const bool store = X.pair_q != nullptr;
   if (P.Lq > kMaxLq || P.K > 16 || P.Lq * P.K > kEpiThreads || P.D % 4 != 0) return MMB200_OK;
   if (P.B * (int64_t)P.C >= (1ll << 31) || P.B >= (1ll << 31) - 8) return MMB200_OK;
   const size_t fixed = (size_t)kOps * kQopBytes + 2 * (size_t)kMaxLq * kCsStride * sizeof(float) + sizeof(TsShared) + 1024;
@@ -741,7 +770,7 @@ int tkl_window_ts_launch(TklParams& P, const DeviceInfo& dev, cudaStream_t strea
   const size_t smem = fixed + (size_t)n_raw * kRawBytes;
   CUtensorMap tq, tc;
   {
-    const uint64_t dims[3] = {(uint64_t)P.D, (uint64_t)P.Lq, (uint64_t)P.B};
+    const uint64_t dims[3] = {(uint64_t)P.D, (uint64_t)P.Lq, (uint64_t)(store ? X.n_q : P.B)};
     const uint64_t strides[2] = {(uint64_t)P.D * 4, (uint64_t)P.Lq * P.D * 4};
     const uint32_t box[3] = {32, (uint32_t)kMaxLq, 1};
     if (int rc = encode_tensor_map(&tq, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, P.q, dims, strides, box,
@@ -749,8 +778,8 @@ int tkl_window_ts_launch(TklParams& P, const DeviceInfo& dev, cudaStream_t strea
       return rc;
   }
   {
-    // the packed chunk count is not part of the C ABI: every index the kernel uses comes from slot_to_packed, so the
-    // outer extent only has to be an upper bound (B * C slots)
+    // the packed chunk count is not part of the padded C ABI: every index the kernel uses comes from slot_to_packed, so
+    // the outer extent only has to be an upper bound (B * C slots); the store entry passes its chunk count
     const uint64_t dims[3] = {(uint64_t)P.D, (uint64_t)kChunk, (uint64_t)(P.n_chunks > 0 ? P.n_chunks : P.B * P.C)};
     const uint64_t strides[2] = {(uint64_t)P.D * 4, (uint64_t)kChunk * P.D * 4};
     const uint32_t box[3] = {32, (uint32_t)kChunk, 1};
@@ -767,8 +796,12 @@ int tkl_window_ts_launch(TklParams& P, const DeviceInfo& dev, cudaStream_t strea
 #endif
   // the zero fill first: the window-score kernel is a programmatic dependent of the plan kernel (nothing may sit between them)
   MMB_CHECK_CUDA(cudaMemsetAsync(P.window_score, 0, (size_t)P.B * P.W * sizeof(float), stream));
-  tkl_plan_kernel<<<1, 1024, 0, stream>>>(P.slot_to_packed, P.q_mask, P.mask_dtype, P.B, P.C, P.Lq, P.mu, P.sigma, P.K, grid,
-                                          force, plan);
+  if (store)
+    tkl_plan_store_kernel<<<1, 1024, 0, stream>>>(P.slot_to_packed, P.q_mask, P.mask_dtype, P.B, P.C, P.Lq, P.mu, P.sigma,
+                                                  P.K, grid, force, plan, X);
+  else
+    tkl_plan_kernel<<<1, 1024, 0, stream>>>(P.slot_to_packed, P.q_mask, P.mask_dtype, P.B, P.C, P.Lq, P.mu, P.sigma, P.K, grid,
+                                            force, plan);
   MMB_CHECK_CUDA(cudaGetLastError());
   P.plan = plan;
   *plan_out = plan;
@@ -784,23 +817,23 @@ int tkl_window_ts_launch(TklParams& P, const DeviceInfo& dev, cudaStream_t strea
     attr.val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = &attr;
     cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, kernel, tq, tc, P, n_raw, fallback);
+    return cudaLaunchKernelEx(&cfg, kernel, tq, tc, P, n_raw, fallback, X);
   };
-  static bool attr_set[2][64] = {};
+  static bool attr_set[2][2][64] = {};
   const int di = dev.device & 63;
-  if (P.saturation == 0) {
-    if (!attr_set[0][di]) {
-      MMB_CHECK_CUDA(cudaFuncSetAttribute(tkl_ts_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dev.max_smem_optin));
-      attr_set[0][di] = true;
+  auto launch = [&](auto kernel, bool& attr) -> cudaError_t {
+    if (!attr) {
+      if (cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dev.max_smem_optin))
+        return e;
+      attr = true;
     }
-    MMB_CHECK_CUDA(launch_pdl(tkl_ts_kernel<0>));
-  } else {
-    if (!attr_set[1][di]) {
-      MMB_CHECK_CUDA(cudaFuncSetAttribute(tkl_ts_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dev.max_smem_optin));
-      attr_set[1][di] = true;
-    }
-    MMB_CHECK_CUDA(launch_pdl(tkl_ts_kernel<1>));
-  }
+    return launch_pdl(kernel);
+  };
+  bool& attr = attr_set[P.saturation][store ? 1 : 0][di];
+  if (P.saturation == 0)
+    MMB_CHECK_CUDA(store ? launch(tkl_ts_kernel<0, true>, attr) : launch(tkl_ts_kernel<0, false>, attr));
+  else
+    MMB_CHECK_CUDA(store ? launch(tkl_ts_kernel<1, true>, attr) : launch(tkl_ts_kernel<1, false>, attr));
   MMB_CHECK_CUDA(cudaGetLastError());
   *handled = true;
   return MMB200_OK;

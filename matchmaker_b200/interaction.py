@@ -443,9 +443,10 @@ def _tkl_slot_map(packed_indices: torch.Tensor) -> torch.Tensor:
 
 def _tkl_operands(q_mask, chunk_mask, packed_indices, mu, sigma, dense_weight, sat_red_weight, sat_params,
                   saturation: str):
-    """The operands both TKL entries share: masks of one element type and their code, the slot map, the kernel and
-    saturation parameters as flat fp32, and the saturation code."""
-    slot = _tkl_slot_map(packed_indices)
+    """The operands the TKL entries share: masks of one element type and their code, the slot map (None without
+    ``packed_indices``: the store entry takes a slot table), the kernel and saturation parameters as flat fp32, and the
+    saturation code."""
+    slot = None if packed_indices is None else _tkl_slot_map(packed_indices)
     q_mask, chunk_mask, mcode = _common_mask_dtype(_prep_mask(q_mask), _prep_mask(chunk_mask))
     mu, sigma, dense_weight = _f32c(mu).view(-1), _f32c(sigma).view(-1), _f32c(dense_weight).view(-1)
     sat_params = _f32c(sat_params).view(-1)
@@ -474,12 +475,62 @@ def tkl_window_scores(q_ctx: torch.Tensor, q_mask: torch.Tensor, doc_chunks: tor
     K = mu.numel()
     W = (C * TKL_CHUNK - TKL_WINDOW) // 2 + 1
     out = torch.empty((B, W), dtype=torch.float32, device=dev)
-    if impl == "auto":
-        # decide on the host (cached per parameter version) so that only ONE of the two kernels is enqueued; the library's
-        # own device-side check stays in force (a forced tensor-core call on a kernel set without cover writes zeros)
-        impl = "tcgen05" if (Lq * K <= 512 and K <= 16 and tkl_kernel_set_covers(mu, sigma)) else "simt"
+    impl = _tkl_impl(impl, Lq, K, mu, sigma)
     _launch(dev, "mmb200_tkl_window_scores", q_ctx, q_mask, doc_chunks, chunk_mask, slot, mu, sigma, dense_weight, red,
             sat_params, out, B, doc_chunks.shape[0], Lq, D, C, K, sat_code, mcode, _IMPLS[impl])
+    return out
+
+
+def _tkl_impl(impl: str, Lq: int, K: int, mu: torch.Tensor, sigma: torch.Tensor) -> str:
+    """``impl="auto"`` of the window-score entries, decided on the host (cached per parameter version) so that only ONE
+    of the two kernels is enqueued; the library's own device-side check stays in force (a forced tensor-core call on a
+    kernel set without cover writes zeros)."""
+    if impl != "auto":
+        return impl
+    return "tcgen05" if (Lq * K <= 512 and K <= 16 and tkl_kernel_set_covers(mu, sigma)) else "simt"
+
+
+def tkl_store_window_scores(q_ctx: torch.Tensor, q_mask: Optional[torch.Tensor], chunks: torch.Tensor,
+                            chunk_mask: Optional[torch.Tensor], doc_slots: torch.Tensor, pair_q: torch.Tensor,
+                            pair_d: torch.Tensor, mu: torch.Tensor, sigma: torch.Tensor, dense_weight: torch.Tensor,
+                            saturation: str, sat_params: torch.Tensor, sat_red_weight: Optional[torch.Tensor] = None,
+                            impl: str = "auto") -> torch.Tensor:
+    """:func:`tkl_window_scores` against a store of packed chunks that was encoded once: window scores [n_pairs, W]
+    (inference), W = (C*40 - 30) // 2 + 1.
+
+    chunks [n_chunks, 40, D] fp32 / chunk_mask [n_chunks, 40] are packed, contextualised chunks without overlap;
+    doc_slots [n_docs, C] int32 holds the chunk index of every slot of every passage (-1: dropped by the packing, or
+    past the passage).  Pair p scores query ``pair_q[p]`` of q_ctx [n_q, Lq, D] (q_mask [n_q, Lq]) against passage
+    ``pair_d[p]``; ``pair_d[p] < 0`` has no slots and all-zero windows.  Same kernels and bit-identical windows as
+    :func:`tkl_window_scores` on the same chunks gathered into the padded layout with ``q_ctx[pair_q]`` (same impl);
+    :func:`tkl_top_hills` selects on them."""
+    if q_ctx.dim() != 3 or chunks.dim() != 3 or chunks.shape[1] != TKL_CHUNK or q_ctx.shape[-1] != chunks.shape[-1]:
+        raise _lib.MatchmakerB200Error(f"tkl_store_window_scores: expected q [n_q, Lq, D], chunks [n_chunks, 40, D]; got "
+                                       f"{tuple(q_ctx.shape)}, {tuple(chunks.shape)}")
+    if doc_slots.dim() != 2 or doc_slots.shape[0] < 1 or doc_slots.shape[1] < 1:
+        raise _lib.MatchmakerB200Error("tkl_store_window_scores: doc_slots must be [n_docs, C] with n_docs, C >= 1")
+    n_q, Lq, D = q_ctx.shape
+    if chunks.shape[0] < 1 or n_q < 1:
+        raise _lib.MatchmakerB200Error("tkl_store_window_scores: need at least one query and one chunk")
+    if q_mask is not None and tuple(q_mask.shape) != (n_q, Lq):
+        raise _lib.MatchmakerB200Error("tkl_store_window_scores: q_mask shape mismatch")
+    if chunk_mask is not None and tuple(chunk_mask.shape) != tuple(chunks.shape[:2]):
+        raise _lib.MatchmakerB200Error("tkl_store_window_scores: chunk_mask shape mismatch")
+    dev = _require_cuda(q_ctx, q_mask, chunks, chunk_mask, doc_slots, pair_q, pair_d, mu, sigma, dense_weight,
+                        sat_params, sat_red_weight)
+    q_ctx, chunks = _f32c(q_ctx), _f32c(chunks)
+    doc_slots = doc_slots.to(torch.int32).contiguous()
+    pair_q, pair_d = _pairs(pair_q, pair_d)
+    q_mask, chunk_mask, mcode, _, mu, sigma, dense_weight, red, sat_params, sat_code = _tkl_operands(
+        q_mask, chunk_mask, None, mu, sigma, dense_weight, sat_red_weight, sat_params, saturation)
+    K = mu.numel()
+    n_docs, C = doc_slots.shape
+    W = (C * TKL_CHUNK - TKL_WINDOW) // 2 + 1
+    out = torch.empty((pair_q.numel(), W), dtype=torch.float32, device=dev)
+    impl = _tkl_impl(impl, Lq, K, mu, sigma)
+    _launch(dev, "mmb200_tkl_store_window_scores", q_ctx, q_mask, chunks, chunk_mask, doc_slots, pair_q, pair_d, mu,
+            sigma, dense_weight, red, sat_params, out, n_q, chunks.shape[0], n_docs, pair_q.numel(), Lq, D, C, K,
+            sat_code, mcode, _IMPLS[impl])
     return out
 
 

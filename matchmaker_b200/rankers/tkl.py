@@ -11,7 +11,7 @@ from typing import List
 import torch
 import torch.nn as nn
 
-from .. import autograd
+from .. import autograd, interaction
 from .tk import sinusoid_position_features
 
 
@@ -32,6 +32,13 @@ def chunk_documents(document_embeddings: torch.Tensor, document_mask: torch.Tens
     cmask2 = cmask.reshape(-1, ext)
     packed = cmask2[:, overlap:-overlap].sum(-1) != 0
     return chunks2, cmask2, packed, pieces
+
+
+def chunk_slots(doc_length: int, chunk_size: int = 40, overlap: int = 5) -> int:
+    """Chunk slots C of a document padded to doc_length positions: the ``pieces`` of :func:`chunk_documents`."""
+    ext = chunk_size + 2 * overlap
+    needed = ext - ((doc_length - overlap) % chunk_size) if doc_length > overlap else ext - overlap - doc_length
+    return (overlap + doc_length + needed - ext) // chunk_size + 1
 
 
 class TKL_sigir20(nn.Module):
@@ -59,6 +66,7 @@ class TKL_sigir20(nn.Module):
             # the reference's "idf" / "linear" branches read an undefined `query_idfs` (sigir20_tkl.py:215,237)
             raise ValueError("tk_saturation_type must be 'embedding' or 'log' (the other reference branches are dead code)")
         n_kernels = len(kernels_mu)
+        self.max_length = max_length
         self.use_pos_encoding = use_pos_encoding
         self.use_diff_posencoding = use_diff_posencoding
         self.re_use_encoding = True
@@ -134,6 +142,43 @@ class TKL_sigir20(nn.Module):
         return score, {"score": score, "orig_score": orig_score, "top_non_overlapping_idx": top_idx,
                        "orig_doc_len": document_pad_oov_mask.sum(dim=-1), "top_k_non_overlapping": top15,
                        "total_chunks": chunks2.shape[0], "packed_chunks": docs_packed.shape[0]}
+
+    @torch.no_grad()
+    def encode_documents(self, document_embeddings: torch.Tensor, document_mask: torch.Tensor):
+        """The document half of ``forward`` (sigir20_tkl.py:142-175) for a store that is encoded once: chunking,
+        packing, the transformer over every packed chunk (alone, with the same positions) and the overlap trim.  None of
+        it depends on the query or on the rest of the batch.  Returns (chunks [n_packed, 40, D] fp32, chunk masks
+        [n_packed, 40], the slot of every chunk within its passage [n_packed] int64, packed chunks per passage [B]
+        int64), passages in batch order and each passage's chunks in slot order.  ``score_store`` over them gives what
+        ``forward`` gives the passages padded to any length at least as long as them."""
+        chunks2, cmask2, packed, pieces = self.chunk_documents(document_embeddings, document_mask)
+        docs_packed = chunks2[packed]
+        pad_packed = cmask2[packed]
+        docs_ctx, _ = self.forward_representation(docs_packed, pad_packed,
+                                                  self.positional_features_d[:, :docs_packed.shape[1], :])
+        chunks = docs_ctx[:, self.overlap:-self.overlap, :].float().contiguous()
+        chunk_mask = pad_packed[:, self.overlap:-self.overlap].contiguous()
+        slots = torch.arange(packed.numel(), device=packed.device)[packed] % pieces
+        return chunks, chunk_mask, slots, packed.view(-1, pieces).sum(dim=1)
+
+    @torch.no_grad()
+    def score_store(self, query_ctx: torch.Tensor, query_mask: torch.Tensor, chunks: torch.Tensor,
+                    chunk_mask: torch.Tensor, doc_slots: torch.Tensor, pair_q: torch.Tensor, pair_d: torch.Tensor,
+                    output_secondary_output: bool = False):
+        """The interaction stage of ``forward`` over chunks from ``encode_documents`` (inference): pair p scores query
+        ``pair_q[p]`` of query_ctx [n_q, Lq, D] (``forward_representation`` with ``positional_features_q``) against the
+        chunk slots ``doc_slots[pair_d[p]]`` (see ``interaction.tkl_store_window_scores``), then the top-3 windows.
+        With ``output_secondary_output`` also returns ``forward``'s ``score`` / ``orig_score`` /
+        ``top_non_overlapping_idx`` / ``top_k_non_overlapping`` entries: the selected regions of every pair."""
+        sat_params, sat_red = self._saturation_params()
+        window = interaction.tkl_store_window_scores(query_ctx, query_mask, chunks, chunk_mask, doc_slots, pair_q, pair_d,
+                                                     self.mu, self.sigma, self.dense.weight, self.saturation_type,
+                                                     sat_params, sat_red)
+        score, orig_score, top_idx, top15 = interaction.tkl_top_hills(window, self.chunk_scoring)
+        if not output_secondary_output:
+            return score
+        return score, {"score": score, "orig_score": orig_score, "top_non_overlapping_idx": top_idx,
+                       "top_k_non_overlapping": top15}
 
     def forward_representation(self, sequence_embeddings: torch.Tensor, sequence_mask: torch.Tensor,
                                positional_features=None):
