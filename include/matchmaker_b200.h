@@ -365,6 +365,29 @@ MMB200_API int mmb200_tkl_bwd(const float* q, const void* q_mask, const float* c
                               float* workspace, int64_t B, int64_t n_chunks, int32_t Lq, int32_t D, int32_t C,
                               int32_t K, int32_t saturation, int32_t mask_dtype, void* stream);
 
+/* The same backward with shared memory independent of D, for BERT-width embeddings (DESIGN 3.3c): same arguments and
+ * outputs as mmb200_tkl_bwd; the work is split by 64-feature blocks over the union of the positions that the gathered
+ * windows cover (<= 114 per document), with fp32 FFMA throughout.
+ *   Envelope: 1 <= Lq <= 40, 1 <= K <= 16, D a multiple of 4 with 4 <= D <= 1024, C >= 1, either saturation; outside it
+ *   the call returns MMB200_ERR_UNSUPPORTED before any launch.
+ *   workspace: mmb200_tkl_bwd_wide_workspace_floats(B, D, K, saturation) floats (the per-document parameter partials,
+ *   then the per-feature-block partial products and the per-document gradient coefficients).
+ * No allocation and no synchronisation; every output has one writer and one summation order, so two runs give the same
+ * bits and the call can be captured in a CUDA graph. */
+MMB200_API int mmb200_tkl_bwd_wide(const float* q, const void* q_mask, const float* chunks, const void* chunk_mask,
+                                   const int32_t* slot_to_packed, const float* mu, const float* sigma,
+                                   const float* dense_w, const float* sat_red_w, const float* sat_params,
+                                   const float* chunk_scoring, const int64_t* top_idx, const float* orig_score,
+                                   const float* grad_score, float* grad_q, float* grad_chunks, float* grad_params,
+                                   float* workspace, int64_t B, int64_t n_chunks, int32_t Lq, int32_t D, int32_t C,
+                                   int32_t K, int32_t saturation, int32_t mask_dtype, void* stream);
+MMB200_API int64_t mmb200_tkl_bwd_wide_workspace_floats(int64_t B, int32_t D, int32_t K, int32_t saturation);
+
+/* Which TKL backward takes (Lq, D, K), on sm_90a's 227 KB of opt-in shared memory per block (a pure function of the
+ * shape): 1 = mmb200_tkl_bwd (its one-CTA-per-document plan fits: D <= 356), 2 = mmb200_tkl_bwd_wide (up to D = 1024),
+ * 0 = neither. */
+MMB200_API int32_t mmb200_tkl_bwd_route(int32_t Lq, int32_t D, int32_t K);
+
 /* ------------------------------------------------------------------------------------------
  * Exact maximum-inner-product search with fused per-query top-k (BERT_DOT dense retrieval scoring)
  *

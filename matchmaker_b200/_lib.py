@@ -39,6 +39,9 @@ SIGNATURES = {
     "mmb200_tkl_window_scores": (_c.c_int, [_vp] * 11 + [_i64, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
     "mmb200_tkl_store_window_scores": (_c.c_int, [_vp] * 13 + [_i64] * 4 + [_i32] * 7 + [_vp]),
     "mmb200_tkl_bwd": (_c.c_int, [_vp] * 18 + [_i64, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "mmb200_tkl_bwd_wide": (_c.c_int, [_vp] * 18 + [_i64, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "mmb200_tkl_bwd_wide_workspace_floats": (_i64, [_i64, _i32, _i32, _i32]),
+    "mmb200_tkl_bwd_route": (_i32, [_i32, _i32, _i32]),
     "mmb200_tkl_top_hills": (_c.c_int, [_vp] * 6 + [_i64, _i32, _vp]),
     "mmb200_tkl_slot_map": (_c.c_int, [_vp, _vp, _i64, _vp]),
     "mmb200_flat_ip_workspace_bytes": (_i64, [_i64, _i64, _i32]),

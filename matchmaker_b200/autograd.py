@@ -155,9 +155,12 @@ class _TklInteraction(torch.autograd.Function):
         (q_ctx, q_mask, doc_chunks, chunk_mask, packed, mu, sigma, dense_w, sat_params, sat_red_w, chunk_scoring, top_idx,
          orig) = ctx.saved_tensors
         red = sat_red_w if ctx.has_red else None
-        gq, gc, g_dense, g_cs, g_sat, g_red = interaction.tkl_bwd(q_ctx, q_mask, doc_chunks, chunk_mask, packed, ctx.pieces,
-                                                                  mu, sigma, dense_w, ctx.saturation, sat_params, red,
-                                                                  chunk_scoring, top_idx, orig, g_score)
+        # the one-CTA-per-document kernel where its shared-memory plan fits, the feature-split one at BERT widths
+        route = interaction.tkl_bwd_route(q_ctx.shape[1], q_ctx.shape[2], mu.numel())
+        bwd = interaction.tkl_bwd_wide if route == "tkl_bwd_wide" else interaction.tkl_bwd
+        gq, gc, g_dense, g_cs, g_sat, g_red = bwd(q_ctx, q_mask, doc_chunks, chunk_mask, packed, ctx.pieces,
+                                                  mu, sigma, dense_w, ctx.saturation, sat_params, red, chunk_scoring,
+                                                  top_idx, orig, g_score)
         return (gq.to(q_ctx.dtype), None, gc.to(doc_chunks.dtype), None, None, None, None, None, g_dense.view_as(dense_w),
                 None, g_sat.view_as(sat_params), None if g_red is None else g_red.view_as(sat_red_w),
                 g_cs.view_as(chunk_scoring))

@@ -1214,14 +1214,18 @@ def maxsim_store(q: torch.Tensor, store: torch.Tensor, doc_offsets: torch.Tensor
     return out
 
 
-def tkl_bwd(q_ctx, q_mask, doc_chunks, chunk_mask, packed_indices, chunk_pieces, mu, sigma, dense_weight, saturation,
-            sat_params, sat_red_weight, chunk_scoring, top_idx, orig_score, grad_score):
-    """Gradients of the TKL interaction stage: returns (grad_q_ctx, grad_doc_chunks, grad_dense_weight [K],
-    grad_chunk_scoring [15], grad_sat_params, grad_sat_red_weight or None).
+TKL_BWD_ROUTES = {0: None, 1: "tkl_bwd", 2: "tkl_bwd_wide"}
 
-    Envelope: 1 <= Lq <= 40, 1 <= K <= 16, D a multiple of 4 up to what the kernel's shared-memory plan holds, D <= 356
-    on an H100 (227 KB per block); outside it the call raises MatchmakerB200Error before any launch.  The forward accepts
-    wider D through the tensor-core kernel, so a model with D > 356 can score but not train."""
+
+def tkl_bwd_route(Lq: int, D: int, K: int) -> Optional[str]:
+    """Which TKL backward takes (Lq, D, K) on an H100: "tkl_bwd" where its one-CTA-per-document shared-memory plan fits
+    (D <= 356), "tkl_bwd_wide" above that up to D = 1024, None outside both envelopes (mmb200_tkl_bwd_route)."""
+    return TKL_BWD_ROUTES[int(_lib.load().mmb200_tkl_bwd_route(int(Lq), int(D), int(K)))]
+
+
+def _tkl_bwd_call(entry, q_ctx, q_mask, doc_chunks, chunk_mask, packed_indices, chunk_pieces, mu, sigma, dense_weight,
+                  saturation, sat_params, sat_red_weight, chunk_scoring, top_idx, orig_score, grad_score):
+    """The launch both TKL backward entries share; ``entry`` picks the library call and sizes its workspace."""
     dev = _require_cuda(q_ctx, doc_chunks, grad_score)
     q_ctx = q_ctx.float().contiguous()
     doc_chunks = doc_chunks.float().contiguous()
@@ -1235,10 +1239,40 @@ def tkl_bwd(q_ctx, q_mask, doc_chunks, chunk_mask, packed_indices, chunk_pieces,
     gq = torch.empty_like(q_ctx)
     gc = torch.empty_like(doc_chunks)
     gp = torch.empty(stride, dtype=torch.float32, device=dev)
-    ws = torch.empty(max(1, B) * stride, dtype=torch.float32, device=dev)
-    _launch(dev, "mmb200_tkl_bwd", q_ctx, q_mask, doc_chunks, chunk_mask, slot, mu, sigma, dense_weight, red, sat_params,
+    if entry == "mmb200_tkl_bwd":
+        n_ws = max(1, B) * stride
+    else:
+        n_ws = max(1, int(_lib.load().mmb200_tkl_bwd_wide_workspace_floats(B, D, K, sat_code)))
+    ws = torch.empty(n_ws, dtype=torch.float32, device=dev)
+    _launch(dev, entry, q_ctx, q_mask, doc_chunks, chunk_mask, slot, mu, sigma, dense_weight, red, sat_params,
             _f32c(chunk_scoring).view(-1), top_idx.contiguous(), orig_score.contiguous(), _f32c(grad_score), gq, gc, gp,
             ws, B, doc_chunks.shape[0], Lq, D, C, K, sat_code, mcode)
     g_dense, g_cs, g_sat = gp[:K], gp[K:K + 15], gp[K + 15:K + 15 + n_sat]
     g_red = gp[K + 15 + n_sat:] if sat_code == 0 else None
     return gq, gc, g_dense, g_cs, g_sat, g_red
+
+
+def tkl_bwd(q_ctx, q_mask, doc_chunks, chunk_mask, packed_indices, chunk_pieces, mu, sigma, dense_weight, saturation,
+            sat_params, sat_red_weight, chunk_scoring, top_idx, orig_score, grad_score):
+    """Gradients of the TKL interaction stage: returns (grad_q_ctx, grad_doc_chunks, grad_dense_weight [K],
+    grad_chunk_scoring [15], grad_sat_params, grad_sat_red_weight or None).
+
+    Envelope: 1 <= Lq <= 40, 1 <= K <= 16, D a multiple of 4 up to what the kernel's shared-memory plan holds, D <= 356
+    on an H100 (227 KB per block); outside it the call raises MatchmakerB200Error before any launch.  Wider embeddings,
+    up to D = 1024, train through :func:`tkl_bwd_wide`; :func:`tkl_bwd_route` says which of the two takes a shape."""
+    return _tkl_bwd_call("mmb200_tkl_bwd", q_ctx, q_mask, doc_chunks, chunk_mask, packed_indices, chunk_pieces, mu,
+                         sigma, dense_weight, saturation, sat_params, sat_red_weight, chunk_scoring, top_idx, orig_score,
+                         grad_score)
+
+
+def tkl_bwd_wide(q_ctx, q_mask, doc_chunks, chunk_mask, packed_indices, chunk_pieces, mu, sigma, dense_weight,
+                 saturation, sat_params, sat_red_weight, chunk_scoring, top_idx, orig_score, grad_score):
+    """:func:`tkl_bwd` with shared memory independent of D: the same arguments and outputs, for BERT-width embeddings.
+
+    Envelope: 1 <= Lq <= 40, 1 <= K <= 16, D a multiple of 4 with 4 <= D <= 1024; outside it the call raises
+    MatchmakerB200Error before any launch.  It also takes D <= 356, where :func:`tkl_bwd` runs too; the two agree within
+    fp32 rounding, not bit for bit.  fp32 FFMA throughout; deterministic, and free of allocation and synchronisation
+    inside the library call (the workspace is allocated here)."""
+    return _tkl_bwd_call("mmb200_tkl_bwd_wide", q_ctx, q_mask, doc_chunks, chunk_mask, packed_indices, chunk_pieces, mu,
+                         sigma, dense_weight, saturation, sat_params, sat_red_weight, chunk_scoring, top_idx, orig_score,
+                         grad_score)
