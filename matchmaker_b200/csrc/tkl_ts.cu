@@ -237,8 +237,10 @@ __device__ __forceinline__ void tkl_plan_body(const int32_t* __restrict__ slot_t
   if (in_smem)
     for (int64_t i = t; i <= B; i += 1024) { plan[2 + i] = s_tile[i]; plan[3 + B + i] = s_cost[i]; }
   // Cover: activation k is non-zero (ex2_approx) for |c - mu_k| * a_k <= sqrt(126); 11.0 leaves a margin.  The union of
-  // the intervals [klo, khi] covers [-1.01, 1.01] iff the left end and every right end inside the range lie inside an
-  // interval that extends beyond them -- one thread per end point instead of a serial sweep.
+  // the intervals [klo, khi) covers [-1.01, 1.01) iff the left end and every right end inside the range lie inside an
+  // interval that extends beyond them -- one thread per end point instead of a serial sweep.  interaction.py's
+  // tkl_kernel_set_covers restates this test in float32, rounding for rounding: where it says covered, impl="auto"
+  // enqueues this kernel alone, so an answer of "not covered" here would leave the windows at the memset zeros.
   __shared__ int uncovered;
   if (t == 0) uncovered = 0;
   __syncthreads();

@@ -6,6 +6,7 @@ PyTorch is plumbing here: it owns device memory and the current stream; the arit
 from __future__ import annotations
 
 import ctypes
+import weakref
 from typing import Optional, Tuple
 
 import torch
@@ -406,27 +407,34 @@ _TKL_COVER_CACHE = {}
 def tkl_kernel_set_covers(mu: torch.Tensor, sigma: torch.Tensor) -> bool:
     """True when every cosine in [-1, 1] activates at least one RBF kernel under ex2.approx.ftz, i.e. when the window
     token count of sigir20_tkl.py:210 equals the count of unmasked positions (tkl_ts.cu explains why that matters).
-    Same sweep as the device-side plan kernel; evaluated on the host once per (mu, sigma) tensor version -- they are
-    constant buffers of the model -- so that the launch path knows which kernel to enqueue without a device round trip."""
+    Evaluated on the host once per (mu, sigma) tensor version -- they are constant buffers of the model -- so that the
+    launch path knows which kernel to enqueue without a device round trip.
+
+    It is the plan kernel's own test (tkl_ts.cu: tkl_plan_body), every step rounded to float32 as there: the intervals
+    [mu - h, mu + h) with h = 11 sigma / rbf_scale(1), and the left end -1.01 and every right end below 1.01 inside an
+    interval that extends past it.  The answers must agree: when this one says covered, ``impl="auto"`` enqueues the
+    tensor-core kernel alone, and that kernel writes nothing for a set the plan kernel finds uncovered.  In doubles,
+    intervals that miss each other by one float32 ulp overlap."""
+    # The address and version alone do not name a tensor: once it is freed, the caching allocator hands its address to
+    # the next one, at version 0 again.  An entry also holds weak references to the storages it was computed for (one
+    # Python object per storage, shared by its views and detached aliases) and counts only while they are alive.
+    mb, sb = mu.untyped_storage(), sigma.untyped_storage()
     key = (mu.data_ptr(), mu._version, sigma.data_ptr(), sigma._version, mu.numel())
     hit = _TKL_COVER_CACHE.get(key)
-    if hit is not None:
-        return hit
-    m, sg = mu.detach().float().view(-1).cpu().tolist(), sigma.detach().float().view(-1).cpu().tolist()
-    x, ok = -1.01, True
-    while x < 1.01:
-        reach = x
-        for mk, sk in zip(m, sg):
-            h = 11.0 * sk / (0.5 * 1.4426950408889634) ** 0.5
-            if mk - h <= x and mk + h > reach:
-                reach = mk + h
-        if reach <= x:
-            ok = False
-            break
-        x = reach
+    if hit is not None and hit[1]() is mb and hit[2]() is sb:
+        return hit[0]
+    f32 = torch.float32
+    m, sg = mu.detach().to("cpu", f32).view(-1), sigma.detach().to("cpu", f32).view(-1)
+    scale = torch.sqrt(torch.tensor(0.5, dtype=f32) * torch.tensor(1.4426950408889634, dtype=f32))   # rbf_scale(1.0f)
+    h = (sg * torch.tensor(11.0, dtype=f32)) / scale
+    klo, khi = m - h, m + h
+    lo, hi = torch.tensor(-1.01, dtype=f32), torch.tensor(1.01, dtype=f32)
+    ends = torch.cat([lo.view(1), khi])
+    inside = ((klo[None, :] <= ends[:, None]) & (khi[None, :] > ends[:, None])).any(dim=1)
+    ok = bool((inside | ~((ends >= lo) & (ends < hi))).all())
     if len(_TKL_COVER_CACHE) > 64:
         _TKL_COVER_CACHE.clear()
-    _TKL_COVER_CACHE[key] = ok
+    _TKL_COVER_CACHE[key] = (ok, weakref.ref(mb), weakref.ref(sb))
     return ok
 
 
