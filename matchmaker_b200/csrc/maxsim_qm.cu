@@ -16,7 +16,9 @@
 // Only live rows are fetched.  A document's live rows are [0, live) with live = 1 + its last unmasked row (Ld without a
 // mask; the passage's length in store mode); it takes nch = max(1, ceil(live / 64)) chunks of the stage ring.  In the
 // padded layout the chunks are END-aligned: chunk ch starts at row live - 64 (nch - ch), so the first one may start
-// below row 0, where TMA zero-fills without reading HBM, and no padding row is read.  Store mode stays start-aligned
+// below row 0, where TMA zero-fills without reading HBM, and no padding row is read.  A first chunk whose lower half
+// lies wholly below row 0 loads only its upper half (a 32-row box per k-block): skipping the zero fill measured
+// faster.  Store mode stays start-aligned
 // (below a passage's first row lie the previous passage's rows), so its last chunk holds rows past `live`.  A document
 // with no live row takes one chunk that is not fetched (the stage holds whatever it held before).  The mask is applied
 // in the reduction as an fp32 penalty per row, 0 for live unmasked rows and -inf for every other row (rows below 0
@@ -35,8 +37,9 @@
 //
 // Per CTA (persistent, one per SM, 384 threads = 3 warpgroups):
 //   warp 0        TMA producer: query tile (2-slot ring, re-fetched when the query changes), document chunks: one
-//                 {64, 64 rows, dim / 64} box per chunk (rows below 0 and past Ld are zero-filled by TMA and cost no
-//                 HBM traffic), issued by one elected lane of the converged warp
+//                 {64, 64 rows, dim / 64} box per chunk, or one 32-row box per k-block for the upper half of a first
+//                 chunk whose lower half is below row 0 (rows below 0 and past Ld are zero-filled by TMA and cost no HBM
+//                 traffic), issued by one elected lane of the converged warp
 //   warps 1-3     mask scouts: scout s takes the CTA's documents s, s + 3, ...; per document it ballots the mask words
 //                 of its rows (keeping its next two documents' words in flight) and fills the document's record
 //   warpgroups 1, 2  consumers: warpgroup c takes the CTA's documents c, c + 2, ...; per chunk 4 * dim / 64 wgmma
@@ -130,10 +133,12 @@ struct RecCursor {
   }
 };
 
-// Tensor maps of the query tile and of the document chunks ({64, 64 rows, kblocks, 1} boxes).
+// Tensor maps of the query tile and of the document chunks: {64, 64 rows, kblocks, 1} boxes, and {64, 32 rows, 1, 1}
+// boxes for the upper half of one k-block of a padded first chunk whose lower half lies wholly below row 0.
 struct QmMaps {
   CUtensorMap q;
   CUtensorMap d;
+  CUtensorMap dh;
 };
 
 // One warp's own sequence of pairs p = first, first + step, ... < end and what the warp needs of each: its query, its
@@ -254,6 +259,7 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
   if (threadIdx.x == 0) {
     prefetch_tensormap(&M.q);
     prefetch_tensormap(&M.d);
+    if (!kStore) prefetch_tensormap(&M.dh);
     for (int s = 0; s < L.stages; ++s) { mbar_init(&S->full[s], 1); mbar_init(&S->empty[s], 4); }
     for (int s = 0; s < kQSlots; ++s) { mbar_init(&S->qfull[s], 1); mbar_init(&S->qempty[s], 8); }
     for (int r = 0; r < L.records; ++r) {
@@ -323,13 +329,22 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
         mbar_wait(&S->empty[stage], ph_cur ^ 1u);
         QM_PROF(prof[kPrEmpty] += clock64() - t_; t_ = clock64(); ++prof[kPrChunks];)
         if (elect_one_sync()) {
+          uint8_t* dst = stage_base + (size_t)stage * L.chunk_bytes;
           if (live == 0) {
             mbar_arrive(&S->full[stage]);
+          } else if (!kStore && row + kChunkRows / 2 <= 0) {
+            // a first chunk with at most 32 rows at or above row 0: only the upper half of each k-block is loaded.
+            // The lower half keeps whatever the stage held; those rows are below 0, so their penalty is -inf and no
+            // value there (NaN and inf included) can win a max.
+            mbar_arrive_expect_tx(&S->full[stage], (uint32_t)(L.chunk_bytes / 2));
+            for (int kb = 0; kb < L.kblocks; ++kb)
+              tma_load_4d(&M.dh, dst + kb * kChunkKBlockBytes + kChunkKBlockBytes / 2, &S->full[stage], 0,
+                          row + kChunkRows / 2, kb, dcoord, kEvictFirst);
           } else {
             // one full box per chunk: the zero fill below row 0 and past Ld costs no HBM traffic, and short boxes
             // cost more TMA issues and handshakes than they save
             mbar_arrive_expect_tx(&S->full[stage], (uint32_t)L.chunk_bytes);
-            tma_load_4d(&M.d, stage_base + (size_t)stage * L.chunk_bytes, &S->full[stage], 0, row, 0, dcoord, kEvictFirst);
+            tma_load_4d(&M.d, dst, &S->full[stage], 0, row, 0, dcoord, kEvictFirst);
           }
         }
         __syncwarp();
@@ -357,19 +372,15 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
     PairStream<kStore> meta(P, p_begin + s, p_end, kScouts, lane);
     RecCursor rc{s, 0};
     int64_t fp = p_begin + s;           // next pair whose mask words are loaded
-    // mask words folded to 32 bits (an int64 word's halves OR-ed: only zero / nonzero matters; fp32 keeps its bits)
-    auto load_win = [&](uint32_t (&raw)[kW], int64_t dm, int w) {
+    // mask words as loaded: nothing reads them before the document is scanned, so the loads stay in flight until then
+    auto load_win = [&](uint64_t (&raw)[kW], int64_t dm, int w) {
 #pragma unroll
       for (int k = 0; k < kW; ++k) {
         const int g = w * 32 * kW + 32 * k + lane;
-        raw[k] = 1;
-        if (dmt != MMB200_MASK_NONE && g < P.Ld) {
-          const uint64_t v = mask_raw(P.d_mask, dmt, dm * (int64_t)P.Ld + g);
-          raw[k] = (uint32_t)(v | (v >> 32));
-        }
+        raw[k] = (dmt != MMB200_MASK_NONE && g < P.Ld) ? mask_raw(P.d_mask, dmt, dm * (int64_t)P.Ld + g) : 1;
       }
     };
-    auto fetch = [&](uint32_t (&raw)[kW], int64_t& dm, int& lim) {
+    auto fetch = [&](uint64_t (&raw)[kW], int64_t& dm, int& lim) {
       if (fp < p_end) {
         meta.next();
         dm = meta.dm();
@@ -381,7 +392,7 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
     // one document: wait for its record slot, scan its mask into the record, prefetch the scout's document after next
     // into `raw`, hand the record over
     QM_PROF(unsigned long long prof_re = 0; const long long t_start = clock64();)
-    auto doc = [&](uint32_t (&raw)[kW], int64_t& dm, int& lim) {
+    auto doc = [&](uint64_t (&raw)[kW], int64_t& dm, int& lim) {
       QM_PROF(const long long t_ = clock64();)
       mbar_wait(&S->rempty[rc.slot], rc.phase ^ 1u);
       QM_PROF(prof_re += clock64() - t_;)
@@ -411,7 +422,7 @@ maxsim_qm_kernel(const __grid_constant__ QmMaps M, MaxsimParams P, QmLaunch L) {
       }
       rc.advance(kScouts, L.records);
     };
-    uint32_t ra[kW], rb[kW];
+    uint64_t ra[kW], rb[kW];
     int64_t dma = 0, dmb = 0;
     int la = 0, lb = 0;
     fetch(ra, dma, la);
@@ -717,6 +728,11 @@ int maxsim_qm_launch(const MaxsimParams& P, int dtype, const DeviceInfo& dev, cu
     if (int rc = encode_tensor_map(&M.d, tdt, 4, P.d, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B,
                                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B))
       return rc;
+    const uint32_t half[4] = {64, (uint32_t)kChunkRows / 2, 1, 1};
+    if (!P.doc_offsets)   // store mode never takes half boxes
+      if (int rc = encode_tensor_map(&M.dh, tdt, 4, P.d, dims, strides, half, CU_TENSOR_MAP_SWIZZLE_128B,
+                                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B))
+        return rc;
   }
   *handled = true;
   const int grid = (int)std::min<int64_t>(dev.sm_count, P.n_pairs);
